@@ -33,17 +33,36 @@
 //   3. EPILOGUE (the same warpgroup, after each pass): add rowsum * bias to the accumulator registers, ReLU, store.
 // No reference counterpart as a kernel; callers cogdl/layers/gcn_layer.py:51-64 (and sage_layer.py:69-87 for the
 // aggregate-then-linear order).  K (input width) must be 128, Fout <= 128.
+//
+// GraphSAGE form (cogdl/layers/sage_layer.py:69-87, fc(cat[x, agg]) with fc.weight = [W_self | W_neigh]):
+//     OUT[i,:] = act( S[i,:] + agg_i(X) . W_neigh^T ),   S = X[:n] . W_self^T + b   (library GEMM, beforehand)
+// The same kernel, templated on the aggregation (AGG) and on the epilogue addend (EPI):
+//   AGG_SUM  the gather above, optionally times a per-row fp32 scale (graph.in_norm of a CSR-only graph, applied
+//            to the fp32 row before the split, hub rows included: bit-identical to `in_norm * spmm(...)`);
+//            mean is SUM with row-normalised edge weights or with that scale;
+//   AGG_MAX  running max from -inf with the strict `<` update of scatter_max.cu, degree-0 rows 0 (bit-identical to
+//            scatter_max_fwd's values; no argmax: the backward recomputes it).  Hub rows come from a pre-pass of
+//            scatter_max's row-stream kernel (hub chunks only, argmax stores compiled out);
+//   EPI_BIAS add rowsum * bias (GCN);  EPI_SELF add S[row, c] (SAGE).
+// The self half is not put on the tensor cores: a bf16x3 W^T for K = 256 takes 192 KB, and the two 48 KB operand
+// tiles do not fit beside it in the SM's 227 KB.  W_neigh ([Fout,128]) fills the 96 KB W^T buffer as W does for GCN.
 #include "common.cuh"
 #include "stream.cuh"
 
 #include <cuda_bf16.h>
+#include <math_constants.h>
 
 namespace cogdl_b200 {
 
 int spmm_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X, float *Y,
                        int64_t F, const cogdl_b200_hub_plan_t *plan, cudaStream_t stream);
+int smax_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float *X, float *Y, int64_t F,
+                       const cogdl_b200_hub_plan_t *plan, cudaStream_t stream);
 
 namespace fg {
+
+enum { AGG_SUM = 0, AGG_MAX = 1 };
+enum { EPI_BIAS = 0, EPI_SELF = 1 };
 
 constexpr int TILE_M = 64;                            // rows per tile (wgmma M = 64); two tiles are in flight per CTA
 constexpr int GROUPS = 2;                             // independent warp groups, one tile each, W^T shared
@@ -82,6 +101,9 @@ struct Params {
   int chunk_edges;         // 0: no hub rows anywhere
   int relu;
   int n_tiles;
+  // EPI_SELF only (appended so the fields above keep their offsets)
+  const float *row_scale;  // nullable [n_rows]: multiplies the aggregated row (AGG_SUM)
+  const float *S;          // [n_rows, Fout]: epilogue addend
 };
 
 // ------------------------------------------------------------------ PTX wrappers
@@ -158,6 +180,22 @@ __device__ __forceinline__ void store_row(unsigned char *tileA, int r, int lane,
   *reinterpret_cast<uint2 *>(tileA + 2 * 2 * SLAB_BYTES_A + off) = make_uint2(pack2(s3[0], s3[1]), pack2(s3[2], s3[3]));
 }
 
+// AGG_MAX accumulator: strict `<` as scatter_max.cu (first value wins ties, a NaN never replaces the running max)
+__device__ __forceinline__ void max_upd(float4 &m, const float4 &x) {
+  if (m.x < x.x) m.x = x.x;
+  if (m.y < x.y) m.y = x.y;
+  if (m.z < x.z) m.z = x.z;
+  if (m.w < x.w) m.w = x.w;
+}
+template <int AGG> __device__ __forceinline__ float4 agg_init() {
+  return AGG == AGG_MAX ? make_float4(-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F)
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+// the row scale as `in_norm * x` applies it: one rounded product (never contracted into the split's subtractions)
+__device__ __forceinline__ float4 scale_row(const float4 &a, float s) {
+  return make_float4(__fmul_rn(s, a.x), __fmul_rn(s, a.y), __fmul_rn(s, a.z), __fmul_rn(s, a.w));
+}
+
 // rowptr and cost prefix of one 64-row tile -> shared memory (one warp: lane L takes rows 2L, 2L+1).  cost(row) =
 // 1 + (hub ? 4 : deg): hub rows are one 512-byte read here, their edges were consumed by the hub pre-pass
 __device__ __forceinline__ void stage_tile(const Params &p, int row0, int lane, int *tile_rp, int *tile_cost) {
@@ -187,7 +225,8 @@ __device__ __forceinline__ void stage_tile(const Params &p, int row0, int lane, 
   if (lane == 31) { tile_rp[TILE_M] = rp[2]; tile_cost[TILE_M] = run; }
 }
 
-__global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p) {
+template <int AGG, int EPI>
+__global__ void __launch_bounds__(WARPS * 32, 1) fused_layer_kernel(const Params p) {
   extern __shared__ unsigned char fg_smem_raw[];
   // SWIZZLE_128B atoms need a 1024-byte aligned base
   unsigned char *smem = fg_smem_raw + ((1024u - (smem_u32(fg_smem_raw) & 1023u)) & 1023u);   // stays a shared-space pointer
@@ -255,7 +294,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
       auto zero_rows = [&](int upto) {   // rows [next_row, upto): no edges -> zeros
         for (; next_row < upto; ++next_row) {
           store_row(tileA, next_row - row0, lane, make_float4(0.f, 0.f, 0.f, 0.f));
-          if (lane == 0) rowsum_s[next_row - row0] = 0.f;
+          if (EPI == EPI_BIAS && lane == 0) rowsum_s[next_row - row0] = 0.f;
         }
       };
       int r = r_begin;
@@ -263,9 +302,11 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
         const int lb = tile_rp[r - row0], hb = tile_rp[r - row0 + 1];
         if (p.chunk_edges > 0 && hb - lb > p.chunk_edges) {
           // hub row: aggregated beforehand (hub chunks of the row-stream kernel)
-          const float4 a = __ldg(H4 + (int64_t)r * (KDIM / 4) + lane);
+          float4 a = __ldg(H4 + (int64_t)r * (KDIM / 4) + lane);
           float s = 0.f;
-          if (p.rowsum) {
+          if (EPI == EPI_SELF) {
+            if (p.row_scale) a = scale_row(a, __ldg(p.row_scale + r));
+          } else if (p.rowsum) {
             s = __ldg(p.rowsum + r);
           } else if (p.val) {      // no cached row sums: one warp sums the hub's weights, 8 loads in flight per lane
             float sa[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -281,7 +322,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
             s = (float)(hb - lb);
           }
           store_row(tileA, r - row0, lane, a);
-          if (lane == 0) rowsum_s[r - row0] = s;
+          if (EPI == EPI_BIAS && lane == 0) rowsum_s[r - row0] = s;
           next_row = r + 1;
           ++r;
           continue;
@@ -290,14 +331,15 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
         int rb = r + 1;
         while (rb < r_end && !(p.chunk_edges > 0 && tile_rp[rb - row0 + 1] - tile_rp[rb - row0] > p.chunk_edges)) ++rb;
         const int e_begin = lb, e_end = tile_rp[rb - row0];
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 acc = agg_init<AGG>();
         float rs = 0.f;
         auto flush = [&](int rj) {                       // last edge of row rj
           zero_rows(rj);
-          store_row(tileA, rj - row0, lane, acc);
-          if (lane == 0) rowsum_s[rj - row0] = rs;
+          if (EPI == EPI_SELF && p.row_scale) store_row(tileA, rj - row0, lane, scale_row(acc, __ldg(p.row_scale + rj)));
+          else store_row(tileA, rj - row0, lane, acc);
+          if (EPI == EPI_BIAS && lane == 0) rowsum_s[rj - row0] = rs;
           next_row = rj + 1;
-          acc = make_float4(0.f, 0.f, 0.f, 0.f);
+          acc = agg_init<AGG>();
           rs = 0.f;
         };
         // slab registers (column, value, row, row of the next edge); the NEXT slab is fetched while this one is used
@@ -337,7 +379,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
             for (int u = 0; u < U; ++u) {
               if (j + u < cnt) {
                 const float vj = __int_as_float(s_cv[j + u].y);
-                if (p.val) axpy_rn(acc, vj, x[u]); else add_rn(acc, x[u]);
+                if (AGG == AGG_MAX) max_upd(acc, x[u]);
+                else if (p.val) axpy_rn(acc, vj, x[u]); else add_rn(acc, x[u]);
                 rs += vj;
                 if (em != 0u && ((em >> u) & 1u)) flush(s_r[j + u]);
               }
@@ -359,7 +402,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
       // rows of the tile beyond n_rows (last tile): zeros, dealt round-robin
       for (int rr = rows_here + gw; rr < TILE_M; rr += GWARPS) {
         store_row(tileA, rr, lane, make_float4(0.f, 0.f, 0.f, 0.f));
-        if (lane == 0) rowsum_s[rr] = 0.f;
+        if (EPI == EPI_BIAS && lane == 0) rowsum_s[rr] = 0.f;
       }
     }
     fence_async_smem();          // generic-proxy writes of the tile -> visible to the tensor core (async proxy)
@@ -403,12 +446,25 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
         const int r = wq * 16 + (lane >> 2) + 8 * i;
         const int grow = row0 + r;
         if (grow < p.n_rows) {
-          const float rsum = rowsum_s[r];
+          const float rsum = EPI == EPI_BIAS ? rowsum_s[r] : 0.f;
           float *o = p.out + (int64_t)grow * p.Fout;
 #pragma unroll
           for (int j = 0; j < WG_NP / 8; ++j) {
             const int c = col0 + 8 * j + 2 * (lane & 3);
-            float2 y = make_float2(d[4 * j + 2 * i] + rsum * bias_s[c], d[4 * j + 2 * i + 1] + rsum * bias_s[c + 1]);
+            float2 y;
+            if (EPI == EPI_BIAS) {
+              y = make_float2(d[4 * j + 2 * i] + rsum * bias_s[c], d[4 * j + 2 * i + 1] + rsum * bias_s[c + 1]);
+            } else {
+              const float *srow = p.S + (int64_t)grow * p.Fout;
+              float2 sv = make_float2(0.f, 0.f);
+              if (vec && c + 1 < p.Fout) {
+                sv = __ldcs(reinterpret_cast<const float2 *>(srow + c));
+              } else {
+                if (c < p.Fout) sv.x = __ldcs(srow + c);
+                if (c + 1 < p.Fout) sv.y = __ldcs(srow + c + 1);
+              }
+              y = make_float2(d[4 * j + 2 * i] + sv.x, d[4 * j + 2 * i + 1] + sv.y);
+            }
             if (p.relu) { y.x = fmaxf(y.x, 0.f); y.y = fmaxf(y.y, 0.f); }
             if (vec && c + 1 < p.Fout) {
               __stcs(reinterpret_cast<float2 *>(o + c), y);
@@ -422,6 +478,21 @@ __global__ void __launch_bounds__(WARPS * 32, 1) gcn_fused_kernel(const Params p
     }
     group_sync(g);               // operand tile and staged rowptr are free / ready for the next tile
   }
+}
+
+// one persistent CTA per SM (at most one per pair of tiles)
+template <int AGG, int EPI>
+static int launch(const Params &p, cudaStream_t s) {
+  static unsigned long long attr_done = 0;
+  int dev = 0, n_sms = NUM_SMS;
+  if (first_use_on_device(attr_done, &dev))
+    CB_CUDA(cudaFuncSetAttribute(fused_layer_kernel<AGG, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  CB_CUDA(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, dev));
+  const int want = (p.n_tiles + GROUPS - 1) / GROUPS;
+  const int grid = want < n_sms ? want : n_sms;
+  fused_layer_kernel<AGG, EPI><<<grid, WARPS * 32, SMEM_BYTES, s>>>(p);
+  CB_LAUNCH_CHECK();
+  return COGDL_B200_OK;
 }
 
 }  // namespace fg
@@ -458,15 +529,49 @@ extern "C" int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t *co
   p.hub_agg = hub_agg ? hub_agg : X; p.rowsum = rowsum; p.out = out; p.n_rows = (int)n_rows; p.Fout = (int)Fout;
   p.Npad = Fout <= fg::WG_N ? fg::WG_N : 2 * fg::WG_N; p.chunk_edges = plan->chunk_edges; p.relu = relu;
   p.n_tiles = (int)ceil_div(n_rows, fg::TILE_M);
-  static unsigned long long attr_done = 0;
-  int dev = 0, n_sms = NUM_SMS;
-  if (first_use_on_device(attr_done, &dev))
-    CB_CUDA(cudaFuncSetAttribute(fg::gcn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fg::SMEM_BYTES));
-  CB_CUDA(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, dev));
-  const int want = (p.n_tiles + fg::GROUPS - 1) / fg::GROUPS;
-  const int grid = want < n_sms ? want : n_sms;
-  note_kernel("cogdl_b200::fg::gcn_fused_kernel<2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>", p.Npad);
-  fg::gcn_fused_kernel<<<grid, fg::WARPS * 32, fg::SMEM_BYTES, s>>>(p);
-  CB_LAUNCH_CHECK();
-  return COGDL_B200_OK;
+  p.row_scale = nullptr; p.S = nullptr;
+  note_kernel("cogdl_b200::fg::fused_layer_kernel<gcn, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>", p.Npad);
+  return fg::launch<fg::AGG_SUM, fg::EPI_BIAS>(p, s);
+}
+
+extern "C" int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_t *colind, const float *val, const float *row_scale,
+                                         const float *X, const float *W_neigh, const float *S, float *out, float *hub_agg,
+                                         int64_t n_rows, int64_t K, int64_t Fout, int32_t aggr, int32_t relu,
+                                         const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
+  const char *who = "cogdl_b200_sage_fused_f32";
+  CB_REQUIRE(n_rows >= 0 && K >= 0 && Fout >= 0, "%s: negative size", who);
+  CB_REQUIRE(aggr == COGDL_B200_AGGR_SUM || aggr == COGDL_B200_AGGR_MAX, "%s: aggr must be COGDL_B200_AGGR_SUM or _MAX (got %d)",
+             who, (int)aggr);
+  if (n_rows == 0 || Fout == 0) return COGDL_B200_OK;
+  CB_REQUIRE(cogdl_b200_gcn_fused_supported(K, Fout), "%s: needs K == 128 and 1 <= Fout <= 128 (got K=%lld, Fout=%lld)", who,
+             (long long)K, (long long)Fout);
+  CB_REQUIRE(rowptr && colind && X && W_neigh && S && out, "%s: null pointer", who);
+  CB_REQUIRE(aggr == COGDL_B200_AGGR_SUM || (!val && !row_scale), "%s: max aggregation takes no edge values or row scale", who);
+  CB_REQUIRE(n_rows < 0x7fffff00LL, "%s: n_rows must fit int32", who);
+  CB_REQUIRE(plan && plan->chunk_edges > 0 && plan->edge_row, "%s: needs a hub plan with edge_row (row-stream form)", who);
+  CB_REQUIRE(aligned16(X) && aligned16(W_neigh) && aligned16(S) && aligned16(out), "%s: X, W_neigh, S and out must be 16-byte aligned",
+             who);
+  const int64_t elem = aggr == COGDL_B200_AGGR_MAX ? 8 : 4;       // max partials carry (value, argmax)
+  int rc = check_plan(plan, (int64_t)plan->n_chunks * K * elem);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (plan->n_chunks > 0) {
+    CB_REQUIRE(hub_agg && aligned16(hub_agg), "%s: hub_agg scratch [n_rows, 128] is required when the plan has hub rows", who);
+    rc = aggr == COGDL_B200_AGGR_MAX ? smax_hub_rows_only(rowptr, colind, X, hub_agg, K, plan, s)
+                                     : spmm_hub_rows_only(rowptr, colind, val, X, hub_agg, K, plan, s);
+    if (rc) return rc;
+  }
+  fg::Params p;
+  p.rowptr = rowptr; p.colind = colind; p.val = val; p.edge_row = plan->edge_row; p.X = X; p.W = W_neigh; p.bias = nullptr;
+  p.hub_agg = hub_agg ? hub_agg : X; p.rowsum = nullptr; p.out = out; p.n_rows = (int)n_rows; p.Fout = (int)Fout;
+  p.Npad = Fout <= fg::WG_N ? fg::WG_N : 2 * fg::WG_N; p.chunk_edges = plan->chunk_edges; p.relu = relu;
+  p.n_tiles = (int)ceil_div(n_rows, fg::TILE_M);
+  p.row_scale = row_scale; p.S = S;
+  if (aggr == COGDL_B200_AGGR_MAX) {
+    note_kernel("cogdl_b200::fg::fused_layer_kernel<sage-max, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>", p.Npad);
+    return fg::launch<fg::AGG_MAX, fg::EPI_SELF>(p, s);
+  }
+  note_kernel("cogdl_b200::fg::fused_layer_kernel<sage-sum%s, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>",
+              row_scale ? "+row_scale" : "", p.Npad);
+  return fg::launch<fg::AGG_SUM, fg::EPI_SELF>(p, s);
 }

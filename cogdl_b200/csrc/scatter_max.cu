@@ -167,8 +167,10 @@ __global__ void __launch_bounds__(256) scatter_max_fwd_kernel(const SmaxParams p
 // carries segments and a full warp owns the row (F >= 68 on the float4 path).  Hub chunks write
 // (value, argmax) partials that the last chunk to arrive combines in chunk order with the strict
 // `<` rule, so "first max wins" holds across chunks as well: results stay bit-exact.
+// ARGMAX == false tracks values only (hub-only pre-pass of the fused SAGE layer): no argmax output and no id
+// partials; the values are the same, since the in-order strict `<` combine of the partial maxima is the row's max.
 // ------------------------------------------------------------------------------------------
-template <int NV, int U>
+template <int NV, int U, bool ARGMAX = true>
 __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParams p) {
   constexpr int TILE = 32 * NV;
   const int lane = threadIdx.x & 31;
@@ -211,7 +213,7 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
           for (int k = 0; k < NV; ++k)
             if (colok[k]) {
               st_stream(O + (int64_t)(rb + k0) * p.FV + cv + k * 32, make_float4(0.f, 0.f, 0.f, 0.f));
-              st_stream(A + (int64_t)(rb + k0) * p.FV + cv + k * 32, make_int4(-1, -1, -1, -1));
+              if (ARGMAX) st_stream(A + (int64_t)(rb + k0) * p.FV + cv + k * 32, make_int4(-1, -1, -1, -1));
             }
         }
       }
@@ -254,7 +256,7 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
               for (int k = 0; k < NV; ++k)
                 if (colok[k]) {
                   st_stream(O + (int64_t)rj * p.FV + cv + k * 32, acc[k]);
-                  st_stream(A + (int64_t)rj * p.FV + cv + k * 32, id[k]);
+                  if (ARGMAX) st_stream(A + (int64_t)rj * p.FV + cv + k * 32, id[k]);
                   init_acc(acc[k], id[k]);
                 }
             }
@@ -267,7 +269,7 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
       for (int k = 0; k < NV; ++k)
         if (colok[k]) {
           st_cg(PV + (int64_t)w.slot * p.FV + cv + k * 32, acc[k]);
-          st_cg(PI + (int64_t)w.slot * p.FV + cv + k * 32, id[k]);
+          if (ARGMAX) st_cg(PI + (int64_t)w.slot * p.FV + cv + k * 32, id[k]);
         }
     }
   }
@@ -278,9 +280,9 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
         int4 idm;
         init_acc(m, idm);
         for (int q = 0; q < w.n_row_chunks; ++q)
-          upd2(m, idm, ld_cg(PV + (int64_t)(w.first + q) * p.FV + cv), ld_cg(PI + (int64_t)(w.first + q) * p.FV + cv));
+          upd2(m, idm, ld_cg(PV + (int64_t)(w.first + q) * p.FV + cv), ARGMAX ? ld_cg(PI + (int64_t)(w.first + q) * p.FV + cv) : idm);
         st_stream(O + (int64_t)w.row * p.FV + cv, m);
-        st_stream(A + (int64_t)w.row * p.FV + cv, idm);
+        if (ARGMAX) st_stream(A + (int64_t)w.row * p.FV + cv, idm);
       }
     }
   }
@@ -325,6 +327,25 @@ static int dispatch_smax(const SmaxParams &p, cudaStream_t s) {
   if (fv <= 16) return launch_smax<VecT, 16, 1>(p, s);
   if (fv <= 32) return launch_smax<VecT, 32, 1>(p, s);
   return launch_smax<VecT, 32, 2>(p, s);
+}
+
+// Only the hub rows (degree > plan chunk) of the max values, no argmax: the hub-chunk items of the row-stream
+// kernel with their in-order combine, no segments (so independent of COGDL_B200_SMAX_STREAM).  Used by the fused
+// SAGE layer (fused_gcn.cu), which aggregates every other row straight into shared memory.  F == 128, 16-byte
+// aligned X / Y; plan->partials n_chunks * F * 8 bytes.
+int smax_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float *X, float *Y, int64_t F,
+                       const cogdl_b200_hub_plan_t *plan, cudaStream_t stream) {
+  SmaxParams p;
+  p.rowptr = rowptr; p.colind = colind; p.X = X; p.out = Y; p.argmax = nullptr; p.n_rows = 0;
+  p.hub = hub_view(plan);
+  p.hub.n_segs = 0;
+  p.FV = (int)(F / 4);
+  if (p.hub.n_chunks == 0) return COGDL_B200_OK;
+  if (p.FV != 32) return set_error(COGDL_B200_EINVAL, "smax_hub_rows_only: F must be 128");
+  const int64_t blocks = ceil_div((int64_t)p.hub.n_chunks * 32, 256);
+  scatter_max_stream_kernel<1, 4, false><<<(unsigned)blocks, 256, 0, stream>>>(p);
+  CB_LAUNCH_CHECK();
+  return COGDL_B200_OK;
 }
 
 // gx[argmax[i,f], f] += g[i,f]  (red.global.add.f32; gx zero-filled by the caller below)

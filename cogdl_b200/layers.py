@@ -137,10 +137,16 @@ class MaxAggregator:
 
 
 class SAGELayer(nn.Module):
+    """fused=True (opt-in): the aggregation and the neighbour half of `fc` in one kernel (cogdl_b200/csrc/fused_gcn.cu,
+    wgmma epilogue), the self half and bias as one GEMM before it; the aggregated features are never written out.
+    Taken for CUDA fp32 x with in_feats == 128, out_feats <= 128, x.shape[0] == the graph's rows, no out_norm on
+    the graph and edge weights without grad (mean / sum); otherwise the unfused path runs."""
+
     def __init__(self, in_feats, out_feats, normalize=False, aggr="mean", dropout=0.0, norm=None, activation=None,
-                 residual=False):
+                 residual=False, fused=False):
         super().__init__()
         self.in_feats, self.out_feats = in_feats, out_feats
+        self.fused, self._aggr_name, self._act_name = bool(fused), aggr, activation
         self.fc = nn.Linear(2 * in_feats, out_feats)
         self.normalize = normalize
         self.dropout = nn.Dropout(dropout) if dropout > 0 else None
@@ -149,14 +155,33 @@ class SAGELayer(nn.Module):
         self.norm = _norm(norm, out_feats)
         self.residual = nn.Linear(in_feats, out_feats) if residual else None
 
+    def _fused_applies(self, graph, x):
+        from .operators import fused_sage
+
+        if not (self.fused and x.is_cuda and x.dtype == torch.float32 and getattr(graph, "grb_adj", None) is None
+                and fused_sage.supported(self.in_feats, self.out_feats) and x.shape[0] == graph.row_indptr.shape[0] - 1):
+            return False
+        if self._aggr_name == "mean":
+            graph.row_norm()             # as MeanAggregator, before the norms are looked at
+        if graph.out_norm is not None:
+            return False
+        return self._aggr_name == "max" or not graph.raw_edge_weight.requires_grad
+
     def forward(self, graph, x):
-        out = self.aggr(graph, x)
-        out = self.fc(torch.cat([x, out], dim=-1))
+        relu = False
+        if self._fused_applies(graph, x):
+            from .operators import fused_sage
+
+            relu = self._act_name == "relu" and not self.normalize and self.norm is None
+            out = fused_sage.fused_sage_layer(graph, x, self.fc.weight, self.fc.bias, self._aggr_name, relu=relu)
+        else:
+            out = self.aggr(graph, x)
+            out = self.fc(torch.cat([x, out], dim=-1))
         if self.normalize:
             out = F.normalize(out, p=2.0, dim=-1)
         if self.norm is not None:
             out = self.norm(out)
-        if self.act is not None:
+        if self.act is not None and not relu:
             out = self.act(out)
         if self.residual is not None:
             out = out + self.residual(x)
@@ -193,10 +218,10 @@ class GAT(nn.Module):
 
 
 class SAGE(nn.Module):
-    def __init__(self, in_feats, hidden_size, out_feats, aggr="max", dropout=0.0):
+    def __init__(self, in_feats, hidden_size, out_feats, aggr="max", dropout=0.0, fused=False):
         super().__init__()
-        self.l1 = SAGELayer(in_feats, hidden_size, aggr=aggr, dropout=dropout, activation="relu")
-        self.l2 = SAGELayer(hidden_size, out_feats, aggr=aggr)
+        self.l1 = SAGELayer(in_feats, hidden_size, aggr=aggr, dropout=dropout, activation="relu", fused=fused)
+        self.l2 = SAGELayer(hidden_size, out_feats, aggr=aggr, fused=fused)
 
     def forward(self, graph):
         return self.l2(graph, self.l1(graph, graph.x))

@@ -307,6 +307,31 @@ COGDL_B200_API int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t
                              int64_t K, int64_t Fout, int32_t relu, const cogdl_b200_hub_plan_t *plan,
                              cogdl_b200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Fused GraphSAGE layer: OUT = act( S + agg(X).W_neigh^T ), the reference's  fc(cat[x, agg])
+ * (cogdl/layers/sage_layer.py:69-87) with fc.weight = [W_self | W_neigh] and S = X[:n_rows].W_self^T + b
+ * computed beforehand by the caller (the self half does not fit on chip beside the operand tiles).
+ * The aggregation runs in the fused GCN kernel and the aggregated tile is never written to global memory:
+ *   aggr == COGDL_B200_AGGR_SUM: agg = row_scale (.) (A.X), A = (rowptr, colind, val), val NULL = ones,
+ *                                row_scale [n_rows] or NULL (graph.in_norm of a CSR-only graph; mean = sum
+ *                                with row-normalised val or with row_scale = 1/deg).  Bit-identical to
+ *                                row_scale * cogdl_b200_spmm_csr_f32(...).
+ *   aggr == COGDL_B200_AGGR_MAX: agg = the values of cogdl_b200_scatter_max_fwd_f32 (strict `<` from -inf,
+ *                                degree-0 rows 0), bit for bit; no argmax is produced.  val and row_scale
+ *                                must be NULL.
+ * The dense product is the bf16x3 wgmma of cogdl_b200_gcn_fused_f32 (~1e-7 of the row scale vs fp64).
+ * X [n_src,K], W_neigh [Fout,K] contiguous, S and out [n_rows,Fout]; constraints as cogdl_b200_gcn_fused_f32
+ * (cogdl_b200_gcn_fused_supported, hub plan with edge_row, 16-byte aligned X / W_neigh / S / out).
+ * hub_agg: scratch [n_rows, K] fp32, required iff the plan has hub rows.  plan->partials: n_chunks*K*4
+ * bytes for sum, n_chunks*K*8 for max.
+ * ------------------------------------------------------------------------------------- */
+#define COGDL_B200_AGGR_SUM 0
+#define COGDL_B200_AGGR_MAX 1
+COGDL_B200_API int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
+                              const float *row_scale, const float *X, const float *W_neigh, const float *S, float *out,
+                              float *hub_agg, int64_t n_rows, int64_t K, int64_t Fout, int32_t aggr, int32_t relu,
+                              const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
 /* Device COO -> CSR (stable): row_ptr[num_nodes+1] and reindex[nnz] (CSR slot -> COO position),
  * int64 as cogdl.data.Graph stores them.
  * Replaces  sampler.coo2csr_cpu_index(row, col, num_nodes)   cogdl/operators/sample/sample.cpp:234-270
