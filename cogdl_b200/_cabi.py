@@ -9,6 +9,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libcogdl_b200.so")
+MAX_PANELS = 8   # COGDL_B200_MAX_PANELS: a hub plan holds n_chunks * MAX_PANELS arrival counters
 
 OK, EINVAL, ECUDA, EDEVICE, ESCRATCH = 0, -1, -2, -3, -4
 
@@ -57,6 +58,7 @@ SIGNATURES = {
     "cogdl_b200_hub_plan_fill": (ctypes.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "cogdl_b200_edge_rows": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp]),
     "cogdl_b200_spmm_csr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_spmm_csr_f32_ex": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f16": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f32_2src": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f32_peers": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _vp, _i64, _i64, _plan_p, _vp]),

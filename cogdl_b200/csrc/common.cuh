@@ -111,6 +111,7 @@ __device__ __forceinline__ float ld_stream(const float *p) {
 }
 // Gathered feature rows: read-only path, default caching (hub columns do get reused).
 __device__ __forceinline__ float4 ld_gather(const float4 *p) { return __ldg(p); }
+__device__ __forceinline__ float2 ld_gather(const float2 *p) { return __ldg(p); }
 __device__ __forceinline__ float ld_gather(const float *p) { return __ldg(p); }
 
 // L2 eviction-priority hints (createpolicy + ld/st .L2::cache_hint): the gathered matrix X is the
@@ -134,14 +135,17 @@ __device__ __forceinline__ float ld_gather_hint(const float *p, uint64_t pol) {
 
 // Output rows are written once and never re-read by the kernel: streaming store.
 __device__ __forceinline__ void st_stream(float4 *p, float4 v) { __stcs(p, v); }
+__device__ __forceinline__ void st_stream(float2 *p, float2 v) { __stcs(p, v); }
 __device__ __forceinline__ void st_stream(float *p, float v) { __stcs(p, v); }
 __device__ __forceinline__ void st_stream(int *p, int v) { __stcs(p, v); }
 
 // L2-coherent accesses for inter-CTA partial results (L1 is not coherent across SMs).
 __device__ __forceinline__ float4 ld_cg(const float4 *p) { return __ldcg(p); }
+__device__ __forceinline__ float2 ld_cg(const float2 *p) { return __ldcg(p); }
 __device__ __forceinline__ float ld_cg(const float *p) { return __ldcg(p); }
 __device__ __forceinline__ int ld_cg(const int *p) { return __ldcg(p); }
 __device__ __forceinline__ void st_cg(float4 *p, float4 v) { __stcg(p, v); }
+__device__ __forceinline__ void st_cg(float2 *p, float2 v) { __stcg(p, v); }
 __device__ __forceinline__ void st_cg(float *p, float v) { __stcg(p, v); }
 __device__ __forceinline__ void st_cg(int *p, int v) { __stcg(p, v); }
 
@@ -153,6 +157,10 @@ __device__ __forceinline__ float mul_add_rn(float acc, float v, float x) {
 }
 // in-place forms, one per vector type
 __device__ __forceinline__ void axpy_rn(float &acc, float v, const float &x) { acc = mul_add_rn(acc, v, x); }
+__device__ __forceinline__ void axpy_rn(float2 &acc, float v, const float2 &x) {
+  acc.x = mul_add_rn(acc.x, v, x.x);
+  acc.y = mul_add_rn(acc.y, v, x.y);
+}
 __device__ __forceinline__ void axpy_rn(float4 &acc, float v, const float4 &x) {
   acc.x = mul_add_rn(acc.x, v, x.x);
   acc.y = mul_add_rn(acc.y, v, x.y);

@@ -201,6 +201,67 @@ static int launch_spmm_stream(const SpmmParams &p, cudaStream_t stream) {
   return launch_stream<VecT, NV, U, 1>(q, mode, stream);
 }
 
+// ------------------------------------------------------------------------------------------
+// Panel mode.  With uniformly random columns a gathered X row survives in the L2 only if it is reused before
+// ~L2-size of other traffic evicts it; once X outgrows the L2 most gathers go to DRAM.  P passes over the graph,
+// pass p gathering only columns [p*F/P, (p+1)*F/P) (panel-major grid, stream.cuh), keep the live panel
+// L2-resident so X comes from DRAM about once.  Every lane owns one VecT of the panel (F/P = 32, 64 or 128
+// floats => float, float2, float4); accumulation order per element is unchanged, so the output is
+// bit-identical to P = 1.
+// ------------------------------------------------------------------------------------------
+static int64_t device_l2_bytes() {
+  static int cache[64] = {0};   // per device; racing first calls store the same value
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;
+  if (cache[dev] == 0) {
+    int v = 0;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, dev) != cudaSuccess || v <= 0) return 0;
+    cache[dev] = v;
+  }
+  return cache[dev];
+}
+
+// Largest share of the L2 one panel of X may take.  7/8 picks 64-float panels on the arxiv shape (F = 128 -> P = 2,
+// F = 256 -> P = 4; 43 MB panels in the 50 MB L2), the fastest measured (DESIGN 3.1): 32-float panels (P = 4 at
+// F = 128) keep X in the L2 better still, but their one-float lanes cost more issue slots than the misses they save.
+constexpr int64_t PANEL_THETA_NUM = 7, PANEL_THETA_DEN = 8;
+
+// A panel is exactly 32 lanes x one VecT: F / P must be 32, 64 or 128 floats (a 96-float panel would leave a
+// partial VecT tile that the launch below does not have).
+static bool panel_width_ok(int64_t F, int P) {
+  if (P < 1 || P > COGDL_B200_MAX_PANELS || F % P != 0) return false;
+  const int64_t w = F / P;
+  return w == 32 || w == 64 || w == 128;
+}
+
+// Smallest power of two P whose panel fits the budget; 1 when X already fits or even the narrowest panels
+// do not (then the extra index passes cost more than the misses they save).
+static int auto_panels(int64_t x_rows, int64_t F) {
+  const int64_t x_bytes = x_rows * F * (int64_t)sizeof(float);
+  const int64_t budget = device_l2_bytes() * PANEL_THETA_NUM / PANEL_THETA_DEN;
+  if (budget <= 0 || x_bytes <= budget) return 1;
+  for (int P = 2; P <= COGDL_B200_MAX_PANELS && 32 * (int64_t)P <= F; P *= 2)
+    if (panel_width_ok(F, P) && x_bytes / P <= budget) return P;
+  return 1;
+}
+
+static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_t stream) {
+  StreamParams q = to_stream(p);
+  q.S = P;
+  const int mode = p.val ? MODE_WEIGHTED : MODE_UNWEIGHTED;
+  switch (F / P) {
+    case 32:
+      q.ldv = q.FVL = (int)F;
+      return launch_stream<float, 1, 8, 6, true, false, true>(q, mode, stream);
+    case 64:
+      q.ldv = q.FVL = (int)(F / 2);
+      return launch_stream<float2, 1, 8, 5, true, false, true>(q, mode, stream);
+    default:
+      q.ldv = q.FVL = (int)(F / 4);
+      return launch_stream<float4, 1, 4, 5, true, false, true>(q, mode, stream);
+  }
+}
+
 template <typename VecT, int GROUP, int NV>
 static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
   const int64_t items = (int64_t)p.hub.n_chunks + p.n_rows;
@@ -244,8 +305,10 @@ static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
 static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X0,
                       int64_t n0, const float *X1, float *Y, int64_t n_rows, int64_t F,
                       const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream, const char *who,
-                      const float *const *peers = nullptr, int n_peers = 0, int peer_shift = 0) {
+                      const float *const *peers = nullptr, int n_peers = 0, int peer_shift = 0,
+                      int64_t x_rows = 0, int panels = 1) {
   CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
+  CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
   CB_REQUIRE(rowptr && colind && X0 && Y, "%s: null pointer", who);
   CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "%s: n_rows / F must fit int32", who);
@@ -265,10 +328,15 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
                "%s: the peer form needs a plan with segments, F %% 4 == 0, F <= 512 and 16-byte aligned buffers", who);
   const bool vec = (F % 4 == 0) && aligned16(X0) && aligned16(p.X1) && aligned16(Y) &&
                    (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
-  if (vec) {
-    p.FV = (int)(F / 4);
-    return dispatch_spmm<float4>(p, (cudaStream_t)stream);
-  }
+  if (vec) p.FV = (int)(F / 4);
+  const bool panel_form = vec && n_peers == 0 && n0 == INT64_MAX && p.hub.n_segs > 0 && F % 32 == 0;
+  if (panels > 1)
+    CB_REQUIRE(panel_form && panel_width_ok(F, panels),
+               "%s: %d panels need a plan with segments, one source, 16-byte aligned buffers and F / panels in "
+               "{32, 64, 128} (F=%lld, at most %d panels)", who, panels, (long long)F, COGDL_B200_MAX_PANELS);
+  const int P = panels == 0 ? (panel_form ? auto_panels(x_rows, F) : 1) : panels;
+  if (P > 1) return launch_spmm_panels(p, F, P, (cudaStream_t)stream);
+  if (vec) return dispatch_spmm<float4>(p, (cudaStream_t)stream);
   p.FV = (int)F;
   return dispatch_spmm<float>(p, (cudaStream_t)stream);
 }
@@ -385,11 +453,18 @@ int spmm_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float
 
 using namespace cogdl_b200;
 
+extern "C" int cogdl_b200_spmm_csr_f32_ex(const int32_t *rowptr, const int32_t *colind, const float *val,
+                                          const float *X, int64_t x_rows, float *Y, int64_t n_rows, int64_t F,
+                                          int32_t panels, const cogdl_b200_hub_plan_t *plan,
+                                          cogdl_b200_stream_t stream) {
+  return spmm_entry(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream,
+                    "cogdl_b200_spmm_csr_f32_ex", nullptr, 0, 0, x_rows, panels);
+}
+
 extern "C" int cogdl_b200_spmm_csr_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
                                        const float *X, float *Y, int64_t n_rows, int64_t F,
                                        const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
-  return spmm_entry(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream,
-                    "cogdl_b200_spmm_csr_f32");
+  return cogdl_b200_spmm_csr_f32_ex(rowptr, colind, val, X, n_rows, Y, n_rows, F, 0, plan, stream);
 }
 
 extern "C" int cogdl_b200_spmm_csr_f32_2src(const int32_t *rowptr, const int32_t *colind, const float *val,

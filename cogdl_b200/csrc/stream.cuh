@@ -5,6 +5,9 @@
 //                                 scratch, combined in chunk order by the last chunk to arrive;
 //   [n_chunks, n_chunks+n_segs)   segments: runs of consecutive NON-hub rows (~seg_cost rows+edges).
 // In multi-head mode every item exists once per 512-byte slice of the [H*F] row (adjacent warps).
+// In panel mode (plain SpMM, X larger than the L2) every item exists once per column panel of X, panel-major:
+// blockIdx.y = panel.  Blocks are dispatched roughly in linear block order (x fastest), so about one panel
+// of X (F/S columns of every row) is live in the L2 at a time and each X line is fetched from DRAM ~once.
 //
 // One warp per item.  A segment's edges are contiguous in colind/val/edge_row, so the warp walks
 // them in 32-edge slabs: one coalesced load each for colind, the value (or permutation) and the
@@ -38,7 +41,7 @@ struct StreamParams {
   int ldv;            // dense row length in VecT units
   int H;              // MODE 2: heads
   int FVL;            // MODE 2: VecT units per head
-  int S;              // MODE 2: 512-byte slices per row (1 otherwise)
+  int S;              // MODE 2: 512-byte slices per row; panel mode: column panels of 32 VecT (1 otherwise)
   HubView hub;
 };
 
@@ -51,8 +54,10 @@ enum { SRC_ONE = 0, SRC_TWO = 1, SRC_PEERS = 2 };
 
 template <typename VecT> __device__ __forceinline__ VecT sk_zero();
 template <> __device__ __forceinline__ float4 sk_zero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+template <> __device__ __forceinline__ float2 sk_zero<float2>() { return make_float2(0.f, 0.f); }
 template <> __device__ __forceinline__ float sk_zero<float>() { return 0.f; }
 __device__ __forceinline__ void sk_add(float &a, const float &b) { a = __fadd_rn(a, b); }
+__device__ __forceinline__ void sk_add(float2 &a, const float2 &b) { a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); }
 __device__ __forceinline__ void sk_add(float4 &a, const float4 &b) { add_rn(a, b); }
 
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
@@ -151,8 +156,9 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
 // (no convergence requirement, column + value in ONE LDS.64), full batches run without per-edge predicates, and
 // the row-end test is made once per batch on the ballot mask: ~15 instructions per edge.  Same accumulation
 // order and rounding as stream_range (CSR order, separate fp32 multiply and add) => still bit-identical to
-// the reference CPU loop on unsplit rows.
-template <typename VecT, int MODE, int SRC, int U, bool ROWS>
+// the reference CPU loop on unsplit rows.  PF: the next slab's indices are loaded while this slab's gathers are
+// in flight (4 more registers; the panel form's narrow gathers leave room for them).
+template <typename VecT, int MODE, int SRC, int U, bool ROWS, bool PF = false>
 __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, const int e_end, const int cv, const bool colok,
                                                   const int lane, int2 *s_cv, int *s_r, VecT &acc) {
   const VecT *X0 = reinterpret_cast<const VecT *>(p.X0) + cv;
@@ -167,12 +173,29 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
   auto accumulate = [&](float vj, const VecT &x) {
     if (MODE == MODE_UNWEIGHTED) sk_add(acc, x); else axpy_rn(acc, vj, x);
   };
+  auto load_slab = [&](int base, int &c, float &v, int &rid, int &rnx) {
+    const int q = base + lane;
+    c = 0; v = 0.f; rid = -1; rnx = -1;
+    if (q < e_end) {
+      c = ld_stream(p.colind + q);
+      if (MODE == MODE_WEIGHTED) v = ld_stream(p.val + q);
+      if (ROWS) {
+        rid = ld_stream(p.hub.edge_row + q);
+        if (q + 1 < e_end) rnx = __ldg(p.hub.edge_row + q + 1);
+      }
+    }
+  };
+  int pc = 0, prid = -1, prnx = -1;                 // PF: the slab loaded one iteration ahead
+  float pv = 0.f;
+  if (PF) load_slab(e, pc, pv, prid, prnx);
   for (; e < e_end; e += 32) {
     const int cnt = min(32, e_end - e);
     const int q = e + lane;
     int c = 0, rid = -1, rnx = -1;
     float v = 0.f;
-    if (q < e_end) {
+    if (PF) {
+      c = pc; v = pv; rid = prid; rnx = prnx;
+    } else if (q < e_end) {
       c = ld_stream(p.colind + q);
       if (MODE == MODE_WEIGHTED) v = ld_stream(p.val + q);
       if (ROWS) {
@@ -185,13 +208,22 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
     s_cv[lane] = make_int2(c, __float_as_int(v));
     if (ROWS) s_r[lane] = rid;
     __syncwarp();
+    if (PF) load_slab(e + 32, pc, pv, prid, prnx);  // consumed by the next iteration only
     int j = 0;
 #pragma unroll 1
     for (; j + U <= cnt; j += U) {                  // full batches: no per-edge predicates
       int2 cw[U];
       VecT x[U];
+      // PF: the values are read back when consumed, not with the columns, so a deep batch does not hold U of
+      // them across the gathers (at U = 8 that is the difference between spilling and not)
+      auto val_of = [&](int u) {
+        return __int_as_float(PF ? reinterpret_cast<const volatile int *>(s_cv + j + u)[1] : cw[u].y);
+      };
 #pragma unroll
-      for (int u = 0; u < U; ++u) cw[u] = s_cv[j + u];            // broadcast LDS.64
+      for (int u = 0; u < U; ++u) {
+        if (PF) cw[u].x = s_cv[j + u].x;                          // broadcast LDS
+        else cw[u] = s_cv[j + u];                                 // broadcast LDS.64
+      }
 #pragma unroll
       for (int u = 0; u < U; ++u)
         if (colok) x[u] = ld_gather(src_ptr(cw[u].x));
@@ -199,11 +231,11 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
       if (em == 0u) {                               // no row ends inside this batch
 #pragma unroll
         for (int u = 0; u < U; ++u)
-          if (colok) accumulate(__int_as_float(cw[u].y), x[u]);
+          if (colok) accumulate(val_of(u), x[u]);
       } else {
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-          if (colok) accumulate(__int_as_float(cw[u].y), x[u]);
+          if (colok) accumulate(val_of(u), x[u]);
           if ((em >> u) & 1u) {                     // last edge of its row: store and restart (warp-uniform)
             const int rj = s_r[j + u];
             if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = sk_zero<VecT>(); }
@@ -223,20 +255,22 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
   }
 }
 
-// One work item (wid = item * S + slice) processed by one warp.
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool HINT>
+// One work item processed by one warp: wid = item * S + slice (multi-head), slice = blockIdx.y (PANEL).
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool HINT, bool PANEL>
 __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t wid, const int lane, int2 *s_cv, int *s_r) {
   constexpr int TILE = 32 * NV;
-  const int64_t item = (MODE == MODE_MULTIHEAD) ? wid / p.S : wid;
-  const int slice = (MODE == MODE_MULTIHEAD) ? (int)(wid - item * p.S) : 0;
+  constexpr bool SLICED = (MODE == MODE_MULTIHEAD || PANEL);
+  int64_t item = wid;
+  int slice = PANEL ? (int)blockIdx.y : 0;
+  if (MODE == MODE_MULTIHEAD) { item = wid / p.S; slice = (int)(wid - item * p.S); }
   VecT *Y = reinterpret_cast<VecT *>(p.Y);
   VecT *P = reinterpret_cast<VecT *>(p.hub.partials);
   constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD && !HINT);
 
-  // column tiles: the multi-head form owns exactly one 32-vector slice; the plain form loops over
+  // column tiles: the multi-head and panel forms own exactly one 32-vector slice; the plain form loops over
   // the row in TILE-vector passes (one pass for F <= 128 * NV)
-  const int t_begin = (MODE == MODE_MULTIHEAD) ? slice * 32 : 0;
-  const int t_end = (MODE == MODE_MULTIHEAD) ? t_begin + 1 : p.ldv;
+  const int t_begin = SLICED ? slice * 32 : 0;
+  const int t_end = SLICED ? t_begin + 1 : p.ldv;
 
   if (item < p.hub.n_chunks) {
     const WorkItem w = decode_item(item, 0, p.rowptr, p.hub);
@@ -247,16 +281,29 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
 #pragma unroll
       for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = sk_zero<VecT>(); }
       const int head = (MODE == MODE_MULTIHEAD && colok[0]) ? cv / p.FVL : 0;
-      if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false>(p, w.lb, w.hb, cv, colok[0], lane, s_cv, s_r, acc[0]);
+      if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false, PANEL && PREFETCH>(p, w.lb, w.hb, cv, colok[0], lane, s_cv, s_r, acc[0]);
       else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH, HINT>(p, w.lb, w.hb, cv, colok, head, lane, acc);
 #pragma unroll
       for (int k = 0; k < NV; ++k)
         if (colok[k]) st_cg(P + (int64_t)w.slot * p.ldv + cv + k * 32, acc[k]);
     }
+    // multi-head: every slice of every chunk arrives at the row's counter and the last one combines the whole
+    // row.  Panel mode: one counter per (row, panel) at counters[panel * n_chunks + first], and the last chunk of
+    // the panel combines just its 32 vectors -- the row's last arrival overall would come in the last panel,
+    // which would turn a long hub's merge into an end-of-kernel tail.
     WorkItem wa = w;
-    wa.n_row_chunks = w.n_row_chunks * p.S;   // every slice of every chunk arrives once
-    if (hub_arrive_last<32>(wa, p.hub, lane)) {
-      for (int cv = lane; cv < p.ldv; cv += 32) {
+    if (MODE == MODE_MULTIHEAD) wa.n_row_chunks = w.n_row_chunks * p.S;
+    bool last;
+    if constexpr (PANEL) {
+      HubView hv = p.hub;
+      hv.counters += (int64_t)slice * p.hub.n_chunks;
+      last = hub_arrive_last<32>(wa, hv, lane);
+    } else {
+      last = hub_arrive_last<32>(wa, p.hub, lane);
+    }
+    if (last) {
+      const int c_begin = PANEL ? t_begin : 0, c_end = PANEL ? min(t_begin + 32, p.ldv) : p.ldv;
+      for (int cv = c_begin + lane; cv < c_end; cv += 32) {
         const VecT *pp = P + (int64_t)w.first * p.ldv + cv;
         VecT s = ld_cg(pp);
         int q = 1;
@@ -300,12 +347,12 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
         }
       }
     }
-    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true>(p, e_begin, e_end, cv, colok[0], lane, s_cv, s_r, acc[0]);
+    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH>(p, e_begin, e_end, cv, colok[0], lane, s_cv, s_r, acc[0]);
     else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, HINT>(p, e_begin, e_end, cv, colok, head, lane, acc);
   }
 }
 
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool HINT>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool HINT, bool PANEL = false>
 __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p) {
   const int lane = threadIdx.x & 31;
   constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD && !HINT);
@@ -314,13 +361,14 @@ __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p)
   int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
   int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, HINT>(p, wid, lane, s_cv, s_r);
+  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, HINT, PANEL>(p, wid, lane, s_cv, s_r);
 }
 
 // Launch helper: picks the instantiation for (mode, perm, two-source); U / MINB fixed by the caller.
-template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, bool HINT = false>
+// PANEL: the panel-major plain SpMM (NV == 1, one source, p.S panels of 32 VecT each).
+template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, bool HINT = false, bool PANEL = false>
 static int launch_stream(const StreamParams &p, int mode, cudaStream_t stream) {
-  const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * p.S;
+  const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * (PANEL ? 1 : p.S);   // PANEL: grid.y = p.S
   // Threads per block: a launch parameter only -- the kernel indexes its per-warp slabs by warp-in-block and takes its
   // item from the global warp index, so every block size runs the same SASS and gives the same bits.  A block's warp
   // slots go to the next block only when its SLOWEST warp has retired; item durations spread (gathers that miss L2,
@@ -334,13 +382,21 @@ static int launch_stream(const StreamParams &p, int mode, cudaStream_t stream) {
   if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "stream kernel: problem too large for one launch");
   const unsigned g = (unsigned)blocks;
   const int src = p.n_peers > 0 ? SRC_PEERS : (p.n0 != INT64_MAX ? SRC_TWO : SRC_ONE);
-  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s,%s,U=%d,MINB=%d%s%s>", sizeof(VecT) == 16 ? "float4" : "float", NV,
+  if (PANEL && (NV != 1 || src != SRC_ONE || mode == MODE_MULTIHEAD))
+    return set_error(COGDL_B200_EINVAL, "stream kernel: panel mode is the one-source plain SpMM with NV == 1");
+  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s,%s,U=%d,MINB=%d%s%s>",
+              sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
               mode == MODE_MULTIHEAD ? "multihead" : (mode == MODE_WEIGHTED ? "weighted" : "unweighted"),
               (mode == MODE_MULTIHEAD && p.perm) ? "+perm" : "",
               src == SRC_PEERS ? "SRC_PEERS" : (src == SRC_TWO ? "SRC_TWO" : "SRC_ONE"), U, MINB,
               PREFETCH ? ",prefetch" : "", HINT ? ",l2hint" : "");
+  if (PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
   if (bs != 256) append_kernel_note(" block=%d", bs);
-  if (mode == MODE_MULTIHEAD) {
+  if constexpr (PANEL) {
+    const dim3 gp(g, (unsigned)p.S);
+    if (mode == MODE_WEIGHTED) stream_kernel<VecT, 1, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, HINT, true><<<gp, bs, 0, stream>>>(p);
+    else stream_kernel<VecT, 1, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, HINT, true><<<gp, bs, 0, stream>>>(p);
+  } else if (mode == MODE_MULTIHEAD) {
     if constexpr (NV == 1) {
       if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
       else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);

@@ -12,8 +12,10 @@ def _f32c(t, name):
     return t.contiguous()
 
 
-def spmm_raw(st: CSRStructure, val, x):
-    """Y = A @ X with A = (st, val).  x: [n_src, F] fp32 or fp16; val: [nnz] or None."""
+def spmm_raw(st: CSRStructure, val, x, panels=0):
+    """Y = A @ X with A = (st, val).  x: [n_src, F] fp32 or fp16; val: [nnz] or None.
+    panels: column panels of X for the fp32 kernel (0 = chosen from X's size against the L2; the output
+    does not depend on it)."""
     dev = require_cuda(x, val)
     if x.dim() != 2:
         raise ValueError("x must be [n_src, F]")
@@ -29,8 +31,8 @@ def spmm_raw(st: CSRStructure, val, x):
         if x.dtype == torch.float32:
             if val is not None and val.dtype != torch.float32:
                 val = val.float()
-            _cabi.call("cogdl_b200_spmm_csr_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), _ptr(y),
-                       st.n_rows, F, plan, _stream(dev))
+            _cabi.call("cogdl_b200_spmm_csr_f32_ex", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
+                       _ptr(y), st.n_rows, F, int(panels), plan, _stream(dev))
         elif x.dtype == torch.float16:
             if val is not None and val.dtype != torch.float16:
                 val = val.half()

@@ -81,7 +81,8 @@ class HubPlan:
             self.n_hub_rows, self.n_chunks, self.n_empty_rows, self.n_segs = n_hub, n_chunks, n_empty, n_segs
             self.hub_rows = torch.empty(max(n_hub, 1), dtype=torch.int32, device=dev)
             self.chunks = torch.empty(max(2 * n_chunks, 2), dtype=torch.int32, device=dev)
-            self.counters = torch.zeros(max(n_chunks, 1), dtype=torch.int32, device=dev)
+            # one set of arrival counters per column panel of the SpMM's panel form (COGDL_B200_MAX_PANELS)
+            self.counters = torch.zeros(max(n_chunks, 1) * _cabi.MAX_PANELS, dtype=torch.int32, device=dev)
             if self.seg_cost > 0 and n_segs > 0:
                 self.segs = torch.empty(2 * n_segs, dtype=torch.int32, device=dev)
                 self.edge_row = torch.empty(int(nnz), dtype=torch.int32, device=dev)

@@ -74,7 +74,9 @@ COGDL_B200_API int cogdl_b200_tuning_value(const char *name, int dflt);
  *   chunks[2*n_chunks]          (row, first_slot) per chunk slot; a row's chunks occupy the
  *                               contiguous slots [first_slot, first_slot + ceil(deg/chunk_edges))
  *                               and chunk j covers edges rowptr[row] + j*chunk_edges ...
- *   counters[n_chunks]          zero on entry; left zero on exit (arrival counters)
+ *   counters[n_chunks * COGDL_B200_MAX_PANELS]
+ *                               zero on entry; left zero on exit (arrival counters; the panel form of
+ *                               the SpMM keeps one set of n_chunks per column panel)
  *   partials                    scratch for per-chunk partial results; `partials_bytes` capacity.
  *                               needs n_chunks*F*4 bytes (SpMM, mh-SpMM: F := H*F) or
  *                               n_chunks*F*8 bytes (scatter_max: value + argmax).
@@ -82,6 +84,7 @@ COGDL_B200_API int cogdl_b200_tuning_value(const char *name, int dflt);
  * Partial results of a hub row are combined in chunk order by the last chunk to finish, so
  * results are deterministic run to run.
  * ------------------------------------------------------------------------------------- */
+#define COGDL_B200_MAX_PANELS 8
 typedef struct cogdl_b200_hub_plan {
   int32_t chunk_edges;
   int32_t n_hub_rows;
@@ -140,6 +143,16 @@ COGDL_B200_API int cogdl_b200_edge_rows(const int32_t *rowptr, int64_t n_rows, i
 COGDL_B200_API int cogdl_b200_spmm_csr_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
                             const float *X, float *Y, int64_t n_rows, int64_t F,
                             const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
+/* Same, with X of x_rows rows and the column-panel count: when X is larger than the L2, the kernel makes one
+ * pass over the graph per column panel of X (panel-major) so that the panel being gathered stays L2-resident;
+ * the output is bit-identical whatever the panel count.  panels = 0 picks it from x_rows * F * 4 against the
+ * device's L2 size (1 unless the plan has segments, F % 32 == 0 and the buffers are 16-byte aligned);
+ * panels > 1 forces it (F / panels must be 32, 64 or 128, panels <= COGDL_B200_MAX_PANELS).
+ * cogdl_b200_spmm_csr_f32 is this call with x_rows = n_rows and panels = 0. */
+COGDL_B200_API int cogdl_b200_spmm_csr_f32_ex(const int32_t *rowptr, const int32_t *colind, const float *val,
+                               const float *X, int64_t x_rows, float *Y, int64_t n_rows, int64_t F,
+                               int32_t panels, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
 /* fp16 storage (X, val, Y are IEEE half), fp32 accumulation (the reference accumulates in
  * half, spmm_kernel.cu:222-250,311-368,442-512 -- documented divergence). */
