@@ -14,11 +14,61 @@ building models.  Two levels are patched:
      spmm / edge_softmax / mh_spmm / fused_gat_op function (or SpMM / EdgeSoftmax / MultiHeadSpMM
      / FusedGATOp class) is rebound to this package's version, which keeps the int32 CSR, hub
      plan and transpose cached on the graph instead of re-casting per call.
+
+With genconv=True, `cogdl.layers.deepergcn_layer.GENConv.forward` (DeeperGCN, RevGCN) is also rebound, to
+genconv_forward below, which sends the aggregation to cogdl_b200.genconv_aggregate.  The original forward stays
+reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores it).
 """
 import sys
 
+import torch
 
-def install(rebind_dispatch=True):
+_GENCONV_KERNEL_AGGRS = ("softmax_sg", "softmax", "mean", "sum", "max", "powermean")
+
+
+def genconv_forward(self, graph, x):
+    """GENConv.forward (cogdl/layers/deepergcn_layer.py:64-102) with the aggregation in the sm_90a kernels.  The
+    edge encoder, message_norm, residual and MLP are the layer's own.  Cases without a kernel -- CPU or non-fp32
+    input, an aggregation name GENConv does not define, max / powermean with an edge encoder -- run the original."""
+    from .operators.softmax_aggr import genconv_aggregate
+    from .utils.spmm_utils import _structure
+
+    original = type(self)._cogdl_b200_original_forward
+    has_edge = self.edge_encoder is not None and graph.edge_attr is not None
+    if (not x.is_cuda or x.dtype != torch.float32 or self.aggr not in _GENCONV_KERNEL_AGGRS
+            or (has_edge and self.aggr in ("max", "powermean"))):
+        return original(self, graph, x)
+    st = _structure(graph)         # puts the graph in CSR order first, edge_attr included (data.py:279-287)
+    edge_term = self.edge_encoder(graph.edge_attr) if has_edge else None
+    h = genconv_aggregate(st, x, self.aggr, beta=self.beta, eps=self.eps, edge_term=edge_term, p=self.p)
+    if self.use_msg_norm:
+        h = self.message_norm(x, h)
+    if self.residual:
+        h = h + x
+    return self.mlp(h)
+
+
+def install_genconv():
+    import cogdl.layers.deepergcn_layer as dl
+
+    cls = dl.GENConv
+    if getattr(cls.forward, "_cogdl_b200", False):
+        return []
+    cls._cogdl_b200_original_forward = cls.forward
+    genconv_forward._cogdl_b200 = True
+    cls.forward = genconv_forward
+    return ["cogdl.layers.deepergcn_layer.GENConv.forward"]
+
+
+def uninstall_genconv():
+    import cogdl.layers.deepergcn_layer as dl
+
+    cls = dl.GENConv
+    if getattr(cls.forward, "_cogdl_b200", False):
+        cls.forward = cls._cogdl_b200_original_forward
+
+
+def install(rebind_dispatch=True, genconv=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -98,4 +148,6 @@ def install(rebind_dispatch=True):
                 if new is not None and val is not new:
                     setattr(mod, attr, new)
                     patched.append(f"{mname}.{attr}")
+    if genconv:
+        patched += install_genconv()
     return patched

@@ -15,3 +15,4 @@ from .edge_softmax import csr_edge_softmax, EdgeSoftmaxFunction  # noqa: F401
 from .mhspmm import csrmhspmm, MHSPMMFunction  # noqa: F401
 from .scatter_max import scatter_max, ScatterMaxFunction  # noqa: F401
 from .fused_gat import fused_gat_func, FusedGATFunction  # noqa: F401
+from .softmax_aggr import genconv_aggregate, SoftmaxAggrFunction  # noqa: F401

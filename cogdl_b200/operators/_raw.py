@@ -200,6 +200,69 @@ def gat_attn_bwd_raw(st: CSRStructure, att, d_att, h_l, h_r, slope):
     return d_edge, g_row
 
 
+def _sa_scratch(st, F):
+    if st.chunk_edges <= 0:
+        return 0
+    return int(_cabi.load().cogdl_b200_softmax_aggr_scratch_bytes(st.plan.n_chunks, F))
+
+
+def _sa_check(st, x, beta, edge_term, n_x_rows):
+    """Shared argument checks of the softmax aggregation: [n_x_rows, F] fp32 x, [nnz, F] fp32 edge term, a
+    one-element fp32 beta on x's device."""
+    require_cuda(x, beta, edge_term)
+    x = _f32c(x, "x")
+    if x.dim() != 2 or x.shape[0] != n_x_rows:
+        raise ValueError(f"x must be [{n_x_rows}, F], got {tuple(x.shape)}")
+    beta = _f32c(beta, "beta").reshape(-1)
+    if beta.numel() != 1:
+        raise ValueError(f"beta must hold one value, got {beta.numel()}")
+    if edge_term is not None:
+        edge_term = _f32c(edge_term, "edge term")
+        if edge_term.shape != (st.nnz, x.shape[1]):
+            raise ValueError(f"edge term must be [nnz={st.nnz}, F={x.shape[1]}], got {tuple(edge_term.shape)}")
+    return x, beta, edge_term
+
+
+def softmax_aggr_fwd_raw(st: CSRStructure, x, beta, eps, edge_term=None, want_lse=False, want_q=False):
+    """GENConv softmax aggregation: out[i] = sum_e softmax_e(beta m_e) m_e, m_e = relu(x[col_e] + edge_term[e]) + eps.
+    x [n_cols, F], beta a one-element CUDA tensor (read on the device), edge_term [nnz, F] in CSR order or None.
+    Returns (out, lse2, q): lse2 (base-2 log-sum-exp of the logits, for the backward) and q (sum_e w_e m_e^2, for
+    d beta) are [n_rows, F] when asked for, else None."""
+    dev = require_cuda(x)
+    x, beta, edge_term = _sa_check(st, x, beta, edge_term, st.n_cols)
+    F = x.shape[1]
+    with torch.cuda.device(dev):
+        out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+        lse2 = torch.empty_like(out) if want_lse else None
+        q = torch.empty_like(out) if want_q else None
+        plan, keep = st.plan_struct(_sa_scratch(st, F))
+        _cabi.call("cogdl_b200_softmax_aggr_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(x), _ptr(edge_term),
+                   _ptr(beta), float(eps), _ptr(out), _ptr(lse2), _ptr(q), st.n_rows, F, plan, _stream(dev))
+        del keep
+    return out, lse2, q
+
+
+def softmax_aggr_bwd_raw(st: CSRStructure, x, beta, eps, g, out, lse2, edge_term=None, want_edge_grad=True):
+    """(dx [n_cols, F], d_edge_term [nnz, F] or None) of softmax_aggr_fwd_raw, over the cached transpose of st."""
+    dev = require_cuda(x, g, out, lse2)
+    x, beta, edge_term = _sa_check(st, x, beta, edge_term, st.n_cols)
+    F = x.shape[1]
+    g, out, lse2 = _f32c(g, "grad"), _f32c(out, "out"), _f32c(lse2, "lse2")
+    for name, t in (("grad", g), ("out", out), ("lse2", lse2)):
+        if t.shape != (st.n_rows, F):
+            raise ValueError(f"{name} must be [{st.n_rows}, {F}], got {tuple(t.shape)}")
+    st_t, perm = st.csc()
+    with torch.cuda.device(dev):
+        dx = torch.empty_like(x)
+        da = torch.empty_like(edge_term) if edge_term is not None and want_edge_grad else None
+        plan, keep = st_t.plan_struct(st_t.plan.n_chunks * F * 4 if st_t.chunk_edges > 0 else 0)
+        _cabi.call("cogdl_b200_softmax_aggr_bwd_f32", _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(x),
+                   _ptr(edge_term), _ptr(beta), float(eps), _ptr(g), _ptr(out), _ptr(lse2), _ptr(dx), _ptr(da),
+                   st_t.n_rows, F, plan, _stream(dev))
+        del keep
+    return dx, da
+
+
 def edge_colsum_raw(st_t: CSRStructure, perm, e):
     """out[j,h] = sum of e[p,h] over the edges p whose column is j (st_t = cached transpose, perm its permutation)."""
     dev = require_cuda(perm, e)

@@ -345,6 +345,36 @@ COGDL_B200_API int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_
                               float *hub_agg, int64_t n_rows, int64_t K, int64_t Fout, int32_t aggr, int32_t relu,
                               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * GENConv softmax aggregation (DeeperGCN / RevGCN; cogdl/layers/deepergcn_layer.py:64-93) without per-edge
+ * feature tensors.  Per row i, channel f, over the CSR edges e = (i, c_e):
+ *   m_e = relu(X[c_e,f] + edge_term[e,f]) + eps        (edge_term: [nnz, F] in CSR order, or NULL)
+ *   out[i,f] = sum_e w_e m_e,  w_e = softmax_e(beta m_e)       degree-0 rows: out = 0
+ * beta is a DEVICE pointer to one float (a trainable parameter needs no host read; beta = 0 is the mean).
+ * X is [n_cols, F], out / lse2 / Q are [n_rows, F].  Optional outputs for the backward:
+ *   lse2[i,f] = log2 sum_e 2^(beta log2(e) m_e)   (base-2 log-sum-exp of the logits)
+ *   Q[i,f]    = sum_e w_e m_e^2                   (d out / d beta = Q - out^2)
+ * Any F >= 1; 16-byte vectors when F % 4 == 0 and every buffer is 16-byte aligned.  Hub rows are cut into the
+ * plan's chunks and merged in chunk order (no float atomics: bit-reproducible).  plan->partials needs
+ * n_chunks*F*12 bytes (16 with Q); cogdl_b200_softmax_aggr_scratch_bytes covers both directions.
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_softmax_aggr_scratch_bytes(int64_t n_chunks, int64_t F);
+COGDL_B200_API int cogdl_b200_softmax_aggr_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
+                                    const float *edge_term, const float *beta, float eps, float *out, float *lse2,
+                                    float *Q, int64_t n_rows, int64_t F, const cogdl_b200_hub_plan_t *plan,
+                                    cogdl_b200_stream_t stream);
+/* Backward over the transpose (colptr, rowind, perm of cogdl_b200_csr2csc; n_cols columns), given G = dL/dout and
+ * the forward's out and lse2:
+ *   dpre_e = G[i] w_e (1 + beta (m_e - out[i])) [X[j] + edge_term[e] > 0]
+ *   dX[j] = sum_{e: c_e = j} dpre_e  (transpose order; hub columns through `plan`, the TRANSPOSE's plan, whose
+ *           partials need n_chunks*F*4 bytes)            d_edge_term[e] = dpre_e  (optional, needs edge_term)
+ * perm is needed only with an edge term.  d beta = sum G (Q - out^2) is left to the caller. */
+COGDL_B200_API int cogdl_b200_softmax_aggr_bwd_f32(const int32_t *colptr, const int32_t *rowind, const int32_t *perm,
+                                    const float *X, const float *edge_term, const float *beta, float eps,
+                                    const float *G, const float *out, const float *lse2, float *dX,
+                                    float *d_edge_term, int64_t n_cols, int64_t F, const cogdl_b200_hub_plan_t *plan,
+                                    cogdl_b200_stream_t stream);
+
 /* Device COO -> CSR (stable): row_ptr[num_nodes+1] and reindex[nnz] (CSR slot -> COO position),
  * int64 as cogdl.data.Graph stores them.
  * Replaces  sampler.coo2csr_cpu_index(row, col, num_nodes)   cogdl/operators/sample/sample.cpp:234-270
