@@ -51,8 +51,6 @@ SIGNATURES = {
     "cogdl_b200_check_device": (ctypes.c_int, []),
     "cogdl_b200_launch_count": (_i64, []),
     "cogdl_b200_last_kernel": (ctypes.c_char_p, []),
-    "cogdl_b200_reload_tuning": (None, []),
-    "cogdl_b200_tuning_value": (ctypes.c_int, [ctypes.c_char_p, ctypes.c_int]),
     "cogdl_b200_hub_plan_layout": (ctypes.c_int, [ctypes.POINTER(ctypes.c_int64), ctypes.c_int]),
     "cogdl_b200_hub_plan_count": (ctypes.c_int, [_vp, _i64, _i32, _i32, _vp, _vp]),
     "cogdl_b200_hub_plan_fill": (ctypes.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
@@ -113,7 +111,7 @@ def load():
             fn = getattr(lib, name)  # AttributeError here = header/library mismatch: fail loudly
             fn.restype = res
             fn.argtypes = args
-        if lib.cogdl_b200_abi_version() != 5:
+        if lib.cogdl_b200_abi_version() != 6:
             raise ImportError("libcogdl_b200.so ABI version mismatch")
         # the ctypes mirror of cogdl_b200_hub_plan_t must have the library's layout, field for field
         want = [ctypes.sizeof(HubPlanStruct)] + [getattr(HubPlanStruct, n).offset for n, _ in HubPlanStruct._fields_]

@@ -6,10 +6,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstddef>
-#include <cstdlib>
 #include <cstring>
-#include <map>
-#include <mutex>
 
 namespace cogdl_b200 {
 
@@ -32,26 +29,6 @@ void note_kernel(const char *fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_kernel, sizeof(g_kernel), fmt, ap);
   va_end(ap);
-}
-
-// keyed by the (string-literal) name itself: no allocation on the lookup path
-struct CStrLess {
-  bool operator()(const char *a, const char *b) const { return strcmp(a, b) < 0; }
-};
-static std::mutex g_tuning_mu;
-static std::map<const char *, int, CStrLess> g_tuning;
-int tuning(const char *env_name, int dflt) {
-  std::lock_guard<std::mutex> lock(g_tuning_mu);
-  auto it = g_tuning.find(env_name);
-  if (it != g_tuning.end()) return it->second;
-  const char *e = getenv(env_name);
-  const int v = (e && *e) ? atoi(e) : dflt;
-  g_tuning.emplace(env_name, v);
-  return v;
-}
-static void tuning_reload() {
-  std::lock_guard<std::mutex> lock(g_tuning_mu);
-  g_tuning.clear();
 }
 
 void append_kernel_note(const char *fmt, ...) {
@@ -159,19 +136,6 @@ extern "C" const char *cogdl_b200_last_error(void) { return g_err; }
 extern "C" int64_t cogdl_b200_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
 extern "C" const char *cogdl_b200_last_kernel(void) { return g_kernel; }
-
-extern "C" void cogdl_b200_reload_tuning(void) { tuning_reload(); }
-
-// What a knob currently resolves to (cached value if the library has read it, else the environment, else dflt).
-// Never inserts: `name` may be a temporary of the caller.
-extern "C" int cogdl_b200_tuning_value(const char *name, int dflt) {
-  if (!name) return dflt;
-  std::lock_guard<std::mutex> lock(g_tuning_mu);
-  auto it = g_tuning.find(name);
-  if (it != g_tuning.end()) return it->second;
-  const char *e = getenv(name);
-  return (e && *e) ? atoi(e) : dflt;
-}
 
 extern "C" int cogdl_b200_hub_plan_layout(int64_t *out, int n) {
   typedef cogdl_b200_hub_plan_t P;

@@ -20,9 +20,6 @@ void count_launch(int n = 1);
 // (cogdl_b200_last_kernel(); bench.py checks it against the profiled kernel's name).
 void note_kernel(const char *fmt, ...);
 void append_kernel_note(const char *fmt, ...);   // launch-shape suffix after the instantiation name
-// Experiment knobs read from the environment (COGDL_B200_*), cached after the first read;
-// cogdl_b200_reload_tuning() drops the cache so a tuning sweep can change them inside one process.
-int tuning(const char *env_name, int dflt);
 
 #define CB_REQUIRE(cond, ...)                                             \
   do {                                                                    \
@@ -113,25 +110,6 @@ __device__ __forceinline__ float ld_stream(const float *p) {
 __device__ __forceinline__ float4 ld_gather(const float4 *p) { return __ldg(p); }
 __device__ __forceinline__ float2 ld_gather(const float2 *p) { return __ldg(p); }
 __device__ __forceinline__ float ld_gather(const float *p) { return __ldg(p); }
-
-// L2 eviction-priority hints (createpolicy + ld/st .L2::cache_hint): the gathered matrix X is the
-// only data with reuse, everything else is touched once.
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ float4 ld_gather_hint(const float4 *p, uint64_t pol) {
-  float4 v;
-  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ float ld_gather_hint(const float *p, uint64_t pol) {
-  float v;
-  asm volatile("ld.global.nc.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
-  return v;
-}
 
 // Output rows are written once and never re-read by the kernel: streaming store.
 __device__ __forceinline__ void st_stream(float4 *p, float4 v) { __stcs(p, v); }

@@ -540,13 +540,14 @@ __global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
   }
 }
 
-// warps per block of the 512-float-tile main kernel (COGDL_B200_ES_WARPS = 8 | 4 | 2): a launch parameter only,
-// bit-identical outputs.  The default is the shape the whole GPU suite is validated with; the smaller blocks are one
-// environment variable away.
-constexpr int ES_WARPS_DEFAULT = 8;
+// Warps per block of the main kernel.  For the 512-float tile this is a launch parameter only (2 and 4 warps give
+// bit-identical outputs); a block's shared memory and warp slots are released when its slowest warp retires, and 8
+// is the shape the whole GPU suite is validated with.
+constexpr int ES_WARPS = 8;
 
-template <int MODE, int CAP, int WARPS = 8>
+template <int MODE, int CAP>
 static int launch_main(const EsParams &p, cudaStream_t s) {
+  constexpr int WARPS = ES_WARPS;
   constexpr bool TWO = (MODE == 1 || MODE == 3);
   constexpr size_t smem = (size_t)WARPS * CAP * 4 * (TWO ? 2 : 1) + (size_t)WARPS * 34 * 4 + (size_t)WARPS * 8;
   static unsigned long long attr_done = 0;
@@ -609,17 +610,9 @@ static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t
     es_stats_kernel<MODE><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
   }
-  const int cap_floor = tuning("COGDL_B200_ES_CAP", 0);   // tuning only: smallest tile (floats per warp) of the staged kernel
-  const int64_t cap = cap_need > cap_floor ? cap_need : cap_floor;
-  const int chosen = cap <= 512 ? 512 : (cap <= 1024 ? 1024 : 2048);
-  // warps per block of the 512-float-tile instantiation (tuning: a block's shared memory and warp slots are released
-  // when its slowest warp retires)
-  const int es_warps = chosen == 512 ? tuning("COGDL_B200_ES_WARPS", ES_WARPS_DEFAULT) : 8;
-  const int warps = (es_warps == 4 || es_warps == 2) ? es_warps : 8;
-  note_kernel("cogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d>%s", MODE, chosen, warps,
+  const int chosen = cap_need <= 512 ? 512 : (cap_need <= 1024 ? 1024 : 2048);   // smallest tile (floats per warp) that fits
+  note_kernel("cogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d>%s", MODE, chosen, ES_WARPS,
               (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
-  if (chosen == 512 && warps == 4) return launch_main<MODE, 512, 4>(p, s);
-  if (chosen == 512 && warps == 2) return launch_main<MODE, 512, 2>(p, s);
   if (chosen == 512) return launch_main<MODE, 512>(p, s);
   if (chosen == 1024) return launch_main<MODE, 1024>(p, s);
   return launch_main<MODE, 2048>(p, s);

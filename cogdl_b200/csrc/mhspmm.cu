@@ -156,7 +156,7 @@ static int dispatch_mh(MhParams &p, cudaStream_t s) {
     q.X0 = p.feat; q.X1 = p.feat; q.n0 = INT64_MAX; q.Y = p.out; q.ldv = p.HFV; q.H = p.H; q.FVL = p.FVL;
     q.S = p.S; q.hub = p.hub; q.n_peers = 0; q.peer_shift = 0;
     if (p.n_rows == 0) q.hub.n_segs = 0;   // chunks-only call (fused GAT hub path)
-    return launch_stream<VecT, 1, 8, 3>(q, MODE_MULTIHEAD, s);
+    return launch_stream<VecT, 1, 8, 3, true, FORM_MULTIHEAD>(q, s);
   }
   switch (g) {
     case 1: return launch_mh<VecT, 1>(p, s);

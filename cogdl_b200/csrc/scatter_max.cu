@@ -288,9 +288,8 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
   }
 }
 
-// bit-exact either way; products shape F=256: 11.38 ms (row-stream form) vs 11.52 ms (row per warp)
-static bool smax_stream_enabled() { return tuning("COGDL_B200_SMAX_STREAM", 1) != 0; }
-
+// Row-stream form whenever the plan has segments and a row is wider than 16 vectors: bit-exact either way; products
+// shape F=256: 11.38 ms (row-stream form) vs 11.52 ms (row per warp)
 template <int NV>
 static int launch_smax_stream(const SmaxParams &p, cudaStream_t stream) {
   const int64_t warps = (int64_t)p.hub.n_chunks + p.hub.n_segs;
@@ -317,7 +316,7 @@ template <typename VecT>
 static int dispatch_smax(const SmaxParams &p, cudaStream_t s) {
   const int fv = p.FV;
   if constexpr (sizeof(VecT) == 16) {
-    if (fv > 16 && p.hub.n_segs > 0 && smax_stream_enabled())
+    if (fv > 16 && p.hub.n_segs > 0)
       return fv <= 32 ? launch_smax_stream<1>(p, s) : launch_smax_stream<2>(p, s);
   }
   if (fv <= 1) return launch_smax<VecT, 1, 1>(p, s);
@@ -330,7 +329,7 @@ static int dispatch_smax(const SmaxParams &p, cudaStream_t s) {
 }
 
 // Only the hub rows (degree > plan chunk) of the max values, no argmax: the hub-chunk items of the row-stream
-// kernel with their in-order combine, no segments (so independent of COGDL_B200_SMAX_STREAM).  Used by the fused
+// kernel with their in-order combine, no segments.  Used by the fused
 // SAGE layer (fused_gcn.cu), which aggregates every other row straight into shared memory.  F == 128, 16-byte
 // aligned X / Y; plan->partials n_chunks * F * 8 bytes.
 int smax_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float *X, float *Y, int64_t F,

@@ -206,10 +206,9 @@ __global__ void __launch_bounds__(256) sddmm_stream_kernel(const SddmmParams p) 
   }
 }
 
-// Stream form on / off (COGDL_B200_SDDMM_STREAM = 1 / 0), measured on an H100 SXM (700 W, arxiv shape, two alternating
-// runs): 220 vs 298 us (F=128), 2.03 vs 2.53 ms (H=8, F=128) -> on by default; the row form serves every other width.
-static bool sddmm_stream_enabled() { return tuning("COGDL_B200_SDDMM_STREAM", 1) != 0; }
-
+// Stream form vs row form, measured on an H100 SXM (700 W, arxiv shape, two alternating runs): 220 vs 298 us (F=128),
+// 2.03 vs 2.53 ms (H=8, F=128) -> the stream form whenever the plan has segments and L is 32 or 64 vectors; the row
+// form serves every other width and plans without segments.
 template <int NV>
 static int launch_sddmm_stream(const SddmmParams &p, cudaStream_t stream) {
   const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * p.NSEG;
@@ -239,7 +238,7 @@ template <typename VecT>
 static int dispatch_sddmm(const SddmmParams &p, cudaStream_t s) {
   const int L = p.L, H = p.NSEG;
   if constexpr (sizeof(VecT) == 16) {
-    if (p.hub.n_segs > 0 && sddmm_stream_enabled()) {
+    if (p.hub.n_segs > 0) {
       if (L == 32) return launch_sddmm_stream<1>(p, s);
       if (L == 64) return launch_sddmm_stream<2>(p, s);
     }

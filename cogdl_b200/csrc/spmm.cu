@@ -166,12 +166,8 @@ __global__ void __launch_bounds__(256) spmm_kernel(const SpmmParams p) {
 
 // ------------------------------------------------------------------------------------------
 // Row-stream form (stream.cuh), used whenever the plan carries segments and a full warp owns the
-// row (F >= 68, or >= 17 on the scalar path).  COGDL_B200_SPMM_VARIANT (experiments only) picks
-// the unroll depth / occupancy target of the F <= 128 instantiation; the default is the only
-// variant the test suite exercises.
+// row (F >= 68, or >= 17 on the scalar path).
 // ------------------------------------------------------------------------------------------
-static int spmm_variant() { return tuning("COGDL_B200_SPMM_VARIANT", 7); }
-
 static StreamParams to_stream(const SpmmParams &p) {
   StreamParams q;
   q.rowptr = p.rowptr; q.colind = p.colind; q.val = p.val; q.att = nullptr; q.perm = nullptr;
@@ -185,20 +181,12 @@ static StreamParams to_stream(const SpmmParams &p) {
 template <typename VecT, int NV>
 static int launch_spmm_stream(const SpmmParams &p, cudaStream_t stream) {
   const StreamParams q = to_stream(p);
-  const int mode = p.val ? MODE_WEIGHTED : MODE_UNWEIGHTED;
   if constexpr (NV == 1 && sizeof(VecT) == 16) {
-    // lean loop (stream_range_lean); the variants differ in gathers per batch (U) and resident blocks per SM
-    switch (spmm_variant()) {
-      case 1: return launch_stream<VecT, 1, 8, 4, false>(q, mode, stream);
-      case 2: return launch_stream<VecT, 1, 8, 3, false>(q, mode, stream);
-      case 3: return launch_stream<VecT, 1, 4, 6, false>(q, mode, stream);
-      case 8: return launch_stream<VecT, 1, 4, 5, false, true>(q, mode, stream);   // round-1 loop + L2 evict_last hint on X (slower)
-      // U=4, 48 registers (40 warps/SM)
-      default: return launch_stream<VecT, 1, 4, 5, false>(q, mode, stream);
-    }
+    return launch_stream<VecT, 1, 4, 5, false>(q, stream);   // lean loop (stream_range_lean), U=4, 48 registers (40 warps/SM)
+  } else {
+    constexpr int U = (NV == 1) ? 8 : (NV == 2 ? 4 : 2);
+    return launch_stream<VecT, NV, U, 1>(q, stream);
   }
-  constexpr int U = (NV == 1) ? 8 : (NV == 2 ? 4 : 2);
-  return launch_stream<VecT, NV, U, 1>(q, mode, stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -248,17 +236,16 @@ static int auto_panels(int64_t x_rows, int64_t F) {
 static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_t stream) {
   StreamParams q = to_stream(p);
   q.S = P;
-  const int mode = p.val ? MODE_WEIGHTED : MODE_UNWEIGHTED;
   switch (F / P) {
     case 32:
       q.ldv = q.FVL = (int)F;
-      return launch_stream<float, 1, 8, 6, true, false, true>(q, mode, stream);
+      return launch_stream<float, 1, 8, 6, true, FORM_PANEL>(q, stream);
     case 64:
       q.ldv = q.FVL = (int)(F / 2);
-      return launch_stream<float2, 1, 8, 5, true, false, true>(q, mode, stream);
+      return launch_stream<float2, 1, 8, 5, true, FORM_PANEL>(q, stream);
     default:
       q.ldv = q.FVL = (int)(F / 4);
-      return launch_stream<float4, 1, 4, 5, true, false, true>(q, mode, stream);
+      return launch_stream<float4, 1, 4, 5, true, FORM_PANEL>(q, stream);
   }
 }
 
@@ -281,6 +268,10 @@ static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
   return COGDL_B200_OK;
 }
 
+// narrow rows (F = 40 -> 10 float4): the lean row-stream form with the idle lanes masked beats the sub-warp
+// row kernel once a row needs at least this many vectors
+constexpr int SPMM_STREAM_MIN_FV = 9;
+
 template <typename VecT>
 static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
   const int fv = p.FV;
@@ -288,17 +279,16 @@ static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
   // sub-warp row kernel below would read them as X1[c - n0].  NV = 1 masks lanes >= fv.
   if (p.n_peers > 0 && fv <= 32) return launch_spmm_stream<VecT, 1>(p, s);
   const bool stream = p.hub.n_segs > 0;
-  // narrow rows (F = 40 -> 10 float4): the lean row-stream form with the idle lanes masked beats the sub-warp
-  // row kernel once a row needs more than `stream_min_fv` vectors (tunable for experiments)
-  const int stream_min_fv = tuning("COGDL_B200_SPMM_STREAM_MINFV", 9);
-  if (stream && fv >= stream_min_fv && fv <= 16) return launch_spmm_stream<VecT, 1>(p, s);
+  if (stream && fv >= SPMM_STREAM_MIN_FV && fv <= 16) return launch_spmm_stream<VecT, 1>(p, s);
   if (fv <= 1) return launch_spmm<VecT, 1, 1>(p, s);
   if (fv <= 2) return launch_spmm<VecT, 2, 1>(p, s);
   if (fv <= 4) return launch_spmm<VecT, 4, 1>(p, s);
   if (fv <= 8) return launch_spmm<VecT, 8, 1>(p, s);
   if (fv <= 16) return launch_spmm<VecT, 16, 1>(p, s);
   if (fv <= 32) return stream ? launch_spmm_stream<VecT, 1>(p, s) : launch_spmm<VecT, 32, 1>(p, s);
-  if (sizeof(VecT) == 4 && fv > 64) return stream ? launch_spmm_stream<VecT, 4>(p, s) : launch_spmm<VecT, 32, 4>(p, s);
+  if constexpr (sizeof(VecT) == 4) {
+    if (fv > 64) return stream ? launch_spmm_stream<VecT, 4>(p, s) : launch_spmm<VecT, 32, 4>(p, s);
+  }
   return stream ? launch_spmm_stream<VecT, 2>(p, s) : launch_spmm<VecT, 32, 2>(p, s);
 }
 
@@ -445,8 +435,8 @@ int spmm_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float
   p.FV = (int)(F / 4);
   if (p.hub.n_chunks == 0) return COGDL_B200_OK;
   const StreamParams q = to_stream(p);
-  if (p.FV <= 32) return launch_stream<float4, 1, 4, 5, false>(q, val ? MODE_WEIGHTED : MODE_UNWEIGHTED, stream);
-  return launch_stream<float4, 2, 4, 1>(q, val ? MODE_WEIGHTED : MODE_UNWEIGHTED, stream);
+  if (p.FV <= 32) return launch_stream<float4, 1, 4, 5, false>(q, stream);
+  return launch_stream<float4, 2, 4, 1>(q, stream);
 }
 
 }  // namespace cogdl_b200

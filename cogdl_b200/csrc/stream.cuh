@@ -25,7 +25,7 @@ namespace cogdl_b200 {
 struct StreamParams {
   const int *rowptr;
   const int *colind;
-  const float *val;   // MODE 1: [nnz]
+  const float *val;   // MODE 1: [nnz]; null => unweighted
   const float *att;   // MODE 2: [nnz, H]
   const int *perm;    // MODE 2, nullable: attention row of edge p is perm[p]
   const float *X0;
@@ -46,11 +46,14 @@ struct StreamParams {
 };
 
 enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2 };
-// Threads per block of every row-stream launch (COGDL_B200_STREAM_BLOCK overrides).  Measured on an H100 SXM (700 W),
-// 128 vs 256, two alternating runs each: SpMM F=40 87 vs 90 us, arxiv / products F=128, mh-SpMM and the papers
-// shard within 1 %; all outputs bit-identical.
-constexpr int STREAM_BLOCK_DEFAULT = 128;
+// Threads per block of every row-stream launch.  Measured on an H100 SXM (700 W), 128 vs 256, two alternating runs
+// each: SpMM F=40 87 vs 90 us, arxiv / products F=128, mh-SpMM and the papers shard within 1 %; all outputs
+// bit-identical.
+constexpr int STREAM_BLOCK = 128;
 enum { SRC_ONE = 0, SRC_TWO = 1, SRC_PEERS = 2 };
+// What a launch_stream call runs: the plain SpMM (weighted iff p.val, any source form), its panel-major form, or
+// the multi-head SpMM.
+enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
 
 template <typename VecT> __device__ __forceinline__ VecT sk_zero();
 template <> __device__ __forceinline__ float4 sk_zero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
@@ -62,14 +65,13 @@ __device__ __forceinline__ void sk_add(float4 &a, const float4 &b) { add_rn(a, b
 
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
 // whole range into acc (hub chunk).
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH, bool HINT>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH>
 __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const int e_end, const int cv,
                                              const bool (&colok)[NV], const int head, const int lane,
                                              VecT (&acc)[NV]) {
   const VecT *X0 = reinterpret_cast<const VecT *>(p.X0) + cv;
   const VecT *X1 = reinterpret_cast<const VecT *>(p.X1) + cv;
   VecT *Y = reinterpret_cast<VecT *>(p.Y) + cv;
-  const uint64_t pol = HINT ? l2_policy_evict_last() : 0;
 
   // slab registers: column, value / attention row, owning row, owning row of the next edge
   int c = 0, rid = -1, rnx = -1, pe = 0;
@@ -119,7 +121,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
           }
 #pragma unroll
           for (int k = 0; k < NV; ++k)
-            if (colok[k]) x[u][k] = HINT ? ld_gather_hint(xp + k * 32, pol) : ld_gather(xp + k * 32);
+            if (colok[k]) x[u][k] = ld_gather(xp + k * 32);
           if (MODE == MODE_MULTIHEAD && colok[0]) a[u] = __ldg(p.att + (int64_t)pj * p.H + head);
         }
       }
@@ -256,7 +258,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
 }
 
 // One work item processed by one warp: wid = item * S + slice (multi-head), slice = blockIdx.y (PANEL).
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool HINT, bool PANEL>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool PANEL>
 __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t wid, const int lane, int2 *s_cv, int *s_r) {
   constexpr int TILE = 32 * NV;
   constexpr bool SLICED = (MODE == MODE_MULTIHEAD || PANEL);
@@ -265,7 +267,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
   if (MODE == MODE_MULTIHEAD) { item = wid / p.S; slice = (int)(wid - item * p.S); }
   VecT *Y = reinterpret_cast<VecT *>(p.Y);
   VecT *P = reinterpret_cast<VecT *>(p.hub.partials);
-  constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD && !HINT);
+  constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD);
 
   // column tiles: the multi-head and panel forms own exactly one 32-vector slice; the plain form loops over
   // the row in TILE-vector passes (one pass for F <= 128 * NV)
@@ -282,7 +284,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
       for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = sk_zero<VecT>(); }
       const int head = (MODE == MODE_MULTIHEAD && colok[0]) ? cv / p.FVL : 0;
       if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false, PANEL && PREFETCH>(p, w.lb, w.hb, cv, colok[0], lane, s_cv, s_r, acc[0]);
-      else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH, HINT>(p, w.lb, w.hb, cv, colok, head, lane, acc);
+      else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH>(p, w.lb, w.hb, cv, colok, head, lane, acc);
 #pragma unroll
       for (int k = 0; k < NV; ++k)
         if (colok[k]) st_cg(P + (int64_t)w.slot * p.ldv + cv + k * 32, acc[k]);
@@ -348,69 +350,63 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
       }
     }
     if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH>(p, e_begin, e_end, cv, colok[0], lane, s_cv, s_r, acc[0]);
-    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, HINT>(p, e_begin, e_end, cv, colok, head, lane, acc);
+    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH>(p, e_begin, e_end, cv, colok, head, lane, acc);
   }
 }
 
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool HINT, bool PANEL = false>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool PANEL = false>
 __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p) {
   const int lane = threadIdx.x & 31;
-  constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD && !HINT);
+  constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD);
   __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
   __shared__ int s_r_all[LEAN ? 8 : 1][32];
   int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
   int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, HINT, PANEL>(p, wid, lane, s_cv, s_r);
+  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, PANEL>(p, wid, lane, s_cv, s_r);
 }
 
-// Launch helper: picks the instantiation for (mode, perm, two-source); U / MINB fixed by the caller.
-// PANEL: the panel-major plain SpMM (NV == 1, one source, p.S panels of 32 VecT each).
-template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, bool HINT = false, bool PANEL = false>
-static int launch_stream(const StreamParams &p, int mode, cudaStream_t stream) {
-  const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * (PANEL ? 1 : p.S);   // PANEL: grid.y = p.S
+// Launch helper: picks the instantiation of FORM for (weighted, perm, source form); U / MINB fixed by the caller.
+// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.
+template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN>
+static int launch_stream(const StreamParams &p, cudaStream_t stream) {
+  static_assert(FORM == FORM_PLAIN || NV == 1, "the panel and multi-head forms have one VecT per lane");
+  const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * (FORM == FORM_MULTIHEAD ? p.S : 1);
   // Threads per block: a launch parameter only -- the kernel indexes its per-warp slabs by warp-in-block and takes its
   // item from the global warp index, so every block size runs the same SASS and gives the same bits.  A block's warp
   // slots go to the next block only when its SLOWEST warp has retired; item durations spread (gathers that miss L2,
   // hub merges), so smaller blocks keep more warp slots busy -- most visibly for the two-vectors-per-lane
   // instantiation (F = 256).  A persistent form (grid = resident warp slots, items drawn from a ticket counter in the
   // plan) was also built and measured slower (the ticket loop needs 64 registers = 32 warps/SM) -- removed.
-  int bs = tuning("COGDL_B200_STREAM_BLOCK", STREAM_BLOCK_DEFAULT);
-  if (bs != 32 && bs != 64 && bs != 128) bs = 256;
-  const int64_t blocks = ceil_div(warps * 32, bs);
+  const int64_t blocks = ceil_div(warps * 32, STREAM_BLOCK);
   if (blocks == 0) return COGDL_B200_OK;
   if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "stream kernel: problem too large for one launch");
-  const unsigned g = (unsigned)blocks;
+  const dim3 grid((unsigned)blocks, FORM == FORM_PANEL ? (unsigned)p.S : 1u);
   const int src = p.n_peers > 0 ? SRC_PEERS : (p.n0 != INT64_MAX ? SRC_TWO : SRC_ONE);
-  if (PANEL && (NV != 1 || src != SRC_ONE || mode == MODE_MULTIHEAD))
-    return set_error(COGDL_B200_EINVAL, "stream kernel: panel mode is the one-source plain SpMM with NV == 1");
-  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s,%s,U=%d,MINB=%d%s%s>",
+  if (FORM != FORM_PLAIN && src != SRC_ONE)
+    return set_error(COGDL_B200_EINVAL, "stream kernel: the panel and multi-head forms read one source");
+  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s,%s,U=%d,MINB=%d%s>",
               sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
-              mode == MODE_MULTIHEAD ? "multihead" : (mode == MODE_WEIGHTED ? "weighted" : "unweighted"),
-              (mode == MODE_MULTIHEAD && p.perm) ? "+perm" : "",
+              FORM == FORM_MULTIHEAD ? "multihead" : (p.val ? "weighted" : "unweighted"),
+              (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "",
               src == SRC_PEERS ? "SRC_PEERS" : (src == SRC_TWO ? "SRC_TWO" : "SRC_ONE"), U, MINB,
-              PREFETCH ? ",prefetch" : "", HINT ? ",l2hint" : "");
-  if (PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
-  if (bs != 256) append_kernel_note(" block=%d", bs);
-  if constexpr (PANEL) {
-    const dim3 gp(g, (unsigned)p.S);
-    if (mode == MODE_WEIGHTED) stream_kernel<VecT, 1, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, HINT, true><<<gp, bs, 0, stream>>>(p);
-    else stream_kernel<VecT, 1, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, HINT, true><<<gp, bs, 0, stream>>>(p);
-  } else if (mode == MODE_MULTIHEAD) {
-    if constexpr (NV == 1) {
-      if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
-      else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
-    } else {
-      return set_error(COGDL_B200_EINVAL, "stream kernel: multi-head form needs NV == 1");
-    }
-  } else if (mode == MODE_WEIGHTED) {
-    if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
-    else if (src == SRC_TWO) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_TWO, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
-    else stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
+              PREFETCH ? ",prefetch" : "");
+  if (FORM == FORM_PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
+  append_kernel_note(" block=%d", STREAM_BLOCK);
+  if constexpr (FORM == FORM_MULTIHEAD) {
+    if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if constexpr (FORM == FORM_PANEL) {
+    if (p.val) stream_kernel<VecT, 1, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_kernel<VecT, 1, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if (p.val) {
+    if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else if (src == SRC_TWO) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_TWO, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
   } else {
-    if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
-    else if (src == SRC_TWO) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_TWO, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
-    else stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, HINT><<<g, bs, 0, stream>>>(p);
+    if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else if (src == SRC_TWO) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_TWO, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
   }
   CB_LAUNCH_CHECK();
   return COGDL_B200_OK;

@@ -17,9 +17,9 @@ from . import _cabi
 import os
 
 # rows with more edges than this are cut into chunks of this many edges (hub plan)
-DEFAULT_CHUNK_EDGES = int(os.environ.get("COGDL_B200_CHUNK_EDGES", "64"))
+DEFAULT_CHUNK_EDGES = 64
 # rows + edges streamed by one warp of the row-stream kernels (0 disables the stream form)
-DEFAULT_SEG_COST = int(os.environ.get("COGDL_B200_SEG_COST", "128"))
+DEFAULT_SEG_COST = 128
 
 
 _EMPTY = {}

@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define COGDL_B200_ABI_VERSION 5
+#define COGDL_B200_ABI_VERSION 6
 
 #define COGDL_B200_OK 0
 #define COGDL_B200_EINVAL (-1)   /* bad argument (null pointer, negative size, unsupported shape) */
@@ -58,11 +58,6 @@ COGDL_B200_API int64_t cogdl_b200_launch_count(void);
  * thread (e.g. "stream_kernel<float4,NV=1,weighted,SRC_ONE,U=4>"); "" before the first call.  Lets a
  * harness check that a profile it cites is of the kernel that actually ran. */
 COGDL_B200_API const char *cogdl_b200_last_kernel(void);
-/* Experiment knobs (environment variables COGDL_B200_*: kernel variants, tile floors) are read once and cached;
- * this drops the cache so that a tuning sweep can change them inside one process.  Not needed in normal use. */
-COGDL_B200_API void cogdl_b200_reload_tuning(void);
-/* What the knob `name` currently resolves to: the cached value, else the environment, else `dflt`. */
-COGDL_B200_API int cogdl_b200_tuning_value(const char *name, int dflt);
 
 /* ---------------------------------------------------------------------------------------
  * Hub plan: how rows with more than `chunk_edges` edges are cut into fixed-size edge chunks

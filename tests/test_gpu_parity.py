@@ -33,10 +33,11 @@ def dev():
     return torch.device("cuda:0")
 
 
-def structure(rp, ci, n_cols, dev, chunk=256):
+def structure(rp, ci, n_cols, dev, chunk=256, seg_cost=None):
     from cogdl_b200.structure import CSRStructure
 
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk)
+    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk,
+                        seg_cost=seg_cost)
 
 
 def T(a, dev):
@@ -405,31 +406,11 @@ def test_errors_are_raised_not_swallowed(dev):
     assert "null pointer" in cogdl_b200._cabi.last_error()
 
 
-# ------------------------------------------------------------------------------------ launch-shape knobs
-def _with_tuning(env, fn):
-    """Run fn() with experiment knobs set (environment + cogdl_b200_reload_tuning), then restore the defaults."""
-    import os
-
-    from cogdl_b200 import _cabi
-
-    old = {k: os.environ.get(k) for k in env}
-    try:
-        os.environ.update({k: str(v) for k, v in env.items()})
-        _cabi.load().cogdl_b200_reload_tuning()
-        return fn()
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-        _cabi.load().cogdl_b200_reload_tuning()
-
-
+# ------------------------------------------------------------------------------------ row-stream launches
 @pytest.mark.parametrize("F", [128, 40, 256])
-def test_stream_block_size_is_a_launch_parameter_only(dev, F):
-    """Threads per block of the row-stream kernels (default 128) changes which warp slots are busy, never the
-    arithmetic: every block size gives the same bits (and the oracle's on unsplit rows)."""
+def test_stream_spmm_on_hub_chunks_matches_the_oracle(dev, F):
+    """The row-stream SpMM with 64-edge hub chunks: the oracle's bits on unsplit rows, the arrival counters left
+    at zero."""
     from cogdl_b200.operators._raw import spmm_raw
 
     rp, ci, n_cols = case("two_hubs")
@@ -437,22 +418,18 @@ def test_stream_block_size_is_a_launch_parameter_only(dev, F):
     X = rng.standard_normal((n_cols, F)).astype(np.float32)
     val = rng.random(ci.shape[0]).astype(np.float32)
     st = structure(rp, ci, n_cols, dev, chunk=64)
-    xd, vd = T(X, dev), T(val, dev)
-    y0 = spmm_raw(st, vd, xd)
+    y = spmm_raw(st, T(val, dev), T(X, dev)).cpu().numpy()
     ref = oracle.spmm_csr(rp, ci, val, X)
     unsplit = np.diff(rp) <= 64
-    assert np.array_equal(y0.cpu().numpy()[unsplit], ref[unsplit]) and rel(y0.cpu().numpy(), ref) <= TOL
-    for block in (256, 64, 32):
-        y = _with_tuning({"COGDL_B200_STREAM_BLOCK": block}, lambda: spmm_raw(st, vd, xd))
-        assert torch.equal(y, y0), f"block={block}"
+    assert np.array_equal(y[unsplit], ref[unsplit]) and rel(y, ref) <= TOL
     assert int(st.plan.counters.abs().sum()) == 0
 
 
 @pytest.mark.parametrize("name", ["two_hubs", "ragged", "empty_graph"])
 @pytest.mark.parametrize("H,F", [(1, 128), (1, 256), (8, 128), (2, 256)])
 def test_sddmm_stream_and_row_forms_match_the_oracle(dev, name, H, F):
-    """Rows of 128 / 256 floats per head take the row-stream SDDMM (default); COGDL_B200_SDDMM_STREAM=0 selects the
-    row form.  Both agree with the oracle, with and without hub chunks."""
+    """Rows of 128 / 256 floats per head take the row-stream SDDMM when the plan has segments and the row form
+    otherwise.  Both agree with the oracle, with and without hub chunks."""
     from cogdl_b200.operators._raw import mhsddmm_raw, sddmm_raw
 
     rp, ci, n_cols = case(name)
@@ -466,17 +443,18 @@ def test_sddmm_stream_and_row_forms_match_the_oracle(dev, name, H, F):
     else:
         ref = oracle.mhsddmm(rp, ci, grad, feat)
         run = lambda st: mhsddmm_raw(st, T(grad, dev), T(feat, dev))
-    for chunk in (64, 0):
-        st = structure(rp, ci, n_cols, dev, chunk)
-        for mode in (1, 0):
-            out = _with_tuning({"COGDL_B200_SDDMM_STREAM": mode}, lambda: run(st)).cpu().numpy()
-            assert rel(out, ref) <= TOL, f"chunk={chunk} stream={mode}"
+    # stream form (default plan), row form with hub chunks (plan without segments), row form without a plan
+    for chunk, seg_cost in ((64, None), (64, 0), (0, None)):
+        st = structure(rp, ci, n_cols, dev, chunk, seg_cost)
+        out = run(st).cpu().numpy()
+        assert rel(out, ref) <= TOL, f"chunk={chunk} seg_cost={seg_cost}"
         if chunk:
             assert int(st.plan.counters.abs().sum()) == 0
 
 
 @pytest.mark.parametrize("H", [8, 4])
-def test_edge_softmax_warps_per_block_is_a_launch_parameter_only(dev, H):
+def test_edge_softmax_512_float_tiles_match_the_oracle(dev, H):
+    """64-edge hub chunks with H <= 8 take the 512-float-tile main kernel, forward and backward."""
     from cogdl_b200.operators._raw import edge_softmax_bwd_raw, edge_softmax_fwd_raw
 
     rp, ci, n_cols = case("two_hubs")
@@ -484,10 +462,8 @@ def test_edge_softmax_warps_per_block_is_a_launch_parameter_only(dev, H):
     e = T(np.clip(rng.standard_normal((ci.shape[0], H)) * 3, -10, 10).astype(np.float32), dev)
     g = T(rng.standard_normal((ci.shape[0], H)).astype(np.float32), dev)
     st = structure(rp, ci, n_cols, dev, chunk=64)
-    y0 = edge_softmax_fwd_raw(st, e)
-    b0 = edge_softmax_bwd_raw(st, y0, g)
-    assert rel(y0.cpu().numpy(), oracle.edge_softmax_fwd(rp, e.cpu().numpy())) <= TOL
-    for warps in (4, 2):
-        y, b = _with_tuning({"COGDL_B200_ES_WARPS": warps},
-                            lambda: (edge_softmax_fwd_raw(st, e), edge_softmax_bwd_raw(st, y0, g)))
-        assert torch.equal(y, y0) and torch.equal(b, b0), f"warps={warps}"
+    y = edge_softmax_fwd_raw(st, e)
+    b = edge_softmax_bwd_raw(st, y, g)
+    assert rel(y.cpu().numpy(), oracle.edge_softmax_fwd(rp, e.cpu().numpy())) <= TOL
+    assert rel(b.cpu().numpy(), oracle.edge_softmax_bwd(rp, y.cpu().numpy(), g.cpu().numpy())) <= TOL
+    assert int(st.plan.counters.abs().sum()) == 0
