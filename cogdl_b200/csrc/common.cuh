@@ -89,6 +89,22 @@ static inline HubView hub_view(const cogdl_b200_hub_plan_t *plan) {
 
 int check_plan(const cogdl_b200_hub_plan_t *plan, int64_t need_partial_bytes);
 
+// Launch helper of the gather kernels that give GROUP lanes to each of `items` work items (256 threads per block):
+// rejects grids beyond int32 under the caller's name `who`, records the instantiation for cogdl_b200_last_kernel()
+// (printf-style `fmt`) and launches.
+template <typename P, typename... Args>
+static int launch_items(void (*kernel)(P), const P &p, int64_t items, int group, cudaStream_t stream, const char *who,
+                        const char *fmt, Args... args) {
+  const int64_t blocks = ceil_div(items * group, 256);
+  if (blocks == 0) return COGDL_B200_OK;
+  if (blocks > 0x7fffffffLL)
+    return set_error(COGDL_B200_EINVAL, "%s: problem too large for one launch (blocks=%lld)", who, (long long)blocks);
+  note_kernel(fmt, args...);
+  kernel<<<(unsigned)blocks, 256, 0, stream>>>(p);
+  CB_LAUNCH_CHECK();
+  return COGDL_B200_OK;
+}
+
 // ------------------------------------------------------------------ device side
 #ifdef __CUDACC__
 
@@ -145,12 +161,21 @@ __device__ __forceinline__ void axpy_rn(float4 &acc, float v, const float4 &x) {
   acc.z = mul_add_rn(acc.z, v, x.z);
   acc.w = mul_add_rn(acc.w, v, x.w);
 }
+__device__ __forceinline__ void add_rn(float &acc, const float &x) { acc = __fadd_rn(acc, x); }
+__device__ __forceinline__ void add_rn(float2 &acc, const float2 &x) {
+  acc.x = __fadd_rn(acc.x, x.x);
+  acc.y = __fadd_rn(acc.y, x.y);
+}
 __device__ __forceinline__ void add_rn(float4 &acc, const float4 &x) {
   acc.x = __fadd_rn(acc.x, x.x);
   acc.y = __fadd_rn(acc.y, x.y);
   acc.z = __fadd_rn(acc.z, x.z);
   acc.w = __fadd_rn(acc.w, x.w);
 }
+template <typename VecT> __device__ __forceinline__ VecT vzero();
+template <> __device__ __forceinline__ float4 vzero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+template <> __device__ __forceinline__ float2 vzero<float2>() { return make_float2(0.f, 0.f); }
+template <> __device__ __forceinline__ float vzero<float>() { return 0.f; }
 
 template <int WIDTH>
 __device__ __forceinline__ int group_max(int v) {
@@ -214,6 +239,28 @@ __device__ __forceinline__ bool hub_arrive_last(const WorkItem &w, const HubView
     __threadfence();                          // acquire side: partials read after this point
   }
   return last;
+}
+
+// The last chunk's combine: folds the n partials of one hub row strictly in chunk order, DEPTH loads in flight, and
+// returns the result.  The fold starts from partial 0, not from an identity: 0.0f + -0.0f would turn a -0.0f sum
+// into +0.0f.  The row-stream SpMM keeps 8 partials in flight (a 22 K-edge hub has 354: that loop is the kernel's
+// tail); the row kernels and scatter_max fold one at a time -- an 8-deep fold there changed their register
+// allocation and measured slower (DESIGN 3.2).
+template <int DEPTH, typename Load, typename Fold>
+__device__ __forceinline__ auto merge_chunks(const int n, Load load, Fold fold) {
+  auto s = load(0);
+  int q = 1;
+  if constexpr (DEPTH > 1) {
+    for (; q + DEPTH <= n; q += DEPTH) {
+      decltype(s) t[DEPTH];
+#pragma unroll
+      for (int u = 0; u < DEPTH; ++u) t[u] = load(q + u);
+#pragma unroll
+      for (int u = 0; u < DEPTH; ++u) fold(s, t[u]);
+    }
+  }
+  for (; q < n; ++q) fold(s, load(q));
+  return s;
 }
 
 #endif  // __CUDACC__

@@ -34,12 +34,6 @@ struct MhParams {
   HubView hub;
 };
 
-template <typename VecT> __device__ __forceinline__ VecT mh_zero();
-template <> __device__ __forceinline__ float4 mh_zero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-template <> __device__ __forceinline__ float mh_zero<float>() { return 0.f; }
-__device__ __forceinline__ void mh_add(float &a, const float &b) { a = __fadd_rn(a, b); }
-__device__ __forceinline__ void mh_add(float4 &a, const float4 &b) { add_rn(a, b); }
-
 template <typename VecT, int GROUP, bool HAS_PERM>
 __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
   constexpr int U0 = 8;
@@ -63,7 +57,7 @@ __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
   int maxdeg = w.hb - w.lb;
   if (GROUP < 32) maxdeg = warp_max(maxdeg);
 
-  VecT acc = mh_zero<VecT>();
+  VecT acc = vzero<VecT>();
   int c = 0, pe = 0;
   {
     const int e = w.lb + gl;
@@ -121,8 +115,8 @@ __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
     if (hub_arrive_last<GROUP>(wa, p.hub, gl)) {
       for (int k = gl; k < p.HFV; k += GROUP) {
         const VecT *pp = P + (int64_t)w.first * p.HFV + k;
-        VecT s = ld_cg(pp);
-        for (int q = 1; q < w.n_row_chunks; ++q) mh_add(s, ld_cg(pp + (int64_t)q * p.HFV));
+        const VecT s = merge_chunks<1>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.HFV); },
+                                       [](VecT &a, const VecT &t) { add_rn(a, t); });
         st_stream(Y + (int64_t)w.row * p.HFV + k, s);
       }
     }
@@ -131,16 +125,10 @@ __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
 
 template <typename VecT, int GROUP>
 static int launch_mh(const MhParams &p, cudaStream_t stream) {
-  const int64_t groups = ((int64_t)p.hub.n_chunks + p.n_rows) * p.S;
-  const int64_t blocks = ceil_div(groups * GROUP, 256);
-  if (blocks == 0) return COGDL_B200_OK;
-  if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "mhspmm: problem too large for one launch");
-  if (p.perm)
-    mhspmm_kernel<VecT, GROUP, true><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  else
-    mhspmm_kernel<VecT, GROUP, false><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  CB_LAUNCH_CHECK();
-  return COGDL_B200_OK;
+  return launch_items(p.perm ? mhspmm_kernel<VecT, GROUP, true> : mhspmm_kernel<VecT, GROUP, false>, p,
+                      ((int64_t)p.hub.n_chunks + p.n_rows) * p.S, GROUP, stream, "mhspmm",
+                      "cogdl_b200::mhspmm_kernel<%s,GROUP=%d,%s>", sizeof(VecT) == 16 ? "float4" : "float", GROUP,
+                      p.perm ? "perm" : "no_perm");
 }
 
 template <typename VecT>
@@ -155,7 +143,6 @@ static int dispatch_mh(MhParams &p, cudaStream_t s) {
     q.rowptr = p.rowptr; q.colind = p.colind; q.val = nullptr; q.att = p.att; q.perm = p.perm;
     q.X0 = p.feat; q.X1 = p.feat; q.n0 = INT64_MAX; q.Y = p.out; q.ldv = p.HFV; q.H = p.H; q.FVL = p.FVL;
     q.S = p.S; q.hub = p.hub; q.n_peers = 0; q.peer_shift = 0;
-    if (p.n_rows == 0) q.hub.n_segs = 0;   // chunks-only call (fused GAT hub path)
     return launch_stream<VecT, 1, 8, 3, true, FORM_MULTIHEAD>(q, s);
   }
   switch (g) {
@@ -168,13 +155,12 @@ static int dispatch_mh(MhParams &p, cudaStream_t s) {
   }
 }
 
-// rows_too == false processes only the hub-chunk items of the plan.
-int mhspmm_run(const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const float *att,
-               const float *feat, float *out, int64_t n_rows, int64_t H, int64_t F,
-               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream, bool rows_too) {
+static int mhspmm_run(const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const float *att,
+                      const float *feat, float *out, int64_t n_rows, int64_t H, int64_t F,
+                      const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
   MhParams p;
   p.rowptr = rowptr; p.colind = colind; p.perm = perm; p.att = att; p.feat = feat; p.out = out;
-  p.n_rows = rows_too ? n_rows : 0; p.H = (int)H; p.hub = hub_view(plan); p.S = 1;
+  p.n_rows = n_rows; p.H = (int)H; p.hub = hub_view(plan); p.S = 1;
   const bool vec = (F % 4 == 0) && aligned16(feat) && aligned16(out) &&
                    (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
   if (vec) {
@@ -201,7 +187,7 @@ extern "C" int cogdl_b200_mhspmm_f32(const int32_t *rowptr, const int32_t *colin
   CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "cogdl_b200_mhspmm_f32: sizes must fit int32");
   int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
   if (rc) return rc;
-  return mhspmm_run(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream, true);
+  return mhspmm_run(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -236,5 +222,5 @@ extern "C" int cogdl_b200_gat_fwd_f32(const int32_t *rowptr, const int32_t *coli
   if (rc) return rc;
   rc = gat_attention(rowptr, colind, h_l, h_r, negative_slope, att_out, n_rows, H, plan, (cudaStream_t)stream);
   if (rc) return rc;
-  return mhspmm_run(rowptr, colind, nullptr, att_out, feat, out, n_rows, H, F, plan, stream, true);
+  return mhspmm_run(rowptr, colind, nullptr, att_out, feat, out, n_rows, H, F, plan, stream);
 }

@@ -53,6 +53,12 @@ __device__ __forceinline__ void init_acc(float4 &m, int4 &id) {
 }
 __device__ __forceinline__ void zero_acc(float &m) { m = 0.f; }
 __device__ __forceinline__ void zero_acc(float4 &m) { m = make_float4(0.f, 0.f, 0.f, 0.f); }
+// (max, argmax) partial of one lane vector, as the last chunk of a hub row combines them
+template <typename VecT>
+struct MaxAcc {
+  VecT m;
+  typename IdxOf<VecT>::type id;
+};
 __device__ __forceinline__ int4 ld_cg(const int4 *p) { return __ldcg(p); }
 __device__ __forceinline__ void st_cg(int4 *p, int4 v) { __stcg(p, v); }
 __device__ __forceinline__ void st_stream(int4 *p, int4 v) { __stcs(p, v); }
@@ -150,13 +156,16 @@ __global__ void __launch_bounds__(256) scatter_max_fwd_kernel(const SmaxParams p
   if (warp_has_chunk) {
     if (hub_arrive_last<GROUP>(w, p.hub, gl)) {
       for (int cv = gl; cv < p.FV; cv += GROUP) {
-        VecT m;
-        IdxT id;
-        init_acc(m, id);
-        for (int q = 0; q < w.n_row_chunks; ++q)   // chunk order + strict `<` keeps "first max wins"
-          upd2(m, id, ld_cg(PV + (int64_t)(w.first + q) * p.FV + cv), ld_cg(PI + (int64_t)(w.first + q) * p.FV + cv));
-        st_stream(O + (int64_t)w.row * p.FV + cv, m);
-        st_stream(A + (int64_t)w.row * p.FV + cv, id);
+        // chunk order + strict `<` keeps "first max wins"
+        const MaxAcc<VecT> m = merge_chunks<1>(
+            w.n_row_chunks,
+            [&](int q) {
+              const int64_t i = (int64_t)(w.first + q) * p.FV + cv;
+              return MaxAcc<VecT>{ld_cg(PV + i), ld_cg(PI + i)};
+            },
+            [](MaxAcc<VecT> &s, const MaxAcc<VecT> &t) { upd2(s.m, s.id, t.m, t.id); });
+        st_stream(O + (int64_t)w.row * p.FV + cv, m.m);
+        st_stream(A + (int64_t)w.row * p.FV + cv, m.id);
       }
     }
   }
@@ -276,13 +285,15 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
   if (is_chunk) {
     if (hub_arrive_last<32>(w, p.hub, lane)) {
       for (int cv = lane; cv < p.FV; cv += 32) {
-        float4 m;
-        int4 idm;
-        init_acc(m, idm);
-        for (int q = 0; q < w.n_row_chunks; ++q)
-          upd2(m, idm, ld_cg(PV + (int64_t)(w.first + q) * p.FV + cv), ARGMAX ? ld_cg(PI + (int64_t)(w.first + q) * p.FV + cv) : idm);
-        st_stream(O + (int64_t)w.row * p.FV + cv, m);
-        if (ARGMAX) st_stream(A + (int64_t)w.row * p.FV + cv, idm);
+        const MaxAcc<float4> m = merge_chunks<1>(
+            w.n_row_chunks,
+            [&](int q) {
+              const int64_t i = (int64_t)(w.first + q) * p.FV + cv;
+              return MaxAcc<float4>{ld_cg(PV + i), ARGMAX ? ld_cg(PI + i) : make_int4(-1, -1, -1, -1)};
+            },
+            [](MaxAcc<float4> &s, const MaxAcc<float4> &t) { upd2(s.m, s.id, t.m, t.id); });
+        st_stream(O + (int64_t)w.row * p.FV + cv, m.m);
+        if (ARGMAX) st_stream(A + (int64_t)w.row * p.FV + cv, m.id);
       }
     }
   }
@@ -292,24 +303,16 @@ __global__ void __launch_bounds__(256) scatter_max_stream_kernel(const SmaxParam
 // shape F=256: 11.38 ms (row-stream form) vs 11.52 ms (row per warp)
 template <int NV>
 static int launch_smax_stream(const SmaxParams &p, cudaStream_t stream) {
-  const int64_t warps = (int64_t)p.hub.n_chunks + p.hub.n_segs;
-  const int64_t blocks = ceil_div(warps * 32, 256);
-  if (blocks == 0) return COGDL_B200_OK;
-  if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "scatter_max: problem too large for one launch");
-  scatter_max_stream_kernel<NV, (NV == 1 ? 4 : 2)><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  CB_LAUNCH_CHECK();
-  return COGDL_B200_OK;
+  constexpr int U = NV == 1 ? 4 : 2;
+  return launch_items(scatter_max_stream_kernel<NV, U>, p, (int64_t)p.hub.n_chunks + p.hub.n_segs, 32, stream,
+                      "scatter_max", "cogdl_b200::scatter_max_stream_kernel<NV=%d,U=%d>", NV, U);
 }
 
 template <typename VecT, int GROUP, int NV>
 static int launch_smax(const SmaxParams &p, cudaStream_t stream) {
-  const int64_t items = (int64_t)p.hub.n_chunks + p.n_rows;
-  const int64_t blocks = ceil_div(items * GROUP, 256);
-  if (blocks == 0) return COGDL_B200_OK;
-  if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "scatter_max: problem too large for one launch");
-  scatter_max_fwd_kernel<VecT, GROUP, NV><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  CB_LAUNCH_CHECK();
-  return COGDL_B200_OK;
+  return launch_items(scatter_max_fwd_kernel<VecT, GROUP, NV>, p, (int64_t)p.hub.n_chunks + p.n_rows, GROUP, stream,
+                      "scatter_max", "cogdl_b200::scatter_max_fwd_kernel<%s,GROUP=%d,NV=%d>",
+                      sizeof(VecT) == 16 ? "float4" : "float", GROUP, NV);
 }
 
 template <typename VecT>

@@ -48,11 +48,6 @@ struct SpmmParams {
   HubView hub;
 };
 
-template <typename VecT> __device__ __forceinline__ VecT vzero();
-template <> __device__ __forceinline__ float4 vzero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-template <> __device__ __forceinline__ float vzero<float>() { return 0.f; }
-__device__ __forceinline__ void add_rn(float &a, const float &b) { a = __fadd_rn(a, b); }
-
 template <typename VecT, int GROUP, int NV, bool HAS_VAL>
 __global__ void __launch_bounds__(256) spmm_kernel(const SpmmParams p) {
   constexpr int U0 = (NV == 1) ? 8 : (NV == 2 ? 4 : 2);
@@ -156,8 +151,8 @@ __global__ void __launch_bounds__(256) spmm_kernel(const SpmmParams p) {
       // combine this row's partial sums in chunk order (deterministic, independent of arrival)
       for (int cv = gl; cv < p.FV; cv += GROUP) {
         const VecT *pp = P + (int64_t)w.first * p.FV + cv;
-        VecT s = ld_cg(pp);
-        for (int q = 1; q < w.n_row_chunks; ++q) add_rn(s, ld_cg(pp + (int64_t)q * p.FV));
+        const VecT s = merge_chunks<1>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.FV); },
+                                       [](VecT &a, const VecT &t) { add_rn(a, t); });
         st_stream(Y + (int64_t)w.row * p.FV + cv, s);
       }
     }
@@ -251,21 +246,10 @@ static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_
 
 template <typename VecT, int GROUP, int NV>
 static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
-  const int64_t items = (int64_t)p.hub.n_chunks + p.n_rows;
-  const int64_t threads = items * GROUP;
-  const int64_t blocks = ceil_div(threads, 256);
-  if (blocks == 0) return COGDL_B200_OK;
-  if (blocks > 0x7fffffffLL)
-    return set_error(COGDL_B200_EINVAL, "spmm: problem too large for one launch (blocks=%lld)", (long long)blocks);
-  dim3 grid((unsigned)blocks);
-  note_kernel("cogdl_b200::spmm_kernel<%s,GROUP=%d,NV=%d,%s>", sizeof(VecT) == 16 ? "float4" : "float", GROUP, NV,
-              p.val ? "weighted" : "unweighted");
-  if (p.val)
-    spmm_kernel<VecT, GROUP, NV, true><<<grid, 256, 0, stream>>>(p);
-  else
-    spmm_kernel<VecT, GROUP, NV, false><<<grid, 256, 0, stream>>>(p);
-  CB_LAUNCH_CHECK();
-  return COGDL_B200_OK;
+  return launch_items(p.val ? spmm_kernel<VecT, GROUP, NV, true> : spmm_kernel<VecT, GROUP, NV, false>, p,
+                      (int64_t)p.hub.n_chunks + p.n_rows, GROUP, stream, "spmm",
+                      "cogdl_b200::spmm_kernel<%s,GROUP=%d,NV=%d,%s>", sizeof(VecT) == 16 ? "float4" : "float", GROUP,
+                      NV, p.val ? "weighted" : "unweighted");
 }
 
 // narrow rows (F = 40 -> 10 float4): the lean row-stream form with the idle lanes masked beats the sub-warp

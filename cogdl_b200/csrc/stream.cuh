@@ -55,14 +55,6 @@ enum { SRC_ONE = 0, SRC_TWO = 1, SRC_PEERS = 2 };
 // the multi-head SpMM.
 enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
 
-template <typename VecT> __device__ __forceinline__ VecT sk_zero();
-template <> __device__ __forceinline__ float4 sk_zero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-template <> __device__ __forceinline__ float2 sk_zero<float2>() { return make_float2(0.f, 0.f); }
-template <> __device__ __forceinline__ float sk_zero<float>() { return 0.f; }
-__device__ __forceinline__ void sk_add(float &a, const float &b) { a = __fadd_rn(a, b); }
-__device__ __forceinline__ void sk_add(float2 &a, const float2 &b) { a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); }
-__device__ __forceinline__ void sk_add(float4 &a, const float4 &b) { add_rn(a, b); }
-
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
 // whole range into acc (hub chunk).
 template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH>
@@ -133,7 +125,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
 #pragma unroll
           for (int k = 0; k < NV; ++k) {
             if (colok[k]) {
-              if (MODE == MODE_UNWEIGHTED) sk_add(acc[k], x[u][k]);          // 1.0f * x == x exactly
+              if (MODE == MODE_UNWEIGHTED) add_rn(acc[k], x[u][k]);          // 1.0f * x == x exactly
               else if (MODE == MODE_WEIGHTED) axpy_rn(acc[k], vj, x[u][k]);
               else axpy_rn(acc[k], a[u], x[u][k]);
             }
@@ -141,7 +133,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
           if (ROWS && ((em >> u) & 1u)) {   // last edge of row rj: store and restart (warp-uniform)
 #pragma unroll
             for (int k = 0; k < NV; ++k)
-              if (colok[k]) { st_stream(Y + (int64_t)rj * p.ldv + k * 32, acc[k]); acc[k] = sk_zero<VecT>(); }
+              if (colok[k]) { st_stream(Y + (int64_t)rj * p.ldv + k * 32, acc[k]); acc[k] = vzero<VecT>(); }
           }
         }
       }
@@ -173,7 +165,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
     return reinterpret_cast<const VecT *>(p.peers[r >> p.peer_shift]) + cv + (int64_t)(r & ((1u << p.peer_shift) - 1u)) * p.ldv;
   };
   auto accumulate = [&](float vj, const VecT &x) {
-    if (MODE == MODE_UNWEIGHTED) sk_add(acc, x); else axpy_rn(acc, vj, x);
+    if (MODE == MODE_UNWEIGHTED) add_rn(acc, x); else axpy_rn(acc, vj, x);
   };
   auto load_slab = [&](int base, int &c, float &v, int &rid, int &rnx) {
     const int q = base + lane;
@@ -240,7 +232,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
           if (colok) accumulate(val_of(u), x[u]);
           if ((em >> u) & 1u) {                     // last edge of its row: store and restart (warp-uniform)
             const int rj = s_r[j + u];
-            if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = sk_zero<VecT>(); }
+            if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = vzero<VecT>(); }
           }
         }
       }
@@ -251,7 +243,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
       if (colok) accumulate(__int_as_float(cw.y), ld_gather(src_ptr(cw.x)));
       if (ROWS && ((endmask >> j) & 1u)) {
         const int rj = s_r[j];
-        if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = sk_zero<VecT>(); }
+        if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = vzero<VecT>(); }
       }
     }
   }
@@ -281,7 +273,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
       bool colok[NV];
       VecT acc[NV];
 #pragma unroll
-      for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = sk_zero<VecT>(); }
+      for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = vzero<VecT>(); }
       const int head = (MODE == MODE_MULTIHEAD && colok[0]) ? cv / p.FVL : 0;
       if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false, PANEL && PREFETCH>(p, w.lb, w.hb, cv, colok[0], lane, s_cv, s_r, acc[0]);
       else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH>(p, w.lb, w.hb, cv, colok, head, lane, acc);
@@ -307,16 +299,8 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
       const int c_begin = PANEL ? t_begin : 0, c_end = PANEL ? min(t_begin + 32, p.ldv) : p.ldv;
       for (int cv = c_begin + lane; cv < c_end; cv += 32) {
         const VecT *pp = P + (int64_t)w.first * p.ldv + cv;
-        VecT s = ld_cg(pp);
-        int q = 1;
-        for (; q + 8 <= w.n_row_chunks; q += 8) {      // 8 partials in flight, added in chunk order (a 22 K-edge
-          VecT t[8];                                   // hub has 354 of them: this loop is the kernel's tail)
-#pragma unroll
-          for (int u = 0; u < 8; ++u) t[u] = ld_cg(pp + (int64_t)(q + u) * p.ldv);
-#pragma unroll
-          for (int u = 0; u < 8; ++u) sk_add(s, t[u]);
-        }
-        for (; q < w.n_row_chunks; ++q) sk_add(s, ld_cg(pp + (int64_t)q * p.ldv));
+        const VecT s = merge_chunks<8>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.ldv); },
+                                       [](VecT &a, const VecT &t) { add_rn(a, t); });
         st_stream(Y + (int64_t)w.row * p.ldv + cv, s);
       }
     }
@@ -333,7 +317,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
     bool colok[NV];
     VecT acc[NV];
 #pragma unroll
-    for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = sk_zero<VecT>(); }
+    for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = vzero<VecT>(); }
     const int head = (MODE == MODE_MULTIHEAD && colok[0]) ? cv / p.FVL : 0;
     if (p.hub.n_empty_rows > 0) {
       // rows without edges never show up in the edge stream: zero-fill them here
@@ -345,7 +329,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
           m &= m - 1;
 #pragma unroll
           for (int k = 0; k < NV; ++k)
-            if (colok[k]) st_stream(Y + (int64_t)(rb + k0) * p.ldv + cv + k * 32, sk_zero<VecT>());
+            if (colok[k]) st_stream(Y + (int64_t)(rb + k0) * p.ldv + cv + k * 32, vzero<VecT>());
         }
       }
     }

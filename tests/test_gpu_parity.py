@@ -56,8 +56,10 @@ def test_spmm_matches_oracle(dev, name, F, weighted):
     X = rng.standard_normal((n_cols, F)).astype(np.float32)
     val = rng.random(ci.shape[0]).astype(np.float32) if weighted else None
     ref = oracle.spmm_csr(rp, ci, val, X)
-    for chunk in (0, 256):  # 0: no hub plan -> strictly sequential -> bit exact everywhere
-        st = structure(rp, ci, n_cols, dev, chunk)
+    # chunk 0: no hub plan -> strictly sequential -> bit exact everywhere; seg_cost 0: a plan without segments, so
+    # every width runs the row kernel with hub chunks
+    for chunk, seg_cost in ((0, None), (256, None), (256, 0)):
+        st = structure(rp, ci, n_cols, dev, chunk, seg_cost)
         y = spmm_raw(st, None if val is None else T(val, dev), T(X, dev)).cpu().numpy()
         assert y.shape == ref.shape
         deg = np.diff(rp)
@@ -256,8 +258,8 @@ def test_mhspmm_and_mhsddmm(dev, name, H, F):
     grad = rng.standard_normal((n, H, F)).astype(np.float32)
     ref = oracle.mhspmm(rp, ci, att, feat)
     ref_sd = oracle.mhsddmm(rp, ci, grad, feat)
-    for chunk in (0, 256):
-        st = structure(rp, ci, n_cols, dev, chunk)
+    for chunk, seg_cost in ((0, None), (256, None), (256, 0)):   # seg_cost 0: row kernel with hub chunks
+        st = structure(rp, ci, n_cols, dev, chunk, seg_cost)
         out = mhspmm_raw(st, T(att, dev), T(feat, dev)).cpu().numpy()
         unsplit = np.diff(rp) <= chunk if chunk else np.ones(n, bool)
         assert np.array_equal(out[unsplit], ref[unsplit])
@@ -295,8 +297,8 @@ def test_scatter_max_fwd_bwd(dev, name, F):
     # mixed sign + deliberate ties (quantised values) to exercise "first max wins"
     X = np.round(rng.standard_normal((n_cols, F)) * 4).astype(np.float32) / 4
     ref, ref_id = oracle.scatter_max_fwd(rp, ci, X)
-    for chunk in (0, 256):
-        out, arg = scatter_max_fwd_raw(structure(rp, ci, n_cols, dev, chunk), T(X, dev))
+    for chunk, seg_cost in ((0, None), (256, None), (256, 0)):   # seg_cost 0: row kernel with hub chunks
+        out, arg = scatter_max_fwd_raw(structure(rp, ci, n_cols, dev, chunk, seg_cost), T(X, dev))
         assert np.array_equal(out.cpu().numpy(), ref)         # max is exact
         assert np.array_equal(arg.cpu().numpy(), ref_id)      # integer output: bit exact, ties included
     g = rng.standard_normal((n, F)).astype(np.float32)
@@ -314,6 +316,27 @@ def test_scatter_max_reference_semantics_agree_on_positive_features(dev):
     out, arg = scatter_max_fwd_raw(structure(rp, ci, n_cols, dev), T(X, dev))
     has = np.diff(rp) > 0
     assert np.array_equal(out.cpu().numpy()[has], ref[has]) and np.array_equal(arg.cpu().numpy()[has], ref_id[has])
+
+
+def test_scatter_max_and_mhspmm_name_their_kernel(dev):
+    """cogdl_b200_last_kernel() names what scatter_max (both forms) and the row form of the multi-head SpMM
+    launched, not the kernel of an earlier call."""
+    from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import mhspmm_raw, scatter_max_fwd_raw, spmm_raw
+
+    rp, ci, n_cols = case("hub")
+    st = structure(rp, ci, n_cols, dev)
+    rng = np.random.default_rng(15)
+    spmm_raw(st, None, T(rng.standard_normal((n_cols, 128)).astype(np.float32), dev))
+    assert "stream_kernel<" in _cabi.last_kernel()
+    scatter_max_fwd_raw(st, T(rng.standard_normal((n_cols, 16)).astype(np.float32), dev))
+    assert _cabi.last_kernel() == "cogdl_b200::scatter_max_fwd_kernel<float4,GROUP=4,NV=1>", _cabi.last_kernel()
+    spmm_raw(st, None, T(rng.standard_normal((n_cols, 128)).astype(np.float32), dev))
+    att = T(rng.random((ci.shape[0], 8)).astype(np.float32), dev)
+    mhspmm_raw(st, att, T(rng.standard_normal((n_cols, 8, 8)).astype(np.float32), dev))
+    assert _cabi.last_kernel() == "cogdl_b200::mhspmm_kernel<float4,GROUP=16,no_perm>", _cabi.last_kernel()
+    scatter_max_fwd_raw(st, T(rng.standard_normal((n_cols, 256)).astype(np.float32), dev))
+    assert _cabi.last_kernel() == "cogdl_b200::scatter_max_stream_kernel<NV=2,U=2>", _cabi.last_kernel()
 
 
 # ------------------------------------------------------------------------------------ fused GAT

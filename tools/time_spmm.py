@@ -1,4 +1,11 @@
-"""SpMM timings on the arxiv shape for several widths (CUDA events, L2 flushed, median of 30)."""
+"""Gather-kernel timings on the arxiv shape (CUDA events, L2 flushed, median of 30), with a SHA-256 of every output.
+
+Inputs are seeded, so the hashes of two builds match exactly when the builds compute the same bits.
+
+  python tools/time_spmm.py              # every workload below
+  python tools/time_spmm.py 128 40       # only the SpMM (default plan) at these widths
+"""
+import hashlib
 import os
 import statistics
 import sys
@@ -8,7 +15,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
 from cogdl_b200 import _cabi, synth  # noqa: E402
-from cogdl_b200.operators._raw import spmm_raw  # noqa: E402
+from cogdl_b200.operators._raw import mhspmm_raw, scatter_max_fwd_raw, spmm_raw  # noqa: E402
 
 dev = torch.device("cuda")
 n, e = synth.SHAPES["arxiv"]
@@ -16,23 +23,55 @@ rp, col = synth.powerlaw_csr(n, e, seed=0)
 w = synth.sym_norm_weights(rp, col).to(dev)
 st = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n)
 st.plan
+st_noplan = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n, chunk_edges=0)
 flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
-for F in [int(a) for a in sys.argv[1:]] or [128, 40, 64, 16, 256]:
-    x = torch.randn(n, F, device=dev)
-    for wt in (w, None):
-        fn = lambda: spmm_raw(st, wt, x)
-        for _ in range(3):
-            fn()
-        ts = []
-        for _ in range(30):
-            flush.zero_()
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            fn()
-            b.record()
-            torch.cuda.synchronize()
-            ts.append(a.elapsed_time(b) * 1e3)
+
+
+def randn(*shape, seed):
+    return torch.randn(*shape, device=dev, generator=torch.Generator(device=dev).manual_seed(seed))
+
+
+def digest(out):
+    h = hashlib.sha256()
+    for t in out if isinstance(out, tuple) else (out,):
+        h.update(t.contiguous().cpu().numpy().tobytes())
+    return h.hexdigest()[:16]
+
+
+def run(label, fn, algo=None):
+    for _ in range(3):
+        out = fn()
+    ts = []
+    for _ in range(30):
+        flush.zero_()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        torch.cuda.synchronize()
+        ts.append(a.elapsed_time(b) * 1e3)
+    med = statistics.median(ts)
+    rate = f"{algo / med / 1e3:7.0f} GB/s" if algo else " " * 12
+    print(f"{label:32s} median {med:8.1f} us min {min(ts):8.1f} us {rate}  sha256 {digest(out)}  [{_cabi.last_kernel()}]")
+
+
+def spmm(F, structure=st, tag="", weights=(w, None)):
+    x = randn(n, F, seed=F)
+    for wt in weights:
         algo = st.nnz * (4 * F + (8 if wt is not None else 4)) + n * (4 * F + 4)
-        med = statistics.median(ts)
-        print(f"F={F:4d} {'weighted  ' if wt is not None else 'unweighted'} median {med:7.1f} us min {min(ts):7.1f} us  {algo / med / 1e3:7.0f} GB/s  "
-              f"frac {algo / med / 1e3 / 6566.1:5.3f}  [{_cabi.last_kernel()}]")
+        run(f"spmm F={F} {'weighted' if wt is not None else 'unweighted'}{tag}", lambda: spmm_raw(structure, wt, x), algo)
+
+
+if sys.argv[1:]:
+    for F in (int(a) for a in sys.argv[1:]):
+        spmm(F)
+    sys.exit(0)
+for F in (7, 16, 32):
+    spmm(F)
+spmm(128, st_noplan, " chunk_edges=0")
+for H, F in ((8, 8), (4, 8), (1, 16)):
+    att, feat = torch.rand(st.nnz, H, device=dev, generator=torch.Generator(device=dev).manual_seed(H)), randn(n, H, F, seed=F)
+    run(f"mhspmm H={H} F={F}", lambda: mhspmm_raw(st, att, feat))
+for F in (4, 7, 8, 16, 40, 128, 256):
+    x = randn(n, F, seed=F)
+    run(f"scatter_max F={F}", lambda: scatter_max_fwd_raw(st, x))
