@@ -17,7 +17,9 @@ building models.  Two levels are patched:
 
 With genconv=True, `cogdl.layers.deepergcn_layer.GENConv.forward` (DeeperGCN, RevGCN) is also rebound, to
 genconv_forward below, which sends the aggregation to cogdl_b200.genconv_aggregate.  The original forward stays
-reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores it).
+reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores it).  disengcn=True does the same for
+`cogdl.layers.disengcn_layer.DisenGCNLayer.forward` (DisenGCN), with disengcn_forward and cogdl_b200.disen_routing
+(uninstall_disengcn()).
 """
 import sys
 
@@ -48,27 +50,63 @@ def genconv_forward(self, graph, x):
     return self.mlp(h)
 
 
-def install_genconv():
-    import cogdl.layers.deepergcn_layer as dl
-
-    cls = dl.GENConv
+def _rebind_forward(cls, forward, name):
+    """cls.forward = forward, keeping the original at cls._cogdl_b200_original_forward; idempotent."""
     if getattr(cls.forward, "_cogdl_b200", False):
         return []
     cls._cogdl_b200_original_forward = cls.forward
-    genconv_forward._cogdl_b200 = True
-    cls.forward = genconv_forward
-    return ["cogdl.layers.deepergcn_layer.GENConv.forward"]
+    forward._cogdl_b200 = True
+    cls.forward = forward
+    return [name]
+
+
+def _restore_forward(cls):
+    if getattr(cls.forward, "_cogdl_b200", False):
+        cls.forward = cls._cogdl_b200_original_forward
+
+
+def install_genconv():
+    import cogdl.layers.deepergcn_layer as dl
+
+    return _rebind_forward(dl.GENConv, genconv_forward, "cogdl.layers.deepergcn_layer.GENConv.forward")
 
 
 def uninstall_genconv():
     import cogdl.layers.deepergcn_layer as dl
 
-    cls = dl.GENConv
-    if getattr(cls.forward, "_cogdl_b200", False):
-        cls.forward = cls._cogdl_b200_original_forward
+    _restore_forward(dl.GENConv)
 
 
-def install(rebind_dispatch=True, genconv=False):
+def disengcn_forward(self, graph, x):
+    """DisenGCNLayer.forward (cogdl/layers/disengcn_layer.py:40-91) with the routing in the sm_90a kernels: the
+    layer's own weight, bias and activation give h, and cogdl_b200.disen_routing does the per-channel
+    normalisation and the iterations.  CPU or non-fp32 input and channel widths without a kernel (d not a power
+    of two up to 32, or out_feats not K * d) run the original."""
+    from .operators.disen_routing import SUPPORTED_D, disen_routing
+    from .utils.spmm_utils import _structure
+
+    original = type(self)._cogdl_b200_original_forward
+    d, K = self.factor_dim, self.K
+    if (not x.is_cuda or x.dtype != torch.float32 or self.weight.dtype != torch.float32 or d not in SUPPORTED_D
+            or self.weight.shape[1] != K * d):
+        return original(self, graph, x)
+    h = self.activation(torch.matmul(x, self.weight) + self.bias)
+    return disen_routing(_structure(graph), h, K, self.iterations, self.tau)
+
+
+def install_disengcn():
+    import cogdl.layers.disengcn_layer as dl
+
+    return _rebind_forward(dl.DisenGCNLayer, disengcn_forward, "cogdl.layers.disengcn_layer.DisenGCNLayer.forward")
+
+
+def uninstall_disengcn():
+    import cogdl.layers.disengcn_layer as dl
+
+    _restore_forward(dl.DisenGCNLayer)
+
+
+def install(rebind_dispatch=True, genconv=False, disengcn=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -150,4 +188,6 @@ def install(rebind_dispatch=True, genconv=False):
                     patched.append(f"{mname}.{attr}")
     if genconv:
         patched += install_genconv()
+    if disengcn:
+        patched += install_disengcn()
     return patched

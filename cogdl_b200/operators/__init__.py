@@ -16,3 +16,4 @@ from .mhspmm import csrmhspmm, MHSPMMFunction  # noqa: F401
 from .scatter_max import scatter_max, ScatterMaxFunction  # noqa: F401
 from .fused_gat import fused_gat_func, FusedGATFunction  # noqa: F401
 from .softmax_aggr import genconv_aggregate, SoftmaxAggrFunction  # noqa: F401
+from .disen_routing import disen_routing, DisenRouteFunction  # noqa: F401

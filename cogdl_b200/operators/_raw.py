@@ -263,6 +263,70 @@ def softmax_aggr_bwd_raw(st: CSRStructure, x, beta, eps, g, out, lse2, edge_term
     return dx, da
 
 
+def _dr_scratch(st, F, K):
+    if st.chunk_edges <= 0:
+        return 0
+    return int(_cabi.load().cogdl_b200_disen_route_scratch_bytes(st.plan.n_chunks, F, K))
+
+
+def _dr_check(st, K, **feats):
+    """[n, F] fp32 contiguous features of one routing step, all on one device."""
+    require_cuda(*feats.values())
+    out = []
+    for name, t in feats.items():
+        t = _f32c(t, name)
+        if t.dim() != 2 or t.shape[0] != st.n_rows:
+            raise ValueError(f"{name} must be [{st.n_rows}, F], got {tuple(t.shape)}")
+        out.append(t)
+    F = out[0].shape[1]
+    if any(t.shape[1] != F for t in out):
+        raise ValueError("the routing features must have the same width")
+    if K < 1 or F % K:
+        raise ValueError(f"F={F} is not a multiple of K={K}")
+    return out, F
+
+
+def disen_route_fwd_raw(st: CSRStructure, q, c, K, tau, want_saved=False):
+    """One DisenGCN routing step: out[i,k] = u / |u|, u = sum_e softmax_e(q[i,k] . c[j,k] / tau) c[j,k] + c[i,k]
+    over row i's edges, per channel k of d = F/K columns.  Returns (out [n, F], lse2 [n, K], r [n, K]); lse2 (base-2
+    log-sum-exp of the logits) and r (|u|) are for the backward and None unless want_saved."""
+    dev = require_cuda(q, c)
+    (q, c), F = _dr_check(st, K, q=q, c=c)
+    n = st.n_rows
+    with torch.cuda.device(dev):
+        out = torch.empty((n, F), dtype=torch.float32, device=dev)
+        lse2 = torch.empty((n, K), dtype=torch.float32, device=dev) if want_saved else None
+        r = torch.empty_like(lse2) if want_saved else None
+        plan, keep = st.plan_struct(_dr_scratch(st, F, K))
+        _cabi.call("cogdl_b200_disen_route_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(q), _ptr(c), _ptr(out),
+                   _ptr(lse2), _ptr(r), n, st.n_cols, F, K, float(tau), plan, _stream(dev))
+        del keep
+    return out, lse2, r
+
+
+def disen_route_bwd_raw(st: CSRStructure, q, c, K, tau, g, out, lse2, r):
+    """(dq, dc) [n, F] of disen_route_fwd_raw given g = dL/dout: a row pass over st and a column pass over its
+    cached transpose.  Scratch g_u [n, F] and D [n, K]; nothing edge-sized."""
+    dev = require_cuda(q, c, g, out, lse2, r)
+    (q, c, g, out), F = _dr_check(st, K, q=q, c=c, grad=g, out=out)
+    lse2, r = _f32c(lse2, "lse2"), _f32c(r, "r")
+    n = st.n_rows
+    for name, t in (("lse2", lse2), ("r", r)):
+        if t.shape != (n, K):
+            raise ValueError(f"{name} must be [{n}, {K}], got {tuple(t.shape)}")
+    st_t, _ = st.csc()
+    with torch.cuda.device(dev):
+        dq, dc, gu = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+        D = torch.empty_like(lse2)
+        plan, keep = st.plan_struct(_dr_scratch(st, F, K))
+        plan_t, keep_t = st_t.plan_struct(_dr_scratch(st_t, F, K))
+        _cabi.call("cogdl_b200_disen_route_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), plan, _ptr(st_t.rowptr),
+                   _ptr(st_t.colind), plan_t, _ptr(q), _ptr(c), _ptr(g), _ptr(out), _ptr(lse2), _ptr(r), _ptr(gu),
+                   _ptr(D), _ptr(dq), _ptr(dc), n, st.n_cols, F, K, float(tau), _stream(dev))
+        del keep, keep_t
+    return dq, dc
+
+
 def edge_colsum_raw(st_t: CSRStructure, perm, e):
     """out[j,h] = sum of e[p,h] over the edges p whose column is j (st_t = cached transpose, perm its permutation)."""
     dev = require_cuda(perm, e)

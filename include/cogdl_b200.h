@@ -370,6 +370,40 @@ COGDL_B200_API int cogdl_b200_softmax_aggr_bwd_f32(const int32_t *colptr, const 
                                     float *d_edge_term, int64_t n_cols, int64_t F, const cogdl_b200_hub_plan_t *plan,
                                     cogdl_b200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * DisenGCN neighbourhood routing, one step (cogdl/layers/disengcn_layer.py:40-91) without per-edge feature
+ * tensors.  Rows of F = K*d floats are K channels of d (channel k = columns [k*d, (k+1)*d)).  c holds the
+ * per-(node, channel) normalised features, q the current routing state ([n, F] each).  Per row i, channel k,
+ * over the CSR edges e = (i, j):
+ *   s_e = (q[i,k] . c[j,k]) / tau,  w_e = softmax over row i's edges of s_e,  u = sum_e w_e c[j,k] + c[i,k]
+ *   out[i,k] = u / |u|           (degree-0 rows: u = c[i,k]; |u| = 0 gives NaN, as the reference)
+ * Optional training outputs, [n, K], both or neither:
+ *   lse2[i,k] = log2 sum_e 2^(s_e log2 e)   (base-2 log-sum-exp of the logits)      r[i,k] = |u|
+ * The structure must be square (n_rows == n_cols); F % K == 0; d = F/K a power of two from 1 to 32; tau > 0.
+ * 16-byte vectors when d % 4 == 0 and every feature buffer is 16-byte aligned.  Hub rows are cut into the plan's
+ * chunks and merged in chunk order (no float atomics: bit-reproducible).  plan->partials needs
+ * cogdl_b200_disen_route_scratch_bytes(n_chunks, F, K) bytes, which also covers the backward.
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_disen_route_scratch_bytes(int64_t n_chunks, int64_t F, int64_t K);
+COGDL_B200_API int cogdl_b200_disen_route_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *q,
+                                   const float *c, float *out, float *lse2, float *r, int64_t n_rows,
+                                   int64_t n_cols, int64_t F, int64_t K, float tau,
+                                   const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+/* Backward of one step, given G = dL/dout and the forward's out, lse2 and r.  Two kernels:
+ *   row kernel (CSR rowptr/colind, its plan `plan`): g_u = (G - out (out . G)) / r into the caller's scratch
+ *     g_u [n, F]; with t_e = g_u[i] . c[j] and D[i,k] = sum_e w_e t_e (into the scratch D [n, K]),
+ *     dq[i] = sum_e w_e (t_e - D[i]) c[j] / tau
+ *   column kernel (transpose colptr/rowind of cogdl_b200_csr2csc, ITS plan `plan_t`):
+ *     dc[j] = g_u[j] + sum_{e=(i,j)} [w_e g_u[i] + w_e (t_e - D[i]) q[i] / tau]
+ * w_e is recomputed from lse2.  plan's partials need n_chunks*(2F+K)*4 bytes, plan_t's n_chunks*F*4 (both within
+ * cogdl_b200_disen_route_scratch_bytes); hub rows / columns are merged in chunk order.  dq and dc are overwritten. */
+COGDL_B200_API int cogdl_b200_disen_route_bwd_f32(const int32_t *rowptr, const int32_t *colind,
+                                   const cogdl_b200_hub_plan_t *plan, const int32_t *colptr,
+                                   const int32_t *rowind, const cogdl_b200_hub_plan_t *plan_t, const float *q,
+                                   const float *c, const float *G, const float *out, const float *lse2,
+                                   const float *r, float *g_u, float *D, float *dq, float *dc, int64_t n_rows,
+                                   int64_t n_cols, int64_t F, int64_t K, float tau, cogdl_b200_stream_t stream);
+
 /* Device COO -> CSR (stable): row_ptr[num_nodes+1] and reindex[nnz] (CSR slot -> COO position),
  * int64 as cogdl.data.Graph stores them.
  * Replaces  sampler.coo2csr_cpu_index(row, col, num_nodes)   cogdl/operators/sample/sample.cpp:234-270
