@@ -10,6 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libcogdl_b200.so")
 MAX_PANELS = 8   # COGDL_B200_MAX_PANELS: a hub plan holds n_chunks * MAX_PANELS arrival counters
+COMP_OPS = {"mult": 0, "sub": 1, "copy": 2}   # COGDL_B200_COMP_MULT / _SUB / _COPY of cogdl_b200_comp_aggr_f32
 
 OK, EINVAL, ECUDA, EDEVICE, ESCRATCH = 0, -1, -2, -3, -4
 
@@ -87,6 +88,9 @@ SIGNATURES = {
                                                       _plan_p, _vp]),
     "cogdl_b200_disen_route_bwd_f32": (ctypes.c_int, [_vp, _vp, _plan_p, _vp, _vp, _plan_p, _vp, _vp, _vp, _vp, _vp, _vp,
                                                       _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _f32, _vp]),
+    "cogdl_b200_comp_aggr_scratch_bytes": (_i64, [_i64, _i64]),
+    "cogdl_b200_comp_aggr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _plan_p,
+                                                _vp]),
     "cogdl_b200_coo2csr_workspace_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_coo2csr_index": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _i64, _vp]),
     "cogdl_b200_narrow_i64_i32": (ctypes.c_int, [_vp, _vp, _i64, _vp]),

@@ -172,6 +172,17 @@ __device__ __forceinline__ void add_rn(float4 &acc, const float4 &x) {
   acc.z = __fadd_rn(acc.z, x.z);
   acc.w = __fadd_rn(acc.w, x.w);
 }
+// elementwise a * b and a - b, correctly rounded (the composition operators of the CompGCN aggregation)
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float2 mul_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float4 mul_rn(float4 a, float4 b) {
+  return make_float4(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y), __fmul_rn(a.z, b.z), __fmul_rn(a.w, b.w));
+}
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ float2 sub_rn(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ float4 sub_rn(float4 a, float4 b) {
+  return make_float4(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z), __fsub_rn(a.w, b.w));
+}
 template <typename VecT> __device__ __forceinline__ VecT vzero();
 template <> __device__ __forceinline__ float4 vzero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 template <> __device__ __forceinline__ float2 vzero<float2>() { return make_float2(0.f, 0.f); }

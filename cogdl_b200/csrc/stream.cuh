@@ -1,4 +1,5 @@
-// stream.cuh -- the row-stream gather kernel shared by the SpMM and the multi-head SpMM (sm_90a).
+// stream.cuh -- the row-stream gather kernel shared by the SpMM, the multi-head SpMM and the CompGCN composition
+// aggregation (sm_90a).
 //
 // Work items, in grid order:
 //   [0, n_chunks)                 hub chunks: <= chunk_edges edges of ONE hub row -> partial sum in
@@ -43,9 +44,16 @@ struct StreamParams {
   int FVL;            // MODE 2: VecT units per head
   int S;              // MODE 2: 512-byte slices per row; panel mode: column panels of 32 VecT (1 otherwise)
   HubView hub;
+  // composition modes (comp_aggr.cu): edge q also reads B[idx2[q]] ([*, ldv], like X0) and accumulates
+  // val[q] * (X0[colind[q]] o B[idx2[q]]) with o = * (MODE_COMP_MULT) or - (MODE_COMP_SUB)
+  const int *idx2;
+  const float *B;
 };
 
-enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2 };
+enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2, MODE_COMP_MULT = 3, MODE_COMP_SUB = 4 };
+template <int MODE> constexpr bool is_comp_mode() { return MODE == MODE_COMP_MULT || MODE == MODE_COMP_SUB; }
+// the shared-memory slab loop (stream_range_lean) serves the one-vector plain SpMM only
+template <int MODE, int NV> constexpr bool is_lean() { return NV == 1 && (MODE == MODE_UNWEIGHTED || MODE == MODE_WEIGHTED); }
 // Threads per block of every row-stream launch.  Measured on an H100 SXM (700 W), 128 vs 256, two alternating runs
 // each: SpMM F=40 87 vs 90 us, arxiv / products F=128, mh-SpMM and the papers shard within 1 %; all outputs
 // bit-identical.
@@ -64,8 +72,10 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
   const VecT *X0 = reinterpret_cast<const VecT *>(p.X0) + cv;
   const VecT *X1 = reinterpret_cast<const VecT *>(p.X1) + cv;
   VecT *Y = reinterpret_cast<VecT *>(p.Y) + cv;
+  constexpr bool COMP = is_comp_mode<MODE>();
+  const VecT *B = COMP ? reinterpret_cast<const VecT *>(p.B) + cv : nullptr;
 
-  // slab registers: column, value / attention row, owning row, owning row of the next edge
+  // slab registers: column, value / attention row / second index, owning row, owning row of the next edge
   int c = 0, rid = -1, rnx = -1, pe = 0;
   float v = 0.f;
   auto load_slab = [&](int base, int &c_, float &v_, int &pe_, int &rid_, int &rnx_) {
@@ -73,8 +83,9 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
     c_ = 0; v_ = 0.f; pe_ = 0; rid_ = -1; rnx_ = -1;
     if (q < e_end) {
       c_ = ld_stream(p.colind + q);
-      if (MODE == MODE_WEIGHTED) v_ = ld_stream(p.val + q);
+      if (MODE == MODE_WEIGHTED || COMP) v_ = ld_stream(p.val + q);
       if (MODE == MODE_MULTIHEAD) pe_ = HAS_PERM ? ld_stream(p.perm + q) : q;
+      if (COMP) pe_ = ld_stream(p.idx2 + q);
       if (ROWS) {
         rid_ = ld_stream(p.hub.edge_row + q);
         if (q + 1 < e_end) rnx_ = __ldg(p.hub.edge_row + q + 1);
@@ -95,11 +106,12 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
       const bool full = (j + U <= cnt);
       const unsigned em = endmask >> j;
       VecT x[U][NV];
+      VecT b[COMP ? U : 1][COMP ? NV : 1];
       float a[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const int cj = __shfl_sync(FULL, c, j + u);
-        const int pj = (MODE == MODE_MULTIHEAD) ? __shfl_sync(FULL, pe, j + u) : 0;
+        const int pj = (MODE == MODE_MULTIHEAD || COMP) ? __shfl_sync(FULL, pe, j + u) : 0;
         if (full || j + u < cnt) {
           const VecT *xp;
           if (SRC == SRC_ONE || cj < p.n0) {
@@ -115,11 +127,17 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
           for (int k = 0; k < NV; ++k)
             if (colok[k]) x[u][k] = ld_gather(xp + k * 32);
           if (MODE == MODE_MULTIHEAD && colok[0]) a[u] = __ldg(p.att + (int64_t)pj * p.H + head);
+          if constexpr (COMP) {
+            const VecT *bp = B + (int64_t)pj * p.ldv;
+#pragma unroll
+            for (int k = 0; k < NV; ++k)
+              if (colok[k]) b[u][k] = ld_gather(bp + k * 32);
+          }
         }
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
-        const float vj = (MODE == MODE_WEIGHTED) ? __shfl_sync(FULL, v, j + u) : 0.f;
+        const float vj = (MODE == MODE_WEIGHTED || COMP) ? __shfl_sync(FULL, v, j + u) : 0.f;
         const int rj = ROWS ? __shfl_sync(FULL, rid, j + u) : 0;
         if (full || j + u < cnt) {
 #pragma unroll
@@ -127,6 +145,8 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
             if (colok[k]) {
               if (MODE == MODE_UNWEIGHTED) add_rn(acc[k], x[u][k]);          // 1.0f * x == x exactly
               else if (MODE == MODE_WEIGHTED) axpy_rn(acc[k], vj, x[u][k]);
+              else if (MODE == MODE_COMP_MULT) axpy_rn(acc[k], vj, mul_rn(x[u][k], b[u][k]));
+              else if (MODE == MODE_COMP_SUB) axpy_rn(acc[k], vj, sub_rn(x[u][k], b[u][k]));
               else axpy_rn(acc[k], a[u], x[u][k]);
             }
           }
@@ -259,7 +279,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
   if (MODE == MODE_MULTIHEAD) { item = wid / p.S; slice = (int)(wid - item * p.S); }
   VecT *Y = reinterpret_cast<VecT *>(p.Y);
   VecT *P = reinterpret_cast<VecT *>(p.hub.partials);
-  constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD);
+  constexpr bool LEAN = is_lean<MODE, NV>();
 
   // column tiles: the multi-head and panel forms own exactly one 32-vector slice; the plain form loops over
   // the row in TILE-vector passes (one pass for F <= 128 * NV)
@@ -341,7 +361,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
 template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool PANEL = false>
 __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p) {
   const int lane = threadIdx.x & 31;
-  constexpr bool LEAN = (NV == 1 && MODE != MODE_MULTIHEAD);
+  constexpr bool LEAN = is_lean<MODE, NV>();
   __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
   __shared__ int s_r_all[LEAN ? 8 : 1][32];
   int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];

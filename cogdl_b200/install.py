@@ -19,7 +19,8 @@ With genconv=True, `cogdl.layers.deepergcn_layer.GENConv.forward` (DeeperGCN, Re
 genconv_forward below, which sends the aggregation to cogdl_b200.genconv_aggregate.  The original forward stays
 reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores it).  disengcn=True does the same for
 `cogdl.layers.disengcn_layer.DisenGCNLayer.forward` (DisenGCN), with disengcn_forward and cogdl_b200.disen_routing
-(uninstall_disengcn()).
+(uninstall_disengcn()).  compgcn=True rebinds `cogdl.models.nn.compgcn.CompGCNLayer.forward` (CompGCN) to
+compgcn_forward, which sends the message passing to cogdl_b200.compgcn_aggregate (uninstall_compgcn()).
 """
 import sys
 
@@ -106,7 +107,49 @@ def uninstall_disengcn():
     _restore_forward(dl.DisenGCNLayer)
 
 
-def install(rebind_dispatch=True, genconv=False, disengcn=False):
+def compgcn_forward(self, graph, x, rel_embed):
+    """CompGCNLayer.forward (cogdl/models/nn/compgcn.py:94-122) with the two per-edge message passings replaced by
+    one cogdl_b200.compgcn_aggregate and two N-row GEMMs (the message is linear in W).  The layer's own weights,
+    basis_weight, dropout (called in the reference's order: in, out, loop), BN, bias and activation are used, and
+    the graph is read as COO in the order given, never sorted.  CPU or non-fp32 input or weights, and an opn
+    other than sub / mult, run the original."""
+    import torch.nn.functional as F
+
+    from .operators.comp_aggr import COMPGCN_OPS, compgcn_aggregate
+
+    original = type(self)._cogdl_b200_original_forward
+    weights = (self.weight_in, self.weight_out, self.weight_rel, self.weight_loop, self.loop_rel)
+    if (not x.is_cuda or x.dtype != torch.float32 or self.opn not in COMPGCN_OPS
+            or any(w.dtype != torch.float32 for w in weights)
+            or (not self.use_bases and rel_embed.dtype != torch.float32)):
+        return original(self, graph, x, rel_embed)
+    if self.use_bases:
+        rel_embed = self.basis_weight()
+    rel_embed = torch.cat((rel_embed, self.loop_rel), dim=0)
+    agg_in, agg_out = compgcn_aggregate(graph.edge_index, graph.edge_attr, x, rel_embed, self.opn)
+    emb = F.dropout(agg_in @ self.weight_in, p=self.dropout, training=self.training)
+    rev_emb = F.dropout(agg_out @ self.weight_out, p=self.dropout, training=self.training)
+    loop_emb = F.dropout(self.rel_transform(x, self.loop_rel) @ self.weight_loop, p=self.dropout, training=self.training)
+    out = 1 / 3 * (emb + rev_emb + loop_emb)
+    if self.bias is not None:
+        out += self.bias
+    out = self.bn(out)
+    return self.activation(out), torch.matmul(rel_embed, self.weight_rel)[:-1]
+
+
+def install_compgcn():
+    import cogdl.models.nn.compgcn as cm
+
+    return _rebind_forward(cm.CompGCNLayer, compgcn_forward, "cogdl.models.nn.compgcn.CompGCNLayer.forward")
+
+
+def uninstall_compgcn():
+    import cogdl.models.nn.compgcn as cm
+
+    _restore_forward(cm.CompGCNLayer)
+
+
+def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -190,4 +233,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False):
         patched += install_genconv()
     if disengcn:
         patched += install_disengcn()
+    if compgcn:
+        patched += install_compgcn()
     return patched

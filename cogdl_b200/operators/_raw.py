@@ -339,3 +339,37 @@ def edge_colsum_raw(st_t: CSRStructure, perm, e):
                    _stream(dev))
         del keep
     return out
+
+
+def comp_aggr_raw(st: CSRStructure, idx2, w, a, b, op):
+    """CompGCN composition aggregation: y[i] = sum over row i's slots q of w[q] * phi(a[colind[q]], b[idx2[q]]), with
+    phi = a * b ("mult"), a - b ("sub") or a ("copy": idx2 and b unused).  a [*, F] and b [*, F] fp32; w [nnz] fp32;
+    idx2 [nnz] int32.  Returns y [st.n_rows, F]; rows without slots are zero."""
+    dev = require_cuda(a, b, w, idx2)
+    if op not in _cabi.COMP_OPS:
+        raise ValueError(f"unknown composition op {op!r} (one of {sorted(_cabi.COMP_OPS)})")
+    two = op != "copy"
+    a = _f32c(a, "a")
+    b = _f32c(b, "b") if two else None
+    if a.dim() != 2 or (two and (b.dim() != 2 or b.shape[1] != a.shape[1])):
+        raise ValueError(f"a and b must be [*, F] of one width, got {tuple(a.shape)} and "
+                         f"{None if b is None else tuple(b.shape)}")
+    F = a.shape[1]
+    if F <= 0:
+        raise ValueError("F must be positive")
+    w = _f32c(w, "w").view(-1)
+    if w.numel() != st.nnz or (two and idx2.numel() != st.nnz):
+        raise ValueError(f"per-slot arrays must have {st.nnz} entries")
+    if two and idx2.dtype != torch.int32:
+        raise TypeError(f"idx2 must be int32, got {idx2.dtype}")
+    with torch.cuda.device(dev):
+        if st.nnz == 0:
+            return torch.zeros((st.n_rows, F), dtype=torch.float32, device=dev)
+        y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+        need = int(_cabi.load().cogdl_b200_comp_aggr_scratch_bytes(st.plan.n_chunks, F))
+        plan, keep = st.plan_struct(need)
+        _cabi.call("cogdl_b200_comp_aggr_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(idx2.contiguous() if two else None),
+                   _ptr(w), _ptr(a), a.shape[0], _ptr(b), b.shape[0] if two else 0, _ptr(y), st.n_rows, F,
+                   _cabi.COMP_OPS[op], plan, _stream(dev))
+        del keep
+    return y

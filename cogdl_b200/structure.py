@@ -265,3 +265,100 @@ def structure_for(rowptr, colind, n_cols=None):
 
 def clear_structure_cache():
     _CACHE.clear()
+    _COMP_CACHE.clear()
+
+
+class CompStructure:
+    """CompGCN's typed COO (cogdl/models/nn/compgcn.py:94-151) in the form the composition aggregation reads.
+
+    The COO is taken in the order given and never reordered in place: edges [0, E // 2) are the "in" half and
+    [E // 2, E) the "out" half.  Owns
+      * `csr`: the two halves stacked into one CSR of 2N rows (rows [0, N) "in", [N, 2N) "out"), built with the
+        stable device COO -> CSR, so each row keeps its edges in COO order, with per-slot `type` and weight
+        `w` = 1 / deg_h(row) (CompGCN's per-half row normalisation);
+      * `transpose()`: the N x 2N transpose with the permuted type and weight (for dx), built on first use;
+      * `by_type(T)`: the CSR with edge types as rows, per slot the stacked row, the column and the weight (for
+        dR'), built on first use.
+    Index bounds are checked once here (one host sync) and raise ValueError, as the reference's indexing raises
+    IndexError; `max_type` lets every call check its relation table's size on the host."""
+
+    def __init__(self, row, col, etype, num_nodes, chunk_edges=DEFAULT_CHUNK_EDGES):
+        from .data import coo2csr_index
+
+        dev = require_cuda(row, col)
+        etype = etype.reshape(-1)
+        E, N = row.numel(), int(num_nodes)
+        if col.numel() != E or etype.numel() != E:
+            raise ValueError(f"edge_index has {E} / {col.numel()} entries and the edge types {etype.numel()}")
+        if 2 * N >= 2**31 or E >= 2**31:
+            raise ValueError("graph too large for int32 indices on one device")
+        row, col = row.to(dev, torch.int64).contiguous(), col.to(dev, torch.int64).contiguous()
+        etype = etype.to(dev, torch.int64).contiguous()   # edge types may come from the host: one copy per build
+        self.device, self.n_nodes, self.nnz, self.chunk_edges = dev, N, E, int(chunk_edges)
+        self.max_type = -1
+        if E > 0:
+            lo_i, lo_t, hi_i, hi_t = (int(v) for v in torch.stack([
+                torch.minimum(row.min(), col.min()), etype.min(), torch.maximum(row.max(), col.max()), etype.max()
+            ]).tolist())                                  # one sync per structure
+            if lo_i < 0 or hi_i >= N:
+                raise ValueError(f"edge index {lo_i if lo_i < 0 else hi_i} is out of range for {N} nodes")
+            if lo_t < 0:
+                raise ValueError(f"edge type {lo_t} is negative")
+            self.max_type = hi_t
+        srow = row + N * (torch.arange(E, device=dev) >= E // 2)   # stacked row: the "out" half is rows [N, 2N)
+        rowptr, reindex = coo2csr_index(srow, 2 * N)
+        self.srow = srow[reindex].int()
+        self.type = etype[reindex].int()
+        deg = rowptr[1:] - rowptr[:-1]
+        self.w = torch.repeat_interleave(1.0 / deg.float(), deg, output_size=E)
+        self.csr = CSRStructure(rowptr.int(), col[reindex].int(), n_cols=N, chunk_edges=self.chunk_edges)
+        self._transpose = None
+        self._by_type = {}
+
+    def transpose(self):
+        """(CSRStructure of the N x 2N transpose, type, w) with type / w in the transpose's slot order."""
+        if self._transpose is None:
+            t, perm = self.csr.csc()
+            p = perm.long()
+            self._transpose = (t, self.type[p], self.w[p])
+        return self._transpose
+
+    def by_type(self, T):
+        """(CSRStructure with T type rows whose colind is the stacked row, col, w) in type-then-COO slot order."""
+        from .data import coo2csr_index
+
+        ent = self._by_type.get(T)
+        if ent is None:
+            if self.max_type >= T:
+                raise ValueError(f"edge type {self.max_type} is out of range for {T} relation rows")
+            rowptr, reindex = coo2csr_index(self.type.long(), T)
+            st = CSRStructure(rowptr.int(), self.srow[reindex], n_cols=2 * self.n_nodes, chunk_edges=self.chunk_edges)
+            ent = self._by_type[T] = (st, self.csr.colind[reindex], self.w[reindex])
+        return ent
+
+
+# CompStructure cache: keyed on the storage identity, size and version of the (row, col, type) tensors, the node
+# count and the chunk size, like structure_for.  Both layers of a model, and repeated predict() calls on one graph,
+# share one entry; the entry keeps its key tensors alive so their addresses cannot be reused under it.
+_COMP_CACHE = OrderedDict()
+_COMP_CACHE_CAP = 4
+comp_cache_stats = {"hit": 0, "miss": 0}
+
+
+def comp_structure_for(row, col, etype, num_nodes, chunk_edges=DEFAULT_CHUNK_EDGES):
+    keys = (row, col, etype)
+    key = tuple((t.data_ptr(), t.numel(), str(t.device), t.dtype) for t in keys) + (int(num_nodes), int(chunk_edges))
+    ent = _COMP_CACHE.get(key)
+    if ent is not None:
+        cs, kept, ver = ent
+        if ver == tuple(t._version for t in kept):
+            _COMP_CACHE.move_to_end(key)
+            comp_cache_stats["hit"] += 1
+            return cs
+        del _COMP_CACHE[key]
+    comp_cache_stats["miss"] += 1
+    cs = CompStructure(row, col, etype, num_nodes, chunk_edges)
+    _COMP_CACHE[key] = (cs, keys, tuple(t._version for t in keys))
+    while len(_COMP_CACHE) > _COMP_CACHE_CAP:
+        _COMP_CACHE.popitem(last=False)
+    return cs

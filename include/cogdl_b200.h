@@ -404,6 +404,27 @@ COGDL_B200_API int cogdl_b200_disen_route_bwd_f32(const int32_t *rowptr, const i
                                    const float *r, float *g_u, float *D, float *dq, float *dc, int64_t n_rows,
                                    int64_t n_cols, int64_t F, int64_t K, float tau, cogdl_b200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * CompGCN composition aggregation (cogdl/models/nn/compgcn.py:124-140) without per-edge feature tensors.
+ * Per row i of the CSR (rowptr, colind) with per-slot second index idx2 and weight w:
+ *   Y[i,:] = sum_{q in row i} w[q] * phi(A[colind[q],:], B[idx2[q],:])
+ *   op COGDL_B200_COMP_MULT: phi = a * b;  COGDL_B200_COMP_SUB: phi = a - b;  COGDL_B200_COMP_COPY: phi = a (idx2
+ *   and B unused, may be NULL).
+ * A is [a_rows, F], B [b_rows, F], Y [n_rows, F], all fp32 row-major; colind < a_rows and idx2 < b_rows are the
+ * caller's to guarantee.  Degree-0 rows give zeros.  Needs a hub plan (chunk_edges > 0) with row-stream
+ * segments; plan->partials needs cogdl_b200_comp_aggr_scratch_bytes(n_chunks, F) bytes.  Hub rows are merged in
+ * chunk order (no float atomics: bit-reproducible).  16-byte vectors when F % 4 == 0 and A, B, Y and the partials
+ * are 16-byte aligned.  Rejects an unknown op, F <= 0 and a plan whose row counts do not match n_rows.
+ * ------------------------------------------------------------------------------------- */
+#define COGDL_B200_COMP_MULT 0
+#define COGDL_B200_COMP_SUB 1
+#define COGDL_B200_COMP_COPY 2
+COGDL_B200_API int64_t cogdl_b200_comp_aggr_scratch_bytes(int64_t n_chunks, int64_t F);
+COGDL_B200_API int cogdl_b200_comp_aggr_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *idx2,
+                                            const float *w, const float *A, int64_t a_rows, const float *B,
+                                            int64_t b_rows, float *Y, int64_t n_rows, int64_t F, int32_t op,
+                                            const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
 /* Device COO -> CSR (stable): row_ptr[num_nodes+1] and reindex[nnz] (CSR slot -> COO position),
  * int64 as cogdl.data.Graph stores them.
  * Replaces  sampler.coo2csr_cpu_index(row, col, num_nodes)   cogdl/operators/sample/sample.cpp:234-270
