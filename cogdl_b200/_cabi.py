@@ -91,6 +91,13 @@ SIGNATURES = {
     "cogdl_b200_comp_aggr_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_comp_aggr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _plan_p,
                                                 _vp]),
+    "cogdl_b200_spgemm_scratch_bytes": (_i64, [_i64, _i64, _i64]),
+    "cogdl_b200_spgemm_count": (ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, ctypes.POINTER(_i64), _vp,
+                                               _i64, _vp]),
+    "cogdl_b200_spgemm_fill_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp,
+                                                  _i64, _vp]),
+    "cogdl_b200_spgemm_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp,
+                                                 _vp, _vp, _vp, _vp, _vp]),
     "cogdl_b200_coo2csr_workspace_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_coo2csr_index": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _i64, _vp]),
     "cogdl_b200_narrow_i64_i32": (ctypes.c_int, [_vp, _vp, _i64, _vp]),

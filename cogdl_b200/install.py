@@ -21,6 +21,8 @@ reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores 
 `cogdl.layers.disengcn_layer.DisenGCNLayer.forward` (DisenGCN), with disengcn_forward and cogdl_b200.disen_routing
 (uninstall_disengcn()).  compgcn=True rebinds `cogdl.models.nn.compgcn.CompGCNLayer.forward` (CompGCN) to
 compgcn_forward, which sends the message passing to cogdl_b200.compgcn_aggregate (uninstall_compgcn()).
+spspmm=True provides torch_sparse's spspmm / spmm (cogdl_b200.spspmm / coo_spmm) to GTN, SRGCN and Graph U-Net, through a
+`torch_sparse` stand-in module when the real package is missing (install_spspmm, uninstall_spspmm()).
 """
 import sys
 
@@ -149,7 +151,56 @@ def uninstall_compgcn():
     _restore_forward(cm.CompGCNLayer)
 
 
-def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False):
+_SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
+_spspmm_state = {"stub": None, "rebound": []}
+
+
+def install_spspmm():
+    """torch_sparse's spspmm / spmm for GTN, SRGCN and Graph U-Net.  Without a loadable torch_sparse, a module of that
+    name providing exactly those two functions goes into sys.modules, so the models import; an importable torch_sparse
+    is left alone.  Either way the two names are rebound in those of the four model modules already imported."""
+    import types
+
+    from .operators.spspmm import coo_spmm, spspmm
+
+    patched = []
+    if _spspmm_state["stub"] is None and "torch_sparse" not in sys.modules:
+        try:
+            import torch_sparse  # noqa: F401
+        except (ImportError, OSError):   # missing, or a binary build that does not load (undefined symbol)
+            stub = types.ModuleType("torch_sparse")
+            stub.__doc__ = "spspmm and spmm of cogdl_b200, seeded by cogdl_b200.install(spspmm=True)"
+            stub.spspmm, stub.spmm = spspmm, coo_spmm
+            sys.modules["torch_sparse"] = _spspmm_state["stub"] = stub
+            patched.append("torch_sparse")
+    for mname in _SPSPMM_MODULES:
+        mod = sys.modules.get(mname)
+        if mod is None:
+            continue
+        for attr, new in (("spspmm", spspmm), ("spmm", coo_spmm)):
+            if attr == "spmm" and mname != "cogdl.utils.srgcn_utils":
+                continue   # srgcn.py's `spmm` is cogdl.utils.spmm (the graph SpMM), not torch_sparse's
+            old = getattr(mod, attr, None)
+            if old is not None and old is not new:
+                _spspmm_state["rebound"].append((mod, attr, old))
+                setattr(mod, attr, new)
+                patched.append(f"{mname}.{attr}")
+    return patched
+
+
+def uninstall_spspmm():
+    """Undo install_spspmm: restore the rebound names and take the torch_sparse stand-in out of sys.modules (models
+    imported while it was there keep their binding)."""
+    for mod, attr, old in reversed(_spspmm_state["rebound"]):
+        setattr(mod, attr, old)
+    _spspmm_state["rebound"] = []
+    stub = _spspmm_state["stub"]
+    if stub is not None and sys.modules.get("torch_sparse") is stub:
+        del sys.modules["torch_sparse"]
+    _spspmm_state["stub"] = None
+
+
+def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -235,4 +286,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False):
         patched += install_disengcn()
     if compgcn:
         patched += install_compgcn()
+    if spspmm:
+        patched += install_spspmm()
     return patched

@@ -266,6 +266,7 @@ def structure_for(rowptr, colind, n_cols=None):
 def clear_structure_cache():
     _CACHE.clear()
     _COMP_CACHE.clear()
+    _COO_CACHE.clear()
 
 
 class CompStructure:
@@ -361,4 +362,122 @@ def comp_structure_for(row, col, etype, num_nodes, chunk_edges=DEFAULT_CHUNK_EDG
     _COMP_CACHE[key] = (cs, keys, tuple(t._version for t in keys))
     while len(_COMP_CACHE) > _COMP_CACHE_CAP:
         _COMP_CACHE.popitem(last=False)
+    return cs
+
+
+def _coo_bounds(row, col, n_rows, n_cols):
+    """Raise ValueError unless every row index is in [0, n_rows) and every column in [0, n_cols) (one host sync)."""
+    if row.numel() == 0:
+        return
+    lo_r, lo_c, hi_r, hi_c = (int(v) for v in torch.stack([row.min(), col.min(), row.max(), col.max()]).tolist())
+    if lo_r < 0 or hi_r >= n_rows:
+        raise ValueError(f"row index {lo_r if lo_r < 0 else hi_r} is out of range for {n_rows} rows")
+    if lo_c < 0 or hi_c >= n_cols:
+        raise ValueError(f"column index {lo_c if lo_c < 0 else hi_c} is out of range for {n_cols} columns")
+
+
+class CooStructure:
+    """A COO index [2, E] (torch_sparse's `index` argument) in the forms the sparse products read.
+
+    * `csr`: the (row, col)-sorted, duplicate-merged CSR (ascending unique columns per row) that the sparse x sparse
+      product needs, built with two stable device sorts (by column, then by row), so entries of one (row, col) keep
+      their input order; `slot[e]` is the CSR slot input entry e was merged into.  `merge(value)` sums the values of
+      each slot in input order (deterministic) and `spread(g)` hands every input entry its slot's gradient.
+    * `coo_csr()`: the stable COO -> CSR with duplicates kept (row order, then input order) and `reindex`, for the
+      sparse x dense product; built on first use.
+    Index bounds are checked once here and raise ValueError."""
+
+    def __init__(self, index, n_rows, n_cols):
+        from .data import coo2csr_index
+
+        require_cuda(index)
+        if index.dim() != 2 or index.shape[0] != 2:
+            raise ValueError(f"index must be [2, E], got {tuple(index.shape)}")
+        n_rows, n_cols = int(n_rows), int(n_cols)
+        E = index.shape[1]
+        if n_rows < 0 or n_cols < 0:
+            raise ValueError(f"negative size {n_rows} x {n_cols}")
+        if n_rows >= 2**31 or n_cols >= 2**31 or E >= 2**31:
+            raise ValueError("sparse matrix too large for int32 indices on one device")
+        dev = index.device
+        row, col = index[0].to(torch.int64).contiguous(), index[1].to(torch.int64).contiguous()
+        _coo_bounds(row, col, n_rows, n_cols)
+        self.device, self.n_rows, self.n_cols, self.nnz_in = dev, n_rows, n_cols, E
+        self._row, self._col = row, col
+        self._coo_csr = None
+        by_col = coo2csr_index(col, n_cols)[1]
+        rowptr_all, by_row = coo2csr_index(row[by_col], n_rows)
+        order = by_col[by_row]                        # input positions in (row, col, input) order
+        srow, scol = row[order], col[order]
+        new = torch.ones(E, dtype=torch.bool, device=dev)
+        if E > 1:
+            new[1:] = (srow[1:] != srow[:-1]) | (scol[1:] != scol[:-1])
+        sorted_slot = torch.cumsum(new, 0) - 1
+        self.nnz = int(sorted_slot[-1]) + 1 if E > 0 else 0       # one host read per structure
+        self.slot = torch.empty(E, dtype=torch.int64, device=dev)
+        self.slot[order] = sorted_slot
+        urow = srow[new]
+        rowptr = torch.searchsorted(urow, torch.arange(n_rows + 1, device=dev))
+        self.csr = CSRStructure(rowptr.to(torch.int32), scol[new].to(torch.int32), n_cols=n_cols)
+        # merge plan: the r-th entry (in input order) of every slot, for r = 0 .. max multiplicity - 1
+        self._groups = []
+        if self.nnz < E:
+            first = torch.nonzero(new).view(-1)
+            rank = torch.arange(E, device=dev) - first[sorted_slot]
+            for r in range(int(rank.max()) + 1):
+                sel = torch.nonzero(rank == r).view(-1)
+                self._groups.append((order[sel], sorted_slot[sel]))
+        else:
+            self._order = order
+
+    def merge(self, value):
+        """[nnz] fp32 CSR values: the input values of each slot summed in input order."""
+        value = value.reshape(-1)
+        if not self._groups:
+            return value[self._order].float().contiguous()
+        out = torch.empty(self.nnz, dtype=torch.float32, device=value.device)
+        src, dst = self._groups[0]
+        out[dst] = value[src].float()
+        for src, dst in self._groups[1:]:
+            out[dst] = out[dst] + value[src].float()
+        return out
+
+    def spread(self, g):
+        """Gradient of the input values from the gradient `g` [nnz] of the merged CSR values."""
+        return g[self.slot]
+
+    def coo_csr(self):
+        """(CSRStructure with duplicates kept, reindex [E] int64: CSR slot -> input position)."""
+        if self._coo_csr is None:
+            from .data import coo2csr_index
+
+            rowptr, reindex = coo2csr_index(self._row, self.n_rows)
+            st = CSRStructure(rowptr.to(torch.int32), self._col[reindex].to(torch.int32), n_cols=self.n_cols)
+            self._coo_csr = (st, reindex)
+        return self._coo_csr
+
+
+# CooStructure cache, keyed like _COMP_CACHE on the storage, size and version of the index tensor and the matrix shape:
+# SRGCN reuses one index across its heads and calls the products on it several times per forward.
+_COO_CACHE = OrderedDict()
+_COO_CACHE_CAP = 8
+coo_cache_stats = {"hit": 0, "miss": 0}
+
+
+def coo_structure_for(index, n_rows, n_cols):
+    key = (index.data_ptr(), tuple(index.shape), tuple(index.stride()), str(index.device), index.dtype, int(n_rows),
+           int(n_cols))
+    ent = _COO_CACHE.get(key)
+    if ent is not None:
+        cs, kept, ver = ent
+        if ver == kept._version:
+            _COO_CACHE.move_to_end(key)
+            coo_cache_stats["hit"] += 1
+            return cs
+        del _COO_CACHE[key]
+    coo_cache_stats["miss"] += 1
+    cs = CooStructure(index, n_rows, n_cols)
+    _COO_CACHE[key] = (cs, index, index._version)
+    while len(_COO_CACHE) > _COO_CACHE_CAP:
+        _COO_CACHE.popitem(last=False)
     return cs

@@ -425,6 +425,45 @@ COGDL_B200_API int cogdl_b200_comp_aggr_f32(const int32_t *rowptr, const int32_t
                                             int64_t b_rows, float *Y, int64_t n_rows, int64_t F, int32_t op,
                                             const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Sparse x sparse product C = A.B, A [a_rows x a_cols] and B [b_rows x b_cols] int32 CSR with fp32 values, columns
+ * ascending and unique inside every row (b_rows must equal a_cols).  C comes out as CSR with ascending, unique columns.
+ * Replaces  torch_sparse.spspmm(indexA, valueA, indexB, valueB, m, k, n)   (cuSPARSE SpGEMM), imported at module level
+ *           by cogdl/models/nn/gtn.py:7 (GTLayer.forward :82), cogdl/models/nn/srgcn.py:6 (nhop powers :79,153),
+ *           cogdl/utils/srgcn_utils.py:7 (NodeAttention :36, PPR :133) and cogdl/models/nn/graph_unet.py:9 (:38).
+ * The pattern is structural: (i, j) is in C when some product a_ik b_kj exists, even if the values sum to 0.
+ * Every value is acc = fmaf(a_ik, b_kj, acc) from 0, in (A's CSR order, B's CSR order), without float atomics: rows
+ * are never split, so C is bit-identical to that sequential loop and reproducible run to run.
+ *   1. ..._count  : rowptrC[a_rows+1] and *nnz_c (host) = nnz(C).  Totals are int64; nnz(C) > INT32_MAX returns
+ *                   EINVAL with nothing written to rowptrC.  Reads the total on the host (synchronises the stream).
+ *   2. ..._fill   : colC / valC [nnz(C)], caller-allocated from step 1.
+ * `scratch`: device memory of at least cogdl_b200_spgemm_scratch_bytes(a_rows, a_cols, b_cols) bytes, for both steps
+ * (about 28 bytes per row of A plus 33 bytes per column of B; the per-column part, a bitmap and its prefix sums for each
+ * of 132 concurrent rows, is written only when a row has more than 4096 possible columns).
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_spgemm_scratch_bytes(int64_t a_rows, int64_t a_cols, int64_t b_cols);
+COGDL_B200_API int cogdl_b200_spgemm_count(const int32_t *rowptrA, const int32_t *colA, int64_t a_rows, int64_t a_cols,
+                                           const int32_t *rowptrB, const int32_t *colB, int64_t b_rows, int64_t b_cols,
+                                           int32_t *rowptrC, int64_t *nnz_c, void *scratch, int64_t scratch_bytes,
+                                           cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_spgemm_fill_f32(const int32_t *rowptrA, const int32_t *colA, const float *valA,
+                                              int64_t a_rows, int64_t a_cols, const int32_t *rowptrB, const int32_t *colB,
+                                              const float *valB, int64_t b_rows, int64_t b_cols, const int32_t *rowptrC,
+                                              int32_t *colC, float *valC, void *scratch, int64_t scratch_bytes,
+                                              cogdl_b200_stream_t stream);
+/* Value gradients of C = A.B given dC [nnz(C)] (the backward of torch_sparse.spspmm's values; GTN's GTConv weights
+ * train only through them):
+ *   dA[p=(i,k)] = sum_{q in B_k} b_q dC[i, col_B(q)]                      (dA [nnz(A)], NULL = not wanted)
+ *   dB[q=(k,j)] = sum_{p in column k of A} a_p dC[row(p), j]              (dB [nnz(B)], NULL = not wanted)
+ * dB walks A's transpose: colptrAT / rowindAT / permAT of cogdl_b200_csr2csc (needed only with dB).  Each output is
+ * written once by one warp (fixed-order lane sums): deterministic. */
+COGDL_B200_API int cogdl_b200_spgemm_bwd_f32(const int32_t *rowptrA, const int32_t *colA, const float *valA,
+                                             int64_t a_rows, int64_t a_cols, const int32_t *rowptrB, const int32_t *colB,
+                                             const float *valB, int64_t b_rows, int64_t b_cols, const int32_t *rowptrC,
+                                             const int32_t *colC, const float *dC, const int32_t *colptrAT,
+                                             const int32_t *rowindAT, const int32_t *permAT, float *dA, float *dB,
+                                             cogdl_b200_stream_t stream);
+
 /* Device COO -> CSR (stable): row_ptr[num_nodes+1] and reindex[nnz] (CSR slot -> COO position),
  * int64 as cogdl.data.Graph stores them.
  * Replaces  sampler.coo2csr_cpu_index(row, col, num_nodes)   cogdl/operators/sample/sample.cpp:234-270
