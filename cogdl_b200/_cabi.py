@@ -75,6 +75,11 @@ SIGNATURES = {
     "cogdl_b200_scatter_max_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_scatter_max_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "cogdl_b200_gat_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_gat_fwd_dropout_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, ctypes.c_uint64, ctypes.c_uint64, _f32,
+                                                      _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_mhspmm_dropout_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _i64, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_gat_attn_bwd_dropout_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _i64, _i64,
+                                                           _plan_p, _vp]),
     "cogdl_b200_gcn_fused_supported": (ctypes.c_int, [_i64, _i64]),
     "cogdl_b200_gcn_fused_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _plan_p, _vp]),
     "cogdl_b200_sage_fused_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32,

@@ -183,6 +183,12 @@ __device__ __forceinline__ float2 sub_rn(float2 a, float2 b) { return make_float
 __device__ __forceinline__ float4 sub_rn(float4 a, float4 b) {
   return make_float4(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z), __fsub_rn(a.w, b.w));
 }
+// Attention that carries a dropout mask in its sign bit (GAT attention dropout, edge_softmax.cu MODE 2): a dropped
+// entry reads as 0, a kept one as a * scale.  The BIT is tested, not a < 0: a dropped softmax that underflowed to 0
+// is stored as -0.0.
+__device__ __forceinline__ float drop_att(float a, float scale) {
+  return (__float_as_uint(a) >> 31) ? 0.f : __fmul_rn(a, scale);
+}
 template <typename VecT> __device__ __forceinline__ VecT vzero();
 template <> __device__ __forceinline__ float4 vzero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 template <> __device__ __forceinline__ float2 vzero<float2>() { return make_float2(0.f, 0.f); }

@@ -38,7 +38,14 @@
 //   MODE 2: attention, a = h_l [N,H], b = h_r [N,H]: logit = leakyrelu(a[row,h] + b[col,h])
 //   MODE 3: attention backward: y = att, g = d att (from mhsddmm), plus h_l / h_r / colind / slope:
 //           out = d logit * leakyrelu'(h_l[row]+h_r[col]) written to [nnz,H], and grow[row,h] = its row sum
+// DROP (template flag of MODES 2 and 3, attention dropout): (edge p, head h) is dropped iff draw(seed, p, h) <
+// drop_below (rng.cuh; p = CSR position, so the CSC backward finds the same mask through perm).  MODE 2 writes a
+// dropped attention as -a: the softmax is >= 0, so its sign bit is free to carry the mask, and the hash runs once per
+// (edge, head) here instead of in the gather loops.  MODE 3 reads y = |att| and g = (sign bit ? 0 : d att * scale),
+// the gradient of the softmax before the dropout.  The bit is tested, never `att < 0`: a dropped softmax that
+// underflowed to 0 is -0.0.
 #include "common.cuh"
+#include "rng.cuh"
 
 #include <math_constants.h>
 
@@ -63,7 +70,25 @@ struct EsParams {
   float2 *stats;          // per chunk slot x head: (max, sum) -- the row's merged value sits in its first slot
   float *part;            // MODE 3: per chunk slot x head partial row sums
   bool bulk;              // tiles may be moved with cp.async.bulk (alignment checked on the host)
+  uint64_t seed;          // DROP: attention-dropout mask (see the header comment)
+  uint64_t drop_below;
+  float scale;            // DROP, MODE 3: 1 / (1 - p_drop), the factor a kept attention was multiplied by
 };
+
+// DROP, MODE 2: the attention a (>= 0) of CSR edge `edge`, head `head`, with the sign bit set if the pair is dropped
+template <bool DROP>
+__device__ __forceinline__ float es_mark(const EsParams &p, int64_t edge, int head, float a) {
+  if (DROP && draw(p.seed, edge, head) < p.drop_below) a = __uint_as_float(__float_as_uint(a) | 0x80000000u);
+  return a;
+}
+// DROP, MODE 3: (y, g) = (saved attention, d attention after dropout) -> (softmax, d softmax)
+template <bool DROP>
+__device__ __forceinline__ void es_unmark(const EsParams &p, float &y, float &g) {
+  if (DROP) {
+    g = (__float_as_uint(y) >> 31) ? 0.f : __fmul_rn(g, p.scale);
+    y = fabsf(y);
+  }
+}
 
 // exp for the plan-based kernels: arguments are x - max <= 0.  ex2.approx(x * log2 e): 2 ulp from the MUFU plus
 // |x| * 2^-24 from the scaling product, i.e. <= ~2e-6 relative for logits within 30 of the row maximum and an
@@ -100,20 +125,30 @@ __device__ __forceinline__ float es_dact(const EsParams &p, int lb, int64_t t, i
 
 // One row handled by a team of NT threads striding the row's elements (tid = index inside the
 // team, NT % H == 0).  reduce(v, is_max) must return the team-wide per-head reduction.
-template <int MODE, int NT, typename Reduce>
+template <int MODE, int NT, bool DROP, typename Reduce>
 __device__ __forceinline__ void es_row(const EsParams &p, int64_t row, int lb, int64_t n, int tid, Reduce reduce) {
   const int head = tid & (p.H - 1);
   float *o = p.out + (int64_t)lb * p.H;
   if (MODE == 1 || MODE == 3) {
     const float *y = p.a + (int64_t)lb * p.H, *g = p.b + (int64_t)lb * p.H;
+    auto yg = [&](int64_t t) {
+      float yv = __ldg(y + t), gv = __ldg(g + t);
+      es_unmark<DROP>(p, yv, gv);
+      return make_float2(yv, gv);
+    };
     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
     int64_t t = tid;
     for (; t + 3 * NT < n; t += 4 * NT) {
-      s0 = fmaf(__ldg(y + t), __ldg(g + t), s0); s1 = fmaf(__ldg(y + t + NT), __ldg(g + t + NT), s1);
-      s2 = fmaf(__ldg(y + t + 2 * NT), __ldg(g + t + 2 * NT), s2);
-      s3 = fmaf(__ldg(y + t + 3 * NT), __ldg(g + t + 3 * NT), s3);
+      float2 v = yg(t);
+      s0 = fmaf(v.x, v.y, s0);
+      v = yg(t + NT);
+      s1 = fmaf(v.x, v.y, s1);
+      v = yg(t + 2 * NT);
+      s2 = fmaf(v.x, v.y, s2);
+      v = yg(t + 3 * NT);
+      s3 = fmaf(v.x, v.y, s3);
     }
-    for (; t < n; t += NT) s0 = fmaf(__ldg(y + t), __ldg(g + t), s0);
+    for (; t < n; t += NT) { const float2 v = yg(t); s0 = fmaf(v.x, v.y, s0); }
     const float s = reduce((s0 + s1) + (s2 + s3), false);
     t = tid;
     if (MODE == 1) {
@@ -123,7 +158,8 @@ __device__ __forceinline__ void es_row(const EsParams &p, int64_t row, int lb, i
       const float hlrow = __ldg(p.hl + row * p.H + head);
       float acc = 0.f;
       for (; t < n; t += NT) {
-        const float v = __ldg(y + t) * (__ldg(g + t) - s) * es_dact(p, lb, t, head, hlrow);
+        const float2 w = yg(t);
+        const float v = w.x * (w.y - s) * es_dact(p, lb, t, head, hlrow);
         st_stream(o + t, v);
         acc += v;
       }
@@ -155,14 +191,18 @@ __device__ __forceinline__ void es_row(const EsParams &p, int64_t row, int lb, i
   for (; t + 3 * NT < n; t += 4 * NT) {
     const float x0 = es_in<MODE>(p, lb, t, head, hl), x1 = es_in<MODE>(p, lb, t + NT, head, hl);
     const float x2 = es_in<MODE>(p, lb, t + 2 * NT, head, hl), x3 = es_in<MODE>(p, lb, t + 3 * NT, head, hl);
-    st_stream(o + t, expf(x0 - m) / s); st_stream(o + t + NT, expf(x1 - m) / s);
-    st_stream(o + t + 2 * NT, expf(x2 - m) / s); st_stream(o + t + 3 * NT, expf(x3 - m) / s);
+    const int64_t e = lb + (t >> p.lgH), de = NT >> p.lgH;     // CSR edge of element t (DROP)
+    st_stream(o + t, es_mark<DROP>(p, e, head, expf(x0 - m) / s));
+    st_stream(o + t + NT, es_mark<DROP>(p, e + de, head, expf(x1 - m) / s));
+    st_stream(o + t + 2 * NT, es_mark<DROP>(p, e + 2 * de, head, expf(x2 - m) / s));
+    st_stream(o + t + 3 * NT, es_mark<DROP>(p, e + 3 * de, head, expf(x3 - m) / s));
   }
-  for (; t < n; t += NT) st_stream(o + t, expf(es_in<MODE>(p, lb, t, head, hl) - m) / s);
+  for (; t < n; t += NT)
+    st_stream(o + t, es_mark<DROP>(p, lb + (t >> p.lgH), head, expf(es_in<MODE>(p, lb, t, head, hl) - m) / s));
 }
 
 // ---------------------------------------------------------------- warp per row (no plan)
-template <int MODE>
+template <int MODE, bool DROP>
 __global__ void __launch_bounds__(256) es_warp_kernel(const EsParams p) {
   const int lane = threadIdx.x & 31;
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -174,13 +214,13 @@ __global__ void __launch_bounds__(256) es_warp_kernel(const EsParams p) {
     if (MODE == 3 && lane < H) p.grow[row * H + lane] = 0.f;
     return;
   }
-  es_row<MODE, 32>(p, row, lb, n, lane, [H](float v, bool is_max) { return is_max ? head_max(v, H) : head_sum(v, H); });
+  es_row<MODE, 32, DROP>(p, row, lb, n, lane, [H](float v, bool is_max) { return is_max ? head_max(v, H) : head_sum(v, H); });
 }
 
 // ---------------------------------------------------------------- hub chunks, pass 1: statistics
 // One warp per chunk slot.  Forward / attention: (max, sum exp(x - max)) per head; backward: sum y*g.
 // The last chunk of the row to arrive merges the chunks' values in chunk order into stats[first].
-template <int MODE>
+template <int MODE, bool DROP>
 __global__ void __launch_bounds__(256) es_stats_kernel(const EsParams p) {
   // programmatic dependent launch: the main kernel may start as soon as every CTA of this grid is running; its
   // segment items need nothing from us, its chunk items wait (griddepcontrol.wait) for this grid to finish
@@ -194,7 +234,11 @@ __global__ void __launch_bounds__(256) es_stats_kernel(const EsParams p) {
   float m = -CUDART_INF_F, s = 0.f;
   if (MODE == 1 || MODE == 3) {
     const float *y = p.a + (int64_t)w.lb * H, *g = p.b + (int64_t)w.lb * H;
-    for (int t = lane; t < n; t += 32) s = fmaf(__ldg(y + t), __ldg(g + t), s);
+    for (int t = lane; t < n; t += 32) {
+      float yv = __ldg(y + t), gv = __ldg(g + t);
+      es_unmark<DROP>(p, yv, gv);
+      s = fmaf(yv, gv, s);
+    }
     s = head_sum(s, H);
   } else {
     const float hl = (MODE == 2) ? __ldg(p.a + (int64_t)w.row * H + head) : 0.f;
@@ -252,7 +296,7 @@ __global__ void __launch_bounds__(256) es_stats_kernel(const EsParams p) {
 
 // ---------------------------------------------------------------- hub chunk, pass 2 (shared by both main kernels)
 // normalise the chunk's elements with its row's merged statistics (stats[first slot])
-template <int MODE>
+template <int MODE, bool DROP>
 __device__ __forceinline__ void es_chunk_item(const EsParams &p, int64_t item, int lane) {
   constexpr bool TWO = (MODE == 1 || MODE == 3);
   const int H = p.H;
@@ -271,7 +315,9 @@ __device__ __forceinline__ void es_chunk_item(const EsParams &p, int64_t item, i
         const float hlrow = __ldg(p.hl + (int64_t)w.row * H + head);
         float acc = 0.f;
         for (int t = lane; t < n; t += 32) {
-          const float v = __ldg(y + t) * (__ldg(g + t) - rs.y) * es_dact(p, w.lb, t, head, hlrow);
+          float yv = __ldg(y + t), gv = __ldg(g + t);
+          es_unmark<DROP>(p, yv, gv);
+          const float v = yv * (gv - rs.y) * es_dact(p, w.lb, t, head, hlrow);
           st_stream(o + t, v);
           acc += v;
         }
@@ -289,7 +335,8 @@ __device__ __forceinline__ void es_chunk_item(const EsParams &p, int64_t item, i
       const float hl = (MODE == 2) ? __ldg(p.a + (int64_t)w.row * H + head) : 0.f;
       const float inv = 1.f / rs.y;
 #pragma unroll 4
-      for (int t = lane; t < n; t += 32) st_stream(o + t, es_exp(es_in<MODE>(p, w.lb, t, head, hl) - rs.x) * inv);
+      for (int t = lane; t < n; t += 32)
+        st_stream(o + t, es_mark<DROP>(p, w.lb + (t >> p.lgH), head, es_exp(es_in<MODE>(p, w.lb, t, head, hl) - rs.x) * inv));
     }
     }
 
@@ -327,7 +374,7 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 
 // ---------------------------------------------------------------- main kernel: chunks + segments
 // Shared memory per warp: CAP floats (+ CAP for the backward's second operand) + 33 row offsets.
-template <int MODE, int CAP, int WARPS>
+template <int MODE, int CAP, int WARPS, bool DROP>
 __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
   constexpr bool TWO = (MODE == 1 || MODE == 3);
   extern __shared__ __align__(128) unsigned char es_smem[];
@@ -343,7 +390,7 @@ __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
   if (item >= p.hub.n_segs) {
     if (item - p.hub.n_segs < p.hub.n_chunks) {
       asm volatile("griddepcontrol.wait;" ::: "memory");
-      es_chunk_item<MODE>(p, item - p.hub.n_segs, lane);
+      es_chunk_item<MODE, DROP>(p, item - p.hub.n_segs, lane);
     }
     return;
   }
@@ -438,7 +485,11 @@ __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
         const int k0 = RP[rl], k1 = RP[rl + 1];
         if (TWO) {
           float s = 0.f;
-          for (int k = k0; k < k1; ++k) s = fmaf(T[k * H + h], T2[k * H + h], s);
+          for (int k = k0; k < k1; ++k) {
+            float yv = T[k * H + h], gv = T2[k * H + h];
+            es_unmark<DROP>(p, yv, gv);
+            s = fmaf(yv, gv, s);
+          }
           if (MODE == 1) {
             for (int k = k0; k < k1; ++k) T[k * H + h] = T[k * H + h] * (T2[k * H + h] - s);
           } else {
@@ -448,7 +499,9 @@ __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
             for (int k = k0; k < k1; ++k) {
               const int c = __ldg(p.colind + base + k);
               const float z = hlrow + __ldg(p.hr + (int64_t)c * H + h);
-              const float v = T[k * H + h] * (T2[k * H + h] - s) * (z > 0.f ? 1.f : p.slope);
+              float yv = T[k * H + h], gv = T2[k * H + h];
+              es_unmark<DROP>(p, yv, gv);
+              const float v = yv * (gv - s) * (z > 0.f ? 1.f : p.slope);
               T[k * H + h] = v;
               acc += v;
             }
@@ -467,7 +520,7 @@ __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
             mx = fmaxf(mx, x);
           }
           const float inv = 1.f / sm;
-          for (int k = k0; k < k1; ++k) T[k * H + h] = es_exp(T[k * H + h] - mx) * inv;
+          for (int k = k0; k < k1; ++k) T[k * H + h] = es_mark<DROP>(p, (int64_t)base + k, h, es_exp(T[k * H + h] - mx) * inv);
         }
       }
     }
@@ -492,7 +545,7 @@ __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
 }
 
 // ---------------------------------------------------------------- generic H: warp per row, loop over heads
-template <int MODE>
+template <int MODE, bool DROP>
 __global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
   const int lane = threadIdx.x & 31;
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -501,14 +554,19 @@ __global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
   for (int h = 0; h < p.H; ++h) {
     if (MODE == 1 || MODE == 3) {
       float s = 0.f;
-      for (int e = lb + lane; e < hb; e += 32)
-        s = fmaf(__ldg(p.a + (int64_t)e * p.H + h), __ldg(p.b + (int64_t)e * p.H + h), s);
+      for (int e = lb + lane; e < hb; e += 32) {
+        float yv = __ldg(p.a + (int64_t)e * p.H + h), gv = __ldg(p.b + (int64_t)e * p.H + h);
+        es_unmark<DROP>(p, yv, gv);
+        s = fmaf(yv, gv, s);
+      }
       s = head_sum(s, 1);
       const float hlrow = (MODE == 3) ? __ldg(p.hl + row * p.H + h) : 0.f;
       float acc = 0.f;
       for (int e = lb + lane; e < hb; e += 32) {
         const int64_t k = (int64_t)e * p.H + h;
-        float v = __ldg(p.a + k) * (__ldg(p.b + k) - s);
+        float yv = __ldg(p.a + k), gv = __ldg(p.b + k);
+        es_unmark<DROP>(p, yv, gv);
+        float v = yv * (gv - s);
         if (MODE == 3) {
           const float z = hlrow + __ldg(p.hr + (int64_t)__ldg(p.colind + e) * p.H + h);
           v *= (z > 0.f ? 1.f : p.slope);
@@ -535,7 +593,7 @@ __global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
       float s = 0.f;
       for (int e = lb + lane; e < hb; e += 32) s += expf(in(e) - m);
       s = head_sum(s, 1);
-      for (int e = lb + lane; e < hb; e += 32) p.out[(int64_t)e * p.H + h] = expf(in(e) - m) / s;
+      for (int e = lb + lane; e < hb; e += 32) p.out[(int64_t)e * p.H + h] = es_mark<DROP>(p, e, h, expf(in(e) - m) / s);
     }
   }
 }
@@ -545,7 +603,7 @@ __global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
 // is the shape the whole GPU suite is validated with.
 constexpr int ES_WARPS = 8;
 
-template <int MODE, int CAP>
+template <int MODE, int CAP, bool DROP>
 static int launch_main(const EsParams &p, cudaStream_t s) {
   constexpr int WARPS = ES_WARPS;
   constexpr bool TWO = (MODE == 1 || MODE == 3);
@@ -553,7 +611,7 @@ static int launch_main(const EsParams &p, cudaStream_t s) {
   static unsigned long long attr_done = 0;
   int dev = 0;
   if (first_use_on_device(attr_done, &dev))
-    CB_CUDA(cudaFuncSetAttribute(es_main_kernel<MODE, CAP, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CB_CUDA(cudaFuncSetAttribute(es_main_kernel<MODE, CAP, WARPS, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t items = (int64_t)p.hub.n_chunks + p.hub.n_segs;
   const int64_t blocks = ceil_div(items, WARPS);
   if (blocks == 0) return COGDL_B200_OK;
@@ -568,14 +626,16 @@ static int launch_main(const EsParams &p, cudaStream_t s) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;     // overlap with the statistics kernel (see es_stats_kernel)
   cfg.attrs = attr;
   cfg.numAttrs = p.hub.n_chunks > 0 ? 1 : 0;
-  CB_CUDA(cudaLaunchKernelEx(&cfg, es_main_kernel<MODE, CAP, WARPS>, p));
+  CB_CUDA(cudaLaunchKernelEx(&cfg, es_main_kernel<MODE, CAP, WARPS, DROP>, p));
   count_launch();
   return COGDL_B200_OK;
 }
 
-// Launch plan (see the header comment).
-template <int MODE>
+// Launch plan (see the header comment).  DROP only with MODE 2 / 3.
+template <int MODE, bool DROP = false>
 static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t s, const char *who) {
+  static_assert(!DROP || MODE == 2 || MODE == 3, "attention dropout is a mode of the GAT attention and its backward");
+  const char *drop_note = DROP ? ",DROP" : "";
   const bool pow2 = p.H <= 32 && (p.H & (p.H - 1)) == 0;
   const int64_t row_blocks = ceil_div(p.n_rows * 32, 256);
   CB_REQUIRE(row_blocks <= 0x7fffffffLL, "%s: problem too large for one launch", who);
@@ -584,16 +644,16 @@ static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t
   p.hub = hub_view(nullptr);
   p.stats = nullptr; p.part = nullptr; p.bulk = false;
   if (!pow2) {
-    note_kernel("cogdl_b200::es_generic_kernel<MODE=%d>", MODE);
-    es_generic_kernel<MODE><<<(unsigned)row_blocks, 256, 0, s>>>(p);
+    note_kernel("cogdl_b200::es_generic_kernel<MODE=%d%s>", MODE, drop_note);
+    es_generic_kernel<MODE, DROP><<<(unsigned)row_blocks, 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
     return COGDL_B200_OK;
   }
   const int64_t cap_need = plan ? (int64_t)plan->chunk_edges * p.H : 0;
   const bool segs = plan && plan->chunk_edges > 0 && plan->segs && plan->edge_row && plan->n_segs > 0 && cap_need <= 2048;
   if (!segs) {   // no plan: every row through the warp kernel (hubs serialise on one warp)
-    note_kernel("cogdl_b200::es_warp_kernel<MODE=%d>", MODE);
-    es_warp_kernel<MODE><<<(unsigned)row_blocks, 256, 0, s>>>(p);
+    note_kernel("cogdl_b200::es_warp_kernel<MODE=%d%s>", MODE, drop_note);
+    es_warp_kernel<MODE, DROP><<<(unsigned)row_blocks, 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
     return COGDL_B200_OK;
   }
@@ -607,15 +667,16 @@ static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t
   // 1-D TMA needs 16-byte aligned global addresses and sizes: rows start at multiples of H floats
   p.bulk = (p.H % 4 == 0) && aligned16(p.a) && aligned16(p.out) && (MODE == 0 || aligned16(p.b));
   if (p.hub.n_chunks > 0) {
-    es_stats_kernel<MODE><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
+    // the attention's statistics come before the dropout: MODE 2 shares the kernel without DROP
+    es_stats_kernel<MODE, DROP && MODE == 3><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
   }
   const int chosen = cap_need <= 512 ? 512 : (cap_need <= 1024 ? 1024 : 2048);   // smallest tile (floats per warp) that fits
-  note_kernel("cogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d>%s", MODE, chosen, ES_WARPS,
+  note_kernel("cogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d%s>%s", MODE, chosen, ES_WARPS, drop_note,
               (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
-  if (chosen == 512) return launch_main<MODE, 512>(p, s);
-  if (chosen == 1024) return launch_main<MODE, 1024>(p, s);
-  return launch_main<MODE, 2048>(p, s);
+  if (chosen == 512) return launch_main<MODE, 512, DROP>(p, s);
+  if (chosen == 1024) return launch_main<MODE, 1024, DROP>(p, s);
+  return launch_main<MODE, 2048, DROP>(p, s);
 }
 
 template <int MODE>
@@ -629,15 +690,20 @@ static int es_entry(const int32_t *rowptr, const float *a, const float *b, float
   EsParams p;
   p.rowptr = rowptr; p.a = a; p.b = b; p.out = out; p.n_rows = n_rows; p.H = (int)H;
   p.colind = nullptr; p.slope = 0.f; p.hl = nullptr; p.hr = nullptr; p.grow = nullptr;
+  p.seed = 0; p.drop_below = 0; p.scale = 1.f;
   return es_launch<MODE>(p, plan, (cudaStream_t)stream, who);
 }
 
-// GAT attention (used by cogdl_b200_gat_fwd_f32, mhspmm.cu): att = softmax_row(leakyrelu(h_l[row] + h_r[col])), any H.
+// GAT attention (used by cogdl_b200_gat_fwd_f32 / _dropout_f32, mhspmm.cu): att = softmax_row(leakyrelu(h_l[row] +
+// h_r[col])), any H; with drop, the dropped (edge, head) pairs carry the sign bit.
 int gat_attention(const int32_t *rowptr, const int32_t *colind, const float *h_l, const float *h_r, float slope,
-                  float *att, int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan, cudaStream_t s) {
+                  float *att, int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan, cudaStream_t s,
+                  bool drop, uint64_t seed, uint64_t drop_below) {
   EsParams p;
   p.rowptr = rowptr; p.a = h_l; p.b = h_r; p.out = att; p.n_rows = n_rows; p.H = (int)H;
   p.colind = colind; p.slope = slope; p.hl = nullptr; p.hr = nullptr; p.grow = nullptr;
+  p.seed = seed; p.drop_below = drop_below; p.scale = 1.f;
+  if (drop) return es_launch<2, true>(p, plan, s, "cogdl_b200_gat_fwd_dropout_f32");
   return es_launch<2>(p, plan, s, "cogdl_b200_gat_fwd_f32");
 }
 
@@ -665,11 +731,11 @@ extern "C" int cogdl_b200_edge_softmax_bwd_f32(const int32_t *rowptr, const floa
 //   d e[p,h]  = att * (d att - sum_row att * d att) * leakyrelu'(h_l[row,h] + h_r[col,h])      -> d_edge [nnz, H]
 //   g_row[i,h] = sum_{p in row i} d e[p,h]                                                      -> [n_rows, H]
 // (g_col is the column-wise sum of d_edge: cogdl_b200_edge_colsum_f32 on the cached transpose.)
-extern "C" int cogdl_b200_gat_attn_bwd_f32(const int32_t *rowptr, const int32_t *colind, const float *att,
-                                           const float *d_att, const float *h_l, const float *h_r,
-                                           float negative_slope, float *d_edge, float *g_row, int64_t n_rows,
-                                           int64_t H, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
-  const char *who = "cogdl_b200_gat_attn_bwd_f32";
+template <bool DROP>
+static int gat_attn_bwd(const int32_t *rowptr, const int32_t *colind, const float *att, const float *d_att,
+                        const float *h_l, const float *h_r, float negative_slope, float scale, float *d_edge,
+                        float *g_row, int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan,
+                        cogdl_b200_stream_t stream, const char *who) {
   CB_REQUIRE(n_rows >= 0 && H >= 0, "%s: negative size", who);
   if (n_rows == 0 || H == 0) return COGDL_B200_OK;
   CB_REQUIRE(rowptr && colind && att && d_att && h_l && h_r && d_edge && g_row, "%s: null pointer", who);
@@ -677,5 +743,28 @@ extern "C" int cogdl_b200_gat_attn_bwd_f32(const int32_t *rowptr, const int32_t 
   EsParams p;
   p.rowptr = rowptr; p.a = att; p.b = d_att; p.out = d_edge; p.n_rows = n_rows; p.H = (int)H;
   p.colind = colind; p.slope = negative_slope; p.hl = h_l; p.hr = h_r; p.grow = g_row;
-  return es_launch<3>(p, plan, (cudaStream_t)stream, who);
+  p.seed = 0; p.drop_below = 0; p.scale = scale;
+  return es_launch<3, DROP>(p, plan, (cudaStream_t)stream, who);
+}
+
+extern "C" int cogdl_b200_gat_attn_bwd_f32(const int32_t *rowptr, const int32_t *colind, const float *att,
+                                           const float *d_att, const float *h_l, const float *h_r,
+                                           float negative_slope, float *d_edge, float *g_row, int64_t n_rows,
+                                           int64_t H, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
+  return gat_attn_bwd<false>(rowptr, colind, att, d_att, h_l, h_r, negative_slope, 1.f, d_edge, g_row, n_rows, H, plan,
+                             stream, "cogdl_b200_gat_attn_bwd_f32");
+}
+
+// The same over the signed attention of cogdl_b200_gat_fwd_dropout_f32: d_att (= mhsddmm(d out, feat)) is the
+// gradient of the dropped, scaled attention; the softmax backward runs on |att| with d_att * scale on the kept
+// entries and 0 on the dropped ones.
+extern "C" int cogdl_b200_gat_attn_bwd_dropout_f32(const int32_t *rowptr, const int32_t *colind, const float *att,
+                                                   const float *d_att, const float *h_l, const float *h_r,
+                                                   float negative_slope, float scale, float *d_edge, float *g_row,
+                                                   int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan,
+                                                   cogdl_b200_stream_t stream) {
+  const char *who = "cogdl_b200_gat_attn_bwd_dropout_f32";
+  CB_REQUIRE(isfinite(scale) && scale > 0.f, "%s: scale must be finite and > 0 (got %g)", who, (double)scale);
+  return gat_attn_bwd<true>(rowptr, colind, att, d_att, h_l, h_r, negative_slope, scale, d_edge, g_row, n_rows, H,
+                            plan, stream, who);
 }

@@ -32,9 +32,10 @@ struct MhParams {
   int FVL;           // F in vector units  (head = col / FVL)
   int S;             // slices per row
   HubView hub;
+  float drop_scale;  // > 0: att carries an attention-dropout mask in its sign bit (drop_att); 0: plain attention
 };
 
-template <typename VecT, int GROUP, bool HAS_PERM>
+template <typename VecT, int GROUP, bool HAS_PERM, bool DROP>
 __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
   constexpr int U0 = 8;
   constexpr int U = U0 < GROUP ? U0 : GROUP;
@@ -96,7 +97,7 @@ __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
       }
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        if (j + u < cnt && colok) axpy_rn(acc, a[u], x[u]);
+        if (j + u < cnt && colok) axpy_rn(acc, DROP ? drop_att(a[u], p.drop_scale) : a[u], x[u]);
     }
     c = cn;
     pe = pn;
@@ -125,10 +126,12 @@ __global__ void __launch_bounds__(256) mhspmm_kernel(const MhParams p) {
 
 template <typename VecT, int GROUP>
 static int launch_mh(const MhParams &p, cudaStream_t stream) {
-  return launch_items(p.perm ? mhspmm_kernel<VecT, GROUP, true> : mhspmm_kernel<VecT, GROUP, false>, p,
-                      ((int64_t)p.hub.n_chunks + p.n_rows) * p.S, GROUP, stream, "mhspmm",
-                      "cogdl_b200::mhspmm_kernel<%s,GROUP=%d,%s>", sizeof(VecT) == 16 ? "float4" : "float", GROUP,
-                      p.perm ? "perm" : "no_perm");
+  const bool drop = p.drop_scale > 0.f;
+  auto kernel = drop ? (p.perm ? mhspmm_kernel<VecT, GROUP, true, true> : mhspmm_kernel<VecT, GROUP, false, true>)
+                     : (p.perm ? mhspmm_kernel<VecT, GROUP, true, false> : mhspmm_kernel<VecT, GROUP, false, false>);
+  return launch_items(kernel, p, ((int64_t)p.hub.n_chunks + p.n_rows) * p.S, GROUP, stream, "mhspmm",
+                      "cogdl_b200::mhspmm_kernel<%s,GROUP=%d,%s%s>", sizeof(VecT) == 16 ? "float4" : "float", GROUP,
+                      p.perm ? "perm" : "no_perm", drop ? ",drop" : "");
 }
 
 template <typename VecT>
@@ -142,7 +145,7 @@ static int dispatch_mh(MhParams &p, cudaStream_t s) {
     StreamParams q;
     q.rowptr = p.rowptr; q.colind = p.colind; q.val = nullptr; q.att = p.att; q.perm = p.perm;
     q.X0 = p.feat; q.X1 = p.feat; q.n0 = INT64_MAX; q.Y = p.out; q.ldv = p.HFV; q.H = p.H; q.FVL = p.FVL;
-    q.S = p.S; q.hub = p.hub; q.n_peers = 0; q.peer_shift = 0;
+    q.S = p.S; q.hub = p.hub; q.n_peers = 0; q.peer_shift = 0; q.drop_scale = p.drop_scale;
     return launch_stream<VecT, 1, 8, 3, true, FORM_MULTIHEAD>(q, s);
   }
   switch (g) {
@@ -155,12 +158,13 @@ static int dispatch_mh(MhParams &p, cudaStream_t s) {
   }
 }
 
+// drop_scale > 0: att carries an attention-dropout mask in its sign bit (see drop_att); 0: plain attention.
 static int mhspmm_run(const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const float *att,
                       const float *feat, float *out, int64_t n_rows, int64_t H, int64_t F,
-                      const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
+                      const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream, float drop_scale = 0.f) {
   MhParams p;
   p.rowptr = rowptr; p.colind = colind; p.perm = perm; p.att = att; p.feat = feat; p.out = out;
-  p.n_rows = n_rows; p.H = (int)H; p.hub = hub_view(plan); p.S = 1;
+  p.n_rows = n_rows; p.H = (int)H; p.hub = hub_view(plan); p.S = 1; p.drop_scale = drop_scale;
   const bool vec = (F % 4 == 0) && aligned16(feat) && aligned16(out) &&
                    (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
   if (vec) {
@@ -177,17 +181,36 @@ static int mhspmm_run(const int32_t *rowptr, const int32_t *colind, const int32_
 
 using namespace cogdl_b200;
 
+static int mhspmm_entry(const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const float *att,
+                        const float *feat, float *out, int64_t n_rows, int64_t H, int64_t F,
+                        const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream, float drop_scale,
+                        const char *who) {
+  CB_REQUIRE(n_rows >= 0 && H >= 0 && F >= 0, "%s: negative size", who);
+  if (n_rows == 0 || H == 0 || F == 0) return COGDL_B200_OK;
+  CB_REQUIRE(rowptr && colind && att && feat && out, "%s: null pointer", who);
+  CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "%s: sizes must fit int32", who);
+  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
+  if (rc) return rc;
+  return mhspmm_run(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream, drop_scale);
+}
+
 extern "C" int cogdl_b200_mhspmm_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                                      const float *att, const float *feat, float *out, int64_t n_rows,
                                      int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan,
                                      cogdl_b200_stream_t stream) {
-  CB_REQUIRE(n_rows >= 0 && H >= 0 && F >= 0, "cogdl_b200_mhspmm_f32: negative size");
-  if (n_rows == 0 || H == 0 || F == 0) return COGDL_B200_OK;
-  CB_REQUIRE(rowptr && colind && att && feat && out, "cogdl_b200_mhspmm_f32: null pointer");
-  CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "cogdl_b200_mhspmm_f32: sizes must fit int32");
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
-  if (rc) return rc;
-  return mhspmm_run(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream);
+  return mhspmm_entry(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream, 0.f, "cogdl_b200_mhspmm_f32");
+}
+
+// The aggregation over an attention written by cogdl_b200_gat_fwd_dropout_f32: entries with the sign bit set are
+// dropped, the others are scaled by `scale`.  With perm (the cached transpose) this is d feat of the dropout GAT.
+extern "C" int cogdl_b200_mhspmm_dropout_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                                             const float *att, const float *feat, float scale, float *out,
+                                             int64_t n_rows, int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan,
+                                             cogdl_b200_stream_t stream) {
+  CB_REQUIRE(isfinite(scale) && scale > 0.f, "cogdl_b200_mhspmm_dropout_f32: scale must be finite and > 0 (got %g)",
+             (double)scale);
+  return mhspmm_entry(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream, scale,
+                      "cogdl_b200_mhspmm_dropout_f32");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -206,21 +229,46 @@ extern "C" int cogdl_b200_mhspmm_f32(const int32_t *rowptr, const int32_t *colin
 // ------------------------------------------------------------------------------------------
 namespace cogdl_b200 {
 int gat_attention(const int32_t *rowptr, const int32_t *colind, const float *h_l, const float *h_r, float slope,
-                  float *att, int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan, cudaStream_t s);
+                  float *att, int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan, cudaStream_t s,
+                  bool drop, uint64_t seed, uint64_t drop_below);
+}
+
+// drop: attention dropout (seed, drop_below, scale) -- see cogdl_b200_gat_fwd_dropout_f32
+static int gat_fwd(const int32_t *rowptr, const int32_t *colind, const float *h_l, const float *h_r, const float *feat,
+                   float negative_slope, bool drop, uint64_t seed, uint64_t drop_below, float scale, float *out,
+                   float *att_out, int64_t n_rows, int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan,
+                   cogdl_b200_stream_t stream, const char *who) {
+  CB_REQUIRE(n_rows >= 0 && H >= 0 && F >= 0, "%s: negative size", who);
+  if (n_rows == 0 || H == 0 || F == 0) return COGDL_B200_OK;
+  CB_REQUIRE(rowptr && colind && h_l && h_r && feat && out, "%s: null pointer", who);
+  CB_REQUIRE(att_out, "%s: att_out ([nnz,H] attention, also scratch) is required", who);
+  CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "%s: sizes must fit int32", who);
+  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
+  if (rc) return rc;
+  rc = gat_attention(rowptr, colind, h_l, h_r, negative_slope, att_out, n_rows, H, plan, (cudaStream_t)stream, drop,
+                     seed, drop_below);
+  if (rc) return rc;
+  return mhspmm_run(rowptr, colind, nullptr, att_out, feat, out, n_rows, H, F, plan, stream, drop ? scale : 0.f);
 }
 
 extern "C" int cogdl_b200_gat_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *h_l,
                                       const float *h_r, const float *feat, float negative_slope, float *out,
                                       float *att_out, int64_t n_rows, int64_t H, int64_t F,
                                       const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
-  CB_REQUIRE(n_rows >= 0 && H >= 0 && F >= 0, "cogdl_b200_gat_fwd_f32: negative size");
-  if (n_rows == 0 || H == 0 || F == 0) return COGDL_B200_OK;
-  CB_REQUIRE(rowptr && colind && h_l && h_r && feat && out, "cogdl_b200_gat_fwd_f32: null pointer");
-  CB_REQUIRE(att_out, "cogdl_b200_gat_fwd_f32: att_out ([nnz,H] attention, also scratch) is required");
-  CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "cogdl_b200_gat_fwd_f32: sizes must fit int32");
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
-  if (rc) return rc;
-  rc = gat_attention(rowptr, colind, h_l, h_r, negative_slope, att_out, n_rows, H, plan, (cudaStream_t)stream);
-  if (rc) return rc;
-  return mhspmm_run(rowptr, colind, nullptr, att_out, feat, out, n_rows, H, F, plan, stream);
+  return gat_fwd(rowptr, colind, h_l, h_r, feat, negative_slope, false, 0, 0, 0.f, out, att_out, n_rows, H, F, plan,
+                 stream, "cogdl_b200_gat_fwd_f32");
+}
+
+// GAT forward with attention dropout: (edge p, head h) is kept iff draw(seed, p, h) >= drop_below (rng.cuh), and a
+// kept attention is scaled by `scale` in the aggregation.  att_out holds the softmax with the sign bit set on the
+// dropped entries -- the mask travels to the backward in the saved attention, nothing else is stored.
+extern "C" int cogdl_b200_gat_fwd_dropout_f32(const int32_t *rowptr, const int32_t *colind, const float *h_l,
+                                              const float *h_r, const float *feat, float negative_slope, uint64_t seed,
+                                              uint64_t drop_below, float scale, float *out, float *att_out,
+                                              int64_t n_rows, int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan,
+                                              cogdl_b200_stream_t stream) {
+  CB_REQUIRE(isfinite(scale) && scale > 0.f, "cogdl_b200_gat_fwd_dropout_f32: scale must be finite and > 0 (got %g)",
+             (double)scale);
+  return gat_fwd(rowptr, colind, h_l, h_r, feat, negative_slope, true, seed, drop_below, scale, out, att_out, n_rows,
+                 H, F, plan, stream, "cogdl_b200_gat_fwd_dropout_f32");
 }

@@ -26,23 +26,13 @@
 // `assoc` scratch contract: int32[num_nodes], every entry COGDL_B200_SAMPLE_UNSEEN (0x7fffffff) on entry;
 // restored to that state before the fill call returns, so one allocation serves every batch.
 #include "common.cuh"
+#include "rng.cuh"
 
 #include <cub/device/device_scan.cuh>
 
 namespace cogdl_b200 {
 
 constexpr int UNSEEN = 0x7fffffff;
-
-__host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-// draw k of batch slot i
-__host__ __device__ __forceinline__ uint64_t draw(uint64_t seed, int64_t i, int64_t k) {
-  return mix64(mix64(seed + (uint64_t)i * 0xD1342543DE82EF95ull) + (uint64_t)k);
-}
 
 __device__ __forceinline__ int64_t row_count(int64_t deg, int64_t k, int replace) {
   if (k < 0) return deg;

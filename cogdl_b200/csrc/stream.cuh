@@ -48,6 +48,10 @@ struct StreamParams {
   // val[q] * (X0[colind[q]] o B[idx2[q]]) with o = * (MODE_COMP_MULT) or - (MODE_COMP_SUB)
   const int *idx2;
   const float *B;
+  // multi-head form with DROP: the attention carries an attention-dropout mask in its sign bit (edge_softmax.cu,
+  // MODE 2); a kept entry is read as att * drop_scale, a dropped one as 0 (drop_att, common.cuh).  Read only by
+  // the multi-head form, which takes the DROP instantiation iff drop_scale > 0.
+  float drop_scale;
 };
 
 enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2, MODE_COMP_MULT = 3, MODE_COMP_SUB = 4 };
@@ -65,7 +69,7 @@ enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
 
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
 // whole range into acc (hub chunk).
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH, bool DROP = false>
 __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const int e_end, const int cv,
                                              const bool (&colok)[NV], const int head, const int lane,
                                              VecT (&acc)[NV]) {
@@ -147,7 +151,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
               else if (MODE == MODE_WEIGHTED) axpy_rn(acc[k], vj, x[u][k]);
               else if (MODE == MODE_COMP_MULT) axpy_rn(acc[k], vj, mul_rn(x[u][k], b[u][k]));
               else if (MODE == MODE_COMP_SUB) axpy_rn(acc[k], vj, sub_rn(x[u][k], b[u][k]));
-              else axpy_rn(acc[k], a[u], x[u][k]);
+              else axpy_rn(acc[k], DROP ? drop_att(a[u], p.drop_scale) : a[u], x[u][k]);
             }
           }
           if (ROWS && ((em >> u) & 1u)) {   // last edge of row rj: store and restart (warp-uniform)
@@ -270,7 +274,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
 }
 
 // One work item processed by one warp: wid = item * S + slice (multi-head), slice = blockIdx.y (PANEL).
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool PANEL>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool PANEL, bool DROP = false>
 __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t wid, const int lane, int2 *s_cv, int *s_r) {
   constexpr int TILE = 32 * NV;
   constexpr bool SLICED = (MODE == MODE_MULTIHEAD || PANEL);
@@ -296,7 +300,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
       for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = vzero<VecT>(); }
       const int head = (MODE == MODE_MULTIHEAD && colok[0]) ? cv / p.FVL : 0;
       if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false, PANEL && PREFETCH>(p, w.lb, w.hb, cv, colok[0], lane, s_cv, s_r, acc[0]);
-      else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH>(p, w.lb, w.hb, cv, colok, head, lane, acc);
+      else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH, DROP>(p, w.lb, w.hb, cv, colok, head, lane, acc);
 #pragma unroll
       for (int k = 0; k < NV; ++k)
         if (colok[k]) st_cg(P + (int64_t)w.slot * p.ldv + cv + k * 32, acc[k]);
@@ -354,11 +358,12 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
       }
     }
     if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH>(p, e_begin, e_end, cv, colok[0], lane, s_cv, s_r, acc[0]);
-    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH>(p, e_begin, e_end, cv, colok, head, lane, acc);
+    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, DROP>(p, e_begin, e_end, cv, colok, head, lane, acc);
   }
 }
 
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool PANEL = false>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool PANEL = false,
+          bool DROP = false>
 __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p) {
   const int lane = threadIdx.x & 31;
   constexpr bool LEAN = is_lean<MODE, NV>();
@@ -367,7 +372,7 @@ __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p)
   int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
   int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, PANEL>(p, wid, lane, s_cv, s_r);
+  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, PANEL, DROP>(p, wid, lane, s_cv, s_r);
 }
 
 // Launch helper: picks the instantiation of FORM for (weighted, perm, source form); U / MINB fixed by the caller.
@@ -389,17 +394,24 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   const int src = p.n_peers > 0 ? SRC_PEERS : (p.n0 != INT64_MAX ? SRC_TWO : SRC_ONE);
   if (FORM != FORM_PLAIN && src != SRC_ONE)
     return set_error(COGDL_B200_EINVAL, "stream kernel: the panel and multi-head forms read one source");
-  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s,%s,U=%d,MINB=%d%s>",
+  const bool drop = FORM == FORM_MULTIHEAD && p.drop_scale > 0.f;
+  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>",
               sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
               FORM == FORM_MULTIHEAD ? "multihead" : (p.val ? "weighted" : "unweighted"),
-              (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "",
+              (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "", drop ? "+drop" : "",
               src == SRC_PEERS ? "SRC_PEERS" : (src == SRC_TWO ? "SRC_TWO" : "SRC_ONE"), U, MINB,
               PREFETCH ? ",prefetch" : "");
   if (FORM == FORM_PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
   append_kernel_note(" block=%d", STREAM_BLOCK);
   if constexpr (FORM == FORM_MULTIHEAD) {
-    if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    if (drop) {
+      if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+      else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    } else if (p.perm) {
+      stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    } else {
+      stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    }
   } else if constexpr (FORM == FORM_PANEL) {
     if (p.val) stream_kernel<VecT, 1, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
     else stream_kernel<VecT, 1, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);

@@ -21,6 +21,8 @@ reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores 
 `cogdl.layers.disengcn_layer.DisenGCNLayer.forward` (DisenGCN), with disengcn_forward and cogdl_b200.disen_routing
 (uninstall_disengcn()).  compgcn=True rebinds `cogdl.models.nn.compgcn.CompGCNLayer.forward` (CompGCN) to
 compgcn_forward, which sends the message passing to cogdl_b200.compgcn_aggregate (uninstall_compgcn()).
+gat=True rebinds `cogdl.layers.gat_layer.GATLayer.forward` (GAT and every model built on GATLayer) to gat_forward, which
+sends the attention, its dropout and the aggregation to the fused GAT kernels (uninstall_gat()).
 spspmm=True provides torch_sparse's spspmm / spmm (cogdl_b200.spspmm / coo_spmm) to GTN, SRGCN and Graph U-Net, through a
 `torch_sparse` stand-in module when the real package is missing (install_spspmm, uninstall_spspmm()).
 """
@@ -151,6 +153,46 @@ def uninstall_compgcn():
     _restore_forward(cm.CompGCNLayer)
 
 
+def gat_forward(self, graph, x):
+    """GATLayer.forward (cogdl/layers/gat_layer.py:59-86) with the attention, its dropout and the aggregation in the
+    fused sm_90a GAT kernels, for any graph (the backward uses the cached transpose, not is_symmetric()).  The layer's
+    own W, a_l, a_r, NaN zeroing, residual, norm and activation are used; the attention dropout is self.dropout.p
+    when training and none in eval, drawn in the kernel (a fresh seed from torch's CPU generator per call).  CPU or
+    non-fp32 input or weights, and a dropout of 1, run the original."""
+    from .utils.spmm_utils import FusedGATFunction, _structure
+
+    original = type(self)._cogdl_b200_original_forward
+    p = self.dropout.p if self.training else 0.0
+    if (not x.is_cuda or x.dtype != torch.float32 or self.W.dtype != torch.float32 or self.a_l.dtype != torch.float32
+            or self.a_r.dtype != torch.float32 or p >= 1.0):
+        return original(self, graph, x)
+    h = torch.matmul(x, self.W).view(-1, self.nhead, self.out_features)
+    h[torch.isnan(h)] = 0.0
+    h_l = (self.a_l * h).sum(dim=-1)
+    h_r = (self.a_r * h).sum(dim=-1)
+    out = FusedGATFunction.apply(h_l, h_r, _structure(graph), None, None, None, self.alpha, h, p, None)
+    out = out.view(out.shape[0], -1)
+    if self.residual is not None:
+        out = out + self.residual(x)
+    if self.norm is not None:
+        out = self.norm(out)
+    if self.act is not None:
+        out = self.act(out)
+    return out
+
+
+def install_gat():
+    import cogdl.layers.gat_layer as gl
+
+    return _rebind_forward(gl.GATLayer, gat_forward, "cogdl.layers.gat_layer.GATLayer.forward")
+
+
+def uninstall_gat():
+    import cogdl.layers.gat_layer as gl
+
+    _restore_forward(gl.GATLayer)
+
+
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
 _spspmm_state = {"stub": None, "rebound": []}
 
@@ -200,7 +242,7 @@ def uninstall_spspmm():
     _spspmm_state["stub"] = None
 
 
-def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False):
+def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -288,4 +330,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_compgcn()
     if spspmm:
         patched += install_spspmm()
+    if gat:
+        patched += install_gat()
     return patched

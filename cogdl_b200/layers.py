@@ -89,7 +89,9 @@ class GATLayer(nn.Module):
         self.act = _activation(activation)
         self.norm = _norm(norm, out_feats * nhead)
         self.residual = nn.Linear(in_feats, out_feats * nhead) if residual else None
-        self.fused = fused  # None: the reference's rule (gat_layer.py:68); True/False forces it
+        # None: the reference's rule (gat_layer.py:68); True/False forces it.  With True the attention dropout runs in
+        # the fused kernels when training.
+        self.fused = fused
         for t in (self.a_l, self.a_r, self.W):
             stdv = math.sqrt(6.0 / (t.size(-2) + t.size(-1)))
             t.data.uniform_(-stdv, stdv)
@@ -102,8 +104,9 @@ class GATLayer(nn.Module):
         use_fused = self.fused
         if use_fused is None:
             use_fused = (self.dropout.p == 0.0 or not self.training) and check_fused_gat()
-        if use_fused:
-            out = fused_gat_op(h_l, h_r, graph, self.alpha, h)
+        p = self.dropout.p if self.training else 0.0
+        if use_fused and p < 1.0:      # p = 1 drops everything: nn.Dropout on the unfused path
+            out = fused_gat_op(h_l, h_r, graph, self.alpha, h, attn_drop=p)
             out = out.view(out.shape[0], -1)
         else:
             row, col = graph.edge_index

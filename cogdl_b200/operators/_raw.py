@@ -116,8 +116,10 @@ def edge_softmax_bwd_raw(st: CSRStructure, y, g):
     return out
 
 
-def mhspmm_raw(st: CSRStructure, att, feat, perm=None):
-    """out[i,h,:] = sum_p att[P(p),h] * feat[col[p],h,:];  feat [n_src,H,F], att [nnz,H]."""
+def mhspmm_raw(st: CSRStructure, att, feat, perm=None, drop_scale=None):
+    """out[i,h,:] = sum_p att[P(p),h] * feat[col[p],h,:];  feat [n_src,H,F], att [nnz,H].
+    drop_scale: att is the signed attention of gat_fwd_raw(drop=...): sign-bit entries count as 0, the others as
+    att * drop_scale."""
     dev = require_cuda(att, feat, perm)
     att, feat = _f32c(att, "attention"), _f32c(feat, "feat")
     if feat.dim() != 3:
@@ -128,8 +130,12 @@ def mhspmm_raw(st: CSRStructure, att, feat, perm=None):
     with torch.cuda.device(dev):
         out = torch.empty((st.n_rows, H, F), dtype=torch.float32, device=dev)
         plan, keep = st.plan_struct(st.plan.n_chunks * H * F * 4 if st.chunk_edges > 0 else 0)
-        _cabi.call("cogdl_b200_mhspmm_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att), _ptr(feat),
-                   _ptr(out), st.n_rows, H, F, plan, _stream(dev))
+        if drop_scale is None:
+            _cabi.call("cogdl_b200_mhspmm_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att), _ptr(feat),
+                       _ptr(out), st.n_rows, H, F, plan, _stream(dev))
+        else:
+            _cabi.call("cogdl_b200_mhspmm_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att),
+                       _ptr(feat), float(drop_scale), _ptr(out), st.n_rows, H, F, plan, _stream(dev))
         del keep
     return out
 
@@ -171,7 +177,18 @@ def scatter_max_bwd_raw(grad, argmax, n_src):
     return gx
 
 
-def gat_fwd_raw(st: CSRStructure, h_l, h_r, feat, slope, want_att):
+def attn_dropout_args(p):
+    """(drop_below, scale) of attention dropout with probability p, 0 <= p < 1: an (edge, head) is kept iff
+    draw(seed, edge, head) >= drop_below = floor(p * 2^64), a kept attention is multiplied by scale = 1 / (1 - p)."""
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise ValueError(f"attention dropout must be in [0, 1), got {p}")
+    return int(p * 2.0 ** 64), 1.0 / (1.0 - p)
+
+
+def gat_fwd_raw(st: CSRStructure, h_l, h_r, feat, slope, want_att, drop=None):
+    """(out [n_rows,H,F], att [nnz,H]).  drop = (seed, drop_below, scale): attention dropout, and att is returned
+    signed (sign bit set on the dropped entries; see cogdl_b200_gat_fwd_dropout_f32)."""
     dev = require_cuda(h_l, h_r, feat)
     h_l, h_r, feat = _f32c(h_l, "attn_row"), _f32c(h_r, "attn_col"), _f32c(feat, "in_feat")
     H, F = feat.shape[1], feat.shape[2]
@@ -179,14 +196,21 @@ def gat_fwd_raw(st: CSRStructure, h_l, h_r, feat, slope, want_att):
         out = torch.empty((st.n_rows, H, F), dtype=torch.float32, device=dev)
         att = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)   # output for training, scratch otherwise
         plan, keep = st.plan_struct(max(st.plan.n_chunks * H * F * 4, _es_scratch(st, H)) if st.chunk_edges > 0 else 0)
-        _cabi.call("cogdl_b200_gat_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r), _ptr(feat),
-                   float(slope), _ptr(out), _ptr(att), st.n_rows, H, F, plan, _stream(dev))
+        if drop is None:
+            _cabi.call("cogdl_b200_gat_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r), _ptr(feat),
+                       float(slope), _ptr(out), _ptr(att), st.n_rows, H, F, plan, _stream(dev))
+        else:
+            seed, drop_below, scale = drop
+            _cabi.call("cogdl_b200_gat_fwd_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r),
+                       _ptr(feat), float(slope), int(seed), int(drop_below), float(scale), _ptr(out), _ptr(att),
+                       st.n_rows, H, F, plan, _stream(dev))
         del keep
     return out, att
 
 
-def gat_attn_bwd_raw(st: CSRStructure, att, d_att, h_l, h_r, slope):
-    """(d_edge [nnz,H], g_row [n_rows,H]): softmax backward * LeakyReLU' and its row sums in one pass."""
+def gat_attn_bwd_raw(st: CSRStructure, att, d_att, h_l, h_r, slope, drop_scale=None):
+    """(d_edge [nnz,H], g_row [n_rows,H]): softmax backward * LeakyReLU' and its row sums in one pass.
+    drop_scale: att is the signed attention of gat_fwd_raw(drop=...) and d_att the gradient after the dropout."""
     dev = require_cuda(att, d_att, h_l, h_r)
     att, d_att, h_l, h_r = _f32c(att, "att"), _f32c(d_att, "d_att"), _f32c(h_l, "attn_row"), _f32c(h_r, "attn_col")
     H = att.shape[1]
@@ -194,8 +218,13 @@ def gat_attn_bwd_raw(st: CSRStructure, att, d_att, h_l, h_r, slope):
         d_edge = torch.empty_like(att)
         g_row = torch.empty((st.n_rows, H), dtype=torch.float32, device=dev)
         plan, keep = st.plan_struct(_es_scratch(st, H))
-        _cabi.call("cogdl_b200_gat_attn_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(att), _ptr(d_att), _ptr(h_l),
-                   _ptr(h_r), float(slope), _ptr(d_edge), _ptr(g_row), st.n_rows, H, plan, _stream(dev))
+        if drop_scale is None:
+            _cabi.call("cogdl_b200_gat_attn_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(att), _ptr(d_att),
+                       _ptr(h_l), _ptr(h_r), float(slope), _ptr(d_edge), _ptr(g_row), st.n_rows, H, plan, _stream(dev))
+        else:
+            _cabi.call("cogdl_b200_gat_attn_bwd_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(att), _ptr(d_att),
+                       _ptr(h_l), _ptr(h_r), float(slope), float(drop_scale), _ptr(d_edge), _ptr(g_row), st.n_rows,
+                       H, plan, _stream(dev))
         del keep
     return d_edge, g_row
 

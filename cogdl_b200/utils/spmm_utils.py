@@ -4,6 +4,7 @@
     edge_softmax(graph, edge_val, csr_edge_softmax=None)                       :172
     mh_spmm(graph, attention, h, csrmhspmm=None, fast_spmm=None)               :201
     fused_gat_op(attn_row, attn_col, graph, negative_slope, in_feat, fused_gat_func=None)   :251
+      (plus attn_drop=0.0, seed=None: attention dropout inside the fused kernels)
     modules SpMM / EdgeSoftmax / MultiHeadSpMM / FusedGATOp, registry CONFIGS  :4-14
 
 Differences (deliberate):
@@ -150,11 +151,16 @@ class MultiHeadSpMM(torch.nn.Module):
         return mh_spmm(graph, attention, h, csrmhspmm=self.csrmhspmm, fast_spmm=self.spmm)
 
 
-def fused_gat_op(attn_row, attn_col, graph, negative_slope, in_feat, fused_gat_func=None):
+def fused_gat_op(attn_row, attn_col, graph, negative_slope, in_feat, fused_gat_func=None, attn_drop=0.0, seed=None):
+    """attn_drop (0 <= attn_drop < 1): dropout on the attention, drawn inside the kernels; apply it when training
+    only.  seed: the mask's 64-bit seed (None: drawn from torch's CPU generator, a fresh mask per call)."""
     if fused_gat_func is not None and fused_gat_func is not CONFIGS["fused_gat_func"]:
+        if attn_drop:
+            raise ValueError("attention dropout needs this package's fused GAT operator, not a custom fused_gat_func")
         rp, ci = graph.row_indptr.int(), graph.col_indices.int()
         return fused_gat_func(attn_row, attn_col, rp, ci, rp, ci, negative_slope, in_feat)
-    return FusedGATFunction.apply(attn_row, attn_col, _structure(graph), None, None, None, negative_slope, in_feat)
+    return FusedGATFunction.apply(attn_row, attn_col, _structure(graph), None, None, None, negative_slope, in_feat,
+                                  attn_drop, seed)
 
 
 class FusedGATOp(torch.nn.Module):

@@ -296,6 +296,31 @@ COGDL_B200_API int cogdl_b200_edge_colsum_f32(const int32_t *colptr, const int32
                                int64_t n_cols, int64_t H, const cogdl_b200_hub_plan_t *plan /* of the transpose; scratch n_chunks*H*4 B */,
                                cogdl_b200_stream_t stream);
 
+/* GAT with attention dropout (the nn.Dropout between edge_softmax and mh_spmm in cogdl/layers/gat_layer.py:73-77).
+ * Mask: (CSR edge position p, head h) is KEPT iff cogdl_b200_sample_draw(seed, p, h) >= drop_below, with
+ * drop_below = floor(p_drop * 2^64) (0 keeps everything); a kept attention is multiplied by scale = 1 / (1 - p_drop)
+ * (finite and > 0, else COGDL_B200_EINVAL).  p_drop = 1 has no kernel.
+ * att_out receives the softmax with the SIGN BIT SET on the dropped entries (-a; the softmax is >= 0, and a dropped
+ * softmax that underflowed to 0 is -0.0): one [nnz,H] tensor carries both the attention and the mask, and the
+ * backward needs no seed.  The other arguments are those of cogdl_b200_gat_fwd_f32; with drop_below = 0 and
+ * scale = 1 the results are bit-identical to it. */
+COGDL_B200_API int cogdl_b200_gat_fwd_dropout_f32(const int32_t *rowptr, const int32_t *colind, const float *h_l,
+                                   const float *h_r, const float *feat, float negative_slope, uint64_t seed,
+                                   uint64_t drop_below, float scale, float *out, float *att_out, int64_t n_rows,
+                                   int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+/* cogdl_b200_mhspmm_f32 over such a signed attention: an entry with the sign bit set counts as 0, the others as
+ * att * scale.  With perm (the cached transpose) it is d feat of the dropout GAT. */
+COGDL_B200_API int cogdl_b200_mhspmm_dropout_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
+                                  const float *att, const float *feat, float scale, float *out, int64_t n_rows,
+                                  int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+/* cogdl_b200_gat_attn_bwd_f32 over such a signed attention; d_att = mhsddmm(d out, feat) is the gradient of the
+ * dropped, scaled attention: the softmax backward runs on |att| with d_att * scale on the kept entries, 0 on the
+ * dropped ones. */
+COGDL_B200_API int cogdl_b200_gat_attn_bwd_dropout_f32(const int32_t *rowptr, const int32_t *colind, const float *att,
+                                        const float *d_att, const float *h_l, const float *h_r, float negative_slope,
+                                        float scale, float *d_edge, float *g_row, int64_t n_rows, int64_t H,
+                                        const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * Fused GCN layer (SURVEY 8f-3): OUT = act( (A.X).W^T + (A.1) b^T ), A = (rowptr, colind, val).
  * Equal to the reference layer  act( A.(X.W^T + 1 b^T) )  (cogdl/layers/gcn_layer.py:51-64, bias inside the
