@@ -401,6 +401,7 @@ extern "C" int cogdl_b200_scatter_max_bwd_f32(const float *g, const int32_t *arg
   const int64_t total = n_rows * F;
   int64_t blocks = ceil_div(total, 256);
   if (blocks > NUM_SMS * 32) blocks = NUM_SMS * 32;
+  note_kernel("cogdl_b200::scatter_max_bwd_kernel");
   scatter_max_bwd_kernel<<<(unsigned)blocks, 256, 0, s>>>(g, argmax, gx, total, (int)F);
   CB_LAUNCH_CHECK();
   return COGDL_B200_OK;

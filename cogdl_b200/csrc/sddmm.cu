@@ -215,7 +215,9 @@ static int launch_sddmm_stream(const SddmmParams &p, cudaStream_t stream) {
   const int64_t blocks = ceil_div(warps * 32, 256);
   if (blocks == 0) return COGDL_B200_OK;
   if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "sddmm: problem too large for one launch");
-  sddmm_stream_kernel<NV, (NV == 1 ? 4 : 2)><<<(unsigned)blocks, 256, 0, stream>>>(p);
+  constexpr int U = NV == 1 ? 4 : 2;
+  note_kernel("cogdl_b200::sddmm_stream_kernel<NV=%d,U=%d>", NV, U);
+  sddmm_stream_kernel<NV, U><<<(unsigned)blocks, 256, 0, stream>>>(p);
   CB_LAUNCH_CHECK();
   return COGDL_B200_OK;
 }
@@ -228,6 +230,7 @@ static int launch_sddmm(const SddmmParams &p, cudaStream_t stream) {
   if (blocks == 0 || ytiles == 0) return COGDL_B200_OK;
   if (blocks > 0x7fffffffLL || ytiles > 65535)
     return set_error(COGDL_B200_EINVAL, "sddmm: problem too large for one launch");
+  note_kernel("cogdl_b200::sddmm_kernel<%s,GROUP=%d,SUB=%d,NV=%d>", sizeof(VecT) == 16 ? "float4" : "float", GROUP, SUB, NV);
   sddmm_kernel<VecT, GROUP, SUB, NV><<<dim3((unsigned)blocks, (unsigned)ytiles), 256, 0, stream>>>(p);
   CB_LAUNCH_CHECK();
   return COGDL_B200_OK;

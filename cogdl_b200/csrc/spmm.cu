@@ -469,6 +469,7 @@ extern "C" int cogdl_b200_spmm_csr_f16(const int32_t *rowptr, const int32_t *col
   CB_REQUIRE(blocks <= 0x7fffffffLL, "cogdl_b200_spmm_csr_f16: problem too large");
   dim3 grid((unsigned)blocks);
   cudaStream_t s = (cudaStream_t)stream;
+  note_kernel("cogdl_b200::spmm_half_kernel<%s,%s>", val ? "weighted" : "unweighted", vec ? "vec" : "scalar");
   if (vec) {
     if (val) spmm_half_kernel<true, true><<<grid, 256, 0, s>>>(p);
     else spmm_half_kernel<false, true><<<grid, 256, 0, s>>>(p);

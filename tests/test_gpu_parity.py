@@ -46,7 +46,7 @@ def T(a, dev):
 
 # ------------------------------------------------------------------------------------ SpMM
 @pytest.mark.parametrize("name", list(CASES))
-@pytest.mark.parametrize("F", [128, 16, 40, 7, 256, 1, 64, 33, 300])
+@pytest.mark.parametrize("F", [128, 16, 40, 7, 256, 1, 64, 33, 300, 9, 17, 65, 1433])
 @pytest.mark.parametrize("weighted", [True, False])
 def test_spmm_matches_oracle(dev, name, F, weighted):
     from cogdl_b200.operators._raw import spmm_raw
@@ -287,7 +287,7 @@ def test_mhspmm_transpose_with_fused_perm(dev):
 
 # ------------------------------------------------------------------------------------ scatter_max
 @pytest.mark.parametrize("name", ["tiny", "ragged", "hub", "two_hubs", "rect", "empty_graph"])
-@pytest.mark.parametrize("F", [256, 128, 16, 7, 40])
+@pytest.mark.parametrize("F", [256, 128, 16, 7, 40, 1, 3, 9, 17, 33])
 def test_scatter_max_fwd_bwd(dev, name, F):
     from cogdl_b200.operators._raw import scatter_max_fwd_raw, scatter_max_bwd_raw
 
