@@ -175,10 +175,18 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
 // the row-end test is made once per batch on the ballot mask: ~15 instructions per edge.  Same accumulation
 // order and rounding as stream_range (CSR order, separate fp32 multiply and add) => still bit-identical to
 // the reference CPU loop on unsplit rows.  PF: the next slab's indices are loaded while this slab's gathers are
-// in flight (4 more registers; the panel form's narrow gathers leave room for them).
+// in flight (3 more registers; the panel form's narrow gathers leave room for them).
+//
+// Row ends (ROWS).  The panel form (PF) finds them from rowptr: a row cursor r (the first row of the segment
+// [r, r_end) whose end lies past the slab start) is kept in a register, lane k reads rowptr[r + k + 1], and every
+// non-empty row whose end falls inside the slab sets its bit of the row-end mask.  That is one 128-byte line per slab,
+// mostly re-read by the next slab, instead of edge_row's 4 bytes per edge (plus the neighbour's) in every pass.  The
+// one-pass form keeps the edge_row test (`row != row of the next edge`, one ballot): there the cursor's longer
+// dependent chain per slab costs more than the bytes it saves (SpMM F=40 +2 %, DESIGN 3.1).
 template <typename VecT, int MODE, int SRC, int U, bool ROWS, bool PF = false>
-__device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, const int e_end, const int cv, const bool colok,
-                                                  const int lane, int2 *s_cv, int *s_r, VecT &acc) {
+__device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, const int e_end, int r, const int r_end,
+                                                  const int cv, const bool colok, const int lane, int2 *s_cv, int *s_r,
+                                                  VecT &acc) {
   const VecT *X0 = reinterpret_cast<const VecT *>(p.X0) + cv;
   const VecT *X1 = reinterpret_cast<const VecT *>(p.X1) + cv;
   VecT *Y = reinterpret_cast<VecT *>(p.Y) + cv;
@@ -191,42 +199,59 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
   auto accumulate = [&](float vj, const VecT &x) {
     if (MODE == MODE_UNWEIGHTED) add_rn(acc, x); else axpy_rn(acc, vj, x);
   };
-  auto load_slab = [&](int base, int &c, float &v, int &rid, int &rnx) {
+  constexpr bool CURSOR = ROWS && PF;               // row ends from rowptr; otherwise (ROWS) from edge_row
+  // column, value and (CURSOR) the end of row r + lane; INT_MAX past the segment's last row
+  auto load_slab = [&](int base, int &c, float &v, int &end) {
     const int q = base + lane;
-    c = 0; v = 0.f; rid = -1; rnx = -1;
+    c = 0; v = 0.f; end = INT_MAX;
     if (q < e_end) {
       c = ld_stream(p.colind + q);
       if (MODE == MODE_WEIGHTED) v = ld_stream(p.val + q);
-      if (ROWS) {
-        rid = ld_stream(p.hub.edge_row + q);
-        if (q + 1 < e_end) rnx = __ldg(p.hub.edge_row + q + 1);
-      }
+    }
+    if (CURSOR && base < e_end && r + lane < r_end) end = ld_stream(p.rowptr + r + lane + 1);
+  };
+  // Row-end mask of the slab [base, base + 32) from `end` (as load_slab left it), s_r[t] = the row whose last edge
+  // is base + t, and r moved past every row that ends inside the slab.  A row is empty iff its end equals the end
+  // of the row before; rows ending at or before base (empty rows at the segment's start) set no bit.  More than 32
+  // rows can end inside one slab only through empty rows: then the next 32 are read.
+  auto row_ends = [&](int base, int end) {
+    unsigned mask = 0u;
+    int end_before = base;
+    for (;;) {
+      int before = __shfl_up_sync(FULL, end, 1);
+      if (lane == 0) before = end_before;
+      const bool inside = end <= base + 32;
+      const bool last_edge = inside && end > before;
+      if (last_edge) s_r[end - 1 - base] = r + lane;
+      mask |= __reduce_or_sync(FULL, last_edge ? 1u << (end - 1 - base) : 0u);
+      const unsigned done = __ballot_sync(FULL, inside);   // a prefix of the lanes: ends do not decrease
+      r += __popc(done);
+      if (done != FULL) return mask;
+      end_before = __shfl_sync(FULL, end, 31);
+      end = r + lane < r_end ? ld_stream(p.rowptr + r + lane + 1) : INT_MAX;
     }
   };
-  int pc = 0, prid = -1, prnx = -1;                 // PF: the slab loaded one iteration ahead
+  int pc = 0, pend = INT_MAX;                       // PF: the slab loaded one iteration ahead
   float pv = 0.f;
-  if (PF) load_slab(e, pc, pv, prid, prnx);
+  if (PF) load_slab(e, pc, pv, pend);
   for (; e < e_end; e += 32) {
     const int cnt = min(32, e_end - e);
     const int q = e + lane;
-    int c = 0, rid = -1, rnx = -1;
-    float v = 0.f;
-    if (PF) {
-      c = pc; v = pv; rid = prid; rnx = prnx;
-    } else if (q < e_end) {
-      c = ld_stream(p.colind + q);
-      if (MODE == MODE_WEIGHTED) v = ld_stream(p.val + q);
-      if (ROWS) {
-        rid = ld_stream(p.hub.edge_row + q);
-        if (q + 1 < e_end) rnx = __ldg(p.hub.edge_row + q + 1);
-      }
+    int c, end, rid = -1, rnx = -1;
+    float v;
+    if (PF) { c = pc; v = pv; end = pend; }
+    else load_slab(e, c, v, end);
+    if (ROWS && !CURSOR && q < e_end) {
+      rid = ld_stream(p.hub.edge_row + q);
+      if (q + 1 < e_end) rnx = __ldg(p.hub.edge_row + q + 1);
     }
-    const unsigned endmask = ROWS ? __ballot_sync(FULL, lane < cnt && rid != rnx) : 0u;
+    unsigned endmask = ROWS && !CURSOR ? __ballot_sync(FULL, lane < cnt && rid != rnx) : 0u;
     __syncwarp();                                   // everybody is done reading the previous slab
     s_cv[lane] = make_int2(c, __float_as_int(v));
-    if (ROWS) s_r[lane] = rid;
+    if (CURSOR) endmask = row_ends(e, end);
+    else if (ROWS) s_r[lane] = rid;
     __syncwarp();
-    if (PF) load_slab(e + 32, pc, pv, prid, prnx);  // consumed by the next iteration only
+    if (PF) load_slab(e + 32, pc, pv, pend);        // consumed by the next iteration only (r is already past this slab)
     int j = 0;
 #pragma unroll 1
     for (; j + U <= cnt; j += U) {                  // full batches: no per-edge predicates
@@ -299,7 +324,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
 #pragma unroll
       for (int k = 0; k < NV; ++k) { colok[k] = (cv + k * 32) < p.ldv; acc[k] = vzero<VecT>(); }
       const int head = (MODE == MODE_MULTIHEAD && colok[0]) ? cv / p.FVL : 0;
-      if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false, PANEL && PREFETCH>(p, w.lb, w.hb, cv, colok[0], lane, s_cv, s_r, acc[0]);
+      if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, false, PANEL && PREFETCH>(p, w.lb, w.hb, 0, 0, cv, colok[0], lane, s_cv, s_r, acc[0]);
       else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, false, PREFETCH, DROP>(p, w.lb, w.hb, cv, colok, head, lane, acc);
 #pragma unroll
       for (int k = 0; k < NV; ++k)
@@ -357,7 +382,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
         }
       }
     }
-    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH>(p, e_begin, e_end, cv, colok[0], lane, s_cv, s_r, acc[0]);
+    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH>(p, e_begin, e_end, rr.x, rr.y, cv, colok[0], lane, s_cv, s_r, acc[0]);
     else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, DROP>(p, e_begin, e_end, cv, colok, head, lane, acc);
   }
 }
