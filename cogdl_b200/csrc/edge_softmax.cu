@@ -49,6 +49,8 @@
 
 #include <math_constants.h>
 
+#include <cfloat>
+#include <cstdio>
 #include <cstdlib>
 
 namespace cogdl_b200 {
@@ -510,8 +512,10 @@ __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
         } else {
           // online max / sum (one pass, one exp per element: e = exp(-|x - m|) is the rescale factor of the running
           // sum when x is a new maximum and the new term otherwise), then one normalising pass: 2 LDS + 1 STS and
-          // 2 MUFU per element instead of 3 LDS + 2 STS -- the kernel is issue-bound
-          float mx = -CUDART_INF_F, sm = 0.f;
+          // 2 MUFU per element instead of 3 LDS + 2 STS -- the kernel is issue-bound.  The running max starts at
+          // -FLT_MAX, not -inf: a leading -inf logit then gives d = -inf and e = 0 instead of -inf - -inf = NaN, and
+          // a (row, head) whose logits are all -inf still ends in 0 * (1 / 0) = NaN, as the softmax does.
+          float mx = -FLT_MAX, sm = 0.f;
           for (int k = k0; k < k1; ++k) {
             const float x = T[k * H + h];
             const float d = x - mx;
@@ -672,8 +676,13 @@ static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t
     CB_LAUNCH_CHECK();
   }
   const int chosen = cap_need <= 512 ? 512 : (cap_need <= 1024 ? 1024 : 2048);   // smallest tile (floats per warp) that fits
-  note_kernel("cogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d%s>%s", MODE, chosen, ES_WARPS, drop_note,
-              (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
+  // both launches, in launch order, when the statistics kernel ran
+  char stats_note[64] = "";
+  if (p.hub.n_chunks > 0)
+    snprintf(stats_note, sizeof(stats_note), "cogdl_b200::es_stats_kernel<MODE=%d%s> + ", MODE,
+             (DROP && MODE == 3) ? ",DROP" : "");
+  note_kernel("%scogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d%s>%s", stats_note, MODE, chosen, ES_WARPS,
+              drop_note, (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
   if (chosen == 512) return launch_main<MODE, 512, DROP>(p, s);
   if (chosen == 1024) return launch_main<MODE, 1024, DROP>(p, s);
   return launch_main<MODE, 2048, DROP>(p, s);

@@ -17,6 +17,8 @@
 #include "common.cuh"
 #include "stream.cuh"
 
+#include <cstdio>
+
 namespace cogdl_b200 {
 
 struct MhParams {
@@ -248,7 +250,14 @@ static int gat_fwd(const int32_t *rowptr, const int32_t *colind, const float *h_
   rc = gat_attention(rowptr, colind, h_l, h_r, negative_slope, att_out, n_rows, H, plan, (cudaStream_t)stream, drop,
                      seed, drop_below);
   if (rc) return rc;
-  return mhspmm_run(rowptr, colind, nullptr, att_out, feat, out, n_rows, H, F, plan, stream, drop ? scale : 0.f);
+  // cogdl_b200_last_kernel() names both stages: "<attention> + <aggregation>" (each note is under 128 bytes)
+  char att_note[128], agg_note[128];
+  snprintf(att_note, sizeof(att_note), "%s", cogdl_b200_last_kernel());
+  rc = mhspmm_run(rowptr, colind, nullptr, att_out, feat, out, n_rows, H, F, plan, stream, drop ? scale : 0.f);
+  if (rc) return rc;
+  snprintf(agg_note, sizeof(agg_note), "%s", cogdl_b200_last_kernel());
+  note_kernel("%s + %s", att_note, agg_note);
+  return COGDL_B200_OK;
 }
 
 extern "C" int cogdl_b200_gat_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *h_l,

@@ -1,9 +1,10 @@
-"""One row per dispatch branch of the gather kernels in spmm.cu, sddmm.cu, mhspmm.cu and scatter_max.cu.
+"""One row per dispatch branch of the gather kernels in spmm.cu, sddmm.cu, mhspmm.cu and scatter_max.cu, and of the
+edge softmax and GAT attention kernels in edge_softmax.cu.
 
 Each row names the inputs that select a kernel instantiation (op, graph, width, alignment, plan form, weights,
 perm, dropout, source form) and the exact cogdl_b200_last_kernel() string the call must record.  The GPU test
 (test_gpu_dispatch.py) runs every row and checks the output against a reference; the CPU test
-(test_cpu_kernel_inventory.py) checks that the rows cover every kernel compiled into those four objects, and
+(test_cpu_kernel_inventory.py) checks that the rows cover every kernel compiled into those five objects, and
 that every kernel named here is compiled.  Plain Python, no torch: the CPU test imports it without a GPU.
 """
 from dataclasses import dataclass
@@ -14,29 +15,36 @@ STREAM_BLOCK = 128
 
 @dataclass(frozen=True)
 class Case:
-    op: str                 # spmm | spmm_f16 | sddmm | mhspmm | scatter_max | scatter_max_bwd
-    graph: str              # a name in tests/graphs.py CASES
+    op: str                 # spmm | spmm_f16 | sddmm | mhspmm | scatter_max | scatter_max_bwd | edge_softmax |
+                            # edge_softmax_bwd | gat_fwd | gat_attn_bwd
+    graph: str              # a name in tests/graphs.py CASES, or "bounds": boundary_csr(chunk)
     F: int                  # features per head
     kernel: str             # exact cogdl_b200_last_kernel() after the call
     H: int = 1              # heads (sddmm: H > 1 calls the multi-head SDDMM)
-    aligned: bool = True    # False: the feature input is a view one element past an aligned allocation
+    aligned: bool = True    # False: the feature input (edge_softmax: the logits; the backwards: g) is a view one
+                            # element past an aligned allocation
     plan: str = "default"   # none (no hub plan) | chunks (hub chunks, seg_cost 0) | default (chunks + segments)
     chunk: int = 64         # hub chunk edges of the plan
     weighted: bool = True   # spmm / spmm_f16: edge values, or the unweighted form
     perm: bool = False      # mhspmm: the transposed pass with the attention permutation fused
     drop: bool = False      # mhspmm: attention carrying a dropout mask in its sign bit (cogdl_b200_mhspmm_dropout_f32)
+                            # gat_fwd / gat_attn_bwd: the attention-dropout entry points
     src: str = "one"        # spmm: one | two (cogdl_b200_spmm_csr_f32_2src) | peers (cogdl_b200_spmm_csr_f32_peers)
     panels: int = 0         # spmm: column panels of X (0: chosen by the library)
     partials_offset: int = 0  # bytes the plan's partial scratch starts past a 16-byte boundary
+    masked: bool = False    # edge_softmax: -inf logits (leading, middle and trailing in a row, a whole first hub chunk,
+                            # a (row, head) of nothing but -inf)
 
     @property
     def id(self):
         s = f"{self.op}-{self.graph}-H{self.H}F{self.F}-{self.plan}"
+        if self.op in ES_OPS:
+            s += f"-C{self.chunk}"
         if self.op in ("spmm", "spmm_f16"):
             s += "-w" if self.weighted else "-u"
         if not self.aligned:
             s += "-misaligned"
-        for flag in ("perm", "drop"):
+        for flag in ("perm", "drop", "masked"):
             if getattr(self, flag):
                 s += "-" + flag
         if self.src != "one":
@@ -265,7 +273,96 @@ SCATTER_MAX = [
     Case("scatter_max_bwd", "two_hubs", 33, SMAX_BWD),
 ]
 
-TABLE = SPMM + SPMM_F16 + SDDMM + MHSPMM + SCATTER_MAX
+# ------------------------------------------------------------------ edge softmax and the GAT attention (edge_softmax.cu)
+# cogdl_b200_edge_softmax_fwd_f32 (MODE 0) / _bwd_f32 (MODE 1), the attention of cogdl_b200_gat_fwd_f32 /
+# _dropout_f32 (MODE 2, followed by the multi-head SpMM) and cogdl_b200_gat_attn_bwd_f32 / _dropout_f32 (MODE 3).
+# With a plan that has segments and chunk_edges * H <= 2048 the main kernel runs with the smallest tile of 512, 1024
+# or 2048 floats that holds chunk_edges * H, after the statistics kernel when the graph has hub rows; otherwise a warp
+# per row.  Head counts that are not a power of two <= 32 take the generic kernel.
+ES_OPS = ("edge_softmax", "edge_softmax_bwd", "gat_fwd", "gat_attn_bwd")
+ES_WARPS = 8
+
+
+def es_main(mode, cap, drop=False, bulk=False, stats=True):
+    """Main kernel, staged by cp.async.bulk (bulk) or coalesced loads, preceded by the statistics kernel (stats), whose
+    forward attention runs without the dropout flag."""
+    s = f"cogdl_b200::es_main_kernel<MODE={mode},CAP={cap},WARPS={ES_WARPS}{',DROP' if drop else ''}>"
+    s += " cp.async.bulk tiles" if bulk else ""
+    if stats:
+        s = f"cogdl_b200::es_stats_kernel<MODE={mode}{',DROP' if drop and mode == 3 else ''}> + " + s
+    return s
+
+
+def es_warp(mode, drop=False):
+    return f"cogdl_b200::es_warp_kernel<MODE={mode}{',DROP' if drop else ''}>"
+
+
+def es_generic(mode, drop=False):
+    return f"cogdl_b200::es_generic_kernel<MODE={mode}{',DROP' if drop else ''}>"
+
+
+def gat_k(attention, aggregation):
+    return f"{attention} + {aggregation}"
+
+
+def _es_rows(op, mode):
+    """edge_softmax (MODE 0) or edge_softmax_bwd (MODE 1): the forward's logits carry -inf masks."""
+    m = mode == 0
+    C = lambda graph, kernel, **kw: Case(op, graph, 0, kernel, masked=m, **kw)  # noqa: E731
+    return [
+        C("bounds", es_main(mode, 512, bulk=True), H=8, chunk=64),
+        C("bounds", es_main(mode, 512), H=8, chunk=64, aligned=False),
+        C("bounds", es_main(mode, 1024, bulk=True), H=4, chunk=256),
+        C("bounds", es_main(mode, 2048, bulk=True), H=32, chunk=64),
+        C("bounds", es_main(mode, 2048), H=1, chunk=2048),              # H % 4 != 0: coalesced staging
+        C("bounds", es_warp(mode), H=16, chunk=256),                    # 4096 floats: no tile holds a chunk
+        C("bounds", es_warp(mode), H=8, chunk=64, plan="none"),
+        C("bounds", es_generic(mode), H=3, chunk=64),
+        C("bounds", es_generic(mode), H=6, chunk=64),
+        C("bounds", es_generic(mode), H=64, chunk=64),                  # a power of two above 32
+        C("ragged", es_main(mode, 512, bulk=True, stats=False), H=8, chunk=64),     # no hub rows
+        # 512-float tiles on a graph with a 700-edge hub, without masks
+        Case(op, "two_hubs", 0, es_main(mode, 512, bulk=True), H=8, chunk=64),
+        Case(op, "two_hubs", 0, es_main(mode, 512, bulk=True), H=4, chunk=64),
+    ]
+
+
+EDGE_SOFTMAX = _es_rows("edge_softmax", 0) + _es_rows("edge_softmax_bwd", 1)
+
+GAT_FWD = []
+GAT_ATTN_BWD = []
+for _d in (False, True):
+    _S = lambda vec: mh_stream_k(vec, False, _d)  # noqa: E731
+    _M = lambda vec, group: mh_k(vec, group, False, _d)  # noqa: E731
+    _G = lambda graph, F, att, agg, **kw: Case("gat_fwd", graph, F, gat_k(att, agg), drop=_d, **kw)  # noqa: E731
+    GAT_FWD += [
+        _G("bounds", 16, es_main(2, 512, _d), _S("float4"), H=8, chunk=64),
+        _G("bounds", 32, es_main(2, 1024, _d), _S("float4"), H=4, chunk=256),
+        _G("bounds", 4, es_main(2, 2048, _d), _S("float4"), H=32, chunk=64),
+        _G("bounds", 8, es_main(2, 2048, _d), _M("float4", 2), H=1, chunk=2048),
+        _G("bounds", 8, es_warp(2, _d), _S("float4"), H=16, chunk=256),
+        _G("bounds", 16, es_warp(2, _d), _M("float4", 32), H=8, chunk=64, plan="none"),
+        _G("bounds", 5, es_generic(2, _d), _M("float", 16), H=3, chunk=64),
+        _G("bounds", 4, es_generic(2, _d), _M("float4", 8), H=6, chunk=64),
+        _G("bounds", 4, es_generic(2, _d), _S("float4"), H=64, chunk=64),
+        _G("ragged", 16, es_main(2, 512, _d, stats=False), _S("float4"), H=8, chunk=64),
+    ]
+    _B = lambda graph, kernel, **kw: Case("gat_attn_bwd", graph, 0, kernel, drop=_d, **kw)  # noqa: E731
+    GAT_ATTN_BWD += [
+        _B("bounds", es_main(3, 512, _d, bulk=True), H=8, chunk=64),
+        _B("bounds", es_main(3, 512, _d), H=8, chunk=64, aligned=False),
+        _B("bounds", es_main(3, 1024, _d, bulk=True), H=4, chunk=256),
+        _B("bounds", es_main(3, 2048, _d, bulk=True), H=32, chunk=64),
+        _B("bounds", es_main(3, 2048, _d), H=1, chunk=2048),
+        _B("bounds", es_warp(3, _d), H=16, chunk=256),
+        _B("bounds", es_warp(3, _d), H=8, chunk=64, plan="none"),
+        _B("bounds", es_generic(3, _d), H=3, chunk=64),
+        _B("bounds", es_generic(3, _d), H=6, chunk=64),
+        _B("bounds", es_generic(3, _d), H=64, chunk=64),
+        _B("ragged", es_main(3, 512, _d, bulk=True, stats=False), H=8, chunk=64),
+    ]
+
+TABLE = SPMM + SPMM_F16 + SDDMM + MHSPMM + SCATTER_MAX + EDGE_SOFTMAX + GAT_FWD + GAT_ATTN_BWD
 
 # Compiled instantiations no public entry point above reaches: launched only by the fused layers' hub-row pre-pass.
 EXEMPT = {

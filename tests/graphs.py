@@ -36,3 +36,26 @@ def case(name, seed=0):
     rp, ci = random_csr(n, e, seed=seed, **kw)
     n_cols = kw.get("n_cols", n)
     return rp, ci, n_cols
+
+
+def boundary_csr(C, seed=0):
+    """Square CSR whose rows sit on the boundaries of a hub plan with C-edge chunks (not in CASES: the parity tests
+    parametrised over CASES do not grow).  Returns (rowptr, colind, n_cols) like case().
+
+    Rows, in order (a hub row ends a run of short rows, so the runs after hubs start fresh windows):
+      0, 1, C - 1, C       the largest non-hub row fills a tile exactly when C * H is the tile size
+      C + 1                a hub whose last chunk has one edge
+      40 x 1               a full 32-row window of one-edge rows and a remainder of 8
+      2C                   a hub of full chunks
+      9, 7, 6, 4, 3, 2, 1  descending degrees in one window: the degree sort reverses them
+      129 C + 5            a hub of 130 chunks: at H = 1 the statistics merge loop (128 chunks a pass) runs twice
+      2, 0, 0, 0, 1, 3     empty rows inside a run of short rows
+      then C, 2, C - 1, 5, 0 and 40 random degrees in [0, min(C, 16))."""
+    rng = np.random.default_rng(seed)
+    deg = [0, 1, C - 1, C, C + 1] + [1] * 40 + [2 * C, 9, 7, 6, 4, 3, 2, 1, 129 * C + 5, 2, 0, 0, 0, 1, 3]
+    deg += [C, 2, C - 1, 5, 0] + list(rng.integers(0, min(C, 16), 40))
+    n = len(deg)
+    rowptr = np.zeros(n + 1, np.int32)
+    rowptr[1:] = np.cumsum(deg)
+    colind = rng.integers(0, n, int(rowptr[-1])).astype(np.int32)
+    return rowptr, colind, n

@@ -1,4 +1,5 @@
-"""Every gather kernel compiled into spmm.o, sddmm.o, mhspmm.o and scatter_max.o has a row in the dispatch table
+"""Every gather kernel compiled into spmm.o, sddmm.o, mhspmm.o and scatter_max.o, and every edge-softmax / GAT attention
+kernel compiled into edge_softmax.o, has a row in the dispatch table
 (tests/dispatch_table.py) that the GPU suite runs and checks, and every kernel the table names is compiled.  A new
 dispatch branch without a test case fails here, on a machine without a GPU.
 
@@ -11,11 +12,11 @@ import subprocess
 
 import pytest
 
-from tests.dispatch_table import EXEMPT, TABLE
+from tests.dispatch_table import ES_OPS, EXEMPT, TABLE
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBJ_DIR = os.path.join(ROOT, "cogdl_b200", "csrc", "build")
-OBJECTS = ("spmm", "sddmm", "mhspmm", "scatter_max")
+OBJECTS = ("spmm", "sddmm", "mhspmm", "scatter_max", "edge_softmax")
 
 
 def _tool(name):
@@ -26,7 +27,7 @@ def _tool(name):
 
 
 def compiled_kernels():
-    """Demangled kernel entry points (global functions) of the four objects."""
+    """Demangled kernel entry points (global functions) of the objects."""
     cuobjdump, cufilt = _tool("cuobjdump"), _tool("cu++filt")
     if not cuobjdump or not cufilt:
         pytest.skip("cuobjdump / cu++filt from the CUDA toolkit are not available")
@@ -94,13 +95,26 @@ def note_of(sym):
         return f"cogdl_b200::scatter_max_stream_kernel<NV={nv},U={u}{'' if argmax else ',values_only'}>"
     if name == "scatter_max_bwd_kernel":
         return "cogdl_b200::scatter_max_bwd_kernel"
+    if name == "es_main_kernel":
+        mode, cap, warps, drop = a
+        return f"cogdl_b200::es_main_kernel<MODE={mode},CAP={cap},WARPS={warps}{',DROP' if drop else ''}>"
+    if name in ("es_stats_kernel", "es_warp_kernel", "es_generic_kernel"):
+        mode, drop = a
+        return f"cogdl_b200::{name}<MODE={mode}{',DROP' if drop else ''}>"
     raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
 
 
 def canonical(note):
-    """A recorded name without its launch-shape suffixes: the panel count becomes ',panels' (the instantiation is
-    the same for every count) and ' block=N' goes."""
-    return re.sub(r",panels=\d+", ",panels", re.sub(r" block=\d+$", "", note))
+    """The instantiations a recorded name lists, without their launch-shape suffixes.  A note of several launches
+    ('a + b': the edge-softmax statistics and main kernels, the GAT attention and aggregation) is split; the panel count
+    becomes ',panels' (the instantiation is the same for every count), ' block=N' and the staging note
+    ' cp.async.bulk tiles' go."""
+    out = []
+    for part in note.split(" + "):
+        part = re.sub(r" block=\d+$", "", part)
+        part = re.sub(r" cp\.async\.bulk tiles$", "", part)
+        out.append(re.sub(r",panels=\d+", ",panels", part))
+    return out
 
 
 def test_note_of_maps_known_symbols():
@@ -110,14 +124,21 @@ def test_note_of_maps_known_symbols():
                    "(bool)1, (bool)0>(cogdl_b200::StreamParams)") == \
         "cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"
     assert canonical("cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels=4 block=128") \
-        == "cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"
+        == ["cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"]
+    assert note_of("void cogdl_b200::es_main_kernel<(int)3, (int)512, (int)8, (bool)1>(cogdl_b200::EsParams)") == \
+        "cogdl_b200::es_main_kernel<MODE=3,CAP=512,WARPS=8,DROP>"
+    assert note_of("void cogdl_b200::es_stats_kernel<(int)2, (bool)0>(cogdl_b200::EsParams)") == \
+        "cogdl_b200::es_stats_kernel<MODE=2>"
+    assert canonical("cogdl_b200::es_stats_kernel<MODE=0> + cogdl_b200::es_main_kernel<MODE=0,CAP=512,WARPS=8> "
+                     "cp.async.bulk tiles") == ["cogdl_b200::es_stats_kernel<MODE=0>",
+                                                "cogdl_b200::es_main_kernel<MODE=0,CAP=512,WARPS=8>"]
 
 
 def test_table_covers_every_compiled_kernel():
     compiled = {}
     for sym in compiled_kernels():
         compiled.setdefault(note_of(sym), sym)
-    table = {canonical(c.kernel) for c in TABLE}
+    table = {k for c in TABLE for k in canonical(c.kernel)}
     untested = sorted(set(compiled) - table - set(EXEMPT))
     assert not untested, "compiled kernels without a row in tests/dispatch_table.py:\n" + "\n".join(
         f"  {n}   ({compiled[n]})" for n in untested)
@@ -131,3 +152,84 @@ def test_table_rows_are_distinct():
     ids = [c.id for c in TABLE]
     dup = sorted({i for i in ids if ids.count(i) > 1})
     assert not dup, f"duplicate table rows: {dup}"
+
+
+def test_recorded_names_fit_the_note_buffer():
+    """cogdl_b200_last_kernel() is kept in a 256-byte buffer: the longest name the table expects (a GAT forward:
+    statistics + main kernel of the attention, then the row-stream aggregation) must fit whole."""
+    longest = max(TABLE, key=lambda c: len(c.kernel.encode()))
+    assert len(longest.kernel.encode()) < 256, longest.kernel
+
+
+_ES_OP = {0: "edge_softmax", 1: "edge_softmax_bwd", 2: "gat_fwd", 3: "gat_attn_bwd"}
+
+
+def es_form(c):
+    """The launch form of an edge-softmax row: op, dropout, the attention part of the recorded name (statistics kernel
+    or not, cp.async.bulk or coalesced staging), and what else decides how the kernel runs: for the main kernel the
+    graph (boundary degrees or a random power-law graph), one head or several, and whether a chunk fills the tile
+    exactly; how a warp-kernel row got there (no plan, or no tile holds a chunk); a generic row's head count."""
+    att = c.kernel.split(" + cogdl_b200::stream_kernel")[0].split(" + cogdl_b200::mhspmm_kernel")[0]
+    if "es_main_kernel" in att:
+        cap = int(re.search(r"CAP=(\d+)", att).group(1))
+        detail = (c.graph == "bounds", c.H == 1, c.chunk * c.H == cap)
+    elif "es_warp_kernel" in att:
+        detail = c.plan
+    else:
+        detail = c.H
+    return (c.op, c.drop, att, detail)
+
+
+def required_es_forms():
+    """Every launch form es_launch can take with the compiled instantiations, on the boundary-degree graph unless
+    said otherwise: the main kernel after the statistics kernel at every tile, with several heads filling it exactly
+    and with bulk staging where the mode allows it; at the 2048-float tile also one head (coalesced staging: rows are
+    4 bytes apart); at the 512-float tile coalesced staging of a misaligned operand, no hub rows (a random graph),
+    and for the edge softmax the random graph with a 700-edge hub with the tile filled and half filled; the warp
+    kernel without a plan and when no tile holds a chunk; the generic kernel at 3 and 6 heads and at 64 (a power of
+    two above 32)."""
+    forms = set()
+    for sym in compiled_kernels():
+        m = re.fullmatch(r"(?:void )?cogdl_b200::(es_\w+)<(.*)>\(.*\)", sym)
+        if not m:
+            continue
+        name, a = m.group(1), _args("<" + m.group(2) + ">")
+        mode, drop = a[0], a[-1]
+        op = _ES_OP[mode]
+        dn = ",DROP" if drop else ""
+        if name == "es_main_kernel":
+            cap, warps = a[1], a[2]
+            main = f"cogdl_b200::es_main_kernel<MODE={mode},CAP={cap},WARPS={warps}{dn}>"
+            st = f"cogdl_b200::es_stats_kernel<MODE={mode}{dn if mode == 3 else ''}> + "
+            bulk = " cp.async.bulk tiles" if mode != 2 else ""
+            forms.add((op, drop, st + main + bulk, (True, False, True)))
+            if cap == 2048:
+                forms.add((op, drop, st + main, (True, True, True)))
+            if cap == 512:
+                forms.add((op, drop, main + bulk, (False, False, True)))
+                if mode != 2:
+                    forms.add((op, drop, st + main, (True, False, True)))
+                if mode in (0, 1):
+                    forms.add((op, drop, st + main + bulk, (False, False, True)))
+                    forms.add((op, drop, st + main + bulk, (False, False, False)))
+        elif name == "es_warp_kernel":
+            for route in ("none", "default"):
+                forms.add((op, drop, f"cogdl_b200::es_warp_kernel<MODE={mode}{dn}>", route))
+        elif name == "es_generic_kernel":
+            for H in (3, 6, 64):
+                forms.add((op, drop, f"cogdl_b200::es_generic_kernel<MODE={mode}{dn}>", H))
+    return forms
+
+
+def test_edge_softmax_rows_cover_every_launch_form():
+    """Every launch form has a row and every row is the only one of its form, so removing any edge-softmax row fails
+    here."""
+    rows = [es_form(c) for c in TABLE if c.op in ES_OPS]
+    required = required_es_forms()
+    missing = sorted(required - set(rows), key=str)
+    assert not missing, "edge-softmax launch forms without a row in tests/dispatch_table.py:\n" + "\n".join(
+        f"  {f}" for f in missing)
+    extra = sorted(set(rows) - required, key=str)
+    assert not extra, f"rows in launch forms the compiled kernels do not have: {extra}"
+    dup = sorted({f for f in rows if rows.count(f) > 1}, key=str)
+    assert not dup, f"several rows of one launch form: {dup}"

@@ -1,6 +1,6 @@
-"""Every dispatch branch of the SpMM (fp32 and fp16), SDDMM, multi-head SpMM and scatter_max entry points, one
-row of tests/dispatch_table.py each: the call must record exactly the kernel the row names, and its output must
-match a reference.
+"""Every dispatch branch of the SpMM (fp32 and fp16), SDDMM, multi-head SpMM, scatter_max, edge softmax and GAT
+attention entry points, one row of tests/dispatch_table.py each: the call must record exactly the kernel the row
+names, and its output must match a reference.
 
 - fp32 SpMM: rows the hub plan does not split are bit-identical to the oracle (CSR order, separate fp32 multiply
   and add); every element is within the fp64 bound below.
@@ -11,6 +11,25 @@ match a reference.
 - fp16 SpMM: fp64 over the fp16-rounded inputs, bound 2^-11 |ref| + deg * 2^-24 * sum|v x| + 2^-24 (one fp16
   rounding of the output plus the fp32 accumulation), with outputs in the fp16 subnormal range and a row whose
   terms cancel exactly.
+- Edge softmax forward and the GAT attention, per element against the fp64 softmax of the fp32 logits (for the
+  attention, leakyrelu(h_l[row] + h_r[col]) formed in fp32 as the kernels do: an IEEE add, then the product with the
+  slope).  With t = x - m, T the row's largest finite |t| and d the degree:
+
+      |y - y64| <= y64 ((d + 3) 2^-22 + d 2^-24 + (2|t| + 2T) 2^-23) + 2^-126
+
+  An exp evaluated as MUFU.EX2 of fl(fl(x - m) * log2 e) is off by 2 ulp plus about 1.17 |t| ulp from the argument's
+  two roundings (2^-22 + 1.7 |t| 2^-23 relative): once in the numerator, and in every rescale of the running sum by
+  exp(m_old - m_new), which are at most d per row and whose arguments add up to at most T.  The terms of the sum carry
+  the same relative error (their exp(-|t|) |t| is at most 1/e), the fp32 sum of d terms d 2^-24, the reciprocal and
+  the product two more roundings.  MUFU.EX2 flushes results below 2^-126 to zero, hence the absolute term.  NaN
+  positions (a (row, head) of nothing but -inf logits) must equal the reference's; a -inf logit in any other row gives
+  exactly 0.  With dropout, the sign bits of the attention must equal the keep rule's mask bit for bit.
+- Edge softmax backward and the GAT attention backward: y (g - sum_row y g) dact, dact the LeakyReLU derivative at
+  the fp32 pre-activation (the slope at exactly 0), per element within (d + 3) 2^-24 dact y (|g| + sum_row |y g|)
+  (the fp32 dot product of d terms, then the subtraction and two products); the row sums g_row within the row sum of
+  those bounds plus d 2^-24 sum_row |d_edge|.  With dropout, y = |att| and g = d_att * scale rounded to fp32 on the
+  kept entries and 0 on the dropped ones, as the kernels read them.
+- Every row with hub chunks leaves the plan's arrival counters at zero.
 """
 import ctypes
 
@@ -21,7 +40,7 @@ import torch
 
 import oracle
 from tests.dispatch_table import TABLE
-from tests.graphs import case
+from tests.graphs import boundary_csr, case
 
 pytestmark = pytest.mark.gpu
 
@@ -283,8 +302,188 @@ def run_scatter_max(dev, c):
         assert st.plan.n_chunks > 0 and int(st.plan.counters.abs().sum()) == 0
 
 
+# ------------------------------------------------------------------------------------------ edge softmax, GAT attention
+SLOPE = np.float32(0.2)
+P_DROP = 0.4
+
+
+def es_graph(c):
+    return boundary_csr(c.chunk) if c.graph == "bounds" else case(c.graph)
+
+
+def es_logits(rp, H, rng, masked=False, chunk=0):
+    """[nnz, H] fp32 logits: even rows uniform over [-90, 0] (exp of the smallest is below 2^-126, where MUFU.EX2
+    flushes to zero), odd rows N(0, 4).  masked: per row a leading, middle or trailing -inf in one head, the whole first
+    chunk of the largest hub in head 0, and every logit of a 3-edge row and (H > 1) of the 2 * chunk hub in head H - 1."""
+    n, deg = rp.shape[0] - 1, np.diff(rp)
+    rows = np.repeat(np.arange(n), deg)
+    x = np.where((rows % 2 == 0)[:, None], rng.uniform(-90, 0, (rows.size, H)), rng.standard_normal((rows.size, H)) * 2)
+    x = x.astype(np.float32)
+    if masked:
+        for r in np.nonzero(deg >= 2)[0]:
+            x[rp[r] + (0, deg[r] // 2, deg[r] - 1)[r % 3], (r // 3) % H] = -np.inf
+        big = int(np.argmax(deg))
+        if chunk and deg[big] > chunk:
+            x[rp[big]:rp[big] + chunk, 0] = -np.inf
+        full = np.nonzero(deg == 3)[0][:1].tolist() + (np.nonzero(deg == 2 * chunk)[0][:1].tolist() if H > 1 else [])
+        for r in full:
+            x[rp[r]:rp[r + 1], H - 1] = -np.inf
+    return x
+
+
+def softmax64(rp, x):
+    """fp64 softmax of fp32 logits over each row's edges, per head, with what its error bound needs: (y, |t|, T, d) per
+    element, t = x - row max (0 where x is -inf), T the row's largest |t|, d the row's degree.  A (row, head) of
+    nothing but -inf gives NaN."""
+    n, deg = rp.shape[0] - 1, np.diff(rp)
+    rows = np.repeat(np.arange(n), deg)
+    x64 = x.astype(np.float64)
+    m = np.full((n, x.shape[1]), -np.inf)
+    np.maximum.at(m, rows, x64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        t = x64 - m[rows]
+        ex = np.exp(t)
+        s = np.zeros_like(m)
+        np.add.at(s, rows, ex)
+        y = ex / s[rows]
+    t = np.where(np.isfinite(t), np.abs(t), 0.0)
+    T = np.zeros_like(m)
+    np.maximum.at(T, rows, t)
+    return y, t, T[rows], deg[rows][:, None].astype(np.float64)
+
+
+def check_softmax(got, x, rp, what):
+    """got against the fp64 softmax of the fp32 logits x: NaN exactly where the reference is NaN, every other element
+    within the forward bound of the module docstring."""
+    y, t, T, d = softmax64(rp, x)
+    nan = np.isnan(y)
+    assert np.array_equal(np.isnan(got), nan), (f"{what}: NaN at {np.argwhere(np.isnan(got) != nan)[:4].tolist()}, "
+                                                f"{int(np.isnan(got).sum())} NaN, reference {int(nan.sum())}")
+    bound = y * ((d + 3) * 2.0 ** -22 + d * U32 + (2 * t + 2 * T) * 2.0 ** -23) + 2.0 ** -126
+    assert_within(np.where(nan, 0, got), np.where(nan, 0, y), np.where(nan, 1, bound), what)
+
+
+def softmax_bwd64(rp, y, g, dact):
+    """fp64 y * (g - sum_row y * g) * dact from the fp32 y, g the kernel reads, with the per-element bound
+    (d + 3) 2^-24 dact y (|g| + sum_row |y g|) and the row sums with theirs."""
+    n, deg = rp.shape[0] - 1, np.diff(rp)
+    rows = np.repeat(np.arange(n), deg)
+    y64, g64 = y.astype(np.float64), g.astype(np.float64)
+    s, mag = np.zeros((n, y.shape[1])), np.zeros((n, y.shape[1]))
+    np.add.at(s, rows, y64 * g64)
+    np.add.at(mag, rows, np.abs(y64 * g64))
+    out = y64 * (g64 - s[rows]) * dact
+    bound = (deg[rows][:, None] + 3) * U32 * dact * y64 * (np.abs(g64) + mag[rows]) + TINY
+    grow, gmag, gbound = np.zeros_like(s), np.zeros_like(s), np.zeros_like(s)
+    np.add.at(grow, rows, out)
+    np.add.at(gmag, rows, np.abs(out))
+    np.add.at(gbound, rows, bound)
+    return out, bound, grow, gbound + deg[:, None] * U32 * gmag + TINY
+
+
+def check_counters(c, st):
+    if c.plan != "none" and st.plan.n_chunks > 0:
+        assert int(st.plan.counters.abs().sum()) == 0, f"{c.id}: arrival counters not back at zero"
+
+
+def run_edge_softmax(dev, c):
+    from cogdl_b200.operators._raw import edge_softmax_bwd_raw, edge_softmax_fwd_raw
+
+    rp, ci, n_cols = es_graph(c)
+    rng = np.random.default_rng(600 + c.H * 10 + c.chunk)
+    x = es_logits(rp, c.H, rng, c.masked, c.chunk)
+    st = structure(rp, ci, n_cols, dev, c)
+    if c.op == "edge_softmax":
+        got = edge_softmax_fwd_raw(st, T(x, dev) if c.aligned else misaligned(T(x, dev)))
+        check_kernel(c)
+        check_softmax(got.cpu().numpy(), x, rp, c.id)
+    else:
+        y = softmax64(rp, x)[0].astype(np.float32)
+        g = rng.standard_normal(y.shape).astype(np.float32)
+        got = edge_softmax_bwd_raw(st, T(y, dev), T(g, dev) if c.aligned else misaligned(T(g, dev)))
+        check_kernel(c)
+        ref, bound, _, _ = softmax_bwd64(rp, y, g, 1.0)
+        assert_within(got.cpu().numpy(), ref, bound, c.id)
+    check_counters(c, st)
+
+
+def gat_logits32(rp, ci, hl, hr):
+    """leakyrelu(h_l[row] + h_r[col]) as the kernels form it: an IEEE fp32 add, then the fp32 product with the slope."""
+    rows = np.repeat(np.arange(rp.shape[0] - 1), np.diff(rp))
+    z = hl[rows] + hr[ci]
+    return z, np.where(z > 0, z, z * SLOPE).astype(np.float32)
+
+
+def run_gat_fwd(dev, c):
+    from cogdl_b200.operators._raw import gat_fwd_raw
+    from tests.gat_dropout_ref import drop_below, keep_mask
+
+    rp, ci, n = es_graph(c)
+    rng = np.random.default_rng(700 + c.H * 10 + c.chunk)
+    hl = rng.standard_normal((n, c.H)).astype(np.float32)
+    hr = rng.uniform(-20, 90, (n, c.H)).astype(np.float32)          # logits spread over ~90 in a row
+    feat = rng.standard_normal((n, c.H, c.F)).astype(np.float32)
+    st = structure(rp, ci, n, dev, c)
+    scale = np.float32(1.0 / (1.0 - P_DROP))
+    seed = 0x5EED + c.H
+    drop = (seed, drop_below(P_DROP), float(scale)) if c.drop else None
+    out, att = gat_fwd_raw(st, T(hl, dev), T(hr, dev), T(feat, dev), float(SLOPE), True, drop=drop)
+    check_kernel(c)
+    att = att.cpu().numpy()
+    check_softmax(np.abs(att), gat_logits32(rp, ci, hl, hr)[1], rp, f"{c.id} attention")
+    eff = att
+    if c.drop:
+        keep = keep_mask(seed, ci.size, c.H, P_DROP)
+        assert np.array_equal(np.signbit(att), ~keep), f"{c.id}: the sign bits are not the dropout mask"
+        eff = np.where(keep, np.abs(att) * scale, np.float32(0)).astype(np.float32)
+    else:
+        assert not np.signbit(att).any()
+    # the aggregation over the attention the kernel wrote (the multi-head SpMM bound)
+    got, deg = out.cpu().numpy(), np.diff(rp)[:, None]
+    for h in range(c.H):
+        A = csr64(rp, ci, eff[:, h], n)
+        f64 = feat[:, h, :].astype(np.float64)
+        assert_within(got[:, h, :], A @ f64, deg * U32 * (abs(A) @ np.abs(f64)) + TINY, f"{c.id} head {h}")
+    check_counters(c, st)
+
+
+def run_gat_attn_bwd(dev, c):
+    from cogdl_b200.operators._raw import gat_attn_bwd_raw
+    from tests.gat_dropout_ref import keep_mask
+
+    rp, ci, n = es_graph(c)
+    rng = np.random.default_rng(800 + c.H * 10 + c.chunk)
+    att = softmax64(rp, es_logits(rp, c.H, rng))[0].astype(np.float32)
+    d_att = rng.standard_normal(att.shape).astype(np.float32)
+    hl = rng.standard_normal((n, c.H)).astype(np.float32)
+    hr = rng.standard_normal((n, c.H)).astype(np.float32)
+    # the first edge of every row gets a pre-activation of exactly +0.0: LeakyReLU'(0) is the slope (z > 0 is the test)
+    first = rp[:-1][np.diff(rp) > 0]
+    hl[np.diff(rp) > 0] = -hr[ci[first]]
+    z = gat_logits32(rp, ci, hl, hr)[0]
+    assert np.all(z[first] == 0)
+    dact = np.where(z > 0, 1.0, np.float64(SLOPE))
+    st = structure(rp, ci, n, dev, c)
+    y, g, ds = att, d_att, None
+    if c.drop:
+        scale = np.float32(1.0 / (1.0 - P_DROP))
+        keep = keep_mask(0xD0 + c.H, ci.size, c.H, P_DROP)
+        att = np.where(keep, att, -att).astype(np.float32)            # the dropped entries carry the sign bit
+        g = np.where(keep, d_att * scale, np.float32(0)).astype(np.float32)
+        ds = float(scale)
+    gd = T(d_att, dev)
+    d_edge, g_row = gat_attn_bwd_raw(st, T(att, dev), gd if c.aligned else misaligned(gd), T(hl, dev), T(hr, dev),
+                                     float(SLOPE), drop_scale=ds)
+    check_kernel(c)
+    ref, bound, grow, gbound = softmax_bwd64(rp, y, g, dact)
+    assert_within(d_edge.cpu().numpy(), ref, bound, f"{c.id} d_edge")
+    assert_within(g_row.cpu().numpy(), grow, gbound, f"{c.id} g_row")
+    check_counters(c, st)
+
+
 RUN = {"spmm": run_spmm, "spmm_f16": run_spmm_f16, "sddmm": run_sddmm, "mhspmm": run_mhspmm,
-       "scatter_max": run_scatter_max, "scatter_max_bwd": run_scatter_max}
+       "scatter_max": run_scatter_max, "scatter_max_bwd": run_scatter_max, "edge_softmax": run_edge_softmax,
+       "edge_softmax_bwd": run_edge_softmax, "gat_fwd": run_gat_fwd, "gat_attn_bwd": run_gat_attn_bwd}
 
 
 @pytest.mark.parametrize("c", TABLE, ids=lambda c: c.id)

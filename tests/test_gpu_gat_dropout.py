@@ -214,20 +214,26 @@ def test_eval_and_p0_are_bit_identical_to_the_plain_fused_op(dev):
     assert torch.equal(ya, yb)
 
 
-def test_kernel_names_carry_the_dropout_flag(dev):
+def test_kernel_names_list_every_launch_with_the_dropout_flag(dev):
+    """The attention backward names the statistics kernel and the main kernel it launched, the GAT forward its
+    attention launches and then the aggregation; each instantiation carries the dropout flag."""
     from cogdl_b200 import _cabi
     from cogdl_b200.operators._raw import gat_attn_bwd_raw, gat_fwd_raw, mhsddmm_raw
 
     rp, ci, n, h_l, h_r, feat = inputs("hub", 8, 128, dev)
     st = structure(rp, ci, n, dev, 256)
     _, att = gat_fwd_raw(st, h_l, h_r, feat, 0.2, True, drop=drop_args(1, 0.5))
-    assert "multihead" in _cabi.last_kernel() and "+drop" in _cabi.last_kernel()
+    assert _cabi.last_kernel() == ("cogdl_b200::es_stats_kernel<MODE=2> + cogdl_b200::es_main_kernel<MODE=2,CAP=2048,WARPS=8,DROP>"
+                                   " + cogdl_b200::stream_kernel<float4,NV=1,multihead+drop,SRC_ONE,U=8,MINB=3,prefetch>"
+                                   " block=128")
     d_att = mhsddmm_raw(st, torch.randn(n, 8, 128, device=dev), feat)
     gat_attn_bwd_raw(st, att, d_att, h_l, h_r, 0.2, drop_scale=2.0)
-    assert _cabi.last_kernel().startswith("cogdl_b200::es_main_kernel<MODE=3,CAP=2048,WARPS=8,DROP>")
+    assert _cabi.last_kernel() == ("cogdl_b200::es_stats_kernel<MODE=3,DROP> + "
+                                   "cogdl_b200::es_main_kernel<MODE=3,CAP=2048,WARPS=8,DROP> cp.async.bulk tiles")
     rp1, ci1, n1, hl1, hr1, f1 = inputs("hub", 1, 8, dev)
     gat_fwd_raw(structure(rp1, ci1, n1, dev, 256), hl1, hr1, f1, 0.2, True, drop=drop_args(1, 0.5))
-    assert _cabi.last_kernel() == "cogdl_b200::mhspmm_kernel<float4,GROUP=2,no_perm,drop>"
+    assert _cabi.last_kernel() == ("cogdl_b200::es_stats_kernel<MODE=2> + cogdl_b200::es_main_kernel<MODE=2,CAP=512,WARPS=8,DROP>"
+                                   " + cogdl_b200::mhspmm_kernel<float4,GROUP=2,no_perm,drop>")
 
 
 def test_bad_arguments_raise_the_library_error(dev):

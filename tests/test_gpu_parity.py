@@ -473,20 +473,3 @@ def test_sddmm_stream_and_row_forms_match_the_oracle(dev, name, H, F):
         assert rel(out, ref) <= TOL, f"chunk={chunk} seg_cost={seg_cost}"
         if chunk:
             assert int(st.plan.counters.abs().sum()) == 0
-
-
-@pytest.mark.parametrize("H", [8, 4])
-def test_edge_softmax_512_float_tiles_match_the_oracle(dev, H):
-    """64-edge hub chunks with H <= 8 take the 512-float-tile main kernel, forward and backward."""
-    from cogdl_b200.operators._raw import edge_softmax_bwd_raw, edge_softmax_fwd_raw
-
-    rp, ci, n_cols = case("two_hubs")
-    rng = np.random.default_rng(22)
-    e = T(np.clip(rng.standard_normal((ci.shape[0], H)) * 3, -10, 10).astype(np.float32), dev)
-    g = T(rng.standard_normal((ci.shape[0], H)).astype(np.float32), dev)
-    st = structure(rp, ci, n_cols, dev, chunk=64)
-    y = edge_softmax_fwd_raw(st, e)
-    b = edge_softmax_bwd_raw(st, y, g)
-    assert rel(y.cpu().numpy(), oracle.edge_softmax_fwd(rp, e.cpu().numpy())) <= TOL
-    assert rel(b.cpu().numpy(), oracle.edge_softmax_bwd(rp, y.cpu().numpy(), g.cpu().numpy())) <= TOL
-    assert int(st.plan.counters.abs().sum()) == 0
