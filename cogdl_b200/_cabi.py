@@ -113,6 +113,17 @@ SIGNATURES = {
                                                   _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "cogdl_b200_subgraph_count": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp]),
     "cogdl_b200_subgraph_fill": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "cogdl_b200_actnn_minmax_f32": (ctypes.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _vp]),
+    "cogdl_b200_actnn_pack_f32": (ctypes.c_int, [_vp, _i64, _i64, _i32, _vp, _i32, _vp, _i32, ctypes.c_uint64, _vp, _vp,
+                                                 _vp, _vp]),
+    "cogdl_b200_actnn_unpack_f32": (ctypes.c_int, [_vp, _i64, _i64, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "cogdl_b200_actnn_relu_fwd_f32": (ctypes.c_int, [_vp, _i64, _vp, _vp, _vp]),
+    "cogdl_b200_actnn_relu_bwd_f32": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp]),
+    "cogdl_b200_actnn_dropout_fwd_f32": (ctypes.c_int, [_vp, _i64, _f32, ctypes.c_uint64, ctypes.c_uint64, _vp, _vp,
+                                                        _vp]),
+    "cogdl_b200_actnn_dropout_bwd_f32": (ctypes.c_int, [_vp, _vp, _i64, _f32, _vp, _vp]),
+    "cogdl_b200_actnn_bits_scratch_bytes": (_i64, [_i64]),
+    "cogdl_b200_actnn_bits": (ctypes.c_int, [_vp, _i64, _i32, _i64, _vp, _vp, _i64, _vp]),
 }
 
 _lib = None

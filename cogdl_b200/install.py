@@ -25,6 +25,8 @@ gat=True rebinds `cogdl.layers.gat_layer.GATLayer.forward` (GAT and every model 
 sends the attention, its dropout and the aggregation to the fused GAT kernels (uninstall_gat()).
 spspmm=True provides torch_sparse's spspmm / spmm (cogdl_b200.spspmm / coo_spmm) to GTN, SRGCN and Graph U-Net, through a
 `torch_sparse` stand-in module when the real package is missing (install_spspmm, uninstall_spspmm()).
+actnn=True provides the `actnn` API (cogdl_b200.actnn) to ActGCN, GCNII(actnn=True), GraphSAGE(actnn=True) and the trainer's
+--actnn, through an `actnn` stand-in package when the real one does not import (install_actnn, uninstall_actnn()).
 """
 import sys
 
@@ -242,7 +244,61 @@ def uninstall_spspmm():
     _spspmm_state["stub"] = None
 
 
-def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False):
+_ACTNN_SUBMODULES = ("conf", "ops", "qscheme", "qbnscheme", "layers", "utils")
+_ACTNN_NAMES = {"cogdl.operators.linear": ("quantize_activation", "dequantize_activation", "config", "empty_cache"),
+                "cogdl.operators.spmm": ("quantize_activation", "dequantize_activation")}
+_actnn_state = {"stub": None, "rebound": []}
+
+
+def install_actnn():
+    """The `actnn` API for CogDL's activation-compressed models.  Without an importable actnn, cogdl_b200.actnn and its
+    submodules go into sys.modules as `actnn` and `actnn.<name>`, so the models' imports resolve to them; an importable
+    actnn is left alone.  cogdl.operators.linear imports actnn inside a try at import time: if it was imported before,
+    its names are bound here."""
+    from . import actnn as stub
+
+    patched = []
+    if _actnn_state["stub"] is None and "actnn" not in sys.modules:
+        try:
+            import actnn  # noqa: F401
+        except (ImportError, OSError):   # missing, or a binary build that does not load
+            sys.modules["actnn"] = stub
+            for name in _ACTNN_SUBMODULES:
+                sys.modules["actnn." + name] = getattr(stub, name)
+            _actnn_state["stub"] = stub
+            patched.append("actnn")
+    actnn_mod = sys.modules["actnn"]
+    for mname, attrs in _ACTNN_NAMES.items():
+        mod = sys.modules.get(mname)
+        if mod is None:
+            continue
+        for attr in attrs:
+            src = actnn_mod.conf if attr == "config" else (actnn_mod.utils if attr == "empty_cache" else actnn_mod.ops)
+            new, old = getattr(src, attr), getattr(mod, attr, None)
+            if old is not new:
+                _actnn_state["rebound"].append((mod, attr, old))
+                setattr(mod, attr, new)
+                patched.append(f"{mname}.{attr}")
+    return patched
+
+
+def uninstall_actnn():
+    """Undo install_actnn: restore the bound names and take the actnn stand-in out of sys.modules (modules imported
+    while it was there keep their binding)."""
+    for mod, attr, old in reversed(_actnn_state["rebound"]):
+        if old is None:
+            delattr(mod, attr)
+        else:
+            setattr(mod, attr, old)
+    _actnn_state["rebound"] = []
+    if _actnn_state["stub"] is not None:
+        for name in ("actnn",) + tuple("actnn." + n for n in _ACTNN_SUBMODULES):
+            if sys.modules.get(name) is not None and getattr(sys.modules[name], "__name__", "").startswith("cogdl_b200."):
+                del sys.modules[name]
+    _actnn_state["stub"] = None
+
+
+def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -332,4 +388,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_spspmm()
     if gat:
         patched += install_gat()
+    if actnn:
+        patched += install_actnn()
     return patched

@@ -46,9 +46,52 @@ class SPMMFunction(torch.autograd.Function):
         return None, None, grad_feat, grad_w, None
 
 
+class ActSPMMFunction(torch.autograd.Function):
+    """SPMMFunction with an activation-compressed feature (the reference's ActSPMMFunction, spmm.py:89-133): when the
+    edge weights require grad, feat is saved quantized (cogdl_b200.actnn.ops.quantize_activation, no scheme) and
+    dequantized for the SDDMM weight gradient; otherwise nothing of feat is saved and it is SPMMFunction."""
+
+    @staticmethod
+    def forward(ctx, rowptr, colind, feat, edge_weight_csr=None, sym=False):
+        from ..actnn.ops import quantize_activation
+
+        st = _as_structure(rowptr, colind, feat.shape[0])
+        out = spmm_raw(st, edge_weight_csr, feat)
+        ctx.st, ctx.sym = st, bool(sym)
+        ctx.has_w = edge_weight_csr is not None
+        ctx.quantized = None
+        if ctx.has_w and edge_weight_csr.requires_grad:
+            ctx.quantized, ctx.feat_shape = quantize_activation(feat, None), feat.shape
+        ctx.save_for_backward(edge_weight_csr if ctx.has_w else None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from ..actnn.ops import dequantize_activation
+
+        (w,) = ctx.saved_tensors
+        feat = None
+        if ctx.quantized is not None:
+            feat = dequantize_activation(ctx.quantized, ctx.feat_shape)
+            ctx.quantized = None
+        st = ctx.st
+        grad_out = grad_out.contiguous()
+        grad_feat = grad_w = None
+        if ctx.needs_input_grad[2]:
+            if ctx.sym:
+                grad_feat = spmm_raw(st, w, grad_out)
+            else:
+                st_t, perm = st.csc()
+                w_t = None if w is None else gather_rows_raw(perm, w.detach().float())
+                grad_feat = spmm_raw(st_t, w_t, grad_out)
+        if feat is not None and ctx.needs_input_grad[3]:
+            grad_w = sddmm_raw(st, grad_out.float(), feat.float()).to(w.dtype)
+        return None, None, grad_feat, grad_w, None
+
+
 def csrspmm(rowptr, colind, x, csr_data, sym=False, actnn=False):
-    """Same signature as the reference.  `actnn` (activation-compressed training) is an optional
-    third-party back-end outside this path's scope (SURVEY 2.1): refuse rather than ignore."""
+    """Same signature as the reference.  actnn=True saves the features activation-compressed for the edge-weight
+    gradient (ActSPMMFunction); the output is the same as with actnn=False."""
     if actnn:
-        raise NotImplementedError("actnn=True is not supported by cogdl_b200 (ActNN is out of scope)")
+        return ActSPMMFunction.apply(rowptr, colind, x, csr_data, sym)
     return SPMMFunction.apply(rowptr, colind, x, csr_data, sym)

@@ -548,6 +548,44 @@ COGDL_B200_API int cogdl_b200_subgraph_fill(const int64_t *indptr, const int64_t
                              int64_t n_sub, int32_t *assoc, const int64_t *out_indptr, int64_t *out_indices,
                              int64_t *out_edges, cogdl_b200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Activation-compressed training (ActNN's activation quantization, third_party/actnn; actnn.cu has the rules).
+ *
+ * x: [N, D] fp32 row-major; D is zero-padded to Dp = ceil(D / group_size) * group_size, group_size 64 or 256,
+ * G = Dp / group_size groups per row.
+ * _minmax: mn, mx [N * G] fp32 = min / max of each padded group (the C of the bit allocation is built from them).
+ * _pack: codes of every padded element; scale_bf16 / mn_bf16 [N * G] bf16.  Bit widths: bits = NULL and
+ *   uniform_bits in {1, 2, 4, 8}, packed = N * Dp * uniform_bits / 8 bytes; or bits [N] int32 in 1..8 with
+ *   row_offsets [N] int64 = exclusive prefix sum of bits * Dp / 8, packed = sum(bits) * Dp / 8 bytes.
+ *   stochastic != 0 adds draw(seed, n * Dp + d, 0) noise (rng.cuh) before rounding; 0 rounds to nearest.
+ * _unpack: out [N, D] fp32 = code / scale + mn, same width arguments as the pack.
+ * Masks: uint32 [ceil(n / 32)] words, bit i % 32 of word i / 32 = element i.  The dropout keeps element i iff
+ *   draw(seed, i, 0) >= drop_below (= floor(p * 2^64)) and scales it by 1 / (1 - p); p in [0, 1).
+ * _bits: the reference greedy (calc_precision.cc, w = 1) on the device: bits [N] from initial_bits (1..8) down to at
+ *   least 1 until sum(bits) <= target.  C [N] fp32 must be finite and >= 0 (else EINVAL; one 4-byte status word is
+ *   read back, C is not).  N < 2^28; scratch >= cogdl_b200_actnn_bits_scratch_bytes(N) bytes of device memory.
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int cogdl_b200_actnn_minmax_f32(const float *x, int64_t N, int64_t D, int32_t group_size, float *mn,
+                                float *mx, cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_actnn_pack_f32(const float *x, int64_t N, int64_t D, int32_t group_size,
+                              const int32_t *bits, int32_t uniform_bits, const int64_t *row_offsets,
+                              int32_t stochastic, uint64_t seed, uint8_t *packed, void *scale_bf16, void *mn_bf16,
+                              cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_actnn_unpack_f32(const uint8_t *packed, int64_t N, int64_t D, int32_t group_size,
+                                const int32_t *bits, int32_t uniform_bits, const int64_t *row_offsets,
+                                const void *scale_bf16, const void *mn_bf16, float *out, cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_actnn_relu_fwd_f32(const float *x, int64_t n, float *y, uint32_t *mask,
+                                  cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_actnn_relu_bwd_f32(const float *g, const uint32_t *mask, int64_t n, float *gx,
+                                  cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_actnn_dropout_fwd_f32(const float *x, int64_t n, float p, uint64_t seed,
+                                     uint64_t drop_below, float *y, uint32_t *mask, cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_actnn_dropout_bwd_f32(const float *g, const uint32_t *mask, int64_t n, float p,
+                                     float *gx, cogdl_b200_stream_t stream);
+COGDL_B200_API int64_t cogdl_b200_actnn_bits_scratch_bytes(int64_t N);
+COGDL_B200_API int cogdl_b200_actnn_bits(const float *C, int64_t N, int32_t initial_bits, int64_t target,
+                          int32_t *bits, void *scratch, int64_t scratch_bytes, cogdl_b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
