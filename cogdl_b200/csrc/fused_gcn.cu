@@ -500,6 +500,10 @@ static int launch(const Params &p, cudaStream_t s) {
 
 using namespace cogdl_b200;
 
+// cogdl_b200_last_kernel() of a fused layer: with hub rows, the pre-pass kernel (recorded by its launcher), " + ", then
+// the fused kernel; without, the fused kernel alone
+#define FG_NOTE(prepass, fmt, ...) ((prepass) ? append_kernel_note(" + " fmt, __VA_ARGS__) : note_kernel(fmt, __VA_ARGS__))
+
 extern "C" int cogdl_b200_gcn_fused_supported(int64_t K, int64_t Fout) { return (K == fg::KDIM && Fout >= 1 && Fout <= 128) ? 1 : 0; }
 
 extern "C" int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X,
@@ -530,7 +534,8 @@ extern "C" int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t *co
   p.Npad = Fout <= fg::WG_N ? fg::WG_N : 2 * fg::WG_N; p.chunk_edges = plan->chunk_edges; p.relu = relu;
   p.n_tiles = (int)ceil_div(n_rows, fg::TILE_M);
   p.row_scale = nullptr; p.S = nullptr;
-  note_kernel("cogdl_b200::fg::fused_layer_kernel<gcn, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>", p.Npad);
+  FG_NOTE(plan->n_chunks > 0, "cogdl_b200::fg::fused_layer_kernel<gcn, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>",
+          p.Npad);
   return fg::launch<fg::AGG_SUM, fg::EPI_BIAS>(p, s);
 }
 
@@ -568,10 +573,12 @@ extern "C" int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_t *c
   p.n_tiles = (int)ceil_div(n_rows, fg::TILE_M);
   p.row_scale = row_scale; p.S = S;
   if (aggr == COGDL_B200_AGGR_MAX) {
-    note_kernel("cogdl_b200::fg::fused_layer_kernel<sage-max, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>", p.Npad);
+    FG_NOTE(plan->n_chunks > 0,
+            "cogdl_b200::fg::fused_layer_kernel<sage-max, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>", p.Npad);
     return fg::launch<fg::AGG_MAX, fg::EPI_SELF>(p, s);
   }
-  note_kernel("cogdl_b200::fg::fused_layer_kernel<sage-sum%s, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>",
-              row_scale ? "+row_scale" : "", p.Npad);
+  FG_NOTE(plan->n_chunks > 0,
+          "cogdl_b200::fg::fused_layer_kernel<sage-sum%s, 2 groups x tile 64x%d, K=128, bf16x3 split, wgmma m64n32k16>",
+          row_scale ? "+row_scale" : "", p.Npad);
   return fg::launch<fg::AGG_SUM, fg::EPI_SELF>(p, s);
 }

@@ -345,6 +345,7 @@ int smax_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float
   if (p.hub.n_chunks == 0) return COGDL_B200_OK;
   if (p.FV != 32) return set_error(COGDL_B200_EINVAL, "smax_hub_rows_only: F must be 128");
   const int64_t blocks = ceil_div((int64_t)p.hub.n_chunks * 32, 256);
+  note_kernel("cogdl_b200::scatter_max_stream_kernel<NV=1,U=4,values_only>");
   scatter_max_stream_kernel<1, 4, false><<<(unsigned)blocks, 256, 0, stream>>>(p);
   CB_LAUNCH_CHECK();
   return COGDL_B200_OK;

@@ -364,8 +364,196 @@ for _d in (False, True):
 
 TABLE = SPMM + SPMM_F16 + SDDMM + MHSPMM + SCATTER_MAX + EDGE_SOFTMAX + GAT_FWD + GAT_ATTN_BWD
 
-# Compiled instantiations no public entry point above reaches: launched only by the fused layers' hub-row pre-pass.
-EXEMPT = {
-    "cogdl_b200::scatter_max_stream_kernel<NV=1,U=4,values_only>":
-        "smax_hub_rows_only (fused SAGE max layer): tests/test_gpu_fused_sage.py",
+
+# ================================================================== message operators and the fused layers
+# GENConv's softmax aggregation (softmax_aggr.cu), DisenGCN's routing (disen_routing.cu), CompGCN's composition
+# aggregation (comp_aggr.cu) and the fused GCN / SAGE layers (fused_gcn.cu).  Run by test_gpu_dispatch_message.py.
+@dataclass(frozen=True)
+class MessageCase:
+    op: str                 # sa_fwd | sa_bwd | disen_fwd | disen_bwd | comp | fused_gcn | fused_sage_sum | fused_sage_max
+    graph: str              # "bounds": boundary_csr(chunk); "bounds_t": boundary_csc(chunk), whose transpose (walked by
+                            # the backwards) has the boundary degrees; else a name in tests/graphs.py CASES
+    F: int                  # features (fused layers: Fout; their input width is 128)
+    kernel: str             # exact cogdl_b200_last_kernel() after the call
+    plan: str = "chunks"    # none | chunks (hub chunks, no segments) | default (chunks + segments)
+    chunk: int = 64         # hub chunk edges of the plan (of the transpose's too)
+    aligned: bool = True    # False: the feature inputs are views one element past an aligned allocation
+    partials_offset: int = 0  # bytes the plan's partial scratch starts past a 16-byte boundary
+    # GENConv
+    beta: float = 1.0
+    edge_term: bool = False
+    want_q: bool = False
+    want_edge_grad: bool = True
+    # DisenGCN
+    K: int = 1              # channels (d = F / K)
+    tau: float = 1.0
+    want_saved: bool = True
+    zero_norm: bool = False  # one node's channel of c is NaN, as normalising a zero-norm channel gives
+    # CompGCN
+    comp: str = "mult"      # mult | sub | copy
+    T: int = 1              # edge types (rows of the relation table)
+    # fused layers
+    relu: bool = False
+    bias: bool = False
+    row_scale: bool = False
+    weighted: bool = True
+
+    @property
+    def id(self):
+        s = f"{self.op}-{self.graph}-F{self.F}-{self.plan}-C{self.chunk}"
+        if self.op.startswith("sa_"):
+            s += f"-beta{self.beta:g}" + ("-A" if self.edge_term else "") + ("-Q" if self.want_q else "")
+            s += "" if self.want_edge_grad else "-no_dA"
+        if self.op.startswith("disen"):
+            s += f"-K{self.K}-tau{self.tau:g}" + ("" if self.want_saved else "-unsaved") + ("-nan" if self.zero_norm else "")
+        if self.op == "comp":
+            s += f"-{self.comp}-T{self.T}"
+        if self.op.startswith("fused"):
+            s += ("-relu" if self.relu else "") + ("-bias" if self.bias else "") + ("-rs" if self.row_scale else "")
+            s += "-w" if self.weighted else "-u"
+        if not self.aligned:
+            s += "-misaligned"
+        if self.partials_offset:
+            s += f"-partials+{self.partials_offset}"
+        return s
+
+    @property
+    def vec(self):
+        """Vector width W of the kernel the row selects: 4 (float4) or 1."""
+        return 4 if "<float4" in self.kernel.split(" + ")[-1] else 1
+
+
+def sa_fwd_k(vec, edge_term, q):
+    return (f"cogdl_b200::softmax_aggr_fwd_kernel<{vec},{'edge_term' if edge_term else 'no_edge_term'},"
+            f"{'Q' if q else 'no_Q'}>")
+
+
+def sa_bwd_k(vec, edge_term):
+    return f"cogdl_b200::softmax_aggr_bwd_kernel<{vec},{'edge_term' if edge_term else 'no_edge_term'}>"
+
+
+def dr_fwd_k(vec, group):
+    return f"cogdl_b200::disen_route_fwd_kernel<{vec},GROUP={group}>"
+
+
+def dr_bwd_k(vec, group):
+    return (f"cogdl_b200::disen_route_bwd_row_kernel<{vec},GROUP={group}> + "
+            f"cogdl_b200::disen_route_bwd_col_kernel<{vec},GROUP={group}>")
+
+
+COMP_WHAT = {"mult": "comp_mult", "sub": "comp_sub", "copy": "weighted"}
+
+
+def comp_k(vec, nv, comp):
+    return stream_k(vec, nv, COMP_WHAT[comp], "SRC_ONE", 4 if nv == 1 else 2, 1, True)
+
+
+FUSED_AGG = {"fused_gcn": "gcn", "fused_sage_sum": "sage-sum", "fused_sage_max": "sage-max"}
+
+
+def fused_k(op, npad, hub, weighted=True, row_scale=False):
+    """The fused layer; with hub rows after its pre-pass (the SpMM's hub chunks, or scatter_max's without argmax)."""
+    s = (f"cogdl_b200::fg::fused_layer_kernel<{FUSED_AGG[op]}{'+row_scale' if row_scale else ''}, 2 groups x tile "
+         f"64x{npad}, K=128, bf16x3 split, wgmma m64n32k16>")
+    if not hub:
+        return s
+    pre = ("cogdl_b200::scatter_max_stream_kernel<NV=1,U=4,values_only>" if op == "fused_sage_max"
+           else stream_k("float4", 1, _w(weighted), "SRC_ONE", 4, 5, False))
+    return f"{pre} + {s}"
+
+
+# ------------------------------------------------------------------ GENConv: cogdl_b200_softmax_aggr_fwd_f32 / _bwd_f32
+# float4 iff F % 4 == 0 and every operand (the partial scratch too) is 16-byte aligned; a warp per row or hub chunk,
+# 32 vectors per pass.  Betas 0, 0.5, 4 and 20 spread over the rows.
+_SA = lambda F, kernel, beta, **kw: MessageCase("sa_fwd", "bounds", F, kernel, beta=beta, **kw)  # noqa: E731
+SOFTMAX_AGGR = [
+    _SA(64, sa_fwd_k("float4", False, False), 0.5),
+    _SA(32, sa_fwd_k("float4", False, True), 4.0, want_q=True),
+    _SA(128, sa_fwd_k("float4", True, False), 20.0, edge_term=True),          # 32 vectors: one full pass
+    _SA(16, sa_fwd_k("float4", True, True), 0.0, edge_term=True, want_q=True),
+    _SA(7, sa_fwd_k("float", False, False), 4.0),
+    _SA(1, sa_fwd_k("float", False, True), 20.0, want_q=True),
+    _SA(13, sa_fwd_k("float", True, False), 0.5, edge_term=True),
+    _SA(31, sa_fwd_k("float", True, True), 20.0, edge_term=True, want_q=True),
+    # more than 32 vectors per row: the pass loop runs 3 times, the last pass partial
+    _SA(264, sa_fwd_k("float4", True, True), 4.0, edge_term=True, want_q=True),
+    _SA(70, sa_fwd_k("float", True, True), 0.5, edge_term=True, want_q=True),
+    # no plan: every row (the 129 C + 5 hub too) is one warp's
+    _SA(128, sa_fwd_k("float4", False, False), 20.0, plan="none"),
+    _SA(33, sa_fwd_k("float", False, False), 4.0, plan="none"),
+    # a float4 width and aligned operands, but the partial scratch 4 bytes off: the scalar kernel
+    _SA(64, sa_fwd_k("float", True, True), 4.0, edge_term=True, want_q=True, partials_offset=4),
+]
+_SB = lambda F, kernel, beta, **kw: MessageCase("sa_bwd", "bounds_t", F, kernel, beta=beta, **kw)  # noqa: E731
+SOFTMAX_AGGR += [
+    _SB(64, sa_bwd_k("float4", False), 4.0),
+    _SB(128, sa_bwd_k("float4", True), 0.5, edge_term=True),
+    _SB(7, sa_bwd_k("float", False), 20.0),
+    _SB(33, sa_bwd_k("float", True), 0.0, edge_term=True),                     # two passes
+    _SB(32, sa_bwd_k("float4", True), 20.0, edge_term=True, want_edge_grad=False),   # dA == nullptr
+]
+
+# ------------------------------------------------------------------ DisenGCN: cogdl_b200_disen_route_fwd_f32 / _bwd_f32
+# F = K d; float4 iff d % 4 == 0 and the operands are aligned; GROUP = the row's vectors rounded up to a power of two,
+# at most 32 (wider rows loop over 32-vector tiles); L = d / W lanes per channel reduce its dot products.
+_DR_SHAPES = [   # (vec, GROUP, K, d, aligned, tau)
+    ("float4", 1, 1, 4, True, 1.0),
+    ("float4", 2, 2, 4, True, 0.1),
+    ("float4", 4, 1, 16, True, 5.0),
+    ("float4", 8, 4, 8, True, 1.0),
+    ("float4", 16, 2, 32, True, 0.1),
+    ("float4", 32, 8, 16, True, 5.0),
+    ("float", 1, 1, 1, True, 1.0),
+    ("float", 2, 1, 2, True, 0.1),
+    ("float", 4, 2, 2, True, 5.0),
+    ("float", 8, 8, 1, True, 1.0),
+    ("float", 16, 4, 4, False, 0.1),
+    ("float", 32, 8, 4, False, 5.0),
+]
+_DR_EXTRA = [    # GROUP = 32 with idle lanes (K = 3) and with several 32-vector tiles
+    ("float4", 32, 3, 32, True, 1.0),
+    ("float4", 32, 16, 32, True, 0.1),           # 128 vectors: four tiles
+    ("float", 32, 3, 8, False, 1.0),
+    ("float", 32, 2, 32, False, 5.0),            # 64 floats: two tiles
+]
+DISEN = []
+for _op, _k in (("disen_fwd", dr_fwd_k), ("disen_bwd", dr_bwd_k)):
+    for _vec, _g, _K, _d, _al, _tau in _DR_SHAPES + _DR_EXTRA:
+        DISEN.append(MessageCase(_op, "bounds" if _op == "disen_fwd" else "bounds_t", _K * _d, _k(_vec, _g), K=_K,
+                                 tau=_tau, aligned=_al))
+DISEN += [
+    MessageCase("disen_fwd", "bounds", 32, dr_fwd_k("float4", 8), K=4, tau=1.0, want_saved=False),
+    MessageCase("disen_fwd", "bounds", 64, dr_fwd_k("float4", 16), K=2, tau=0.1, zero_norm=True),
+]
+
+# ------------------------------------------------------------------ CompGCN: cogdl_b200_comp_aggr_f32
+# The row-stream kernel with a second gathered row: one vector per lane up to 32 vectors, two beyond (rows wider than
+# 64 vectors loop over column tiles).  "copy" is the weighted SpMM form at the composition's U and MINB.
+COMP = []
+for _comp in ("mult", "sub", "copy"):
+    for _vec, (_f1, _f2, _f3) in (("float4", (64, 200, 264)), ("float", (7, 50, 133))):
+        COMP += [
+            MessageCase("comp", "bounds", _f1, comp_k(_vec, 1, _comp), plan="default", comp=_comp, T=1),
+            MessageCase("comp", "bounds", _f2, comp_k(_vec, 2, _comp), plan="default", comp=_comp, T=300),
+            MessageCase("comp", "bounds", _f3, comp_k(_vec, 2, _comp), plan="default", comp=_comp, T=1),
+        ]
+
+# ------------------------------------------------------------------ fused layers: cogdl_b200_gcn_fused_f32 / _sage_fused_f32
+# 400 rows: 7 tiles of 64, the last one of 16 rows.  Fout <= 64 fills a 64-row W^T, Fout > 64 a 128-row one.  Chunk 64
+# makes hub rows (the pre-pass runs first); chunk 4096 leaves none.
+_FUSED_SHAPES = {   # op -> rows (Npad, hub, Fout, relu, bias, row_scale, weighted)
+    "fused_gcn": [(64, True, 33, True, True, False, True), (64, False, 1, False, False, False, False),
+                  (128, True, 128, False, True, False, True), (128, False, 65, True, False, False, False)],
+    "fused_sage_sum": [(64, True, 64, False, True, True, True), (64, False, 33, True, False, False, True),
+                       (128, True, 65, True, True, False, False), (128, False, 128, False, False, True, True)],
+    "fused_sage_max": [(64, True, 1, True, True, False, False), (64, False, 64, False, True, False, False),
+                       (128, True, 128, True, False, False, False), (128, False, 65, False, False, False, False)],
 }
+FUSED = [MessageCase(_op, "hub", _fo, fused_k(_op, _np, _hub, _wt, _rs), plan="default", chunk=64 if _hub else 4096,
+                     relu=_relu, bias=_b, row_scale=_rs, weighted=_wt)
+         for _op, _rows in _FUSED_SHAPES.items() for _np, _hub, _fo, _relu, _b, _rs, _wt in _rows]
+
+MESSAGE_TABLE = SOFTMAX_AGGR + DISEN + COMP + FUSED
+
+# Compiled instantiations no row above reaches (none: the fused layers record their hub pre-pass).
+EXEMPT = {}

@@ -59,3 +59,15 @@ def boundary_csr(C, seed=0):
     rowptr[1:] = np.cumsum(deg)
     colind = rng.integers(0, n, int(rowptr[-1])).astype(np.int32)
     return rowptr, colind, n
+
+
+def boundary_csc(C, seed=0):
+    """The transpose of boundary_csr(C), as a CSR: its COLUMNS have the boundary degrees, so a backward that walks the
+    transpose (under the transpose's own hub plan) meets them.  Its rows are the random columns of boundary_csr: the
+    129 C + 5 hub spreads over every row, so rows with more than C edges occur here too.  Returns (rowptr, colind, n)."""
+    rp, ci, n = boundary_csr(C, seed)
+    rows = np.repeat(np.arange(n), np.diff(rp))
+    order = np.lexsort((rows, ci))                   # by column, then row: CSR order of the transpose
+    rowptr = np.zeros(n + 1, np.int32)
+    rowptr[1:] = np.cumsum(np.bincount(ci, minlength=n))
+    return rowptr, rows[order].astype(np.int32), n

@@ -1,7 +1,12 @@
-"""Every gather kernel compiled into spmm.o, sddmm.o, mhspmm.o and scatter_max.o, and every edge-softmax / GAT attention
-kernel compiled into edge_softmax.o, has a row in the dispatch table
+"""Every gather kernel compiled into spmm.o, sddmm.o, mhspmm.o and scatter_max.o, every edge-softmax / GAT attention
+kernel compiled into edge_softmax.o, every message-operator kernel of softmax_aggr.o (GENConv), disen_routing.o
+(DisenGCN) and comp_aggr.o (CompGCN), and every fused layer of fused_gcn.o has a row in the dispatch table
 (tests/dispatch_table.py) that the GPU suite runs and checks, and every kernel the table names is compiled.  A new
 dispatch branch without a test case fails here, on a machine without a GPU.
+
+Objects left out on purpose: spgemm.o (its forward is bit-identical to the oracle on every graph,
+test_gpu_spspmm.py), actnn.o (bit-identical to the numpy restatement, test_gpu_actnn.py), sampler.o and csr_tools.o
+(integer and permutation kernels, checked exactly by test_gpu_sampler.py and the structure tests).
 
 The kernel entry points are read from the objects with cuobjdump and demangled with cu++filt; each instantiation
 is mapped to the string its launcher records for cogdl_b200_last_kernel()."""
@@ -12,11 +17,13 @@ import subprocess
 
 import pytest
 
-from tests.dispatch_table import ES_OPS, EXEMPT, TABLE
+from tests.dispatch_table import ES_OPS, EXEMPT, MESSAGE_TABLE, TABLE
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBJ_DIR = os.path.join(ROOT, "cogdl_b200", "csrc", "build")
-OBJECTS = ("spmm", "sddmm", "mhspmm", "scatter_max", "edge_softmax")
+OBJECTS = ("spmm", "sddmm", "mhspmm", "scatter_max", "edge_softmax", "softmax_aggr", "disen_routing", "comp_aggr",
+           "fused_gcn")
+ROWS = TABLE + MESSAGE_TABLE
 
 
 def _tool(name):
@@ -26,12 +33,12 @@ def _tool(name):
     return shutil.which(name)
 
 
-def compiled_kernels():
+def compiled_kernels(objects=OBJECTS):
     """Demangled kernel entry points (global functions) of the objects."""
     cuobjdump, cufilt = _tool("cuobjdump"), _tool("cu++filt")
     if not cuobjdump or not cufilt:
         pytest.skip("cuobjdump / cu++filt from the CUDA toolkit are not available")
-    paths = [os.path.join(OBJ_DIR, f"{o}.o") for o in OBJECTS]
+    paths = [os.path.join(OBJ_DIR, f"{o}.o") for o in objects]
     missing = [p for p in paths if not os.path.exists(p)]
     if missing:
         pytest.skip(f"library objects not built (run build()): {', '.join(missing)}")
@@ -60,7 +67,7 @@ def _args(sig):
 
 def note_of(sym):
     """The cogdl_b200_last_kernel() string of one demangled instantiation (canonical form, see canonical())."""
-    m = re.fullmatch(r"(?:void )?cogdl_b200::(\w+)(<.*>)?\(.*\)", sym)
+    m = re.fullmatch(r"(?:void )?cogdl_b200::((?:fg::)?\w+)(<.*>)?\(.*\)", sym)
     assert m, f"unexpected symbol {sym!r}"
     name = m.group(1)
     a = _args(m.group(2)) if m.group(2) else []
@@ -73,7 +80,7 @@ def note_of(sym):
         return f"cogdl_b200::spmm_half_kernel<{w(has_val)},{'vec' if vec else 'scalar'}>"
     if name == "stream_kernel":
         vec, nv, mode, perm, src, u, minb, prefetch, panel, drop = a
-        what = {0: "unweighted", 1: "weighted", 2: "multihead"}[mode]
+        what = {0: "unweighted", 1: "weighted", 2: "multihead", 3: "comp_mult", 4: "comp_sub"}[mode]
         if mode == 2:
             what += ("+perm" if perm else "") + ("+drop" if drop else "")
         s = f"cogdl_b200::stream_kernel<{vec},NV={nv},{what},{_SRC[src]},U={u},MINB={minb}{',prefetch' if prefetch else ''}>"
@@ -101,17 +108,35 @@ def note_of(sym):
     if name in ("es_stats_kernel", "es_warp_kernel", "es_generic_kernel"):
         mode, drop = a
         return f"cogdl_b200::{name}<MODE={mode}{',DROP' if drop else ''}>"
+    if name == "softmax_aggr_fwd_kernel":
+        w_, has_a, want_q = a
+        return (f"cogdl_b200::softmax_aggr_fwd_kernel<{'float4' if w_ == 4 else 'float'},"
+                f"{'edge_term' if has_a else 'no_edge_term'},{'Q' if want_q else 'no_Q'}>")
+    if name == "softmax_aggr_bwd_kernel":
+        w_, has_a = a
+        return f"cogdl_b200::softmax_aggr_bwd_kernel<{'float4' if w_ == 4 else 'float'},{'edge_term' if has_a else 'no_edge_term'}>"
+    if name in ("disen_route_fwd_kernel", "disen_route_bwd_row_kernel", "disen_route_bwd_col_kernel"):
+        w_, group = a
+        return f"cogdl_b200::{name}<{'float4' if w_ == 4 else 'float'},GROUP={group}>"
+    if name == "fg::fused_layer_kernel":
+        agg, epi = a
+        what = {(0, 0): "gcn", (0, 1): "sage-sum", (1, 1): "sage-max"}[(agg, epi)]
+        return f"cogdl_b200::fg::fused_layer_kernel<{what}, 2 groups x tile 64xN, K=128, bf16x3 split, wgmma m64n32k16>"
     raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
 
 
 def canonical(note):
     """The instantiations a recorded name lists, without their launch-shape suffixes.  A note of several launches
-    ('a + b': the edge-softmax statistics and main kernels, the GAT attention and aggregation) is split; the panel count
-    becomes ',panels' (the instantiation is the same for every count), ' block=N' and the staging note
-    ' cp.async.bulk tiles' go."""
+    ('a + b': the edge-softmax statistics and main kernels, the GAT attention and aggregation, the DisenGCN row and
+    column kernels, a fused layer's hub pre-pass and the layer) is split; the panel count becomes ',panels' (the
+    instantiation is the same for every count), a fused layer's W^T rows '64xN' and its '+row_scale' go (one
+    instantiation serves every Fout and both forms of the sum), as do ' block=N' and the staging note
+    ' cp.async.bulk tiles'."""
     out = []
     for part in note.split(" + "):
         part = re.sub(r" block=\d+$", "", part)
+        part = re.sub(r"(fused_layer_kernel<[\w-]+)\+row_scale,", r"\1,", part)
+        part = re.sub(r" tile 64x\d+,", " tile 64xN,", part)
         part = re.sub(r" cp\.async\.bulk tiles$", "", part)
         out.append(re.sub(r",panels=\d+", ",panels", part))
     return out
@@ -132,13 +157,27 @@ def test_note_of_maps_known_symbols():
     assert canonical("cogdl_b200::es_stats_kernel<MODE=0> + cogdl_b200::es_main_kernel<MODE=0,CAP=512,WARPS=8> "
                      "cp.async.bulk tiles") == ["cogdl_b200::es_stats_kernel<MODE=0>",
                                                 "cogdl_b200::es_main_kernel<MODE=0,CAP=512,WARPS=8>"]
+    assert note_of("void cogdl_b200::fg::fused_layer_kernel<(int)0, (int)1>(cogdl_b200::fg::Params)") == \
+        "cogdl_b200::fg::fused_layer_kernel<sage-sum, 2 groups x tile 64xN, K=128, bf16x3 split, wgmma m64n32k16>"
+    assert canonical("cogdl_b200::stream_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=5> block=128 + "
+                     "cogdl_b200::fg::fused_layer_kernel<sage-sum+row_scale, 2 groups x tile 64x128, K=128, bf16x3 split, "
+                     "wgmma m64n32k16>") == [
+        "cogdl_b200::stream_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=5>",
+        "cogdl_b200::fg::fused_layer_kernel<sage-sum, 2 groups x tile 64xN, K=128, bf16x3 split, wgmma m64n32k16>"]
+    assert note_of("void cogdl_b200::stream_kernel<float, (int)2, (int)4, (bool)0, (int)0, (int)2, (int)1, (bool)1, "
+                   "(bool)0, (bool)0>(cogdl_b200::StreamParams)") == \
+        "cogdl_b200::stream_kernel<float,NV=2,comp_sub,SRC_ONE,U=2,MINB=1,prefetch>"
+    assert note_of("void cogdl_b200::softmax_aggr_fwd_kernel<(int)4, (bool)1, (bool)0>(cogdl_b200::SaFwdParams)") == \
+        "cogdl_b200::softmax_aggr_fwd_kernel<float4,edge_term,no_Q>"
+    assert note_of("void cogdl_b200::disen_route_bwd_col_kernel<(int)1, (int)16>(cogdl_b200::DrColBwdParams)") == \
+        "cogdl_b200::disen_route_bwd_col_kernel<float,GROUP=16>"
 
 
 def test_table_covers_every_compiled_kernel():
     compiled = {}
     for sym in compiled_kernels():
         compiled.setdefault(note_of(sym), sym)
-    table = {k for c in TABLE for k in canonical(c.kernel)}
+    table = {k for c in ROWS for k in canonical(c.kernel)}
     untested = sorted(set(compiled) - table - set(EXEMPT))
     assert not untested, "compiled kernels without a row in tests/dispatch_table.py:\n" + "\n".join(
         f"  {n}   ({compiled[n]})" for n in untested)
@@ -149,15 +188,16 @@ def test_table_covers_every_compiled_kernel():
 
 
 def test_table_rows_are_distinct():
-    ids = [c.id for c in TABLE]
+    ids = [c.id for c in ROWS]
     dup = sorted({i for i in ids if ids.count(i) > 1})
     assert not dup, f"duplicate table rows: {dup}"
 
 
 def test_recorded_names_fit_the_note_buffer():
     """cogdl_b200_last_kernel() is kept in a 256-byte buffer: the longest name the table expects (a GAT forward:
-    statistics + main kernel of the attention, then the row-stream aggregation) must fit whole."""
-    longest = max(TABLE, key=lambda c: len(c.kernel.encode()))
+    statistics + main kernel of the attention, then the row-stream aggregation; a fused layer after its hub pre-pass)
+    must fit whole."""
+    longest = max(ROWS, key=lambda c: len(c.kernel.encode()))
     assert len(longest.kernel.encode()) < 256, longest.kernel
 
 
@@ -233,3 +273,109 @@ def test_edge_softmax_rows_cover_every_launch_form():
     assert not extra, f"rows in launch forms the compiled kernels do not have: {extra}"
     dup = sorted({f for f in rows if rows.count(f) > 1}, key=str)
     assert not dup, f"several rows of one launch form: {dup}"
+
+
+def message_form(c):
+    """The launch form of a message-operator or fused-layer row: op, the instantiations it records, and what else
+    decides how they run.  GENConv forward: no plan, a partial scratch off alignment, more than 32 vectors a row (several
+    passes), or hub chunks; backward: with or without d edge_term.  DisenGCN: without saved state, a NaN channel, several
+    32-vector tiles, idle lanes of a 32-lane group, or none of these.  CompGCN: the row's vectors (<= 32, <= 64, more:
+    column tiles) and whether there is one edge type.  Fused layers: W^T rows (Npad), hub rows, row scale."""
+    k = tuple(canonical(c.kernel))
+    fv = c.F // c.vec
+    if c.op == "sa_fwd":
+        tag = "none" if c.plan == "none" else "partials+4" if c.partials_offset else "tiles" if fv > 32 else "chunks"
+    elif c.op == "sa_bwd":
+        tag = "chunks" if c.want_edge_grad else "no_dA"
+    elif c.op in ("disen_fwd", "disen_bwd"):
+        tag = ("unsaved" if not c.want_saved else "nan" if c.zero_norm else "tiles" if fv > 32 else
+               "idle" if 16 < fv < 32 else "")
+    elif c.op == "comp":
+        tag = ("one" if fv <= 32 else "two" if fv <= 64 else "tiles", c.T == 1)
+    else:    # the pre-pass of a hub row: test_fused_rows_name_their_pre_pass
+        k, tag = k[-1:], (64 if c.F <= 64 else 128, " + " in c.kernel, c.row_scale)
+    return (c.op, k, tag)
+
+
+_FUSED_OP = {"gcn": "fused_gcn", "sage-sum": "fused_sage_sum", "sage-max": "fused_sage_max"}
+
+
+def required_message_forms():
+    """Every launch form the compiled message kernels and fused layers can take.  GENConv forward: every instantiation
+    with hub chunks; per vector width a row without a plan, a row of several passes, and (scalar only) a row sent to
+    the scalar kernel by a partial scratch 4 bytes off alignment.  Backward: every instantiation with hub chunks on the
+    transpose, and the float4 edge-term kernel without d edge_term.  DisenGCN: every (kernel, W, GROUP), forward and
+    backward (the backward records its row and column kernels); at GROUP 32 and both widths, idle lanes and several
+    tiles; a forward without saved state and one with a NaN channel.  CompGCN: every instantiation, NV = 2 both within
+    64 vectors and over several column tiles, each width and op with one edge type and with 300.  Fused layers: each
+    at Npad 64 and 128, with and without hub rows; the sum of the SAGE layer with and without a row scale."""
+    forms = set()
+    comp = {note_of(s) for s in compiled_kernels(("comp_aggr",))}
+    for sym in compiled_kernels(("softmax_aggr", "disen_routing", "comp_aggr", "fused_gcn")):
+        n = note_of(sym)
+        if "softmax_aggr_fwd_kernel" in n:
+            forms.add(("sa_fwd", (n,), "chunks"))
+            if "no_edge_term,no_Q" in n:
+                forms.add(("sa_fwd", (n,), "none"))
+            if ",edge_term,Q" in n:
+                forms.add(("sa_fwd", (n,), "tiles"))
+                if "<float," in n:
+                    forms.add(("sa_fwd", (n,), "partials+4"))
+        elif "softmax_aggr_bwd_kernel" in n:
+            forms.add(("sa_bwd", (n,), "chunks"))
+            if n.endswith("<float4,edge_term>"):
+                forms.add(("sa_bwd", (n,), "no_dA"))
+        elif "disen_route_bwd_col_kernel" in n:
+            continue
+        elif "disen_route_" in n:
+            op = "disen_fwd" if "fwd" in n else "disen_bwd"
+            k = (n,) if op == "disen_fwd" else (n, n.replace("bwd_row", "bwd_col"))
+            forms.add((op, k, ""))
+            if n.endswith("GROUP=32>"):
+                forms.update({(op, k, "idle"), (op, k, "tiles")})
+            if op == "disen_fwd" and n.endswith("<float4,GROUP=8>"):
+                forms.add((op, k, "unsaved"))
+            if op == "disen_fwd" and n.endswith("<float4,GROUP=16>"):
+                forms.add((op, k, "nan"))
+        elif n in comp:
+            if ",NV=1," in n:
+                forms.add(("comp", (n,), ("one", True)))
+            else:
+                forms.update({("comp", (n,), ("two", False)), ("comp", (n,), ("tiles", True))})
+        elif "fused_layer_kernel" in n:
+            op = _FUSED_OP[re.search(r"<([\w-]+),", n).group(1)]
+            for npad in (64, 128):
+                for hub in (False, True):
+                    rs = op == "fused_sage_sum" and hub == (npad == 64)
+                    forms.add((op, (n,), (npad, hub, rs)))
+    return forms
+
+
+def test_message_rows_cover_every_launch_form():
+    """Every launch form of the message operators and fused layers has exactly one row, so removing any of those rows
+    fails here."""
+    rows = [message_form(c) for c in MESSAGE_TABLE]
+    required = required_message_forms()
+    missing = sorted(required - set(rows), key=str)
+    assert not missing, "message launch forms without a row in tests/dispatch_table.py:\n" + "\n".join(
+        f"  {f}" for f in missing)
+    extra = sorted(set(rows) - required, key=str)
+    assert not extra, "rows in launch forms the compiled kernels do not have:\n" + "\n".join(f"  {f}" for f in extra)
+    dup = sorted({f for f in rows if rows.count(f) > 1}, key=str)
+    assert not dup, f"several rows of one launch form: {dup}"
+
+
+def test_fused_rows_name_their_pre_pass():
+    """A fused row with hub rows names the pre-pass its layer launches (the SpMM's hub chunks, weighted iff the row has
+    edge values; scatter_max's without argmax for the max layer), one without names the layer alone."""
+    for c in MESSAGE_TABLE:
+        if not c.op.startswith("fused"):
+            continue
+        parts = canonical(c.kernel)
+        hub = c.chunk < 1500                      # the 400-row graph's hub has 1500 edges
+        assert len(parts) == (2 if hub else 1), c.id
+        if hub and c.op == "fused_sage_max":
+            assert parts[0] == "cogdl_b200::scatter_max_stream_kernel<NV=1,U=4,values_only>", c.id
+        elif hub:
+            assert parts[0] == f"cogdl_b200::stream_kernel<float4,NV=1,{'weighted' if c.weighted else 'unweighted'}," \
+                               "SRC_ONE,U=4,MINB=5>", c.id
