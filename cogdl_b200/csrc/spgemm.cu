@@ -546,7 +546,7 @@ extern "C" int cogdl_b200_spgemm_bwd_f32(const int32_t *rowptrA, const int32_t *
     CB_LAUNCH_CHECK();
   }
   if (dB) {
-    note_kernel(dA ? "cogdl_b200::spg_dA_kernel+spg_dB_kernel" : "cogdl_b200::spg_dB_kernel");
+    note_kernel(dA ? "cogdl_b200::spg_dA_kernel + cogdl_b200::spg_dB_kernel" : "cogdl_b200::spg_dB_kernel");
     spg_dB_kernel<<<NUM_SMS * 16, 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
   }

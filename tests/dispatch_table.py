@@ -6,6 +6,9 @@ perm, dropout, source form) and the exact cogdl_b200_last_kernel() string the ca
 (test_gpu_dispatch.py) runs every row and checks the output against a reference; the CPU test
 (test_cpu_kernel_inventory.py) checks that the rows cover every kernel compiled into those five objects, and
 that every kernel named here is compiled.  Plain Python, no torch: the CPU test imports it without a GPU.
+
+The message operators and fused layers (MESSAGE_TABLE) and the sparse x sparse product's tier edges (SPGEMM_TABLE)
+follow, each with its own GPU test.
 """
 from dataclasses import dataclass
 
@@ -557,3 +560,65 @@ MESSAGE_TABLE = SOFTMAX_AGGR + DISEN + COMP + FUSED
 
 # Compiled instantiations no row above reaches (none: the fused layers record their hub pre-pass).
 EXEMPT = {}
+
+
+# ================================================================== sparse x sparse product (spgemm.cu)
+# cogdl_b200_spgemm_count / _fill_f32 put every output row into a tier by bound = min(sum_{k in A_i} deg_B(k), n):
+# nothing to do (0), a warp with a 512-slot hash table (<= 256), a block with an 8192-slot table (<= 4096), or a
+# block with a bitmap of the n columns in one of 132 global slots.  Every tier kernel and the classifier launch on every
+# call and the call records one name per phase, so a row names the edges of the tiers its product reaches
+# (tests/spgemm_oracle.py edges(), which test_cpu_kernel_inventory.py checks against the row's builder), and
+# cogdl_b200_spgemm_bwd_f32's one-warp-per-entry reductions.  Run by test_gpu_dispatch_spgemm.py.
+SPG_COUNT = "cogdl_b200::spg_count<warp=256,block=4096,bitmap>"
+SPG_FILL = "cogdl_b200::spg_fill<warp=256,block=4096,bitmap>"
+SPG_DA = "cogdl_b200::spg_dA_kernel"
+SPG_DB = "cogdl_b200::spg_dB_kernel"
+SPG_DA_DB = f"{SPG_DA} + {SPG_DB}"
+
+
+@dataclass(frozen=True)
+class SpgemmCase:
+    name: str               # the product: tests/graphs.py spgemm_case(name)
+    edges: tuple            # the (tier, edge) pairs it is built for
+
+    @property
+    def id(self):
+        return f"spgemm-{self.name}"
+
+    # what every row's calls record: count, fill, and the backward for dA, dB and both
+    kernels = (SPG_COUNT, SPG_FILL, SPG_DA, SPG_DB, SPG_DA_DB)
+
+
+def _spg(name, *edges):
+    return SpgemmCase(name, tuple(edges))
+
+
+SPGEMM_TABLE = [
+    _spg("empty-rows", ("empty", "A row without entries"), ("empty", "A row meeting only empty B rows")),
+    _spg("m0", ("shape", "m = 0")),
+    _spg("k0", ("shape", "k = 0")),
+    _spg("n0", ("shape", "n = 0")),
+    _spg("A-empty", ("shape", "A without entries")),
+    _spg("B-empty", ("shape", "B without entries")),
+    _spg("rect", ("shape", "m, k, n distinct, every tier")),
+    _spg("warp-counts", ("warp", "1 columns"), ("warp", "255 columns"), ("warp", "256 columns")),
+    _spg("warp-bound256-c1", ("warp", "bound 256, 1 columns")),
+    _spg("warp-hash-wrap", ("warp", "hash wrap-around")),
+    _spg("warp-n-capped", ("warp", "n <= 256, full row")),
+    _spg("block-counts", ("block", "257 columns"), ("block", "4095 columns"), ("block", "4096 columns")),
+    _spg("block-bound300-c2", ("block", "bound 300, 2 columns")),
+    _spg("block-hash-wrap", ("block", "hash wrap-around")),
+    _spg("block-n-capped", ("block", "n = 4096, full row")),
+    _spg("bitmap-counts", ("bitmap", "4097 columns")),
+    _spg("bitmap-bound5000-c3", ("bitmap", "bound 5000, 3 columns")),
+    _spg("bitmap-full", ("bitmap", "all n columns")),
+    _spg("bitmap-n32w+1", ("bitmap", "n = 32w + 1")),
+    _spg("bitmap-n8192", ("bitmap", "n = 8192")),
+    _spg("bitmap-n8193", ("bitmap", "n = 8193")),
+    _spg("grid-loops", ("warp", "grid loop"), ("block", "grid loop"), ("bitmap", "grid loop")),
+    _spg("cancel", ("values", "exact cancellation")),
+    _spg("subnormal", ("values", "subnormal")),
+    _spg("negzero", ("values", "-0.0 factors")),
+    *[_spg(f"bwd-{d}", ("dA", f"{d} terms"), ("dB", f"{d} terms")) for d in (1, 31, 32, 33, 65, 2000)],
+    _spg("bwd-duplicates", ("dA", "duplicate entries"), ("dB", "duplicate entries")),
+]

@@ -1,12 +1,13 @@
 """Every gather kernel compiled into spmm.o, sddmm.o, mhspmm.o and scatter_max.o, every edge-softmax / GAT attention
 kernel compiled into edge_softmax.o, every message-operator kernel of softmax_aggr.o (GENConv), disen_routing.o
-(DisenGCN) and comp_aggr.o (CompGCN), and every fused layer of fused_gcn.o has a row in the dispatch table
-(tests/dispatch_table.py) that the GPU suite runs and checks, and every kernel the table names is compiled.  A new
-dispatch branch without a test case fails here, on a machine without a GPU.
+(DisenGCN) and comp_aggr.o (CompGCN), every fused layer of fused_gcn.o and every tier kernel of the sparse x sparse
+product in spgemm.o has a row in the dispatch table (tests/dispatch_table.py) that the GPU suite runs and checks, and
+every kernel the table names is compiled.  A new dispatch branch without a test case fails here, on a machine without
+a GPU.
 
-Objects left out on purpose: spgemm.o (its forward is bit-identical to the oracle on every graph,
-test_gpu_spspmm.py), actnn.o (bit-identical to the numpy restatement, test_gpu_actnn.py), sampler.o and csr_tools.o
-(integer and permutation kernels, checked exactly by test_gpu_sampler.py and the structure tests).
+Objects left out on purpose, none of which picks a kernel by size and all of which are checked bit for bit: actnn.o
+(against the numpy restatement, test_gpu_actnn.py), sampler.o (against the oracle, test_gpu_sampler.py) and
+csr_tools.o (integer and permutation kernels, checked exactly by the structure tests).
 
 The kernel entry points are read from the objects with cuobjdump and demangled with cu++filt; each instantiation
 is mapped to the string its launcher records for cogdl_b200_last_kernel()."""
@@ -17,13 +18,20 @@ import subprocess
 
 import pytest
 
-from tests.dispatch_table import ES_OPS, EXEMPT, MESSAGE_TABLE, TABLE
+from tests import graphs
+from tests import spgemm_oracle as so
+from tests.dispatch_table import ES_OPS, EXEMPT, MESSAGE_TABLE, SPG_COUNT, SPG_FILL, SPGEMM_TABLE, TABLE
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBJ_DIR = os.path.join(ROOT, "cogdl_b200", "csrc", "build")
 OBJECTS = ("spmm", "sddmm", "mhspmm", "scatter_max", "edge_softmax", "softmax_aggr", "disen_routing", "comp_aggr",
-           "fused_gcn")
+           "fused_gcn", "spgemm")
 ROWS = TABLE + MESSAGE_TABLE
+
+
+def table_names():
+    """The recorded name of every row; a sparse x sparse row's calls record several."""
+    return [c.kernel for c in ROWS] + [k for c in SPGEMM_TABLE for k in c.kernels]
 
 
 def _tool(name):
@@ -67,6 +75,8 @@ def _args(sig):
 
 def note_of(sym):
     """The cogdl_b200_last_kernel() string of one demangled instantiation (canonical form, see canonical())."""
+    if re.match(r"void cub::\w+::(DeviceScan\w*Kernel|EmptyKernel)<", sym):
+        return SPG_COUNT      # spgemm.o: the count phase's scan of the row counts (cub compiles EmptyKernel beside it)
     m = re.fullmatch(r"(?:void )?cogdl_b200::((?:fg::)?\w+)(<.*>)?\(.*\)", sym)
     assert m, f"unexpected symbol {sym!r}"
     name = m.group(1)
@@ -122,6 +132,10 @@ def note_of(sym):
         agg, epi = a
         what = {(0, 0): "gcn", (0, 1): "sage-sum", (1, 1): "sage-max"}[(agg, epi)]
         return f"cogdl_b200::fg::fused_layer_kernel<{what}, 2 groups x tile 64xN, K=128, bf16x3 split, wgmma m64n32k16>"
+    if name in ("spg_classify_kernel", "spg_warp_kernel", "spg_block_kernel", "spg_large_kernel"):
+        return SPG_FILL if a == [True] else SPG_COUNT     # the classifier runs in both phases, first in the count
+    if name in ("spg_dA_kernel", "spg_dB_kernel"):
+        return f"cogdl_b200::{name}"
     raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
 
 
@@ -171,13 +185,19 @@ def test_note_of_maps_known_symbols():
         "cogdl_b200::softmax_aggr_fwd_kernel<float4,edge_term,no_Q>"
     assert note_of("void cogdl_b200::disen_route_bwd_col_kernel<(int)1, (int)16>(cogdl_b200::DrColBwdParams)") == \
         "cogdl_b200::disen_route_bwd_col_kernel<float,GROUP=16>"
+    assert note_of("cogdl_b200::spg_classify_kernel(cogdl_b200::SpgParams, bool)") == SPG_COUNT
+    assert note_of("void cogdl_b200::spg_block_kernel<(bool)0>(cogdl_b200::SpgParams)") == SPG_COUNT
+    assert note_of("void cogdl_b200::spg_large_kernel<(bool)1>(cogdl_b200::SpgParams)") == SPG_FILL
+    assert note_of("cogdl_b200::spg_dB_kernel(cogdl_b200::SpgBwdParams)") == "cogdl_b200::spg_dB_kernel"
+    assert canonical("cogdl_b200::spg_dA_kernel + cogdl_b200::spg_dB_kernel") == ["cogdl_b200::spg_dA_kernel",
+                                                                                  "cogdl_b200::spg_dB_kernel"]
 
 
 def test_table_covers_every_compiled_kernel():
     compiled = {}
     for sym in compiled_kernels():
         compiled.setdefault(note_of(sym), sym)
-    table = {k for c in ROWS for k in canonical(c.kernel)}
+    table = {k for name in table_names() for k in canonical(name)}
     untested = sorted(set(compiled) - table - set(EXEMPT))
     assert not untested, "compiled kernels without a row in tests/dispatch_table.py:\n" + "\n".join(
         f"  {n}   ({compiled[n]})" for n in untested)
@@ -188,7 +208,7 @@ def test_table_covers_every_compiled_kernel():
 
 
 def test_table_rows_are_distinct():
-    ids = [c.id for c in ROWS]
+    ids = [c.id for c in ROWS + SPGEMM_TABLE]
     dup = sorted({i for i in ids if ids.count(i) > 1})
     assert not dup, f"duplicate table rows: {dup}"
 
@@ -197,8 +217,8 @@ def test_recorded_names_fit_the_note_buffer():
     """cogdl_b200_last_kernel() is kept in a 256-byte buffer: the longest name the table expects (a GAT forward:
     statistics + main kernel of the attention, then the row-stream aggregation; a fused layer after its hub pre-pass)
     must fit whole."""
-    longest = max(ROWS, key=lambda c: len(c.kernel.encode()))
-    assert len(longest.kernel.encode()) < 256, longest.kernel
+    longest = max(table_names(), key=lambda k: len(k.encode()))
+    assert len(longest.encode()) < 256, longest
 
 
 _ES_OP = {0: "edge_softmax", 1: "edge_softmax_bwd", 2: "gat_fwd", 3: "gat_attn_bwd"}
@@ -379,3 +399,58 @@ def test_fused_rows_name_their_pre_pass():
         elif hub:
             assert parts[0] == f"cogdl_b200::stream_kernel<float4,NV=1,{'weighted' if c.weighted else 'unweighted'}," \
                                "SRC_ONE,U=4,MINB=5>", c.id
+
+
+# The edges of each tier of the sparse x sparse product, as tests/spgemm_oracle.py edges() names them.  The classifier
+# owns the rows with nothing to do and the degenerate shapes; each fill kernel also owns the values its fmaf chains
+# produce, in a row of every tier.
+_SPG_TIERS = {"spg_classify_kernel": ("empty", "shape"), "spg_warp_kernel": ("warp",), "spg_block_kernel": ("block",),
+              "spg_large_kernel": ("bitmap",), "spg_dA_kernel": ("dA",), "spg_dB_kernel": ("dB",)}
+_SPG_EDGES = {
+    "empty": ("A row without entries", "A row meeting only empty B rows"),
+    "shape": ("m = 0", "k = 0", "n = 0", "A without entries", "B without entries", "m, k, n distinct, every tier"),
+    "warp": ("1 columns", "255 columns", "256 columns", "bound 256, 1 columns", "hash wrap-around",
+             "n <= 256, full row", "grid loop"),
+    "block": ("257 columns", "4095 columns", "4096 columns", "bound 300, 2 columns", "hash wrap-around",
+              "n = 4096, full row", "grid loop"),
+    "bitmap": ("4097 columns", "bound 5000, 3 columns", "all n columns", "n = 32w + 1", "n = 8192", "n = 8193",
+               "grid loop"),
+    "values": ("exact cancellation", "subnormal", "-0.0 factors"),
+    "dA": tuple(f"{d} terms" for d in so.BWD_TERMS) + ("duplicate entries",),
+    "dB": tuple(f"{d} terms" for d in so.BWD_TERMS) + ("duplicate entries",),
+}
+
+
+def required_spgemm_edges():
+    """The (tier, edge) pairs of every compiled tier kernel of spgemm.o.  Warp and block tiers: rows of distinct
+    count 1 / 255 / 256 and 257 / 4095 / 4096 with distinct count = bound, a bound at or past the cap with 1 or 2
+    columns, a full table whose columns all hash into its last slots (probes wrap to slot 0), the bound capped by
+    n <= 256 and by n = 4096 with a full row, and more rows than the launch has warps or blocks.  The bitmap: 4097
+    columns, bound 5000 with 3 columns, a row of all n columns, n = 32w + 1 with columns 0, 31, 32, 63, 64 and n - 1,
+    n = 8192 (256 words) and 8193 (a scan carry), more rows than slots.  The backward: entries of 1, 31, 32, 33, 65
+    and 2000 terms and duplicated input entries, for dA and dB."""
+    req = set()
+    for sym in compiled_kernels(("spgemm",)):
+        m = re.fullmatch(r"(?:void )?cogdl_b200::(spg_\w+)(<.*>)?\(.*\)", sym)
+        if not m:
+            continue                                      # cub's scan
+        assert m.group(1) in _SPG_TIERS, f"no edges are known for {sym!r}: add them here and rows to SPGEMM_TABLE"
+        tiers = _SPG_TIERS[m.group(1)] + (("values",) if m.group(2) and _args(m.group(2)) == [True] else ())
+        req |= {(t, e) for t in tiers for e in _SPG_EDGES[t]}
+    return req
+
+
+def test_spgemm_rows_cover_every_tier_edge():
+    """Every tier edge has exactly one row built for it, and each row's product (rebuilt here from its numpy builder)
+    reaches the edges it names, so removing any sparse x sparse row, or a builder drifting off its edge, fails here."""
+    rows = [e for c in SPGEMM_TABLE for e in c.edges]
+    required = required_spgemm_edges()
+    missing = sorted(required - set(rows))
+    assert not missing, "tier edges without a row in SPGEMM_TABLE:\n" + "\n".join(f"  {e}" for e in missing)
+    extra = sorted(set(rows) - required)
+    assert not extra, f"rows for edges no compiled kernel has: {extra}"
+    dup = sorted({e for e in rows if rows.count(e) > 1})
+    assert not dup, f"several rows for one edge: {dup}"
+    for c in SPGEMM_TABLE:
+        off = sorted(set(c.edges) - so.edges(*graphs.spgemm_case(c.name)))
+        assert not off, f"{c.id} does not reach {off}"
