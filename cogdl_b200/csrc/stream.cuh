@@ -52,6 +52,11 @@ struct StreamParams {
   // MODE 2); a kept entry is read as att * drop_scale, a dropped one as 0 (drop_att, common.cuh).  Read only by
   // the multi-head form, which takes the DROP instantiation iff drop_scale > 0.
   float drop_scale;
+  // residual epilogue (spmm_residual.cu, RESID): every finished row i is written as
+  // fl(fl(res_a * fl(row_scale[i] * acc)) + fl(res_b * Z[i])); row_scale and Z are optional ([n_rows], [n_rows, ldv]).
+  const float *Z = nullptr;
+  const float *row_scale = nullptr;
+  float res_a = 1.f, res_b = 0.f;
 };
 
 enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2, MODE_COMP_MULT = 3, MODE_COMP_SUB = 4 };
@@ -67,9 +72,35 @@ enum { SRC_ONE = 0, SRC_TWO = 1, SRC_PEERS = 2 };
 // the multi-head SpMM.
 enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
 
+// The residual epilogue of one output element, rounded step by step as the unfused sequence
+// `a * (r * spmm(x)) + b * z` rounds it (no contraction); r and z are used iff has_r / has_z.
+__device__ __forceinline__ float residual_rn(float acc, float z, bool has_r, float r, bool has_z, float a, float b) {
+  const float t = __fmul_rn(a, has_r ? __fmul_rn(r, acc) : acc);
+  return has_z ? __fadd_rn(t, __fmul_rn(b, z)) : t;
+}
+__device__ __forceinline__ float2 residual_rn(float2 acc, float2 z, bool hr, float r, bool hz, float a, float b) {
+  return make_float2(residual_rn(acc.x, z.x, hr, r, hz, a, b), residual_rn(acc.y, z.y, hr, r, hz, a, b));
+}
+__device__ __forceinline__ float4 residual_rn(float4 acc, float4 z, bool hr, float r, bool hz, float a, float b) {
+  return make_float4(residual_rn(acc.x, z.x, hr, r, hz, a, b), residual_rn(acc.y, z.y, hr, r, hz, a, b),
+                     residual_rn(acc.z, z.z, hr, r, hz, a, b), residual_rn(acc.w, z.w, hr, r, hz, a, b));
+}
+
+// acc of output row `row`, to be stored at yp (Z has Y's layout), with the residual epilogue of p (StreamParams or
+// SpmmParams) applied.
+template <typename VecT, typename P>
+__device__ __forceinline__ VecT residual_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
+  const int64_t o = yp - reinterpret_cast<const VecT *>(p.Y);
+  const bool hr = p.row_scale != nullptr, hz = p.Z != nullptr;
+  const float r = hr ? __ldg(p.row_scale + row) : 1.f;
+  const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.Z) + o) : vzero<VecT>();
+  return residual_rn(acc, z, hr, r, hz, p.res_a, p.res_b);
+}
+
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
 // whole range into acc (hub chunk).
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH, bool DROP = false>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH, bool DROP = false,
+          bool RESID = false>
 __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const int e_end, const int cv,
                                              const bool (&colok)[NV], const int head, const int lane,
                                              VecT (&acc)[NV]) {
@@ -157,7 +188,11 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
           if (ROWS && ((em >> u) & 1u)) {   // last edge of row rj: store and restart (warp-uniform)
 #pragma unroll
             for (int k = 0; k < NV; ++k)
-              if (colok[k]) { st_stream(Y + (int64_t)rj * p.ldv + k * 32, acc[k]); acc[k] = vzero<VecT>(); }
+              if (colok[k]) {
+                VecT *yp = Y + (int64_t)rj * p.ldv + k * 32;
+                st_stream(yp, RESID ? residual_out(p, acc[k], rj, yp) : acc[k]);
+                acc[k] = vzero<VecT>();
+              }
           }
         }
       }
@@ -183,7 +218,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
 // mostly re-read by the next slab, instead of edge_row's 4 bytes per edge (plus the neighbour's) in every pass.  The
 // one-pass form keeps the edge_row test (`row != row of the next edge`, one ballot): there the cursor's longer
 // dependent chain per slab costs more than the bytes it saves (SpMM F=40 +2 %, DESIGN 3.1).
-template <typename VecT, int MODE, int SRC, int U, bool ROWS, bool PF = false>
+template <typename VecT, int MODE, int SRC, int U, bool ROWS, bool PF = false, bool RESID = false>
 __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, const int e_end, int r, const int r_end,
                                                   const int cv, const bool colok, const int lane, int2 *s_cv, int *s_r,
                                                   VecT &acc) {
@@ -198,6 +233,11 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
   };
   auto accumulate = [&](float vj, const VecT &x) {
     if (MODE == MODE_UNWEIGHTED) add_rn(acc, x); else axpy_rn(acc, vj, x);
+  };
+  auto store_row = [&](int rj) {                    // row rj is complete: store it (epilogue applied) and restart
+    VecT *yp = Y + (int64_t)rj * p.ldv;
+    st_stream(yp, RESID ? residual_out(p, acc, rj, yp) : acc);
+    acc = vzero<VecT>();
   };
   constexpr bool CURSOR = ROWS && PF;               // row ends from rowptr; otherwise (ROWS) from edge_row
   // column, value and (CURSOR) the end of row r + lane; INT_MAX past the segment's last row
@@ -281,7 +321,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
           if (colok) accumulate(val_of(u), x[u]);
           if ((em >> u) & 1u) {                     // last edge of its row: store and restart (warp-uniform)
             const int rj = s_r[j + u];
-            if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = vzero<VecT>(); }
+            if (colok) store_row(rj);
           }
         }
       }
@@ -292,14 +332,15 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
       if (colok) accumulate(__int_as_float(cw.y), ld_gather(src_ptr(cw.x)));
       if (ROWS && ((endmask >> j) & 1u)) {
         const int rj = s_r[j];
-        if (colok) { st_stream(Y + (int64_t)rj * p.ldv, acc); acc = vzero<VecT>(); }
+        if (colok) store_row(rj);
       }
     }
   }
 }
 
 // One work item processed by one warp: wid = item * S + slice (multi-head), slice = blockIdx.y (PANEL).
-template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool PANEL, bool DROP = false>
+template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool PANEL, bool DROP = false,
+          bool RESID = false>
 __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t wid, const int lane, int2 *s_cv, int *s_r) {
   constexpr int TILE = 32 * NV;
   constexpr bool SLICED = (MODE == MODE_MULTIHEAD || PANEL);
@@ -350,7 +391,8 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
         const VecT *pp = P + (int64_t)w.first * p.ldv + cv;
         const VecT s = merge_chunks<8>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.ldv); },
                                        [](VecT &a, const VecT &t) { add_rn(a, t); });
-        st_stream(Y + (int64_t)w.row * p.ldv + cv, s);
+        VecT *yp = Y + (int64_t)w.row * p.ldv + cv;
+        st_stream(yp, RESID ? residual_out(p, s, w.row, yp) : s);
       }
     }
     return;
@@ -377,13 +419,17 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
           const int k0 = __ffs(m) - 1;
           m &= m - 1;
 #pragma unroll
-          for (int k = 0; k < NV; ++k)
-            if (colok[k]) st_stream(Y + (int64_t)(rb + k0) * p.ldv + cv + k * 32, vzero<VecT>());
+          for (int k = 0; k < NV; ++k) {
+            if (colok[k]) {
+              VecT *yp = Y + (int64_t)(rb + k0) * p.ldv + cv + k * 32;
+              st_stream(yp, RESID ? residual_out(p, vzero<VecT>(), rb + k0, yp) : vzero<VecT>());
+            }
+          }
         }
       }
     }
-    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH>(p, e_begin, e_end, rr.x, rr.y, cv, colok[0], lane, s_cv, s_r, acc[0]);
-    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, DROP>(p, e_begin, e_end, cv, colok, head, lane, acc);
+    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH, RESID>(p, e_begin, e_end, rr.x, rr.y, cv, colok[0], lane, s_cv, s_r, acc[0]);
+    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, DROP, RESID>(p, e_begin, e_end, cv, colok, head, lane, acc);
   }
 }
 
@@ -400,11 +446,26 @@ __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p)
   stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, PANEL, DROP>(p, wid, lane, s_cv, s_r);
 }
 
+// stream_kernel of the plain SpMM (one source) with the residual epilogue (spmm_residual.cu).
+template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
+__global__ void __launch_bounds__(256, MINB) stream_residual_kernel(const StreamParams p) {
+  const int lane = threadIdx.x & 31;
+  constexpr bool LEAN = is_lean<MODE, NV>();
+  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
+  __shared__ int s_r_all[LEAN ? 8 : 1][32];
+  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
+  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
+  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, true>(p, wid, lane, s_cv, s_r);
+}
+
 // Launch helper: picks the instantiation of FORM for (weighted, perm, source form); U / MINB fixed by the caller.
-// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.
-template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN>
+// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.  RESID: the plain
+// or panel form with the residual epilogue (stream_residual_kernel, one source).
+template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN, bool RESID = false>
 static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   static_assert(FORM == FORM_PLAIN || NV == 1, "the panel and multi-head forms have one VecT per lane");
+  static_assert(!RESID || FORM != FORM_MULTIHEAD, "the residual epilogue is a form of the plain SpMM");
   const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * (FORM == FORM_MULTIHEAD ? p.S : 1);
   // Threads per block: a launch parameter only -- the kernel indexes its per-warp slabs by warp-in-block and takes its
   // item from the global warp index, so every block size runs the same SASS and gives the same bits.  A block's warp
@@ -417,10 +478,10 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "stream kernel: problem too large for one launch");
   const dim3 grid((unsigned)blocks, FORM == FORM_PANEL ? (unsigned)p.S : 1u);
   const int src = p.n_peers > 0 ? SRC_PEERS : (p.n0 != INT64_MAX ? SRC_TWO : SRC_ONE);
-  if (FORM != FORM_PLAIN && src != SRC_ONE)
-    return set_error(COGDL_B200_EINVAL, "stream kernel: the panel and multi-head forms read one source");
+  if ((FORM != FORM_PLAIN || RESID) && src != SRC_ONE)
+    return set_error(COGDL_B200_EINVAL, "stream kernel: the panel, multi-head and residual forms read one source");
   const bool drop = FORM == FORM_MULTIHEAD && p.drop_scale > 0.f;
-  note_kernel("cogdl_b200::stream_kernel<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>",
+  note_kernel("cogdl_b200::%s<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>", RESID ? "stream_residual_kernel" : "stream_kernel",
               sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
               FORM == FORM_MULTIHEAD ? "multihead" : (p.val ? "weighted" : "unweighted"),
               (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "", drop ? "+drop" : "",
@@ -428,7 +489,11 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
               PREFETCH ? ",prefetch" : "");
   if (FORM == FORM_PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
   append_kernel_note(" block=%d", STREAM_BLOCK);
-  if constexpr (FORM == FORM_MULTIHEAD) {
+  if constexpr (RESID) {
+    constexpr bool PANEL = FORM == FORM_PANEL;
+    if (p.val) stream_residual_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_residual_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if constexpr (FORM == FORM_MULTIHEAD) {
     if (drop) {
       if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
       else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);

@@ -27,6 +27,9 @@ spspmm=True provides torch_sparse's spspmm / spmm (cogdl_b200.spspmm / coo_spmm)
 `torch_sparse` stand-in module when the real package is missing (install_spspmm, uninstall_spspmm()).
 actnn=True provides the `actnn` API (cogdl_b200.actnn) to ActGCN, GCNII(actnn=True), GraphSAGE(actnn=True) and the trainer's
 --actnn, through an `actnn` stand-in package when the real one does not import (install_actnn, uninstall_actnn()).
+gcnii=True rebinds `cogdl.layers.gcnii_layer.GCNIILayer.forward` (GCNII) to gcnii_forward and appnp=True
+`cogdl.models.nn.ppnp.PPNP.forward` (APPNP) to appnp_forward; both send the initial-residual propagation to
+cogdl_b200.spmm_residual (uninstall_gcnii(), uninstall_appnp()).
 """
 import sys
 
@@ -195,6 +198,81 @@ def uninstall_gat():
     _restore_forward(gl.GATLayer)
 
 
+def gcnii_forward(self, graph, x, init_x):
+    """GCNIILayer.forward (cogdl/layers/gcnii_layer.py:24-30) with the propagation `(1 - alpha) * spmm(graph, x) +
+    alpha * init_x` in one cogdl_b200.spmm_residual launch, and the identity mapping `beta * linear(s) + (1 - beta) * s`
+    folded into the GEMM operand: one addmm with beta * W + (1 - beta) * I, built from the layer's own linear with
+    autograd-tracked ops, so d W and d bias come from autograd.  CPU or non-fp32 input or weights, and graphs with a
+    dense grb_adj, run the original."""
+    from .operators.spmm_residual import spmm_residual
+
+    original = type(self)._cogdl_b200_original_forward
+    lin = self.linear
+    if (not x.is_cuda or x.dtype != torch.float32 or init_x.dtype != torch.float32 or lin.weight.dtype != torch.float32
+            or (lin.bias is not None and lin.bias.dtype != torch.float32) or getattr(graph, "grb_adj", None) is not None):
+        return original(self, graph, x, init_x)
+    s = spmm_residual(graph, x, init_x, 1 - self.alpha, self.alpha)
+    beta = self.beta
+    eye = torch.eye(lin.weight.shape[0], dtype=lin.weight.dtype, device=lin.weight.device)
+    w = beta * lin.weight + (1 - beta) * eye
+    bias = beta * lin.bias if lin.bias is not None else torch.zeros(lin.weight.shape[0], dtype=s.dtype, device=s.device)
+    h = torch.addmm(bias, s, w.t())
+    if self.residual:
+        h = h + x
+    return h
+
+
+def install_gcnii():
+    import cogdl.layers.gcnii_layer as gl
+
+    return _rebind_forward(gl.GCNIILayer, gcnii_forward, "cogdl.layers.gcnii_layer.GCNIILayer.forward")
+
+
+def uninstall_gcnii():
+    import cogdl.layers.gcnii_layer as gl
+
+    _restore_forward(gl.GCNIILayer)
+
+
+def appnp_forward(self, graph):
+    """PPNP.forward (cogdl/models/nn/ppnp.py:56-87) for propagation "appnp": the MLP, the edge-weight dropout in the
+    reference's order (a seeded run draws the same masks), set_symmetric() as the reference does (so the backward runs
+    over the dropped-weight adjacency, not its transpose), then niter cogdl_b200.spmm_residual launches of
+    `(1 - alpha) * spmm(graph, preds) + alpha * local_preds`.  "ppnp" (the dense inverse), CPU or non-fp32 features
+    or weights, and graphs with a dense grb_adj run the original."""
+    import torch.nn.functional as F
+
+    from .operators.spmm_residual import spmm_residual
+
+    original = type(self)._cogdl_b200_original_forward
+    x = graph.x
+    if (self.propagation != "appnp" or not x.is_cuda or x.dtype != torch.float32
+            or any(p.dtype != torch.float32 for p in self.nn.parameters()) or getattr(graph, "grb_adj", None) is not None):
+        return original(self, graph)
+    graph.sym_norm()
+    x = F.dropout(x, p=self.dropout, training=self.training)
+    local_preds = self.nn.forward(x)
+    preds = local_preds
+    with graph.local_graph():
+        graph.edge_weight = F.dropout(graph.edge_weight, p=self.dropout, training=self.training)
+        graph.set_symmetric()
+        for _ in range(self.niter):
+            preds = spmm_residual(graph, preds, local_preds, 1 - self.alpha, self.alpha)
+    return preds
+
+
+def install_appnp():
+    import cogdl.models.nn.ppnp as pm
+
+    return _rebind_forward(pm.PPNP, appnp_forward, "cogdl.models.nn.ppnp.PPNP.forward")
+
+
+def uninstall_appnp():
+    import cogdl.models.nn.ppnp as pm
+
+    _restore_forward(pm.PPNP)
+
+
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
 _spspmm_state = {"stub": None, "rebound": []}
 
@@ -298,7 +376,8 @@ def uninstall_actnn():
     _actnn_state["stub"] = None
 
 
-def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False):
+def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
+            gcnii=False, appnp=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -390,4 +469,8 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_gat()
     if actnn:
         patched += install_actnn()
+    if gcnii:
+        patched += install_gcnii()
+    if appnp:
+        patched += install_appnp()
     return patched

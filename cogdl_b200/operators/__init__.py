@@ -19,3 +19,4 @@ from .softmax_aggr import genconv_aggregate, SoftmaxAggrFunction  # noqa: F401
 from .disen_routing import disen_routing, DisenRouteFunction  # noqa: F401
 from .comp_aggr import compgcn_aggregate, CompAggrFunction  # noqa: F401
 from .spspmm import spspmm, coo_spmm, SpSpMMFunction  # noqa: F401
+from .spmm_residual import spmm_residual, SpmmResidualFunction  # noqa: F401

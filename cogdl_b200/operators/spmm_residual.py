@@ -1,0 +1,101 @@
+"""spmm_residual -- `a * spmm(graph, x) + b * z` in one SpMM launch (the propagation step of GCNII and APPNP).
+
+The reference computes it as `(1 - alpha) * spmm(graph, x) + alpha * init_x` (cogdl/layers/gcnii_layer.py:24-30,
+cogdl/models/nn/ppnp.py:77-83): the SpMM, then the graph's in_norm, then three elementwise passes over [N, F].  Here
+the scaling, the in_norm and the addition run in the SpMM's store (cogdl_b200_spmm_residual_f32), with the same fp32
+roundings in the same order, so the forward is bit-identical to that sequence run with this package's spmm."""
+import torch
+
+from .. import _cabi
+from ..structure import CSRStructure, _ptr, _stream, require_cuda
+from ._raw import _f32c, gather_rows_raw, sddmm_raw
+
+
+def spmm_residual_raw(st: CSRStructure, val, x, z, a, b, row_scale=None, panels=0):
+    """Y = a * (row_scale[:, None] * (A @ x)) + b * z with A = (st, val); z and row_scale may be None.  x [n_src, F]
+    fp32, z [n_rows, F] fp32, row_scale [n_rows] fp32, val [nnz] fp32 or None.  a and b are rounded to fp32.
+    panels: column panels of x, as for spmm_raw (0 = chosen by the library)."""
+    dev = require_cuda(x, z, val, row_scale)
+    x = _f32c(x, "x")
+    if x.dim() != 2:
+        raise ValueError("x must be [n_src, F]")
+    F = x.shape[1]
+    if z is not None:
+        z = _f32c(z, "z")
+        if z.shape != (st.n_rows, F):
+            raise ValueError(f"z must be [{st.n_rows}, {F}], got {tuple(z.shape)}")
+    if row_scale is not None:
+        row_scale = _f32c(row_scale, "row_scale").view(-1)
+        if row_scale.numel() != st.n_rows:
+            raise ValueError(f"row_scale has {row_scale.numel()} entries, the CSR has {st.n_rows} rows")
+    if val is not None:
+        val = _f32c(val, "edge values").view(-1)
+        if val.numel() != st.nnz:
+            raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
+    with torch.cuda.device(dev):
+        y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+        plan, keep = st.plan_struct(st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0)
+        _cabi.call("cogdl_b200_spmm_residual_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
+                   _ptr(z), float(a), float(b), _ptr(row_scale), _ptr(y), st.n_rows, F, int(panels), plan, _stream(dev))
+        del keep
+    return y
+
+
+class SpmmResidualFunction(torch.autograd.Function):
+    """out = a * (r * (A @ x)) + b * z.  Backward: d x = a * (A^T @ (r * g)) through the same kernel (A itself when
+    `sym`, as SPMMFunction does, else the cached transpose), d z = b * g, and d val = SDDMM(a * r * g, x) when the edge
+    weights require grad."""
+
+    @staticmethod
+    def forward(ctx, st, x, z, val, a, b, row_scale, sym):
+        out = spmm_residual_raw(st, val, x, z, a, b, row_scale)
+        ctx.st, ctx.a, ctx.b, ctx.sym = st, a, b, bool(sym)
+        need_w = val is not None and val.requires_grad
+        ctx.save_for_backward(val, x if need_w else None, row_scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        val, x, r = ctx.saved_tensors
+        st = ctx.st
+        g = g.contiguous()
+        gr = g if r is None else r.view(-1, 1) * g
+        dx = dz = dval = None
+        if ctx.needs_input_grad[1]:
+            if ctx.sym:
+                dx = spmm_residual_raw(st, val, gr, None, ctx.a, 0.0)
+            else:
+                st_t, perm = st.csc()
+                val_t = None if val is None else gather_rows_raw(perm, val.detach())
+                dx = spmm_residual_raw(st_t, val_t, gr, None, ctx.a, 0.0)
+        if ctx.needs_input_grad[2]:
+            dz = ctx.b * g
+        if val is not None and ctx.needs_input_grad[3]:
+            dval = sddmm_raw(st, ctx.a * gr, x)
+        return None, dx, dz, dval, None, None, None, None
+
+
+def spmm_residual(graph, x, z, a, b):
+    """a * spmm(graph, x) + b * z (z may be None) for fp32 CUDA tensors, in one SpMM launch.  The graph is taken as
+    cogdl_b200.spmm takes it: the cached int32 CSR and hub plan, out_norm applied to x first, in_norm applied to the
+    SpMM's rows (here inside the kernel), and the backward over A when graph.is_symmetric(), else over the cached
+    transpose.  The result is bit-identical to `a * spmm(graph, x) + b * z` computed by this package."""
+    from ..utils.spmm_utils import _structure
+
+    if getattr(graph, "grb_adj", None) is not None:
+        raise ValueError("spmm_residual: graphs carrying a dense grb_adj are not supported; use spmm")
+    if not x.is_cuda:
+        raise RuntimeError("cogdl_b200.spmm_residual: CPU tensors are not supported (no CPU fallback); move the graph "
+                           "and features to an H100 device")
+    if x.dtype != torch.float32 or (z is not None and z.dtype != torch.float32):
+        raise TypeError(f"spmm_residual takes float32 features, got {x.dtype}"
+                        f"{'' if z is None else ' and ' + str(z.dtype)}")
+    if graph.out_norm is not None:
+        x = graph.out_norm.to(x.device) * x
+    r = graph.in_norm
+    if r is not None:
+        if r.requires_grad:
+            raise ValueError("spmm_residual: an in_norm that requires grad is not supported")
+        r = r.to(x.device).reshape(-1)
+    val = graph.raw_edge_weight
+    return SpmmResidualFunction.apply(_structure(graph), x, z, val, float(a), float(b), r, graph.is_symmetric())

@@ -149,6 +149,20 @@ COGDL_B200_API int cogdl_b200_spmm_csr_f32_ex(const int32_t *rowptr, const int32
                                const float *X, int64_t x_rows, float *Y, int64_t n_rows, int64_t F,
                                int32_t panels, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
+/* SpMM with a residual epilogue: the propagation step of GCNII / APPNP, `a * (r * (A @ X)) + b * Z`, in one launch.
+ *   Y[i,:] = fl( fl(a * fl(r[i] * (A @ X)[i,:])) + fl(b * Z[i,:]) )
+ * A @ X is cogdl_b200_spmm_csr_f32_ex's sum (same kernels, same accumulation order, same x_rows / panels / plan
+ * rules, plan scratch sized as for it); each epilogue step is one fp32 multiply or add, so Y is bit-identical to the
+ * SpMM followed by those operations one at a time.  row_scale ([n_rows], may be NULL: r = 1, no multiply) is the
+ * in-degree normalisation applied after the SpMM; Z ([n_rows, F], may be NULL: no addition).  An empty row is the
+ * epilogue of a zero sum.  x_rows must be the number of rows of X (every colind value is below it).  Y must not
+ * overlap X (x_rows * F floats), Z or row_scale (COGDL_B200_EINVAL): they are still being read, through the read-only
+ * cache, while finished rows of Y are written.  Z, when 16-byte aligned like X and Y, is read as float4. */
+COGDL_B200_API int cogdl_b200_spmm_residual_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
+                               const float *X, int64_t x_rows, const float *Z, float a, float b,
+                               const float *row_scale, float *Y, int64_t n_rows, int64_t F, int32_t panels,
+                               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
 /* fp16 storage (X, val, Y are IEEE half), fp32 accumulation (the reference accumulates in
  * half, spmm_kernel.cu:222-250,311-368,442-512 -- documented divergence). */
 COGDL_B200_API int cogdl_b200_spmm_csr_f16(const int32_t *rowptr, const int32_t *colind, const void *val,
