@@ -31,45 +31,6 @@
 
 namespace cogdl_b200 {
 
-static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X0,
-                      int64_t n0, const float *X1, float *Y, int64_t n_rows, int64_t F,
-                      const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream, const char *who,
-                      const float *const *peers = nullptr, int n_peers = 0, int peer_shift = 0,
-                      int64_t x_rows = 0, int panels = 1) {
-  CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
-  CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
-  if (n_rows == 0 || F == 0) return COGDL_B200_OK;
-  CB_REQUIRE(rowptr && colind && X0 && Y, "%s: null pointer", who);
-  CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "%s: n_rows / F must fit int32", who);
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * F * (int64_t)sizeof(float));
-  if (rc) return rc;
-  SpmmParams p;
-  p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X0; p.X1 = X1 ? X1 : X0; p.n0 = n0;
-  p.Y = Y; p.n_rows = n_rows; p.hub = hub_view(plan);
-  p.n_peers = n_peers; p.peer_shift = peer_shift;
-  bool peers_aligned = true;
-  for (int i = 0; i < 8; ++i) {
-    p.peers[i] = (i < n_peers) ? peers[i] : nullptr;
-    peers_aligned = peers_aligned && aligned16(p.peers[i]);
-  }
-  if (n_peers > 0)
-    CB_REQUIRE(p.hub.n_segs > 0 && F % 4 == 0 && F <= 512 && peers_aligned && aligned16(X0) && aligned16(Y),
-               "%s: the peer form needs a plan with segments, F %% 4 == 0, F <= 512 and 16-byte aligned buffers", who);
-  const bool vec = (F % 4 == 0) && aligned16(X0) && aligned16(p.X1) && aligned16(Y) &&
-                   (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
-  if (vec) p.FV = (int)(F / 4);
-  const bool panel_form = vec && n_peers == 0 && n0 == INT64_MAX && p.hub.n_segs > 0 && F % 32 == 0;
-  if (panels > 1)
-    CB_REQUIRE(panel_form && panel_width_ok(F, panels),
-               "%s: %d panels need a plan with segments, one source, 16-byte aligned buffers and F / panels in "
-               "{32, 64, 128} (F=%lld, at most %d panels)", who, panels, (long long)F, COGDL_B200_MAX_PANELS);
-  const int P = panels == 0 ? (panel_form ? auto_panels(x_rows, F) : 1) : panels;
-  if (P > 1) return launch_spmm_panels(p, F, P, (cudaStream_t)stream);
-  if (vec) return dispatch_spmm<float4>(p, (cudaStream_t)stream);
-  p.FV = (int)F;
-  return dispatch_spmm<float>(p, (cudaStream_t)stream);
-}
-
 // ------------------------------------------------------------------------------------------
 // fp16 storage, fp32 accumulation.  One lane owns 4 halves (8 bytes); a warp covers 128
 // columns per pass.  (Reference: spmm_test{0,1,2}_half accumulate in half, spmm_kernel.cu:
@@ -166,11 +127,9 @@ __global__ void __launch_bounds__(256) spmm_half_kernel(const SpmmHalfParams p) 
 int spmm_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X, float *Y,
                        int64_t F, const cogdl_b200_hub_plan_t *plan, cudaStream_t stream) {
   SpmmParams p;
-  p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X; p.X1 = X; p.n0 = INT64_MAX; p.Y = Y; p.n_rows = 0;
+  p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X; p.X1 = X; p.Y = Y; p.n_rows = 0;
   p.hub = hub_view(plan);
   p.hub.n_segs = 0;
-  p.n_peers = 0; p.peer_shift = 0;
-  for (int i = 0; i < 8; ++i) p.peers[i] = nullptr;
   p.FV = (int)(F / 4);
   if (p.hub.n_chunks == 0) return COGDL_B200_OK;
   const StreamParams q = to_stream(p);
@@ -186,8 +145,8 @@ extern "C" int cogdl_b200_spmm_csr_f32_ex(const int32_t *rowptr, const int32_t *
                                           const float *X, int64_t x_rows, float *Y, int64_t n_rows, int64_t F,
                                           int32_t panels, const cogdl_b200_hub_plan_t *plan,
                                           cogdl_b200_stream_t stream) {
-  return spmm_entry(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream,
-                    "cogdl_b200_spmm_csr_f32_ex", nullptr, 0, 0, x_rows, panels);
+  return spmm_entry<false>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream,
+                           "cogdl_b200_spmm_csr_f32_ex", nullptr, 0, 0, x_rows, panels);
 }
 
 extern "C" int cogdl_b200_spmm_csr_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
@@ -202,8 +161,8 @@ extern "C" int cogdl_b200_spmm_csr_f32_2src(const int32_t *rowptr, const int32_t
                                             cogdl_b200_stream_t stream) {
   CB_REQUIRE(n0 >= 0, "cogdl_b200_spmm_csr_f32_2src: n0 < 0");
   CB_REQUIRE(X1 != nullptr || n0 == INT64_MAX, "cogdl_b200_spmm_csr_f32_2src: X1 is null");
-  return spmm_entry(rowptr, colind, val, X0, n0, X1, Y, n_rows, F, plan, stream,
-                    "cogdl_b200_spmm_csr_f32_2src");
+  return spmm_entry<false>(rowptr, colind, val, X0, n0, X1, Y, n_rows, F, plan, stream,
+                           "cogdl_b200_spmm_csr_f32_2src");
 }
 
 extern "C" int cogdl_b200_spmm_csr_f16(const int32_t *rowptr, const int32_t *colind, const void *val,
@@ -244,6 +203,6 @@ extern "C" int cogdl_b200_spmm_csr_f32_peers(const int32_t *rowptr, const int32_
   CB_REQUIRE(peer_ptrs && n_peers >= 1 && n_peers <= 8, "cogdl_b200_spmm_csr_f32_peers: need 1..8 peer pointers");
   CB_REQUIRE(owner_shift >= 1 && owner_shift <= 28 && n_local >= 0, "cogdl_b200_spmm_csr_f32_peers: bad owner_shift / n_local");
   for (int i = 0; i < n_peers; ++i) CB_REQUIRE(peer_ptrs[i], "cogdl_b200_spmm_csr_f32_peers: null peer pointer %d", i);
-  return spmm_entry(rowptr, colind, val, X_local, n_local, nullptr, Y, n_rows, F, plan, stream,
-                    "cogdl_b200_spmm_csr_f32_peers", peer_ptrs, n_peers, owner_shift);
+  return spmm_entry<false>(rowptr, colind, val, X_local, n_local, nullptr, Y, n_rows, F, plan, stream,
+                           "cogdl_b200_spmm_csr_f32_peers", peer_ptrs, n_peers, owner_shift);
 }

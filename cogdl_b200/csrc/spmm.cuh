@@ -1,6 +1,7 @@
-// spmm.cuh -- the fp32 SpMM's sub-warp row kernel and its dispatch by width, alignment, plan form and panel count,
-// shared by the plain SpMM (spmm.cu) and the SpMM with a residual epilogue (spmm_residual.cu).  RESID selects the
-// epilogue: every finished row is written as residual_out(acc) (stream.cuh) instead of acc.  Design notes: spmm.cu.
+// spmm.cuh -- the fp32 SpMM's sub-warp row kernel, its dispatch by width, alignment, plan form and panel count, and
+// the host entry in front of it, shared by the plain SpMM (spmm.cu) and the SpMM with a residual epilogue
+// (spmm_residual.cu).  RESID selects the epilogue: every finished row is written as residual_out(acc) (stream.cuh)
+// instead of acc.  Design notes: spmm.cu.
 #pragma once
 #include "common.cuh"
 #include "stream.cuh"
@@ -8,15 +9,15 @@
 namespace cogdl_b200 {
 
 struct SpmmParams {
-  const float *peers[8];
-  int n_peers;
-  int peer_shift;
+  const float *peers[8] = {};
+  int n_peers = 0;
+  int peer_shift = 0;
   const int *rowptr;
   const int *colind;
   const float *val;
   const float *X0;
   const float *X1;
-  int64_t n0;  // columns < n0 read X0, others X1[c - n0]
+  int64_t n0 = INT64_MAX;  // columns < n0 read X0, others X1[c - n0]
   float *Y;
   int64_t n_rows;
   int FV;      // feature row length in VecT units
@@ -223,7 +224,7 @@ static int auto_panels(int64_t x_rows, int64_t F) {
   return 1;
 }
 
-template <bool RESID = false>
+template <bool RESID>
 static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_t stream) {
   StreamParams q = to_stream(p);
   q.S = P;
@@ -258,7 +259,7 @@ static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
 // row kernel once a row needs at least this many vectors
 constexpr int SPMM_STREAM_MIN_FV = 9;
 
-template <typename VecT, bool RESID = false>
+template <typename VecT, bool RESID>
 static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
   const int fv = p.FV;
   // peer form: only the row-stream kernel decodes (owner << shift | row) columns (SRC_PEERS); the
@@ -276,6 +277,51 @@ static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
     if (fv > 64) return stream ? launch_spmm_stream<VecT, 4, RESID>(p, s) : launch_spmm<VecT, 32, 4, RESID>(p, s);
   }
   return stream ? launch_spmm_stream<VecT, 2, RESID>(p, s) : launch_spmm<VecT, 32, 2, RESID>(p, s);
+}
+
+// The host side of every fp32 SpMM entry point: argument checks, the parameters, the panel count and the dispatch.
+// X1 (nullptr = X0) serves the columns >= n0 (two-source form); peers are the peer form's shards; Z, row_scale, a and
+// b are the RESID epilogue's.  x_rows, X0's row count, sizes the automatic panel count (panels = 0).  Static, so each
+// object instantiates only the form it calls.
+template <bool RESID>
+static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X0, int64_t n0,
+                      const float *X1, float *Y, int64_t n_rows, int64_t F, const cogdl_b200_hub_plan_t *plan,
+                      cogdl_b200_stream_t stream, const char *who, const float *const *peers = nullptr,
+                      int n_peers = 0, int peer_shift = 0, int64_t x_rows = 0, int panels = 1,
+                      const float *Z = nullptr, const float *row_scale = nullptr, float a = 1.f, float b = 0.f) {
+  CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
+  CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
+  if (n_rows == 0 || F == 0) return COGDL_B200_OK;
+  CB_REQUIRE(rowptr && colind && X0 && Y, "%s: null pointer", who);
+  CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "%s: n_rows / F must fit int32", who);
+  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * F * (int64_t)sizeof(float));
+  if (rc) return rc;
+  SpmmParams p;
+  p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X0; p.X1 = X1 ? X1 : X0; p.n0 = n0;
+  p.Y = Y; p.n_rows = n_rows; p.hub = hub_view(plan);
+  p.n_peers = n_peers; p.peer_shift = peer_shift;
+  p.Z = Z; p.row_scale = row_scale; p.res_a = a; p.res_b = b;
+  bool peers_aligned = true;
+  for (int i = 0; i < n_peers; ++i) {
+    p.peers[i] = peers[i];
+    peers_aligned = peers_aligned && aligned16(peers[i]);
+  }
+  if (n_peers > 0)
+    CB_REQUIRE(p.hub.n_segs > 0 && F % 4 == 0 && F <= 512 && peers_aligned && aligned16(X0) && aligned16(Y),
+               "%s: the peer form needs a plan with segments, F %% 4 == 0, F <= 512 and 16-byte aligned buffers", who);
+  const bool vec = (F % 4 == 0) && aligned16(X0) && aligned16(p.X1) && aligned16(Y) && aligned16(Z) &&
+                   (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
+  if (vec) p.FV = (int)(F / 4);
+  const bool panel_form = vec && n_peers == 0 && n0 == INT64_MAX && p.hub.n_segs > 0 && F % 32 == 0;
+  if (panels > 1)
+    CB_REQUIRE(panel_form && panel_width_ok(F, panels),
+               "%s: %d panels need a plan with segments, one source, 16-byte aligned buffers and F / panels in "
+               "{32, 64, 128} (F=%lld, at most %d panels)", who, panels, (long long)F, COGDL_B200_MAX_PANELS);
+  const int P = panels == 0 ? (panel_form ? auto_panels(x_rows, F) : 1) : panels;
+  if (P > 1) return launch_spmm_panels<RESID>(p, F, P, (cudaStream_t)stream);
+  if (vec) return dispatch_spmm<float4, RESID>(p, (cudaStream_t)stream);
+  p.FV = (int)F;
+  return dispatch_spmm<float, RESID>(p, (cudaStream_t)stream);
 }
 
 }  // namespace cogdl_b200

@@ -30,35 +30,13 @@ extern "C" int cogdl_b200_spmm_residual_f32(const int32_t *rowptr, const int32_t
                                             int32_t panels, const cogdl_b200_hub_plan_t *plan,
                                             cogdl_b200_stream_t stream) {
   const char *who = "cogdl_b200_spmm_residual_f32";
-  CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
-  CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
-  if (n_rows == 0 || F == 0) return COGDL_B200_OK;
-  CB_REQUIRE(rowptr && colind && X && Y, "%s: null pointer", who);
-  CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "%s: n_rows / F must fit int32", who);
   // the kernels read X, Z and row_scale (read-only cache path) while other warps write finished Y rows; X holds
-  // x_rows rows (colind < x_rows), so an empty X can only coincide with Y
-  CB_REQUIRE(Y != X && !overlaps(Y, n_rows * F, X, x_rows * F), "%s: Y overlaps X", who);
-  CB_REQUIRE(!Z || !overlaps(Y, n_rows * F, Z, n_rows * F), "%s: Y overlaps Z", who);
-  CB_REQUIRE(!row_scale || !overlaps(Y, n_rows * F, row_scale, n_rows), "%s: Y overlaps row_scale", who);
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * F * (int64_t)sizeof(float));
-  if (rc) return rc;
-  SpmmParams p;
-  p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X; p.X1 = X; p.n0 = INT64_MAX;
-  p.Y = Y; p.n_rows = n_rows; p.hub = hub_view(plan);
-  p.n_peers = 0; p.peer_shift = 0;
-  for (int i = 0; i < 8; ++i) p.peers[i] = nullptr;
-  p.Z = Z; p.row_scale = row_scale; p.res_a = a; p.res_b = b;
-  const bool vec = (F % 4 == 0) && aligned16(X) && aligned16(Y) && aligned16(Z) &&
-                   (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
-  if (vec) p.FV = (int)(F / 4);
-  const bool panel_form = vec && p.hub.n_segs > 0 && F % 32 == 0;
-  if (panels > 1)
-    CB_REQUIRE(panel_form && panel_width_ok(F, panels),
-               "%s: %d panels need a plan with segments, 16-byte aligned buffers and F / panels in {32, 64, 128} "
-               "(F=%lld, at most %d panels)", who, panels, (long long)F, COGDL_B200_MAX_PANELS);
-  const int P = panels == 0 ? (panel_form ? auto_panels(x_rows, F) : 1) : panels;
-  if (P > 1) return launch_spmm_panels<true>(p, F, P, (cudaStream_t)stream);
-  if (vec) return dispatch_spmm<float4, true>(p, (cudaStream_t)stream);
-  p.FV = (int)F;
-  return dispatch_spmm<float, true>(p, (cudaStream_t)stream);
+  // x_rows rows (colind < x_rows), so an empty X can only coincide with Y.  An empty Y is written by no one.
+  if (n_rows > 0 && F > 0) {
+    CB_REQUIRE(Y != X && !overlaps(Y, n_rows * F, X, x_rows * F), "%s: Y overlaps X", who);
+    CB_REQUIRE(!Z || !overlaps(Y, n_rows * F, Z, n_rows * F), "%s: Y overlaps Z", who);
+    CB_REQUIRE(!row_scale || !overlaps(Y, n_rows * F, row_scale, n_rows), "%s: Y overlaps row_scale", who);
+  }
+  return spmm_entry<true>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream, who, nullptr, 0, 0,
+                          x_rows, panels, Z, row_scale, a, b);
 }

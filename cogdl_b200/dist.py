@@ -202,18 +202,17 @@ class PartitionedSpMM:
         import ctypes
 
         from . import _cabi
+        from .operators._raw import _spmm_out
         from .structure import _ptr, _stream
 
         buf, hdl, ptrs = self._symm
-        F = buf.shape[1]
         hdl.barrier()   # every rank's shard is written before anyone gathers from it
         dev = self.device
         with torch.cuda.device(dev):
-            y = torch.empty((self.n_local, F), dtype=torch.float32, device=dev)
-            plan, keep = self.st.plan_struct(self.st.plan.n_chunks * F * 4)
+            y, plan, keep = _spmm_out(self.st, self.val, buf)
             _cabi.call("cogdl_b200_spmm_csr_f32_peers", _ptr(self.st.rowptr), _ptr(self.st.colind), _ptr(self.val),
                        _ptr(buf), self.n_local, ctypes.cast(ptrs, ctypes.c_void_p), self.world, self.part.peer_shift,
-                       _ptr(y), self.n_local, F, plan, _stream(dev))
+                       _ptr(y), self.st.n_rows, buf.shape[1], plan, _stream(dev))
             del keep
         return y
 

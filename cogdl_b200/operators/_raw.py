@@ -12,32 +12,42 @@ def _f32c(t, name):
     return t.contiguous()
 
 
+def _spmm_scratch(st: CSRStructure, F):
+    """Bytes of plan scratch an SpMM of width F needs: one fp32 partial row per hub chunk."""
+    return st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0
+
+
+def _spmm_out(st: CSRStructure, val, x):
+    """What every SpMM wrapper shares: checks val against the nnz and x for being 2-D, allocates Y [n_rows, F] in x's
+    dtype and takes the plan with the SpMM's scratch.  Returns (y, plan, keepalive)."""
+    if x.dim() != 2:
+        raise ValueError("x must be [n_src, F]")
+    if val is not None and val.numel() != st.nnz:
+        raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
+    y = torch.empty((st.n_rows, x.shape[1]), dtype=x.dtype, device=x.device)
+    plan, keep = st.plan_struct(_spmm_scratch(st, x.shape[1]))
+    return y, plan, keep
+
+
 def spmm_raw(st: CSRStructure, val, x, panels=0):
     """Y = A @ X with A = (st, val).  x: [n_src, F] fp32 or fp16; val: [nnz] or None.
     panels: column panels of X for the fp32 kernel (0 = chosen from X's size against the L2; the output
     does not depend on it)."""
     dev = require_cuda(x, val)
-    if x.dim() != 2:
-        raise ValueError("x must be [n_src, F]")
     x = x.contiguous()
-    F = x.shape[1]
-    if val is not None:
-        if val.numel() != st.nnz:
-            raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
-        val = val.contiguous().view(-1)
+    val = None if val is None else val.contiguous().view(-1)
     with torch.cuda.device(dev):
-        y = torch.empty((st.n_rows, F), dtype=x.dtype, device=dev)
-        plan, keep = st.plan_struct(st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0)
+        y, plan, keep = _spmm_out(st, val, x)
         if x.dtype == torch.float32:
             if val is not None and val.dtype != torch.float32:
                 val = val.float()
             _cabi.call("cogdl_b200_spmm_csr_f32_ex", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
-                       _ptr(y), st.n_rows, F, int(panels), plan, _stream(dev))
+                       _ptr(y), st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
         elif x.dtype == torch.float16:
             if val is not None and val.dtype != torch.float16:
                 val = val.half()
             _cabi.call("cogdl_b200_spmm_csr_f16", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), _ptr(y),
-                       st.n_rows, F, plan, _stream(dev))
+                       st.n_rows, x.shape[1], plan, _stream(dev))
         else:
             raise TypeError(f"spmm supports float32 / float16 features, got {x.dtype}")
         del keep
@@ -48,18 +58,50 @@ def spmm_2src_raw(st: CSRStructure, val, x0, x1):
     """Partitioned SpMM: columns < x0.shape[0] read x0, the others read x1 (halo rows)."""
     dev = require_cuda(x0, x1, val)
     x0, x1 = _f32c(x0, "x0"), _f32c(x1, "x1")
-    F = x0.shape[1]
-    if x1.shape[1] != F:
+    if x1.shape[1] != x0.shape[1]:
         raise ValueError("x0 / x1 feature widths differ")
     val = None if val is None else _f32c(val, "val").view(-1)
     with torch.cuda.device(dev):
-        y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0)
+        y, plan, keep = _spmm_out(st, val, x0)
         x1p = x1 if x1.numel() > 0 else x0
         _cabi.call("cogdl_b200_spmm_csr_f32_2src", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x0),
-                   x0.shape[0], _ptr(x1p), _ptr(y), st.n_rows, F, plan, _stream(dev))
+                   x0.shape[0], _ptr(x1p), _ptr(y), st.n_rows, x0.shape[1], plan, _stream(dev))
         del keep
     return y
+
+
+def spmm_residual_raw(st: CSRStructure, val, x, z, a, b, row_scale=None, panels=0):
+    """Y = a * (row_scale[:, None] * (A @ x)) + b * z with A = (st, val); z and row_scale may be None.  x [n_src, F]
+    fp32, z [n_rows, F] fp32, row_scale [n_rows] fp32, val [nnz] fp32 or None.  a and b are rounded to fp32.
+    panels: column panels of x, as for spmm_raw (0 = chosen by the library)."""
+    dev = require_cuda(x, z, val, row_scale)
+    x = _f32c(x, "x")
+    z = None if z is None else _f32c(z, "z")
+    row_scale = None if row_scale is None else _f32c(row_scale, "row_scale").view(-1)
+    val = None if val is None else _f32c(val, "edge values").view(-1)
+    with torch.cuda.device(dev):
+        y, plan, keep = _spmm_out(st, val, x)
+        if z is not None and z.shape != y.shape:
+            raise ValueError(f"z must be [{st.n_rows}, {x.shape[1]}], got {tuple(z.shape)}")
+        if row_scale is not None and row_scale.numel() != st.n_rows:
+            raise ValueError(f"row_scale has {row_scale.numel()} entries, the CSR has {st.n_rows} rows")
+        _cabi.call("cogdl_b200_spmm_residual_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
+                   _ptr(z), float(a), float(b), _ptr(row_scale), _ptr(y), st.n_rows, x.shape[1], int(panels), plan,
+                   _stream(dev))
+        del keep
+    return y
+
+
+def spmm_adjoint_raw(st: CSRStructure, val, g, sym, a=None):
+    """A^T @ g, times a when a is given, for A = (st, val): the feature gradient of every SpMM-based operator.  Runs
+    over A itself when sym (A is symmetric), else over the cached transpose with the edge values permuted to it.
+    Without a it is spmm_raw (fp32 or fp16 g); with a it is spmm_residual_raw with b = 0 (fp32)."""
+    if not sym:
+        st, perm = st.csc()
+        val = None if val is None else gather_rows_raw(perm, val.detach().float())
+    if a is None:
+        return spmm_raw(st, val, g)
+    return spmm_residual_raw(st, val, g, None, a, 0.0)
 
 
 def sddmm_raw(st: CSRStructure, d1, d2):

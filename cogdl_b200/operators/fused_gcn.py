@@ -9,7 +9,7 @@ import torch
 
 from .. import _cabi
 from ..structure import CSRStructure, _ptr, _stream, require_cuda
-from ._raw import spmm_raw
+from ._raw import _spmm_scratch, spmm_adjoint_raw, spmm_raw
 
 
 def supported(K, Fout):
@@ -48,7 +48,7 @@ def fused_gcn_raw(st: CSRStructure, val, x, weight, bias=None, relu=False, cache
         return torch.zeros((st.n_rows, Fout), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         out = torch.empty((st.n_rows, Fout), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(st.plan.n_chunks * K * 4)
+        plan, keep = st.plan_struct(_spmm_scratch(st, K))
         hub = torch.empty((st.n_rows, K), dtype=torch.float32, device=dev) if st.plan.n_chunks > 0 else None
         rowsum = cached_rowsum(st, val) if (cache_rowsum and val is not None and bias is not None) else None
         _cabi.call("cogdl_b200_gcn_fused_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), _ptr(weight), _ptr(bias),
@@ -85,14 +85,7 @@ class FusedGCNFunction(torch.autograd.Function):
                 ones = torch.ones((x.shape[0], 4), device=x.device)
                 gb = g.t() @ spmm_raw(st, val, ones)[:, 0]
         if ctx.needs_input_grad[2]:
-            gwm = (g @ weight).contiguous()
-            if ctx.sym:
-                gx = spmm_raw(st, val, gwm)
-            else:
-                from ._raw import gather_rows_raw
-
-                st_t, perm = st.csc()
-                gx = spmm_raw(st_t, None if val is None else gather_rows_raw(perm, val), gwm)
+            gx = spmm_adjoint_raw(st, val, (g @ weight).contiguous(), ctx.sym)
         return None, None, gx, gw, gb, None, None
 
 

@@ -13,7 +13,7 @@ import torch.nn.functional as F
 
 from .. import _cabi
 from ..structure import CSRStructure, _ptr, _stream, require_cuda
-from ._raw import gather_rows_raw, scatter_max_bwd_raw, scatter_max_fwd_raw, spmm_raw
+from ._raw import scatter_max_bwd_raw, scatter_max_fwd_raw, spmm_adjoint_raw, spmm_raw
 from .fused_gcn import supported
 
 AGGR = {"sum": 0, "max": 1}     # COGDL_B200_AGGR_SUM / _MAX; mean is "sum" with row-normalised weights or row_scale
@@ -104,11 +104,7 @@ class FusedSAGEFunction(torch.autograd.Function):
             else:
                 if rs is not None:
                     d = rs * d
-                if ctx.sym:
-                    gx = spmm_raw(st, val, d)
-                else:
-                    st_t, perm = st.csc()
-                    gx = spmm_raw(st_t, None if val is None else gather_rows_raw(perm, val.detach().float()), d)
+                gx = spmm_adjoint_raw(st, val, d, ctx.sym)
             gx[:n] += g @ weight[:, :K]
         return None, None, None, gx, gw, gb, None, None, None
 

@@ -6,39 +6,7 @@ the scaling, the in_norm and the addition run in the SpMM's store (cogdl_b200_sp
 roundings in the same order, so the forward is bit-identical to that sequence run with this package's spmm."""
 import torch
 
-from .. import _cabi
-from ..structure import CSRStructure, _ptr, _stream, require_cuda
-from ._raw import _f32c, gather_rows_raw, sddmm_raw
-
-
-def spmm_residual_raw(st: CSRStructure, val, x, z, a, b, row_scale=None, panels=0):
-    """Y = a * (row_scale[:, None] * (A @ x)) + b * z with A = (st, val); z and row_scale may be None.  x [n_src, F]
-    fp32, z [n_rows, F] fp32, row_scale [n_rows] fp32, val [nnz] fp32 or None.  a and b are rounded to fp32.
-    panels: column panels of x, as for spmm_raw (0 = chosen by the library)."""
-    dev = require_cuda(x, z, val, row_scale)
-    x = _f32c(x, "x")
-    if x.dim() != 2:
-        raise ValueError("x must be [n_src, F]")
-    F = x.shape[1]
-    if z is not None:
-        z = _f32c(z, "z")
-        if z.shape != (st.n_rows, F):
-            raise ValueError(f"z must be [{st.n_rows}, {F}], got {tuple(z.shape)}")
-    if row_scale is not None:
-        row_scale = _f32c(row_scale, "row_scale").view(-1)
-        if row_scale.numel() != st.n_rows:
-            raise ValueError(f"row_scale has {row_scale.numel()} entries, the CSR has {st.n_rows} rows")
-    if val is not None:
-        val = _f32c(val, "edge values").view(-1)
-        if val.numel() != st.nnz:
-            raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
-    with torch.cuda.device(dev):
-        y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0)
-        _cabi.call("cogdl_b200_spmm_residual_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
-                   _ptr(z), float(a), float(b), _ptr(row_scale), _ptr(y), st.n_rows, F, int(panels), plan, _stream(dev))
-        del keep
-    return y
+from ._raw import sddmm_raw, spmm_adjoint_raw, spmm_residual_raw
 
 
 class SpmmResidualFunction(torch.autograd.Function):
@@ -62,12 +30,7 @@ class SpmmResidualFunction(torch.autograd.Function):
         gr = g if r is None else r.view(-1, 1) * g
         dx = dz = dval = None
         if ctx.needs_input_grad[1]:
-            if ctx.sym:
-                dx = spmm_residual_raw(st, val, gr, None, ctx.a, 0.0)
-            else:
-                st_t, perm = st.csc()
-                val_t = None if val is None else gather_rows_raw(perm, val.detach())
-                dx = spmm_residual_raw(st_t, val_t, gr, None, ctx.a, 0.0)
+            dx = spmm_adjoint_raw(st, val, gr, ctx.sym, ctx.a)
         if ctx.needs_input_grad[2]:
             dz = ctx.b * g
         if val is not None and ctx.needs_input_grad[3]:

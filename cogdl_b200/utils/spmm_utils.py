@@ -19,7 +19,7 @@ injection point); the `grb_adj` short-circuit (:86-91) is kept.
 import torch
 
 from ..operators import csrspmm, csr_edge_softmax, csrmhspmm, fused_gat_func
-from ..operators.spmm import ActSPMMFunction, SPMMFunction
+from ..operators.spmm import SPMMFunction
 from ..operators.edge_softmax import EdgeSoftmaxFunction
 from ..operators.mhspmm import MHSPMMFunction
 from ..operators.fused_gat import FusedGATFunction
@@ -83,8 +83,7 @@ def spmm(graph, x, actnn=False, fast_spmm=None, fast_spmm_cpu=None):
     if fast_spmm is not None and fast_spmm is not csrspmm:
         x = fast_spmm(graph.row_indptr.int(), graph.col_indices.int(), x, csr_data, graph.is_symmetric(), actnn=actnn)
     else:
-        fn = ActSPMMFunction if actnn else SPMMFunction
-        x = fn.apply(_structure(graph), None, x, csr_data, graph.is_symmetric())
+        x = SPMMFunction.apply(_structure(graph), None, x, csr_data, graph.is_symmetric(), actnn)
     if graph.in_norm is not None:
         x = graph.in_norm.to(x.device) * x
     return x

@@ -69,8 +69,7 @@ def bits(t):
 @pytest.mark.parametrize("c", TABLE, ids=lambda c: c.id)
 def test_forward_is_the_unfused_sequence_bit_for_bit(dev, c):
     from cogdl_b200 import _cabi
-    from cogdl_b200.operators._raw import spmm_raw
-    from cogdl_b200.operators.spmm_residual import spmm_residual_raw
+    from cogdl_b200.operators._raw import spmm_raw, spmm_residual_raw
 
     rp, ci, n_cols, X, Z, r, val = inputs(c, dev)
     st = structure(rp, ci, n_cols, dev, c)

@@ -193,8 +193,7 @@ def main():
     del models
     torch.cuda.empty_cache()
 
-    from cogdl_b200.operators._raw import spmm_raw
-    from cogdl_b200.operators.spmm_residual import spmm_residual_raw
+    from cogdl_b200.operators._raw import spmm_raw, spmm_residual_raw
 
     st, val = g.structure(), g.raw_edge_weight
     r = torch.rand(n, device="cuda") + 0.5
