@@ -145,7 +145,7 @@ extern "C" int cogdl_b200_spmm_csr_f32_ex(const int32_t *rowptr, const int32_t *
                                           const float *X, int64_t x_rows, float *Y, int64_t n_rows, int64_t F,
                                           int32_t panels, const cogdl_b200_hub_plan_t *plan,
                                           cogdl_b200_stream_t stream) {
-  return spmm_entry<false>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream,
+  return spmm_entry<EPI_NONE>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream,
                            "cogdl_b200_spmm_csr_f32_ex", nullptr, 0, 0, x_rows, panels);
 }
 
@@ -161,7 +161,7 @@ extern "C" int cogdl_b200_spmm_csr_f32_2src(const int32_t *rowptr, const int32_t
                                             cogdl_b200_stream_t stream) {
   CB_REQUIRE(n0 >= 0, "cogdl_b200_spmm_csr_f32_2src: n0 < 0");
   CB_REQUIRE(X1 != nullptr || n0 == INT64_MAX, "cogdl_b200_spmm_csr_f32_2src: X1 is null");
-  return spmm_entry<false>(rowptr, colind, val, X0, n0, X1, Y, n_rows, F, plan, stream,
+  return spmm_entry<EPI_NONE>(rowptr, colind, val, X0, n0, X1, Y, n_rows, F, plan, stream,
                            "cogdl_b200_spmm_csr_f32_2src");
 }
 
@@ -203,6 +203,6 @@ extern "C" int cogdl_b200_spmm_csr_f32_peers(const int32_t *rowptr, const int32_
   CB_REQUIRE(peer_ptrs && n_peers >= 1 && n_peers <= 8, "cogdl_b200_spmm_csr_f32_peers: need 1..8 peer pointers");
   CB_REQUIRE(owner_shift >= 1 && owner_shift <= 28 && n_local >= 0, "cogdl_b200_spmm_csr_f32_peers: bad owner_shift / n_local");
   for (int i = 0; i < n_peers; ++i) CB_REQUIRE(peer_ptrs[i], "cogdl_b200_spmm_csr_f32_peers: null peer pointer %d", i);
-  return spmm_entry<false>(rowptr, colind, val, X_local, n_local, nullptr, Y, n_rows, F, plan, stream,
+  return spmm_entry<EPI_NONE>(rowptr, colind, val, X_local, n_local, nullptr, Y, n_rows, F, plan, stream,
                            "cogdl_b200_spmm_csr_f32_peers", peer_ptrs, n_peers, owner_shift);
 }

@@ -1,7 +1,7 @@
 // spmm.cuh -- the fp32 SpMM's sub-warp row kernel, its dispatch by width, alignment, plan form and panel count, and
-// the host entry in front of it, shared by the plain SpMM (spmm.cu) and the SpMM with a residual epilogue
-// (spmm_residual.cu).  RESID selects the epilogue: every finished row is written as residual_out(acc) (stream.cuh)
-// instead of acc.  Design notes: spmm.cu.
+// the host entry in front of it, shared by the plain SpMM (spmm.cu), the SpMM with a residual epilogue
+// (spmm_residual.cu) and the label-propagation step (label_prop.cu).  EPI selects the epilogue: every finished row is
+// written as epilogue_out<EPI>(acc) (stream.cuh) -- acc itself for EPI_NONE.  Design notes: spmm.cu.
 #pragma once
 #include "common.cuh"
 #include "stream.cuh"
@@ -22,13 +22,17 @@ struct SpmmParams {
   int64_t n_rows;
   int FV;      // feature row length in VecT units
   HubView hub;
-  // residual epilogue (RESID): see StreamParams
+  // residual epilogue (EPI_RESID, EPI_LABELPROP): see StreamParams
   const float *Z = nullptr;
   const float *row_scale = nullptr;
   float res_a = 1.f, res_b = 0.f;
+  // label-propagation epilogue (EPI_LABELPROP): see StreamParams
+  const unsigned char *pin = nullptr;
+  int has_clamp = 0;
+  float clamp_lo = 0.f, clamp_hi = 0.f;
 };
 
-template <typename VecT, int GROUP, int NV, bool HAS_VAL, bool RESID>
+template <typename VecT, int GROUP, int NV, bool HAS_VAL, int EPI>
 __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
   constexpr int U0 = (NV == 1) ? 8 : (NV == 2 ? 4 : 2);
   constexpr int U = U0 < GROUP ? U0 : GROUP;
@@ -116,7 +120,7 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
         VecT *yp = Y + (int64_t)w.row * p.FV + cv;
 #pragma unroll
         for (int k = 0; k < NV; ++k)
-          if (colok[k]) st_stream(yp + k * GROUP, RESID ? residual_out(p, acc[k], w.row, yp + k * GROUP) : acc[k]);
+          if (colok[k]) st_stream(yp + k * GROUP, epilogue_out<EPI>(p, acc[k], w.row, yp + k * GROUP));
       }
     } else {
       VecT *pp = P + (int64_t)w.slot * p.FV + cv;
@@ -134,7 +138,7 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
         const VecT s = merge_chunks<1>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.FV); },
                                        [](VecT &a, const VecT &t) { add_rn(a, t); });
         VecT *yp = Y + (int64_t)w.row * p.FV + cv;
-        st_stream(yp, RESID ? residual_out(p, s, w.row, yp) : s);
+        st_stream(yp, epilogue_out<EPI>(p, s, w.row, yp));
       }
     }
   }
@@ -142,14 +146,20 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
 
 template <typename VecT, int GROUP, int NV, bool HAS_VAL>
 __global__ void __launch_bounds__(256) spmm_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, false>(p);
+  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_NONE>(p);
 }
 
 // at least 3 blocks per SM: left to itself ptxas fits the GROUP=4 float4 weighted instantiation in 64 registers
 // and spills; 80 registers hold every instantiation without spilling
 template <typename VecT, int GROUP, int NV, bool HAS_VAL>
 __global__ void __launch_bounds__(256, 3) spmm_residual_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, true>(p);
+  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_RESID>(p);
+}
+
+// the row kernel with the label-propagation epilogue (label_prop.cu); 3 blocks per SM as for the residual form
+template <typename VecT, int GROUP, int NV, bool HAS_VAL>
+__global__ void __launch_bounds__(256, 3) spmm_labelprop_kernel(const SpmmParams p) {
+  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_LABELPROP>(p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -164,19 +174,20 @@ static StreamParams to_stream(const SpmmParams &p) {
   q.n_peers = p.n_peers; q.peer_shift = p.peer_shift;
   for (int i = 0; i < 8; ++i) q.peers[i] = p.peers[i];
   q.Z = p.Z; q.row_scale = p.row_scale; q.res_a = p.res_a; q.res_b = p.res_b;
+  q.pin = p.pin; q.has_clamp = p.has_clamp; q.clamp_lo = p.clamp_lo; q.clamp_hi = p.clamp_hi;
   return q;
 }
 
-template <typename VecT, int NV, bool RESID>
+template <typename VecT, int NV, int EPI>
 static int launch_spmm_stream(const SpmmParams &p, cudaStream_t stream) {
   const StreamParams q = to_stream(p);
   if constexpr (NV == 1 && sizeof(VecT) == 16) {
     // lean loop (stream_range_lean), U=4, 48 registers (40 warps/SM); the epilogue's Z row needs 4 more registers
-    // than that budget holds, so the residual form runs at 32 warps/SM rather than spill
-    return launch_stream<VecT, 1, 4, RESID ? 4 : 5, false, FORM_PLAIN, RESID>(q, stream);
+    // than that budget holds, so the epilogue forms run at 32 warps/SM rather than spill
+    return launch_stream<VecT, 1, 4, EPI != EPI_NONE ? 4 : 5, false, FORM_PLAIN, EPI>(q, stream);
   } else {
     constexpr int U = (NV == 1) ? 8 : (NV == 2 ? 4 : 2);
-    return launch_stream<VecT, NV, U, 1, true, FORM_PLAIN, RESID>(q, stream);
+    return launch_stream<VecT, NV, U, 1, true, FORM_PLAIN, EPI>(q, stream);
   }
 }
 
@@ -224,29 +235,33 @@ static int auto_panels(int64_t x_rows, int64_t F) {
   return 1;
 }
 
-template <bool RESID>
+template <int EPI>
 static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_t stream) {
   StreamParams q = to_stream(p);
   q.S = P;
   switch (F / P) {
     case 32:
       q.ldv = q.FVL = (int)F;
-      return launch_stream<float, 1, 8, 6, true, FORM_PANEL, RESID>(q, stream);
+      return launch_stream<float, 1, 8, 6, true, FORM_PANEL, EPI>(q, stream);
     case 64:
       q.ldv = q.FVL = (int)(F / 2);
-      return launch_stream<float2, 1, 8, 5, true, FORM_PANEL, RESID>(q, stream);
+      return launch_stream<float2, 1, 8, 5, true, FORM_PANEL, EPI>(q, stream);
     default:
       q.ldv = q.FVL = (int)(F / 4);
-      return launch_stream<float4, 1, 4, RESID ? 4 : 5, true, FORM_PANEL, RESID>(q, stream);
+      return launch_stream<float4, 1, 4, EPI != EPI_NONE ? 4 : 5, true, FORM_PANEL, EPI>(q, stream);
   }
 }
 
-template <typename VecT, int GROUP, int NV, bool RESID>
+template <typename VecT, int GROUP, int NV, int EPI>
 static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
   const char *vec = sizeof(VecT) == 16 ? "float4" : "float";
   const char *what = p.val ? "weighted" : "unweighted";
   const int64_t items = (int64_t)p.hub.n_chunks + p.n_rows;
-  if constexpr (RESID)
+  if constexpr (EPI == EPI_LABELPROP)
+    return launch_items(p.val ? spmm_labelprop_kernel<VecT, GROUP, NV, true> : spmm_labelprop_kernel<VecT, GROUP, NV, false>,
+                        p, items, GROUP, stream, "label_prop",
+                        "cogdl_b200::spmm_labelprop_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
+  else if constexpr (EPI == EPI_RESID)
     return launch_items(p.val ? spmm_residual_kernel<VecT, GROUP, NV, true> : spmm_residual_kernel<VecT, GROUP, NV, false>,
                         p, items, GROUP, stream, "spmm_residual",
                         "cogdl_b200::spmm_residual_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
@@ -259,36 +274,44 @@ static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
 // row kernel once a row needs at least this many vectors
 constexpr int SPMM_STREAM_MIN_FV = 9;
 
-template <typename VecT, bool RESID>
+template <typename VecT, int EPI>
 static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
   const int fv = p.FV;
   // peer form: only the row-stream kernel decodes (owner << shift | row) columns (SRC_PEERS); the
   // sub-warp row kernel below would read them as X1[c - n0].  NV = 1 masks lanes >= fv.
-  if (p.n_peers > 0 && fv <= 32) return launch_spmm_stream<VecT, 1, RESID>(p, s);
+  if (p.n_peers > 0 && fv <= 32) return launch_spmm_stream<VecT, 1, EPI>(p, s);
   const bool stream = p.hub.n_segs > 0;
-  if (stream && fv >= SPMM_STREAM_MIN_FV && fv <= 16) return launch_spmm_stream<VecT, 1, RESID>(p, s);
-  if (fv <= 1) return launch_spmm<VecT, 1, 1, RESID>(p, s);
-  if (fv <= 2) return launch_spmm<VecT, 2, 1, RESID>(p, s);
-  if (fv <= 4) return launch_spmm<VecT, 4, 1, RESID>(p, s);
-  if (fv <= 8) return launch_spmm<VecT, 8, 1, RESID>(p, s);
-  if (fv <= 16) return launch_spmm<VecT, 16, 1, RESID>(p, s);
-  if (fv <= 32) return stream ? launch_spmm_stream<VecT, 1, RESID>(p, s) : launch_spmm<VecT, 32, 1, RESID>(p, s);
+  if (stream && fv >= SPMM_STREAM_MIN_FV && fv <= 16) return launch_spmm_stream<VecT, 1, EPI>(p, s);
+  if (fv <= 1) return launch_spmm<VecT, 1, 1, EPI>(p, s);
+  if (fv <= 2) return launch_spmm<VecT, 2, 1, EPI>(p, s);
+  if (fv <= 4) return launch_spmm<VecT, 4, 1, EPI>(p, s);
+  if (fv <= 8) return launch_spmm<VecT, 8, 1, EPI>(p, s);
+  if (fv <= 16) return launch_spmm<VecT, 16, 1, EPI>(p, s);
+  if (fv <= 32) return stream ? launch_spmm_stream<VecT, 1, EPI>(p, s) : launch_spmm<VecT, 32, 1, EPI>(p, s);
   if constexpr (sizeof(VecT) == 4) {
-    if (fv > 64) return stream ? launch_spmm_stream<VecT, 4, RESID>(p, s) : launch_spmm<VecT, 32, 4, RESID>(p, s);
+    if (fv > 64) return stream ? launch_spmm_stream<VecT, 4, EPI>(p, s) : launch_spmm<VecT, 32, 4, EPI>(p, s);
   }
-  return stream ? launch_spmm_stream<VecT, 2, RESID>(p, s) : launch_spmm<VecT, 32, 2, RESID>(p, s);
+  return stream ? launch_spmm_stream<VecT, 2, EPI>(p, s) : launch_spmm<VecT, 32, 2, EPI>(p, s);
+}
+
+// [p, p + n) and [q, q + m) share a byte: the epilogue entries' output overlap checks
+static inline bool overlaps(const float *p, int64_t n, const float *q, int64_t m) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+  return a < b + (uintptr_t)m * sizeof(float) && b < a + (uintptr_t)n * sizeof(float);
 }
 
 // The host side of every fp32 SpMM entry point: argument checks, the parameters, the panel count and the dispatch.
 // X1 (nullptr = X0) serves the columns >= n0 (two-source form); peers are the peer form's shards; Z, row_scale, a and
-// b are the RESID epilogue's.  x_rows, X0's row count, sizes the automatic panel count (panels = 0).  Static, so each
-// object instantiates only the form it calls.
-template <bool RESID>
+// b are the epilogue's (EPI_RESID, EPI_LABELPROP); pin, has_clamp, lo and hi the label-propagation epilogue's.  x_rows,
+// X0's row count, sizes the automatic panel count (panels = 0).  Static, so each object instantiates only the form it
+// calls.
+template <int EPI>
 static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X0, int64_t n0,
                       const float *X1, float *Y, int64_t n_rows, int64_t F, const cogdl_b200_hub_plan_t *plan,
                       cogdl_b200_stream_t stream, const char *who, const float *const *peers = nullptr,
                       int n_peers = 0, int peer_shift = 0, int64_t x_rows = 0, int panels = 1,
-                      const float *Z = nullptr, const float *row_scale = nullptr, float a = 1.f, float b = 0.f) {
+                      const float *Z = nullptr, const float *row_scale = nullptr, float a = 1.f, float b = 0.f,
+                      const unsigned char *pin = nullptr, int has_clamp = 0, float lo = 0.f, float hi = 0.f) {
   CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
   CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
@@ -301,6 +324,7 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
   p.Y = Y; p.n_rows = n_rows; p.hub = hub_view(plan);
   p.n_peers = n_peers; p.peer_shift = peer_shift;
   p.Z = Z; p.row_scale = row_scale; p.res_a = a; p.res_b = b;
+  p.pin = pin; p.has_clamp = has_clamp; p.clamp_lo = lo; p.clamp_hi = hi;
   bool peers_aligned = true;
   for (int i = 0; i < n_peers; ++i) {
     p.peers[i] = peers[i];
@@ -318,10 +342,10 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
                "%s: %d panels need a plan with segments, one source, 16-byte aligned buffers and F / panels in "
                "{32, 64, 128} (F=%lld, at most %d panels)", who, panels, (long long)F, COGDL_B200_MAX_PANELS);
   const int P = panels == 0 ? (panel_form ? auto_panels(x_rows, F) : 1) : panels;
-  if (P > 1) return launch_spmm_panels<RESID>(p, F, P, (cudaStream_t)stream);
-  if (vec) return dispatch_spmm<float4, RESID>(p, (cudaStream_t)stream);
+  if (P > 1) return launch_spmm_panels<EPI>(p, F, P, (cudaStream_t)stream);
+  if (vec) return dispatch_spmm<float4, EPI>(p, (cudaStream_t)stream);
   p.FV = (int)F;
-  return dispatch_spmm<float, RESID>(p, (cudaStream_t)stream);
+  return dispatch_spmm<float, EPI>(p, (cudaStream_t)stream);
 }
 
 }  // namespace cogdl_b200

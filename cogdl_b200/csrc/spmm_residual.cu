@@ -9,18 +9,8 @@
 // lean panel), their hub merge and the empty-row zero fill (an empty row is the epilogue of a zero sum).  A (A @ X)
 // is the plain SpMM's, in its accumulation order, and each epilogue step is one fp32 multiply or add in the unfused
 // sequence's order, so Y is bit-identical to that sequence.  The kernels and their dispatch are the SpMM's (spmm.cuh,
-// stream.cuh) with RESID set; this file holds their instantiations and the entry point.
+// stream.cuh) with EPI_RESID; this file holds their instantiations and the entry point.
 #include "spmm.cuh"
-
-namespace cogdl_b200 {
-
-// [p, p + n) and [q, q + m) share a byte
-static bool overlaps(const float *p, int64_t n, const float *q, int64_t m) {
-  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
-  return a < b + (uintptr_t)m * sizeof(float) && b < a + (uintptr_t)n * sizeof(float);
-}
-
-}  // namespace cogdl_b200
 
 using namespace cogdl_b200;
 
@@ -37,6 +27,6 @@ extern "C" int cogdl_b200_spmm_residual_f32(const int32_t *rowptr, const int32_t
     CB_REQUIRE(!Z || !overlaps(Y, n_rows * F, Z, n_rows * F), "%s: Y overlaps Z", who);
     CB_REQUIRE(!row_scale || !overlaps(Y, n_rows * F, row_scale, n_rows), "%s: Y overlaps row_scale", who);
   }
-  return spmm_entry<true>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream, who, nullptr, 0, 0,
+  return spmm_entry<EPI_RESID>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream, who, nullptr, 0, 0,
                           x_rows, panels, Z, row_scale, a, b);
 }

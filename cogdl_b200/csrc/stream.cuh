@@ -52,11 +52,17 @@ struct StreamParams {
   // MODE 2); a kept entry is read as att * drop_scale, a dropped one as 0 (drop_att, common.cuh).  Read only by
   // the multi-head form, which takes the DROP instantiation iff drop_scale > 0.
   float drop_scale;
-  // residual epilogue (spmm_residual.cu, RESID): every finished row i is written as
+  // residual epilogue (spmm_residual.cu, EPI_RESID): every finished row i is written as
   // fl(fl(res_a * fl(row_scale[i] * acc)) + fl(res_b * Z[i])); row_scale and Z are optional ([n_rows], [n_rows, ldv]).
   const float *Z = nullptr;
   const float *row_scale = nullptr;
   float res_a = 1.f, res_b = 0.f;
+  // label-propagation epilogue (label_prop.cu, EPI_LABELPROP): the residual epilogue's value, clamped to
+  // [clamp_lo, clamp_hi] as torch.clamp does when has_clamp; a row i with pin[i] != 0 stores Z[i] instead.  pin
+  // ([n_rows] bytes) is optional and needs Z.
+  const unsigned char *pin = nullptr;
+  int has_clamp = 0;
+  float clamp_lo = 0.f, clamp_hi = 0.f;
 };
 
 enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2, MODE_COMP_MULT = 3, MODE_COMP_SUB = 4 };
@@ -71,6 +77,9 @@ enum { SRC_ONE = 0, SRC_TWO = 1, SRC_PEERS = 2 };
 // What a launch_stream call runs: the plain SpMM (weighted iff p.val, any source form), its panel-major form, or
 // the multi-head SpMM.
 enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
+// What a store site of the plain SpMM writes: the sum (EPI_NONE), the residual epilogue of spmm_residual.cu
+// (EPI_RESID) or the label-propagation epilogue of label_prop.cu (EPI_LABELPROP).
+enum { EPI_NONE = 0, EPI_RESID = 1, EPI_LABELPROP = 2 };
 
 // The residual epilogue of one output element, rounded step by step as the unfused sequence
 // `a * (r * spmm(x)) + b * z` rounds it (no contraction); r and z are used iff has_r / has_z.
@@ -97,10 +106,38 @@ __device__ __forceinline__ VecT residual_out(const P &p, const VecT &acc, int64_
   return residual_rn(acc, z, hr, r, hz, p.res_a, p.res_b);
 }
 
+// torch.clamp(v, lo, hi) as its CUDA kernel evaluates it: a NaN passes through, otherwise min(max(v, lo), hi) with the
+// device fmaxf / fminf (so -0.0 against lo = 0 and lo > hi come out as torch gives them).
+__device__ __forceinline__ float clamp_torch(float v, float lo, float hi) { return isnan(v) ? v : fminf(fmaxf(v, lo), hi); }
+__device__ __forceinline__ float2 clamp_torch(float2 v, float lo, float hi) {
+  return make_float2(clamp_torch(v.x, lo, hi), clamp_torch(v.y, lo, hi));
+}
+__device__ __forceinline__ float4 clamp_torch(float4 v, float lo, float hi) {
+  return make_float4(clamp_torch(v.x, lo, hi), clamp_torch(v.y, lo, hi), clamp_torch(v.z, lo, hi), clamp_torch(v.w, lo, hi));
+}
+
+// The label-propagation epilogue of one output element: Z's element for a pinned row (the row reset of Correct &
+// Smooth's fixed_post), else the residual epilogue, clamped when p.has_clamp (autoscale_post).
+template <typename VecT, typename P>
+__device__ __forceinline__ VecT label_prop_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
+  if (p.pin != nullptr && __ldg(p.pin + row) != 0)
+    return __ldg(reinterpret_cast<const VecT *>(p.Z) + (yp - reinterpret_cast<const VecT *>(p.Y)));
+  const VecT v = residual_out(p, acc, row, yp);
+  return p.has_clamp ? clamp_torch(v, p.clamp_lo, p.clamp_hi) : v;
+}
+
+// acc of output row `row`, to be stored at yp, with the epilogue EPI applied.
+template <int EPI, typename VecT, typename P>
+__device__ __forceinline__ VecT epilogue_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
+  if constexpr (EPI == EPI_RESID) return residual_out(p, acc, row, yp);
+  else if constexpr (EPI == EPI_LABELPROP) return label_prop_out(p, acc, row, yp);
+  else return acc;
+}
+
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
 // whole range into acc (hub chunk).
 template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool ROWS, bool PREFETCH, bool DROP = false,
-          bool RESID = false>
+          int EPI = EPI_NONE>
 __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const int e_end, const int cv,
                                              const bool (&colok)[NV], const int head, const int lane,
                                              VecT (&acc)[NV]) {
@@ -190,7 +227,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
             for (int k = 0; k < NV; ++k)
               if (colok[k]) {
                 VecT *yp = Y + (int64_t)rj * p.ldv + k * 32;
-                st_stream(yp, RESID ? residual_out(p, acc[k], rj, yp) : acc[k]);
+                st_stream(yp, epilogue_out<EPI>(p, acc[k], rj, yp));
                 acc[k] = vzero<VecT>();
               }
           }
@@ -218,7 +255,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
 // mostly re-read by the next slab, instead of edge_row's 4 bytes per edge (plus the neighbour's) in every pass.  The
 // one-pass form keeps the edge_row test (`row != row of the next edge`, one ballot): there the cursor's longer
 // dependent chain per slab costs more than the bytes it saves (SpMM F=40 +2 %, DESIGN 3.1).
-template <typename VecT, int MODE, int SRC, int U, bool ROWS, bool PF = false, bool RESID = false>
+template <typename VecT, int MODE, int SRC, int U, bool ROWS, bool PF = false, int EPI = EPI_NONE>
 __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, const int e_end, int r, const int r_end,
                                                   const int cv, const bool colok, const int lane, int2 *s_cv, int *s_r,
                                                   VecT &acc) {
@@ -236,7 +273,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
   };
   auto store_row = [&](int rj) {                    // row rj is complete: store it (epilogue applied) and restart
     VecT *yp = Y + (int64_t)rj * p.ldv;
-    st_stream(yp, RESID ? residual_out(p, acc, rj, yp) : acc);
+    st_stream(yp, epilogue_out<EPI>(p, acc, rj, yp));
     acc = vzero<VecT>();
   };
   constexpr bool CURSOR = ROWS && PF;               // row ends from rowptr; otherwise (ROWS) from edge_row
@@ -340,7 +377,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
 
 // One work item processed by one warp: wid = item * S + slice (multi-head), slice = blockIdx.y (PANEL).
 template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, bool PREFETCH, bool PANEL, bool DROP = false,
-          bool RESID = false>
+          int EPI = EPI_NONE>
 __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t wid, const int lane, int2 *s_cv, int *s_r) {
   constexpr int TILE = 32 * NV;
   constexpr bool SLICED = (MODE == MODE_MULTIHEAD || PANEL);
@@ -392,7 +429,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
         const VecT s = merge_chunks<8>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.ldv); },
                                        [](VecT &a, const VecT &t) { add_rn(a, t); });
         VecT *yp = Y + (int64_t)w.row * p.ldv + cv;
-        st_stream(yp, RESID ? residual_out(p, s, w.row, yp) : s);
+        st_stream(yp, epilogue_out<EPI>(p, s, w.row, yp));
       }
     }
     return;
@@ -422,14 +459,14 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
           for (int k = 0; k < NV; ++k) {
             if (colok[k]) {
               VecT *yp = Y + (int64_t)(rb + k0) * p.ldv + cv + k * 32;
-              st_stream(yp, RESID ? residual_out(p, vzero<VecT>(), rb + k0, yp) : vzero<VecT>());
+              st_stream(yp, epilogue_out<EPI>(p, vzero<VecT>(), rb + k0, yp));
             }
           }
         }
       }
     }
-    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH, RESID>(p, e_begin, e_end, rr.x, rr.y, cv, colok[0], lane, s_cv, s_r, acc[0]);
-    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, DROP, RESID>(p, e_begin, e_end, cv, colok, head, lane, acc);
+    if constexpr (LEAN) stream_range_lean<VecT, MODE, SRC, U, true, PANEL && PREFETCH, EPI>(p, e_begin, e_end, rr.x, rr.y, cv, colok[0], lane, s_cv, s_r, acc[0]);
+    else stream_range<VecT, NV, MODE, HAS_PERM, SRC, U, true, PREFETCH, DROP, EPI>(p, e_begin, e_end, cv, colok, head, lane, acc);
   }
 }
 
@@ -456,16 +493,30 @@ __global__ void __launch_bounds__(256, MINB) stream_residual_kernel(const Stream
   int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
   int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, true>(p, wid, lane, s_cv, s_r);
+  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_RESID>(p, wid, lane, s_cv, s_r);
+}
+
+// stream_kernel of the plain SpMM (one source) with the label-propagation epilogue (label_prop.cu).
+template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
+__global__ void __launch_bounds__(256, MINB) stream_labelprop_kernel(const StreamParams p) {
+  const int lane = threadIdx.x & 31;
+  constexpr bool LEAN = is_lean<MODE, NV>();
+  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
+  __shared__ int s_r_all[LEAN ? 8 : 1][32];
+  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
+  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
+  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_LABELPROP>(p, wid, lane, s_cv, s_r);
 }
 
 // Launch helper: picks the instantiation of FORM for (weighted, perm, source form); U / MINB fixed by the caller.
-// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.  RESID: the plain
-// or panel form with the residual epilogue (stream_residual_kernel, one source).
-template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN, bool RESID = false>
+// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.  EPI: the plain
+// or panel form with the residual (stream_residual_kernel) or label-propagation (stream_labelprop_kernel) epilogue,
+// one source.
+template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN, int EPI = EPI_NONE>
 static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   static_assert(FORM == FORM_PLAIN || NV == 1, "the panel and multi-head forms have one VecT per lane");
-  static_assert(!RESID || FORM != FORM_MULTIHEAD, "the residual epilogue is a form of the plain SpMM");
+  static_assert(EPI == EPI_NONE || FORM != FORM_MULTIHEAD, "the store epilogues are forms of the plain SpMM");
   const int64_t warps = ((int64_t)p.hub.n_chunks + p.hub.n_segs) * (FORM == FORM_MULTIHEAD ? p.S : 1);
   // Threads per block: a launch parameter only -- the kernel indexes its per-warp slabs by warp-in-block and takes its
   // item from the global warp index, so every block size runs the same SASS and gives the same bits.  A block's warp
@@ -478,10 +529,11 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   if (blocks > 0x7fffffffLL) return set_error(COGDL_B200_EINVAL, "stream kernel: problem too large for one launch");
   const dim3 grid((unsigned)blocks, FORM == FORM_PANEL ? (unsigned)p.S : 1u);
   const int src = p.n_peers > 0 ? SRC_PEERS : (p.n0 != INT64_MAX ? SRC_TWO : SRC_ONE);
-  if ((FORM != FORM_PLAIN || RESID) && src != SRC_ONE)
-    return set_error(COGDL_B200_EINVAL, "stream kernel: the panel, multi-head and residual forms read one source");
+  if ((FORM != FORM_PLAIN || EPI != EPI_NONE) && src != SRC_ONE)
+    return set_error(COGDL_B200_EINVAL, "stream kernel: the panel, multi-head and epilogue forms read one source");
   const bool drop = FORM == FORM_MULTIHEAD && p.drop_scale > 0.f;
-  note_kernel("cogdl_b200::%s<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>", RESID ? "stream_residual_kernel" : "stream_kernel",
+  note_kernel("cogdl_b200::%s<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>",
+              EPI == EPI_RESID ? "stream_residual_kernel" : (EPI == EPI_LABELPROP ? "stream_labelprop_kernel" : "stream_kernel"),
               sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
               FORM == FORM_MULTIHEAD ? "multihead" : (p.val ? "weighted" : "unweighted"),
               (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "", drop ? "+drop" : "",
@@ -489,10 +541,14 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
               PREFETCH ? ",prefetch" : "");
   if (FORM == FORM_PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
   append_kernel_note(" block=%d", STREAM_BLOCK);
-  if constexpr (RESID) {
+  if constexpr (EPI == EPI_RESID) {
     constexpr bool PANEL = FORM == FORM_PANEL;
     if (p.val) stream_residual_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
     else stream_residual_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if constexpr (EPI == EPI_LABELPROP) {
+    constexpr bool PANEL = FORM == FORM_PANEL;
+    if (p.val) stream_labelprop_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_labelprop_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
   } else if constexpr (FORM == FORM_MULTIHEAD) {
     if (drop) {
       if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);

@@ -30,6 +30,11 @@ actnn=True provides the `actnn` API (cogdl_b200.actnn) to ActGCN, GCNII(actnn=Tr
 gcnii=True rebinds `cogdl.layers.gcnii_layer.GCNIILayer.forward` (GCNII) to gcnii_forward and appnp=True
 `cogdl.models.nn.ppnp.PPNP.forward` (APPNP) to appnp_forward; both send the initial-residual propagation to
 cogdl_b200.spmm_residual (uninstall_gcnii(), uninstall_appnp()).
+correct_smooth=True rebinds the module globals `outcome_correlation` and `diffusion` of `cogdl.models.nn.correct_smooth`
+(Correct & Smooth, CorrectSmoothMLP) to outcome_correlation / diffusion below: the propagation loops with the clamp or
+the row reset go to cogdl_b200.label_propagate, the p = 1 diffusion steps to cogdl_b200.spmm_residual.  The originals
+stay reachable as `_cogdl_b200_original_outcome_correlation` / `_cogdl_b200_original_diffusion` on that module
+(uninstall_correct_smooth() restores them).
 """
 import sys
 
@@ -273,6 +278,76 @@ def uninstall_appnp():
     _restore_forward(pm.PPNP)
 
 
+def _correct_smooth_module():
+    import cogdl.models.nn.correct_smooth as cs
+
+    return cs
+
+
+def _scalar(v):
+    return isinstance(v, (int, float)) and not isinstance(v, bool)
+
+
+def outcome_correlation(g, labels, alpha, nprop, post_step, alpha_term=True):
+    """outcome_correlation (cogdl/models/nn/correct_smooth.py) with its loop in cogdl_b200.label_propagate, one SpMM
+    launch per step, when post_step is one of the reference's two: partial(autoscale_post, lower=, upper=) with number
+    bounds (the clamp), or partial(fixed_post, y=labels, nid=) (the reset of the rows nid to labels, as every reference
+    call passes y).  Any other post step, CPU or non-fp32 labels, inputs requiring grad under grad mode and graphs with a
+    dense grb_adj run the original."""
+    import functools
+
+    from .operators.label_prop import label_propagate
+
+    cs = _correct_smooth_module()
+    original = cs._cogdl_b200_original_outcome_correlation
+    w = getattr(g, "raw_edge_weight", None)
+    if (not isinstance(post_step, functools.partial) or post_step.args or not torch.is_tensor(labels)
+            or not labels.is_cuda or labels.dtype != torch.float32 or getattr(g, "grb_adj", None) is not None
+            or (torch.is_grad_enabled() and (labels.requires_grad or (w is not None and w.requires_grad)))):
+        return original(g, labels, alpha, nprop, post_step, alpha_term)
+    kw = post_step.keywords
+    if post_step.func is cs.autoscale_post and set(kw) == {"lower", "upper"} and _scalar(kw["lower"]) and _scalar(kw["upper"]):
+        return label_propagate(g, labels, alpha, nprop, lower=kw["lower"], upper=kw["upper"], alpha_term=alpha_term)
+    if post_step.func is cs.fixed_post and set(kw) == {"y", "nid"} and kw["y"] is labels and torch.is_tensor(kw["nid"]):
+        return label_propagate(g, labels, alpha, nprop, pinned=kw["nid"], alpha_term=alpha_term)
+    return original(g, labels, alpha, nprop, post_step, alpha_term)
+
+
+def diffusion(g, x, nhtop, p=1, alpha=0.5):
+    """diffusion (cogdl/models/nn/correct_smooth.py) for p == 1: each step `(1 - alpha) * x + alpha * spmm(g, x)` is
+    cogdl_b200.spmm_residual(g, x, x, alpha, 1 - alpha) (fp32 addition commutes, so the bits are the same) and
+    `x ** 1` is x.  Any other p, CPU or non-fp32 features and graphs with a dense grb_adj run the original."""
+    from .operators.spmm_residual import spmm_residual
+
+    original = _correct_smooth_module()._cogdl_b200_original_diffusion
+    if p != 1 or not x.is_cuda or x.dtype != torch.float32 or getattr(g, "grb_adj", None) is not None:
+        return original(g, x, nhtop, p, alpha)
+    x = x ** p
+    for _ in range(nhtop):
+        x = spmm_residual(g, x, x, alpha, 1 - alpha)
+    return x
+
+
+def install_correct_smooth():
+    """Rebind cogdl.models.nn.correct_smooth.outcome_correlation and diffusion (resolved as module globals at call
+    time by CorrectSmooth.__call__ and CorrectSmoothMLP.forward), keeping the originals on the module; idempotent."""
+    cs = _correct_smooth_module()
+    patched = []
+    for name, new in (("outcome_correlation", outcome_correlation), ("diffusion", diffusion)):
+        if getattr(cs, name) is not new:
+            setattr(cs, "_cogdl_b200_original_" + name, getattr(cs, name))
+            setattr(cs, name, new)
+            patched.append(f"cogdl.models.nn.correct_smooth.{name}")
+    return patched
+
+
+def uninstall_correct_smooth():
+    cs = _correct_smooth_module()
+    for name, new in (("outcome_correlation", outcome_correlation), ("diffusion", diffusion)):
+        if getattr(cs, name) is new:
+            setattr(cs, name, getattr(cs, "_cogdl_b200_original_" + name))
+
+
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
 _spspmm_state = {"stub": None, "rebound": []}
 
@@ -377,7 +452,7 @@ def uninstall_actnn():
 
 
 def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
-            gcnii=False, appnp=False):
+            gcnii=False, appnp=False, correct_smooth=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -473,4 +548,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_gcnii()
     if appnp:
         patched += install_appnp()
+    if correct_smooth:
+        patched += install_correct_smooth()
     return patched

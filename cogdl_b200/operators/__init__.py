@@ -20,3 +20,4 @@ from .disen_routing import disen_routing, DisenRouteFunction  # noqa: F401
 from .comp_aggr import compgcn_aggregate, CompAggrFunction  # noqa: F401
 from .spspmm import spspmm, coo_spmm, SpSpMMFunction  # noqa: F401
 from .spmm_residual import spmm_residual, SpmmResidualFunction  # noqa: F401
+from .label_prop import label_propagate  # noqa: F401

@@ -163,6 +163,19 @@ COGDL_B200_API int cogdl_b200_spmm_residual_f32(const int32_t *rowptr, const int
                                const float *row_scale, float *Y, int64_t n_rows, int64_t F, int32_t panels,
                                const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
+/* One label-propagation step of Correct & Smooth (outcome_correlation) in one launch: the residual epilogue of
+ * cogdl_b200_spmm_residual_f32 followed by the post step.
+ *   Y[i,:] = pin[i] ? Z[i,:] : clamp( fl( fl(a * fl(r[i] * (A @ X)[i,:])) + fl(b * Z[i,:]) ), lo, hi )
+ * The clamp (has_clamp != 0) is torch.clamp's CUDA expression: a NaN passes, otherwise fminf(fmaxf(v, lo), hi).
+ * pin ([n_rows] bytes, may be NULL) marks the rows reset to Z (a non-zero byte; needs Z), which are stored as Z's row
+ * bit for bit.  Everything else -- sums, x_rows, panels, plan scratch, the alignment rules and the overlap checks
+ * (COGDL_B200_EINVAL) -- is as for cogdl_b200_spmm_residual_f32. */
+COGDL_B200_API int cogdl_b200_label_prop_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
+                               const float *X, int64_t x_rows, const float *Z, float a, float b,
+                               const float *row_scale, const uint8_t *pin, int32_t has_clamp, float lo, float hi,
+                               float *Y, int64_t n_rows, int64_t F, int32_t panels,
+                               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
 /* fp16 storage (X, val, Y are IEEE half), fp32 accumulation (the reference accumulates in
  * half, spmm_kernel.cu:222-250,311-368,442-512 -- documented divergence). */
 COGDL_B200_API int cogdl_b200_spmm_csr_f16(const int32_t *rowptr, const int32_t *colind, const void *val,
