@@ -109,6 +109,9 @@ class GATLayer(nn.Module):
             out = fused_gat_op(h_l, h_r, graph, self.alpha, h, attn_drop=p)
             out = out.view(out.shape[0], -1)
         else:
+            # the CSR before edge_index: edge_softmax reads the logits in CSR order, and building the CSR of a graph
+            # held as COO reorders its edges
+            graph.row_indptr
             row, col = graph.edge_index
             e = self.leakyrelu(h_l[row] + h_r[col])      # [E, H]
             a = self.edge_softmax(graph, e)

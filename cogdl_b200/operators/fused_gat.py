@@ -57,7 +57,9 @@ class FusedGATFunction(torch.autograd.Function):
         if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
             grad_att = mhsddmm_raw(st, grad_out, feat)                        # [E,H]
             d_edge, g_row = gat_attn_bwd_raw(st, att, grad_att, attn_row, attn_col, ctx.slope, drop_scale=ds)
-            g_col = edge_colsum_raw(st_t, perm, d_edge)
+            g_col = edge_colsum_raw(st_t, perm, d_edge) if ctx.needs_input_grad[1] else None
+            if not ctx.needs_input_grad[0]:
+                g_row = None
         return g_row, g_col, None, None, None, None, None, grad_feat, None, None
 
 

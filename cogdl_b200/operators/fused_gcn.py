@@ -93,6 +93,8 @@ def fused_gcn_layer(graph, x, weight, bias=None, relu=False):
     """graph: cogdl_b200.Graph or a real cogdl.data.Graph (same attribute surface as spmm())."""
     from ..utils.spmm_utils import _structure
 
+    # the structure before the weights: building the CSR of a graph held as COO puts its edge weights in CSR order
+    st = _structure(graph)
     if graph.out_norm is not None or graph.in_norm is not None:
         raise NotImplementedError("fused GCN layer: graphs with separate in/out norms take the unfused path")
-    return FusedGCNFunction.apply(_structure(graph), graph.raw_edge_weight, x, weight, bias, relu, graph.is_symmetric())
+    return FusedGCNFunction.apply(st, graph.raw_edge_weight, x, weight, bias, relu, graph.is_symmetric())

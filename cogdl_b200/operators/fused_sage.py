@@ -116,6 +116,9 @@ def fused_sage_layer(graph, x, weight, bias=None, aggr="mean", relu=False):
 
     if aggr == "mean":
         graph.row_norm()
+    # the structure before the weights: building the CSR of a graph held as COO puts its edge weights (the 1/deg that
+    # row_norm() just baked in, for a COO graph) in CSR order
+    st = _structure(graph)
     if graph.out_norm is not None:
         raise NotImplementedError("fused SAGE layer: graphs with an out_norm take the unfused path")
     if aggr == "max":
@@ -124,5 +127,5 @@ def fused_sage_layer(graph, x, weight, bias=None, aggr="mean", relu=False):
         val, row_scale = graph.raw_edge_weight, graph.in_norm
         if val.requires_grad:
             raise NotImplementedError("fused SAGE layer: trainable edge weights take the unfused path")
-    return FusedSAGEFunction.apply(_structure(graph), val, row_scale, x, weight, bias, "max" if aggr == "max" else "sum",
-                                   relu, graph.is_symmetric())
+    return FusedSAGEFunction.apply(st, val, row_scale, x, weight, bias, "max" if aggr == "max" else "sum", relu,
+                                   graph.is_symmetric())

@@ -53,6 +53,8 @@ def spmm_residual(graph, x, z, a, b):
     if x.dtype != torch.float32 or (z is not None and z.dtype != torch.float32):
         raise TypeError(f"spmm_residual takes float32 features, got {x.dtype}"
                         f"{'' if z is None else ' and ' + str(z.dtype)}")
+    # the structure first: building the CSR of a graph held as COO puts its edge weights in CSR order
+    st = _structure(graph)
     if graph.out_norm is not None:
         x = graph.out_norm.to(x.device) * x
     r = graph.in_norm
@@ -61,4 +63,4 @@ def spmm_residual(graph, x, z, a, b):
             raise ValueError("spmm_residual: an in_norm that requires grad is not supported")
         r = r.to(x.device).reshape(-1)
     val = graph.raw_edge_weight
-    return SpmmResidualFunction.apply(_structure(graph), x, z, val, float(a), float(b), r, graph.is_symmetric())
+    return SpmmResidualFunction.apply(st, x, z, val, float(a), float(b), r, graph.is_symmetric())

@@ -75,15 +75,21 @@ def spmm(graph, x, actnn=False, fast_spmm=None, fast_spmm_cpu=None):
     if not x.is_cuda:
         raise RuntimeError("cogdl_b200.spmm: CPU tensors are not supported (no CPU fallback); move the graph and "
                            "features to an H100 device")
+    # the CSR before the weights: building it from a graph held as COO puts that graph's edge weights in CSR order
+    custom = fast_spmm is not None and fast_spmm is not csrspmm
+    if custom:
+        row_ptr, col = graph.row_indptr.int(), graph.col_indices.int()
+    else:
+        st = _structure(graph)
     if graph.out_norm is not None:
         x = graph.out_norm.to(x.device) * x
     csr_data = graph.raw_edge_weight
     if x.dtype == torch.half:
         csr_data = csr_data.half()
-    if fast_spmm is not None and fast_spmm is not csrspmm:
-        x = fast_spmm(graph.row_indptr.int(), graph.col_indices.int(), x, csr_data, graph.is_symmetric(), actnn=actnn)
+    if custom:
+        x = fast_spmm(row_ptr, col, x, csr_data, graph.is_symmetric(), actnn=actnn)
     else:
-        x = SPMMFunction.apply(_structure(graph), None, x, csr_data, graph.is_symmetric(), actnn)
+        x = SPMMFunction.apply(st, None, x, csr_data, graph.is_symmetric(), actnn)
     if graph.in_norm is not None:
         x = graph.in_norm.to(x.device) * x
     return x
@@ -100,6 +106,9 @@ class SpMM(torch.nn.Module):
 
 
 def edge_softmax(graph, edge_val, csr_edge_softmax=None):
+    """Softmax of edge_val [E] or [E, H] over each row's edges.  As in the reference, edge_val is taken in the graph's
+    CSR order: a graph still held as COO is put in CSR order by this call, and its edge_index is CSR-ordered after it,
+    so values formed from graph.edge_index before the call are read in an order they were not formed in."""
     if not edge_val.is_cuda:
         raise RuntimeError("cogdl_b200.edge_softmax: CPU tensors are not supported (no CPU fallback)")
     flat = edge_val.dim() == 1
@@ -122,6 +131,9 @@ class EdgeSoftmax(torch.nn.Module):
 
 
 def mh_spmm(graph, attention, h, csrmhspmm=None, fast_spmm=None):
+    """out[i, h] = sum over row i's edges p of attention[p, h] * h[col[p], h], flattened to [N, H * F].  attention
+    [E, H] is taken in the graph's CSR order (as edge_softmax takes its values), for every H: a graph still held as COO
+    is put in CSR order first, so the single-head path's edge weight is not reordered again inside local_graph()."""
     if not h.is_cuda:
         raise RuntimeError("cogdl_b200.mh_spmm: CPU tensors are not supported (no CPU fallback)")
     nhead = h.shape[1]
@@ -132,7 +144,9 @@ def mh_spmm(graph, attention, h, csrmhspmm=None, fast_spmm=None):
             h_prime = MHSPMMFunction.apply(_structure(graph), None, h, attention)
         return h_prime.view(h_prime.shape[0], -1)
     # single head: SpMM with the attention as edge weight inside local_graph() (reference :210-214;
-    # set_weight flips the symmetric flag, so the backward takes the transpose branch)
+    # set_weight flips the symmetric flag, so the backward takes the transpose branch).  The structure is built first, on
+    # the graph itself: built inside the block, it would reorder the attention as a COO-ordered weight.
+    _structure(graph)
     edge_weight = attention.view(-1)
     with graph.local_graph():
         graph.edge_weight = edge_weight
