@@ -40,6 +40,8 @@ import sys
 
 import torch
 
+from .structure import graph_operands, unsupported_operands
+
 _GENCONV_KERNEL_AGGRS = ("softmax_sg", "softmax", "mean", "sum", "max", "powermean")
 
 
@@ -48,14 +50,13 @@ def genconv_forward(self, graph, x):
     edge encoder, message_norm, residual and MLP are the layer's own.  Cases without a kernel -- CPU or non-fp32
     input, an aggregation name GENConv does not define, max / powermean with an edge encoder -- run the original."""
     from .operators.softmax_aggr import genconv_aggregate
-    from .utils.spmm_utils import _structure
 
     original = type(self)._cogdl_b200_original_forward
     has_edge = self.edge_encoder is not None and graph.edge_attr is not None
     if (not x.is_cuda or x.dtype != torch.float32 or self.aggr not in _GENCONV_KERNEL_AGGRS
             or (has_edge and self.aggr in ("max", "powermean"))):
         return original(self, graph, x)
-    st = _structure(graph)         # puts the graph in CSR order first, edge_attr included (data.py:279-287)
+    st = graph_operands(graph).st
     edge_term = self.edge_encoder(graph.edge_attr) if has_edge else None
     h = genconv_aggregate(st, x, self.aggr, beta=self.beta, eps=self.eps, edge_term=edge_term, p=self.p)
     if self.use_msg_norm:
@@ -98,7 +99,6 @@ def disengcn_forward(self, graph, x):
     normalisation and the iterations.  CPU or non-fp32 input and channel widths without a kernel (d not a power
     of two up to 32, or out_feats not K * d) run the original."""
     from .operators.disen_routing import SUPPORTED_D, disen_routing
-    from .utils.spmm_utils import _structure
 
     original = type(self)._cogdl_b200_original_forward
     d, K = self.factor_dim, self.K
@@ -106,7 +106,7 @@ def disengcn_forward(self, graph, x):
             or self.weight.shape[1] != K * d):
         return original(self, graph, x)
     h = self.activation(torch.matmul(x, self.weight) + self.bias)
-    return disen_routing(_structure(graph), h, K, self.iterations, self.tau)
+    return disen_routing(graph_operands(graph).st, h, K, self.iterations, self.tau)
 
 
 def install_disengcn():
@@ -169,7 +169,7 @@ def gat_forward(self, graph, x):
     own W, a_l, a_r, NaN zeroing, residual, norm and activation are used; the attention dropout is self.dropout.p
     when training and none in eval, drawn in the kernel (a fresh seed from torch's CPU generator per call).  CPU or
     non-fp32 input or weights, and a dropout of 1, run the original."""
-    from .utils.spmm_utils import FusedGATFunction, _structure
+    from .utils.spmm_utils import FusedGATFunction
 
     original = type(self)._cogdl_b200_original_forward
     p = self.dropout.p if self.training else 0.0
@@ -180,7 +180,7 @@ def gat_forward(self, graph, x):
     h[torch.isnan(h)] = 0.0
     h_l = (self.a_l * h).sum(dim=-1)
     h_r = (self.a_r * h).sum(dim=-1)
-    out = FusedGATFunction.apply(h_l, h_r, _structure(graph), None, None, None, self.alpha, h, p, None)
+    out = FusedGATFunction.apply(h_l, h_r, graph_operands(graph).st, None, None, None, self.alpha, h, p, None)
     out = out.view(out.shape[0], -1)
     if self.residual is not None:
         out = out + self.residual(x)
@@ -213,8 +213,8 @@ def gcnii_forward(self, graph, x, init_x):
 
     original = type(self)._cogdl_b200_original_forward
     lin = self.linear
-    if (not x.is_cuda or x.dtype != torch.float32 or init_x.dtype != torch.float32 or lin.weight.dtype != torch.float32
-            or (lin.bias is not None and lin.bias.dtype != torch.float32) or getattr(graph, "grb_adj", None) is not None):
+    if (unsupported_operands(graph, x, init_x) is not None or lin.weight.dtype != torch.float32
+            or (lin.bias is not None and lin.bias.dtype != torch.float32)):
         return original(self, graph, x, init_x)
     s = spmm_residual(graph, x, init_x, 1 - self.alpha, self.alpha)
     beta = self.beta
@@ -251,8 +251,8 @@ def appnp_forward(self, graph):
 
     original = type(self)._cogdl_b200_original_forward
     x = graph.x
-    if (self.propagation != "appnp" or not x.is_cuda or x.dtype != torch.float32
-            or any(p.dtype != torch.float32 for p in self.nn.parameters()) or getattr(graph, "grb_adj", None) is not None):
+    if (self.propagation != "appnp" or unsupported_operands(graph, x) is not None
+            or any(p.dtype != torch.float32 for p in self.nn.parameters())):
         return original(self, graph)
     graph.sym_norm()
     x = F.dropout(x, p=self.dropout, training=self.training)
@@ -302,7 +302,7 @@ def outcome_correlation(g, labels, alpha, nprop, post_step, alpha_term=True):
     original = cs._cogdl_b200_original_outcome_correlation
     w = getattr(g, "raw_edge_weight", None)
     if (not isinstance(post_step, functools.partial) or post_step.args or not torch.is_tensor(labels)
-            or not labels.is_cuda or labels.dtype != torch.float32 or getattr(g, "grb_adj", None) is not None
+            or unsupported_operands(g, labels) is not None
             or (torch.is_grad_enabled() and (labels.requires_grad or (w is not None and w.requires_grad)))):
         return original(g, labels, alpha, nprop, post_step, alpha_term)
     kw = post_step.keywords
@@ -320,7 +320,7 @@ def diffusion(g, x, nhtop, p=1, alpha=0.5):
     from .operators.spmm_residual import spmm_residual
 
     original = _correct_smooth_module()._cogdl_b200_original_diffusion
-    if p != 1 or not x.is_cuda or x.dtype != torch.float32 or getattr(g, "grb_adj", None) is not None:
+    if p != 1 or unsupported_operands(g, x) is not None:
         return original(g, x, nhtop, p, alpha)
     x = x ** p
     for _ in range(nhtop):

@@ -12,6 +12,7 @@ import torch.nn.functional as F
 
 from .utils.spmm_utils import spmm, EdgeSoftmax, MultiHeadSpMM, fused_gat_op, check_fused_gat
 from .operators.scatter_max import ScatterMaxFunction
+from .structure import csr_order, graph_operands
 
 
 def _activation(name):
@@ -55,8 +56,9 @@ class GCNLayer(nn.Module):
     def forward(self, graph, x):
         from .operators import fused_gcn
 
-        if (self.fused and self.norm is None and x.is_cuda and x.dtype == torch.float32 and graph.out_norm is None
-                and graph.in_norm is None and fused_gcn.supported(self.in_features, self.out_features)):
+        if (self.fused and self.norm is None and x.is_cuda and x.dtype == torch.float32
+                and fused_gcn.supported(self.in_features, self.out_features)
+                and (ops := graph_operands(graph)).out_norm is None and ops.in_norm is None):
             relu = self._act_name == "relu"
             out = fused_gcn.fused_gcn_layer(graph, x, self.linear.weight, self.linear.bias, relu=relu)
             if self.act is not None and not relu:
@@ -109,9 +111,7 @@ class GATLayer(nn.Module):
             out = fused_gat_op(h_l, h_r, graph, self.alpha, h, attn_drop=p)
             out = out.view(out.shape[0], -1)
         else:
-            # the CSR before edge_index: edge_softmax reads the logits in CSR order, and building the CSR of a graph
-            # held as COO reorders its edges
-            graph.row_indptr
+            csr_order(graph)                             # edge_index in the order edge_softmax reads the logits in
             row, col = graph.edge_index
             e = self.leakyrelu(h_l[row] + h_r[col])      # [E, H]
             a = self.edge_softmax(graph, e)
@@ -169,9 +169,8 @@ class SAGELayer(nn.Module):
             return False
         if self._aggr_name == "mean":
             graph.row_norm()             # as MeanAggregator, before the norms are looked at
-        if graph.out_norm is not None:
-            return False
-        return self._aggr_name == "max" or not graph.raw_edge_weight.requires_grad
+        ops = graph_operands(graph)
+        return ops.out_norm is None and (self._aggr_name == "max" or not ops.val.requires_grad)
 
     def forward(self, graph, x):
         relu = False

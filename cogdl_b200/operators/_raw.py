@@ -17,16 +17,45 @@ def _spmm_scratch(st: CSRStructure, F):
     return st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0
 
 
-def _spmm_out(st: CSRStructure, val, x):
+def _spmm_out(st: CSRStructure, val, x, out=None):
     """What every SpMM wrapper shares: checks val against the nnz and x for being 2-D, allocates Y [n_rows, F] in x's
-    dtype and takes the plan with the SpMM's scratch.  Returns (y, plan, keepalive)."""
+    dtype (unless given `out`) and takes the plan with the SpMM's scratch.  Returns (y, plan, keepalive)."""
     if x.dim() != 2:
         raise ValueError("x must be [n_src, F]")
     if val is not None and val.numel() != st.nnz:
         raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
-    y = torch.empty((st.n_rows, x.shape[1]), dtype=x.dtype, device=x.device)
+    y = torch.empty((st.n_rows, x.shape[1]), dtype=x.dtype, device=x.device) if out is None else out
     plan, keep = st.plan_struct(_spmm_scratch(st, x.shape[1]))
     return y, plan, keep
+
+
+def _epilogue_args(st: CSRStructure, val, x, z, row_scale):
+    """The operands of an SpMM-epilogue entry (residual, label propagation), checked and made fp32 contiguous:
+    (device, val [nnz], x [n_src, F], z [n_rows, F], row_scale [n_rows]); val, z and row_scale may be None."""
+    dev = require_cuda(x, z, val, row_scale)
+    x = _f32c(x, "x")
+    if x.dim() != 2:
+        raise ValueError("x must be [n_src, F]")
+    z = None if z is None else _f32c(z, "z")
+    row_scale = None if row_scale is None else _f32c(row_scale, "row_scale").view(-1)
+    val = None if val is None else _f32c(val, "edge values").view(-1)
+    if z is not None and z.shape != (st.n_rows, x.shape[1]):
+        raise ValueError(f"z must be [{st.n_rows}, {x.shape[1]}], got {tuple(z.shape)}")
+    if row_scale is not None and row_scale.numel() != st.n_rows:
+        raise ValueError(f"row_scale has {row_scale.numel()} entries, the CSR has {st.n_rows} rows")
+    return dev, val, x, z, row_scale
+
+
+def _spmm_epilogue_raw(symbol, st: CSRStructure, val, x, z, a, b, row_scale, extra=(), panels=0, out=None):
+    """One launch of an SpMM-epilogue entry: symbol(rowptr, colind, val, x, n_src, z, a, b, row_scale, *extra, y,
+    n_rows, F, panels, plan, stream), with the operands of _epilogue_args.  Returns y (`out` when given)."""
+    dev, val, x, z, row_scale = _epilogue_args(st, val, x, z, row_scale)
+    with torch.cuda.device(dev):
+        y, plan, keep = _spmm_out(st, val, x, out)
+        _cabi.call(symbol, _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0], _ptr(z), float(a),
+                   float(b), _ptr(row_scale), *extra, _ptr(y), st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
+        del keep
+    return y
 
 
 def spmm_raw(st: CSRStructure, val, x, panels=0):
@@ -74,22 +103,7 @@ def spmm_residual_raw(st: CSRStructure, val, x, z, a, b, row_scale=None, panels=
     """Y = a * (row_scale[:, None] * (A @ x)) + b * z with A = (st, val); z and row_scale may be None.  x [n_src, F]
     fp32, z [n_rows, F] fp32, row_scale [n_rows] fp32, val [nnz] fp32 or None.  a and b are rounded to fp32.
     panels: column panels of x, as for spmm_raw (0 = chosen by the library)."""
-    dev = require_cuda(x, z, val, row_scale)
-    x = _f32c(x, "x")
-    z = None if z is None else _f32c(z, "z")
-    row_scale = None if row_scale is None else _f32c(row_scale, "row_scale").view(-1)
-    val = None if val is None else _f32c(val, "edge values").view(-1)
-    with torch.cuda.device(dev):
-        y, plan, keep = _spmm_out(st, val, x)
-        if z is not None and z.shape != y.shape:
-            raise ValueError(f"z must be [{st.n_rows}, {x.shape[1]}], got {tuple(z.shape)}")
-        if row_scale is not None and row_scale.numel() != st.n_rows:
-            raise ValueError(f"row_scale has {row_scale.numel()} entries, the CSR has {st.n_rows} rows")
-        _cabi.call("cogdl_b200_spmm_residual_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
-                   _ptr(z), float(a), float(b), _ptr(row_scale), _ptr(y), st.n_rows, x.shape[1], int(panels), plan,
-                   _stream(dev))
-        del keep
-    return y
+    return _spmm_epilogue_raw("cogdl_b200_spmm_residual_f32", st, val, x, z, a, b, row_scale, panels=panels)
 
 
 def spmm_adjoint_raw(st: CSRStructure, val, g, sym, a=None):

@@ -9,7 +9,7 @@ backward are bitwise reproducible.
 """
 import torch
 
-from ..structure import CSRStructure
+from ..structure import CSRStructure, graph_operands
 from ._raw import disen_route_bwd_raw, disen_route_fwd_raw
 
 SUPPORTED_D = (1, 2, 4, 8, 16, 32)
@@ -34,14 +34,6 @@ class DisenRouteFunction(torch.autograd.Function):
         return None, dq if ctx.needs_input_grad[1] else None, dc if ctx.needs_input_grad[2] else None, None, None
 
 
-def _structure_of(graph):
-    if isinstance(graph, CSRStructure):
-        return graph
-    from ..utils.spmm_utils import _structure
-
-    return _structure(graph)
-
-
 def disen_routing(graph, h, K, iterations, tau=1.0):
     """The output of CogDL's DisenGCNLayer.forward given h = act(x W + b): h [N, F] is cut into K channels of
     d = F / K columns, each normalised to unit length (c), and `iterations` routing steps run from q = c.  Returns
@@ -57,7 +49,7 @@ def disen_routing(graph, h, K, iterations, tau=1.0):
     N, F = h.shape
     if K < 1 or F % K:
         raise ValueError(f"disen_routing: F={F} is not a multiple of K={K}")
-    st = _structure_of(graph)
+    st = graph if isinstance(graph, CSRStructure) else graph_operands(graph).st
     hk = h.reshape(N, K, F // K)
     c = (hk / hk.pow(2).sum(-1, keepdim=True).sqrt()).reshape(N, F)
     q = c

@@ -8,7 +8,7 @@ against an fp64 evaluation instead of being bit-matched.  Kernel: cogdl_b200/csr
 import torch
 
 from .. import _cabi
-from ..structure import CSRStructure, _ptr, _stream, require_cuda
+from ..structure import CSRStructure, _ptr, _stream, graph_operands, require_cuda
 from ._raw import _spmm_scratch, spmm_adjoint_raw, spmm_raw
 
 
@@ -91,10 +91,7 @@ class FusedGCNFunction(torch.autograd.Function):
 
 def fused_gcn_layer(graph, x, weight, bias=None, relu=False):
     """graph: cogdl_b200.Graph or a real cogdl.data.Graph (same attribute surface as spmm())."""
-    from ..utils.spmm_utils import _structure
-
-    # the structure before the weights: building the CSR of a graph held as COO puts its edge weights in CSR order
-    st = _structure(graph)
-    if graph.out_norm is not None or graph.in_norm is not None:
+    st, val, out_norm, in_norm, sym = graph_operands(graph)
+    if out_norm is not None or in_norm is not None:
         raise NotImplementedError("fused GCN layer: graphs with separate in/out norms take the unfused path")
-    return FusedGCNFunction.apply(st, graph.raw_edge_weight, x, weight, bias, relu, graph.is_symmetric())
+    return FusedGCNFunction.apply(st, val, x, weight, bias, relu, sym)

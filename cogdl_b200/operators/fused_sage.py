@@ -12,7 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _cabi
-from ..structure import CSRStructure, _ptr, _stream, require_cuda
+from ..structure import CSRStructure, _ptr, _stream, graph_operands, require_cuda
 from ._raw import scatter_max_bwd_raw, scatter_max_fwd_raw, spmm_adjoint_raw, spmm_raw
 from .fused_gcn import supported
 
@@ -112,20 +112,13 @@ class FusedSAGEFunction(torch.autograd.Function):
 def fused_sage_layer(graph, x, weight, bias=None, aggr="mean", relu=False):
     """graph: cogdl_b200.Graph or a real cogdl.data.Graph.  aggr "mean" row-normalises the graph first (as the
     reference MeanAggregator); "sum" and "mean" use the edge weights and graph.in_norm as spmm() does."""
-    from ..utils.spmm_utils import _structure
-
     if aggr == "mean":
         graph.row_norm()
-    # the structure before the weights: building the CSR of a graph held as COO puts its edge weights (the 1/deg that
-    # row_norm() just baked in, for a COO graph) in CSR order
-    st = _structure(graph)
-    if graph.out_norm is not None:
+    st, val, out_norm, row_scale, sym = graph_operands(graph)
+    if out_norm is not None:
         raise NotImplementedError("fused SAGE layer: graphs with an out_norm take the unfused path")
     if aggr == "max":
         val = row_scale = None
-    else:
-        val, row_scale = graph.raw_edge_weight, graph.in_norm
-        if val.requires_grad:
-            raise NotImplementedError("fused SAGE layer: trainable edge weights take the unfused path")
-    return FusedSAGEFunction.apply(st, val, row_scale, x, weight, bias, "max" if aggr == "max" else "sum", relu,
-                                   graph.is_symmetric())
+    elif val.requires_grad:
+        raise NotImplementedError("fused SAGE layer: trainable edge weights take the unfused path")
+    return FusedSAGEFunction.apply(st, val, row_scale, x, weight, bias, "max" if aggr == "max" else "sum", relu, sym)

@@ -13,8 +13,8 @@ synchronisation between them."""
 import torch
 
 from .. import _cabi
-from ..structure import _ptr, _stream, require_cuda
-from ._raw import _f32c, _spmm_scratch
+from ..structure import _ptr, _stream, graph_operands, require_cuda, unsupported_operands
+from ._raw import _epilogue_args, _spmm_epilogue_raw, _spmm_out
 
 
 def label_prop_raw(st, val, x, z, a, b, row_scale=None, pin=None, clamp=None, panels=0, out=None):
@@ -22,31 +22,12 @@ def label_prop_raw(st, val, x, z, a, b, row_scale=None, pin=None, clamp=None, pa
     fp32; z [n_rows, F] fp32 or None; row_scale [n_rows] fp32 or None; pin [n_rows] uint8 or None (needs z); clamp
     (lo, hi) or None; val [nnz] fp32 or None.  a, b, lo and hi are rounded to fp32.  out: a preallocated [n_rows, F]
     fp32 Y (must not overlap x, z or row_scale)."""
-    dev = require_cuda(x, z, val, row_scale, pin)
-    x = _f32c(x, "x")
-    if x.dim() != 2:
-        raise ValueError("x must be [n_src, F]")
-    F = x.shape[1]
-    z = None if z is None else _f32c(z, "z")
-    row_scale = None if row_scale is None else _f32c(row_scale, "row_scale").view(-1)
-    val = None if val is None else _f32c(val, "edge values").view(-1)
-    if val is not None and val.numel() != st.nnz:
-        raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
-    if z is not None and z.shape != (st.n_rows, F):
-        raise ValueError(f"z must be [{st.n_rows}, {F}], got {tuple(z.shape)}")
-    if row_scale is not None and row_scale.numel() != st.n_rows:
-        raise ValueError(f"row_scale has {row_scale.numel()} entries, the CSR has {st.n_rows} rows")
+    require_cuda(x, pin)
     if pin is not None and (pin.dtype != torch.uint8 or pin.numel() != st.n_rows):
         raise ValueError(f"pin must be [{st.n_rows}] uint8")
     lo, hi = (0.0, 0.0) if clamp is None else (float(clamp[0]), float(clamp[1]))
-    with torch.cuda.device(dev):
-        y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev) if out is None else out
-        plan, keep = st.plan_struct(_spmm_scratch(st, F))
-        _cabi.call("cogdl_b200_label_prop_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
-                   _ptr(z), float(a), float(b), _ptr(row_scale), _ptr(pin), int(clamp is not None), lo, hi, _ptr(y),
-                   st.n_rows, F, int(panels), plan, _stream(dev))
-        del keep
-    return y
+    return _spmm_epilogue_raw("cogdl_b200_label_prop_f32", st, val, x, z, a, b, row_scale,
+                              (_ptr(pin), int(clamp is not None), lo, hi), panels, out)
 
 
 def pin_mask(n, pinned, device):
@@ -63,22 +44,14 @@ def label_propagate(graph, labels, alpha, nprop, lower=None, upper=None, pinned=
     `pinned` (a node index) is.  The graph is taken as cogdl_b200.spmm takes it: the cached int32 CSR and hub plan,
     out_norm applied to x first and in_norm to the SpMM's rows (here inside the kernel).  Forward only.  The result is
     bit-identical to the reference loop run with this package's spmm; nprop = 0 returns labels.clone()."""
-    from ..utils.spmm_utils import _structure
-
-    if getattr(graph, "grb_adj", None) is not None:
-        raise ValueError("label_propagate: graphs carrying a dense grb_adj are not supported; use spmm")
-    if not labels.is_cuda:
-        raise RuntimeError("cogdl_b200.label_propagate: CPU tensors are not supported (no CPU fallback); move the graph "
-                           "and labels to an H100 device")
-    if labels.dtype != torch.float32:
-        raise TypeError(f"label_propagate takes float32 labels, got {labels.dtype}")
+    err = unsupported_operands(graph, labels, entry="label_propagate", what="labels")
+    if err is not None:
+        raise err
     if (lower is None) != (upper is None):
         raise ValueError("label_propagate clamps to [lower, upper]: give both bounds or neither")
     if lower is not None and pinned is not None:
         raise ValueError("label_propagate: one post step at a time, the clamp or the pinned rows")
-    # the structure first: building the CSR of a graph held as COO puts its edge weights in CSR order
-    st = _structure(graph)
-    val = graph.raw_edge_weight
+    st, val, out_norm, r, _ = graph_operands(graph)
     if torch.is_grad_enabled() and (labels.requires_grad or (val is not None and val.requires_grad)):
         raise RuntimeError("label_propagate is forward only: call it under torch.no_grad() or on inputs that do not "
                            "require grad")
@@ -87,23 +60,18 @@ def label_propagate(graph, labels, alpha, nprop, lower=None, upper=None, pinned=
         raise ValueError(f"nprop must be >= 0, got {nprop}")
     if nprop == 0:
         return labels.clone()
-    labels = labels.contiguous()
-    dev = require_cuda(labels, val)
     if labels.shape[0] != st.n_rows or st.n_cols != st.n_rows:
         raise ValueError(f"labels must be [{st.n_rows}, C] on a square graph, got {tuple(labels.shape)}")
-    val = None if val is None else _f32c(val, "edge values").view(-1)
-    r = graph.in_norm
-    if r is not None:
-        r = _f32c(r.to(dev), "in_norm").reshape(-1)
-    out_norm = None if graph.out_norm is None else graph.out_norm.to(dev)
+    dev, val, labels, _, r = _epilogue_args(st, val, labels, None, None if r is None else r.to(labels.device))
+    out_norm = None if out_norm is None else out_norm.to(dev)
     pin = None if pinned is None else pin_mask(st.n_rows, pinned, dev)
     lo, hi = (0.0, 0.0) if lower is None else (float(lower), float(upper))
     a, b = float(alpha), float((1 - alpha) if alpha_term else 1.0)
     n, F = labels.shape
-    bufs = (torch.empty_like(labels), torch.empty_like(labels))
     step = _cabi.load().cogdl_b200_label_prop_f32
     with torch.cuda.device(dev):
-        plan, keep = st.plan_struct(_spmm_scratch(st, F))
+        y, plan, keep = _spmm_out(st, val, labels)
+        bufs = (y, torch.empty_like(y))
         stream = _stream(dev)
         x = labels
         for k in range(nprop):

@@ -10,7 +10,7 @@ go through the existing scatter_max and SpMM kernels.
 """
 import torch
 
-from ..structure import CSRStructure
+from ..structure import CSRStructure, graph_operands
 from ._raw import softmax_aggr_bwd_raw, softmax_aggr_fwd_raw
 from .scatter_max import ScatterMaxFunction
 from .spmm import SPMMFunction
@@ -44,14 +44,6 @@ class SoftmaxAggrFunction(torch.autograd.Function):
         return None, dx if need_x else None, da, db, None
 
 
-def _structure_of(graph):
-    if isinstance(graph, CSRStructure):
-        return graph
-    from ..utils.spmm_utils import _structure
-
-    return _structure(graph)
-
-
 def _degrees(st):
     return (st.rowptr[1:] - st.rowptr[:-1]).to(torch.float32).unsqueeze(1)
 
@@ -76,7 +68,7 @@ def genconv_aggregate(graph, x, aggr, beta=None, eps=1e-7, edge_term=None, p=1.0
         raise TypeError(f"genconv_aggregate: x must be float32, got {x.dtype}")
     if x.dim() != 2:
         raise ValueError(f"genconv_aggregate: x must be [N, F], got {tuple(x.shape)}")
-    st = _structure_of(graph)
+    st = graph if isinstance(graph, CSRStructure) else graph_operands(graph).st
     if aggr in ("max", "powermean"):
         if edge_term is not None:
             raise NotImplementedError(f"genconv_aggregate: aggr={aggr!r} with an edge term has no kernel")

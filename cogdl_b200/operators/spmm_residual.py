@@ -6,6 +6,7 @@ the scaling, the in_norm and the addition run in the SpMM's store (cogdl_b200_sp
 roundings in the same order, so the forward is bit-identical to that sequence run with this package's spmm."""
 import torch
 
+from ..structure import graph_operands, unsupported_operands
 from ._raw import sddmm_raw, spmm_adjoint_raw, spmm_residual_raw
 
 
@@ -43,24 +44,14 @@ def spmm_residual(graph, x, z, a, b):
     cogdl_b200.spmm takes it: the cached int32 CSR and hub plan, out_norm applied to x first, in_norm applied to the
     SpMM's rows (here inside the kernel), and the backward over A when graph.is_symmetric(), else over the cached
     transpose.  The result is bit-identical to `a * spmm(graph, x) + b * z` computed by this package."""
-    from ..utils.spmm_utils import _structure
-
-    if getattr(graph, "grb_adj", None) is not None:
-        raise ValueError("spmm_residual: graphs carrying a dense grb_adj are not supported; use spmm")
-    if not x.is_cuda:
-        raise RuntimeError("cogdl_b200.spmm_residual: CPU tensors are not supported (no CPU fallback); move the graph "
-                           "and features to an H100 device")
-    if x.dtype != torch.float32 or (z is not None and z.dtype != torch.float32):
-        raise TypeError(f"spmm_residual takes float32 features, got {x.dtype}"
-                        f"{'' if z is None else ' and ' + str(z.dtype)}")
-    # the structure first: building the CSR of a graph held as COO puts its edge weights in CSR order
-    st = _structure(graph)
-    if graph.out_norm is not None:
-        x = graph.out_norm.to(x.device) * x
-    r = graph.in_norm
+    err = unsupported_operands(graph, x, z, entry="spmm_residual")
+    if err is not None:
+        raise err
+    st, val, out_norm, r, sym = graph_operands(graph)
+    if out_norm is not None:
+        x = out_norm.to(x.device) * x
     if r is not None:
         if r.requires_grad:
             raise ValueError("spmm_residual: an in_norm that requires grad is not supported")
         r = r.to(x.device).reshape(-1)
-    val = graph.raw_edge_weight
-    return SpmmResidualFunction.apply(st, x, z, val, float(a), float(b), r, graph.is_symmetric())
+    return SpmmResidualFunction.apply(st, x, z, val, float(a), float(b), r, sym)

@@ -9,6 +9,7 @@ All device work goes through the C ABI (cogdl_b200._cabi); torch only owns the m
 """
 import ctypes
 from collections import OrderedDict
+from typing import NamedTuple, Optional
 
 import torch
 
@@ -194,12 +195,54 @@ class CSRStructure:
         return self._csc
 
 
+class _Entry(NamedTuple):
+    value: object
+    tensors: tuple          # the key tensors, kept alive so their addresses cannot be reused under the key
+    versions: tuple         # their in-place version counters when the entry was made
+    nbytes: int
+
+    def fresh(self):
+        return self.versions == tuple(t._version for t in self.tensors)
+
+
+class IdentityCache:
+    """An LRU of values derived from tensors, keyed on the tensors' storage identity (address, sizes, device and
+    whatever else the caller puts in the key).  An entry keeps its key tensors alive, and is dropped as stale once
+    any of them has been modified in place.  A hit moves the entry to the end; past `cap` entries, or past
+    `max_bytes` of the entries' declared sizes, the oldest entries are evicted (the newest one always stays).
+    `stats["hit"]` counts hits; what counts as a miss is the caller's to say."""
+
+    def __init__(self, cap, stats, max_bytes=None):
+        self.entries = OrderedDict()
+        self.cap, self.stats, self.max_bytes = cap, stats, max_bytes
+
+    def get(self, key):
+        ent = self.entries.get(key)
+        if ent is None:
+            return None
+        if not ent.fresh():
+            del self.entries[key]
+            return None
+        self.entries.move_to_end(key)
+        self.stats["hit"] += 1
+        return ent.value
+
+    def put(self, key, tensors, value, nbytes=0):
+        self.entries[key] = _Entry(value, tensors, tuple(t._version for t in tensors), nbytes)
+        total = sum(e.nbytes for e in self.entries.values())
+        while len(self.entries) > 1 and (len(self.entries) > self.cap
+                                         or (self.max_bytes is not None and total > self.max_bytes)):
+            total -= self.entries.popitem(last=False)[1].nbytes
+
+    def clear(self):
+        self.entries.clear()
+
+
 # ---------------------------------------------------------------------------------------------
 # Structure cache for the operator-level API, where the caller hands us bare (rowptr, colind)
 # tensors (reference signature csrspmm(rowptr, colind, x, csr_data, sym), operators/spmm.py:24).
 #
-# Fast path: keyed on storage identity; the key tensors are kept alive by the entry so an address
-# cannot be recycled under a live key, and the in-place version counter catches mutation.
+# Fast path: the identity lookup of IdentityCache.
 #
 # Slow path: the reference's own dispatch passes `graph.row_indptr.int(), graph.col_indices.int()`
 # -- FRESH tensors on every call (cogdl/utils/spmm_utils.py:106) -- so identity never matches for a
@@ -209,11 +252,9 @@ class CSRStructure:
 # possibly the transpose, and no entry is created for the short-lived tensors (no dead CSR copies
 # pinned by the cache).  The cache is bounded by entries AND by bytes.
 # ---------------------------------------------------------------------------------------------
-_CACHE = OrderedDict()
-_CACHE_CAP = 8
-_CACHE_MAX_BYTES = int(os.environ.get("COGDL_B200_STRUCT_CACHE_BYTES", str(8 << 30)))
 _CONTENT_SCAN = 4
 cache_stats = {"hit": 0, "content_hit": 0, "miss": 0}
+_CACHE = IdentityCache(8, cache_stats, int(os.environ.get("COGDL_B200_STRUCT_CACHE_BYTES", str(8 << 30))))
 
 
 def _entry_bytes(st, rp, ci):
@@ -226,41 +267,82 @@ def _entry_bytes(st, rp, ci):
 def structure_for(rowptr, colind, n_cols=None):
     key = (rowptr.data_ptr(), colind.data_ptr(), rowptr.numel(), colind.numel(), str(rowptr.device),
            rowptr.dtype, n_cols)
-    ent = _CACHE.get(key)
-    if ent is not None:
-        st, rp, ci, ver = ent
-        if ver == (rp._version, ci._version):
-            _CACHE.move_to_end(key)
-            cache_stats["hit"] += 1
-            return st
-        del _CACHE[key]
+    st = _CACHE.get(key)
+    if st is not None:
+        return st
     # content match against recent entries of the same shape (the `.int()`-per-call caller)
     scanned = 0
-    for k in reversed(_CACHE):
+    for k in reversed(_CACHE.entries):
         if scanned >= _CONTENT_SCAN:
             break
         if k[2:5] != key[2:5] or k[6] != n_cols:
             continue
         scanned += 1
-        st, rp, ci, ver = _CACHE[k]
-        if ver != (rp._version, ci._version):
+        ent = _CACHE.entries[k]
+        if not ent.fresh():
             continue
+        st, (rp, ci) = ent.value, ent.tensors
         a_rp = rp if rp.dtype == rowptr.dtype else (st.rowptr if rowptr.dtype == torch.int32 else None)
         a_ci = ci if ci.dtype == colind.dtype else (st.colind if colind.dtype == torch.int32 else None)
         if a_rp is None or a_ci is None:
             continue
         if torch.equal(a_rp, rowptr) and torch.equal(a_ci, colind):
-            _CACHE.move_to_end(k)
+            _CACHE.entries.move_to_end(k)
             cache_stats["content_hit"] += 1
             return st
     cache_stats["miss"] += 1
     st = CSRStructure.from_int64(rowptr, colind, n_cols)
-    _CACHE[key] = (st, rowptr, colind, (rowptr._version, colind._version))
-    total = sum(_entry_bytes(*e[:3]) for e in _CACHE.values())
-    while len(_CACHE) > 1 and (len(_CACHE) > _CACHE_CAP or total > _CACHE_MAX_BYTES):
-        _, old = _CACHE.popitem(last=False)
-        total -= _entry_bytes(*old[:3])
+    _CACHE.put(key, (rowptr, colind), st, _entry_bytes(st, rowptr, colind))
     return st
+
+
+class GraphOperands(NamedTuple):
+    st: CSRStructure
+    val: Optional[torch.Tensor]         # edge weights in CSR order (raw: without the norms)
+    out_norm: Optional[torch.Tensor]
+    in_norm: Optional[torch.Tensor]
+    sym: bool
+
+
+def csr_order(graph):
+    """(row_indptr, col_indices, raw_edge_weight) of a cogdl_b200.Graph or a cogdl.data.Graph, after putting the
+    graph in CSR order.  Host tensors are fine: nothing here needs the device.
+
+    The order is what makes it correct.  Building the CSR of a graph held as COO reorders every edge-aligned tensor
+    the graph holds (its edge weights, and a cogdl.data.Graph's edge_attr) by the sort that builds it.  So the
+    weights are read only once the CSR exists: a weight tensor read before would stay in COO order and pair the
+    CSR's columns with other edges' weights."""
+    rowptr, colind = graph.row_indptr, graph.col_indices
+    return rowptr, colind, graph.raw_edge_weight
+
+
+def graph_operands(graph):
+    """What a graph-level entry point hands its kernels: the cached CSRStructure, the edge weights in CSR order,
+    out_norm, in_norm and is_symmetric(), in that order (see csr_order).
+
+    A cogdl_b200.Graph caches its structure on its adjacency.  A real cogdl.data.Graph filters attribute names
+    (cogdl/data/data.py:352-375: a single leading underscore is stripped, only `keys` survive copy.copy in
+    local_graph()), so nothing can be parked on it; its structure comes from structure_for instead.  Its
+    row_indptr / col_indices are the same tensors on every call and local_graph()'s copies share their storage,
+    so that is a dictionary hit per call, never a rebuild."""
+    rowptr, colind, val = csr_order(graph)
+    st = graph.structure() if hasattr(graph, "structure") else structure_for(rowptr, colind, graph.num_nodes)
+    return GraphOperands(st, val, graph.out_norm, graph.in_norm, graph.is_symmetric())
+
+
+def unsupported_operands(graph, *tensors, entry="", what="features"):
+    """The error a graph-level fp32 entry point raises for operands it has no kernel for, or None: a dense grb_adj
+    on the graph (ValueError), a tensor off the GPU (RuntimeError) or not float32 (TypeError).  `entry` and `what`
+    name the entry point and its tensors in the message."""
+    tensors = [t for t in tensors if t is not None]
+    if getattr(graph, "grb_adj", None) is not None:
+        return ValueError(f"{entry}: graphs carrying a dense grb_adj are not supported; use spmm")
+    if not all(t.is_cuda for t in tensors):
+        return RuntimeError(f"cogdl_b200.{entry}: CPU tensors are not supported (no CPU fallback); move the graph "
+                            f"and {what} to an H100 device")
+    if any(t.dtype != torch.float32 for t in tensors):
+        return TypeError(f"{entry} takes float32 {what}, got {' and '.join(str(t.dtype) for t in tensors)}")
+    return None
 
 
 def clear_structure_cache():
@@ -338,30 +420,20 @@ class CompStructure:
         return ent
 
 
-# CompStructure cache: keyed on the storage identity, size and version of the (row, col, type) tensors, the node
-# count and the chunk size, like structure_for.  Both layers of a model, and repeated predict() calls on one graph,
-# share one entry; the entry keeps its key tensors alive so their addresses cannot be reused under it.
-_COMP_CACHE = OrderedDict()
-_COMP_CACHE_CAP = 4
+# CompStructure cache: keyed on the storage identity and size of the (row, col, type) tensors, the node count and
+# the chunk size.  Both layers of a model, and repeated predict() calls on one graph, share one entry.
 comp_cache_stats = {"hit": 0, "miss": 0}
+_COMP_CACHE = IdentityCache(4, comp_cache_stats)
 
 
 def comp_structure_for(row, col, etype, num_nodes, chunk_edges=DEFAULT_CHUNK_EDGES):
     keys = (row, col, etype)
     key = tuple((t.data_ptr(), t.numel(), str(t.device), t.dtype) for t in keys) + (int(num_nodes), int(chunk_edges))
-    ent = _COMP_CACHE.get(key)
-    if ent is not None:
-        cs, kept, ver = ent
-        if ver == tuple(t._version for t in kept):
-            _COMP_CACHE.move_to_end(key)
-            comp_cache_stats["hit"] += 1
-            return cs
-        del _COMP_CACHE[key]
-    comp_cache_stats["miss"] += 1
-    cs = CompStructure(row, col, etype, num_nodes, chunk_edges)
-    _COMP_CACHE[key] = (cs, keys, tuple(t._version for t in keys))
-    while len(_COMP_CACHE) > _COMP_CACHE_CAP:
-        _COMP_CACHE.popitem(last=False)
+    cs = _COMP_CACHE.get(key)
+    if cs is None:
+        comp_cache_stats["miss"] += 1
+        cs = CompStructure(row, col, etype, num_nodes, chunk_edges)
+        _COMP_CACHE.put(key, keys, cs)
     return cs
 
 
@@ -457,27 +529,18 @@ class CooStructure:
         return self._coo_csr
 
 
-# CooStructure cache, keyed like _COMP_CACHE on the storage, size and version of the index tensor and the matrix shape:
-# SRGCN reuses one index across its heads and calls the products on it several times per forward.
-_COO_CACHE = OrderedDict()
-_COO_CACHE_CAP = 8
+# CooStructure cache, keyed on the storage, size and strides of the index tensor and the matrix shape: SRGCN reuses
+# one index across its heads and calls the products on it several times per forward.
 coo_cache_stats = {"hit": 0, "miss": 0}
+_COO_CACHE = IdentityCache(8, coo_cache_stats)
 
 
 def coo_structure_for(index, n_rows, n_cols):
     key = (index.data_ptr(), tuple(index.shape), tuple(index.stride()), str(index.device), index.dtype, int(n_rows),
            int(n_cols))
-    ent = _COO_CACHE.get(key)
-    if ent is not None:
-        cs, kept, ver = ent
-        if ver == kept._version:
-            _COO_CACHE.move_to_end(key)
-            coo_cache_stats["hit"] += 1
-            return cs
-        del _COO_CACHE[key]
-    coo_cache_stats["miss"] += 1
-    cs = CooStructure(index, n_rows, n_cols)
-    _COO_CACHE[key] = (cs, index, index._version)
-    while len(_COO_CACHE) > _COO_CACHE_CAP:
-        _COO_CACHE.popitem(last=False)
+    cs = _COO_CACHE.get(key)
+    if cs is None:
+        coo_cache_stats["miss"] += 1
+        cs = CooStructure(index, n_rows, n_cols)
+        _COO_CACHE.put(key, (index,), cs)
     return cs

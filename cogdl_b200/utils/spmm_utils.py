@@ -23,6 +23,7 @@ from ..operators.spmm import SPMMFunction
 from ..operators.edge_softmax import EdgeSoftmaxFunction
 from ..operators.mhspmm import MHSPMMFunction
 from ..operators.fused_gat import FusedGATFunction
+from ..structure import csr_order, graph_operands
 
 CONFIGS = {
     "fast_spmm": csrspmm,
@@ -53,20 +54,6 @@ def check_fused_gat():
     return CONFIGS["fused_gat_func"] is not None
 
 
-def _structure(graph):
-    if hasattr(graph, "structure"):
-        return graph.structure()
-    # A real cogdl.data.Graph.  Its Adjacency filters attribute names through __getitem__/keys
-    # (cogdl/data/data.py:352-375: a single leading underscore is stripped, only `keys` survive
-    # copy.copy in local_graph()), so nothing can be parked on the object itself; the int32 CSR, hub
-    # plan and transpose live in the storage-keyed structure cache instead.  graph.row_indptr /
-    # col_indices return the SAME tensors on every call and local_graph()'s shallow copies share their
-    # storage (data.py:381-386), so this is a dictionary hit per call, never a rebuild.
-    from ..structure import structure_for
-
-    return structure_for(graph.row_indptr, graph.col_indices, graph.num_nodes)
-
-
 def spmm(graph, x, actnn=False, fast_spmm=None, fast_spmm_cpu=None):
     if getattr(graph, "grb_adj", None) is not None:
         if graph.grb_adj.is_sparse:
@@ -75,23 +62,22 @@ def spmm(graph, x, actnn=False, fast_spmm=None, fast_spmm_cpu=None):
     if not x.is_cuda:
         raise RuntimeError("cogdl_b200.spmm: CPU tensors are not supported (no CPU fallback); move the graph and "
                            "features to an H100 device")
-    # the CSR before the weights: building it from a graph held as COO puts that graph's edge weights in CSR order
     custom = fast_spmm is not None and fast_spmm is not csrspmm
     if custom:
-        row_ptr, col = graph.row_indptr.int(), graph.col_indices.int()
+        rowptr, colind, val = csr_order(graph)
+        out_norm, in_norm, sym = graph.out_norm, graph.in_norm, graph.is_symmetric()
     else:
-        st = _structure(graph)
-    if graph.out_norm is not None:
-        x = graph.out_norm.to(x.device) * x
-    csr_data = graph.raw_edge_weight
+        st, val, out_norm, in_norm, sym = graph_operands(graph)
+    if out_norm is not None:
+        x = out_norm.to(x.device) * x
     if x.dtype == torch.half:
-        csr_data = csr_data.half()
+        val = val.half()
     if custom:
-        x = fast_spmm(row_ptr, col, x, csr_data, graph.is_symmetric(), actnn=actnn)
+        x = fast_spmm(rowptr.int(), colind.int(), x, val, sym, actnn=actnn)
     else:
-        x = SPMMFunction.apply(st, None, x, csr_data, graph.is_symmetric(), actnn)
-    if graph.in_norm is not None:
-        x = graph.in_norm.to(x.device) * x
+        x = SPMMFunction.apply(st, None, x, val, sym, actnn)
+    if in_norm is not None:
+        x = in_norm.to(x.device) * x
     return x
 
 
@@ -117,7 +103,7 @@ def edge_softmax(graph, edge_val, csr_edge_softmax=None):
     if csr_edge_softmax is not None and csr_edge_softmax is not CONFIGS["csr_edge_softmax"]:
         val = csr_edge_softmax(graph.row_indptr.int(), edge_val)
     else:
-        val = EdgeSoftmaxFunction.apply(_structure(graph), edge_val)
+        val = EdgeSoftmaxFunction.apply(graph_operands(graph).st, edge_val)
     return val.view(-1) if flat else val
 
 
@@ -141,12 +127,11 @@ def mh_spmm(graph, attention, h, csrmhspmm=None, fast_spmm=None):
         if csrmhspmm is not None and csrmhspmm is not CONFIGS["csrmhspmm"]:
             h_prime = csrmhspmm(graph.row_indptr.int(), graph.col_indices.int(), h, attention)
         else:
-            h_prime = MHSPMMFunction.apply(_structure(graph), None, h, attention)
+            h_prime = MHSPMMFunction.apply(graph_operands(graph).st, None, h, attention)
         return h_prime.view(h_prime.shape[0], -1)
     # single head: SpMM with the attention as edge weight inside local_graph() (reference :210-214;
-    # set_weight flips the symmetric flag, so the backward takes the transpose branch).  The structure is built first, on
-    # the graph itself: built inside the block, it would reorder the attention as a COO-ordered weight.
-    _structure(graph)
+    # set_weight flips the symmetric flag, so the backward takes the transpose branch).
+    graph_operands(graph)
     edge_weight = attention.view(-1)
     with graph.local_graph():
         graph.edge_weight = edge_weight
@@ -171,8 +156,8 @@ def fused_gat_op(attn_row, attn_col, graph, negative_slope, in_feat, fused_gat_f
             raise ValueError("attention dropout needs this package's fused GAT operator, not a custom fused_gat_func")
         rp, ci = graph.row_indptr.int(), graph.col_indices.int()
         return fused_gat_func(attn_row, attn_col, rp, ci, rp, ci, negative_slope, in_feat)
-    return FusedGATFunction.apply(attn_row, attn_col, _structure(graph), None, None, None, negative_slope, in_feat,
-                                  attn_drop, seed)
+    return FusedGATFunction.apply(attn_row, attn_col, graph_operands(graph).st, None, None, None, negative_slope,
+                                  in_feat, attn_drop, seed)
 
 
 class FusedGATOp(torch.nn.Module):

@@ -217,6 +217,30 @@ def test_graph_semantics_match_reference_graph():
     assert float(gc.edge_weight[-1]) == gc.num_edges - 1  # restored
 
 
+@pytest.mark.parametrize("trainable", [False, True])
+def test_csr_order_pairs_each_weight_with_its_own_edge(trainable):
+    """The step of the graph resolver that puts a graph held as COO in CSR order and reads its edge weights: every
+    (row, column, weight) it yields is one the user gave, and a trainable weight gets its gradient back in the
+    user's COO order."""
+    import cogdl_b200
+    from cogdl_b200.structure import csr_order
+
+    gen = torch.Generator().manual_seed(5)
+    n, E = 40, 300
+    row, col = torch.randint(0, n, (E,), generator=gen), torch.randint(0, n, (E,), generator=gen)
+    w = (torch.randperm(E, generator=gen).float() + 0.5).requires_grad_(trainable)   # distinct weights
+    g = cogdl_b200.Graph(edge_index=(row, col), edge_weight=w, num_nodes=n)
+    rowptr, colind, val = csr_order(g)
+    csr_row = torch.repeat_interleave(torch.arange(n), rowptr[1:] - rowptr[:-1])
+    assert not torch.equal(csr_row, row)                          # the COO was not in CSR order
+    got = sorted(zip(csr_row.tolist(), colind.tolist(), val.tolist()))
+    assert got == sorted(zip(row.tolist(), col.tolist(), w.tolist()))
+    assert val.requires_grad == trainable
+    if trainable:
+        (val * (colind.float() + 1)).sum().backward()
+        assert torch.equal(w.grad, col.float() + 1)
+
+
 def test_host_coo2csr_index_matches_reference():
     from cogdl_b200.data import coo2csr_index
 
