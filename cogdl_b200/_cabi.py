@@ -62,6 +62,10 @@ SIGNATURES = {
                                                     _plan_p, _vp]),
     "cogdl_b200_label_prop_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _f32, _f32, _vp, _vp, _i32, _f32, _f32, _vp,
                                                  _i64, _i64, _i32, _plan_p, _vp]),
+    "cogdl_b200_spmm_residual_dcoef_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _f32, _vp, _vp, _vp, _i64, _i64,
+                                                          _i32, _plan_p, _vp]),
+    "cogdl_b200_spmm_accum_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i32, _f32, _vp, _i64, _i64, _i32,
+                                                 _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f16": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f32_2src": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f32_peers": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _vp, _i64, _i64, _plan_p, _vp]),

@@ -1,7 +1,8 @@
 // spmm.cuh -- the fp32 SpMM's sub-warp row kernel, its dispatch by width, alignment, plan form and panel count, and
 // the host entry in front of it, shared by the plain SpMM (spmm.cu), the SpMM with a residual epilogue
-// (spmm_residual.cu) and the label-propagation step (label_prop.cu).  EPI selects the epilogue: every finished row is
-// written as epilogue_out<EPI>(acc) (stream.cuh) -- acc itself for EPI_NONE.  Design notes: spmm.cu.
+// (spmm_residual.cu), the label-propagation step (label_prop.cu), the GIN aggregation (gin.cu) and GRAND's propagation
+// hop (spmm_accum.cu).  EPI selects the epilogue: every finished row is written by epilogue_store<EPI> (stream.cuh) --
+// acc itself for EPI_NONE.  Design notes: spmm.cu.
 #pragma once
 #include "common.cuh"
 #include "stream.cuh"
@@ -30,6 +31,11 @@ struct SpmmParams {
   const unsigned char *pin = nullptr;
   int has_clamp = 0;
   float clamp_lo = 0.f, clamp_hi = 0.f;
+  // device-coefficient residual epilogue (EPI_RESID_DEV) and accumulating epilogue (EPI_ACCUM): see StreamParams
+  const float *res_b_dev = nullptr;
+  float *acc = nullptr;
+  int acc_last = 0;
+  float acc_scale = 1.f;
 };
 
 template <typename VecT, int GROUP, int NV, bool HAS_VAL, int EPI>
@@ -62,6 +68,13 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
     VecT acc[NV];
 #pragma unroll
     for (int k = 0; k < NV; ++k) acc[k] = vzero<VecT>();
+    if constexpr (EPI == EPI_ACCUM) {              // ACC_in of this row, ahead of its store (prefetch_l1, stream.cuh)
+      if (!w.is_chunk && w.active) {
+#pragma unroll
+        for (int k = 0; k < NV; ++k)
+          if (colok[k]) prefetch_l1(reinterpret_cast<const VecT *>(p.Z) + (int64_t)w.row * p.FV + cv + k * GROUP);
+      }
+    }
 
     int c = 0;
     float v = 0.f;
@@ -120,7 +133,7 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
         VecT *yp = Y + (int64_t)w.row * p.FV + cv;
 #pragma unroll
         for (int k = 0; k < NV; ++k)
-          if (colok[k]) st_stream(yp + k * GROUP, epilogue_out<EPI>(p, acc[k], w.row, yp + k * GROUP));
+          if (colok[k]) epilogue_store<EPI>(p, acc[k], w.row, yp + k * GROUP);
       }
     } else {
       VecT *pp = P + (int64_t)w.slot * p.FV + cv;
@@ -138,7 +151,7 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
         const VecT s = merge_chunks<1>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.FV); },
                                        [](VecT &a, const VecT &t) { add_rn(a, t); });
         VecT *yp = Y + (int64_t)w.row * p.FV + cv;
-        st_stream(yp, epilogue_out<EPI>(p, s, w.row, yp));
+        epilogue_store<EPI>(p, s, w.row, yp);
       }
     }
   }
@@ -162,6 +175,18 @@ __global__ void __launch_bounds__(256, 3) spmm_labelprop_kernel(const SpmmParams
   spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_LABELPROP>(p);
 }
 
+// the row kernel with the device-coefficient residual epilogue (gin.cu) and with the accumulating epilogue
+// (spmm_accum.cu); 3 blocks per SM as for the residual form
+template <typename VecT, int GROUP, int NV, bool HAS_VAL>
+__global__ void __launch_bounds__(256, 3) spmm_dcoef_kernel(const SpmmParams p) {
+  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_RESID_DEV>(p);
+}
+
+template <typename VecT, int GROUP, int NV, bool HAS_VAL>
+__global__ void __launch_bounds__(256, 3) spmm_accum_kernel(const SpmmParams p) {
+  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_ACCUM>(p);
+}
+
 // ------------------------------------------------------------------------------------------
 // Row-stream form (stream.cuh), used whenever the plan carries segments and a full warp owns the
 // row (F >= 68, or >= 17 on the scalar path).
@@ -175,6 +200,7 @@ static StreamParams to_stream(const SpmmParams &p) {
   for (int i = 0; i < 8; ++i) q.peers[i] = p.peers[i];
   q.Z = p.Z; q.row_scale = p.row_scale; q.res_a = p.res_a; q.res_b = p.res_b;
   q.pin = p.pin; q.has_clamp = p.has_clamp; q.clamp_lo = p.clamp_lo; q.clamp_hi = p.clamp_hi;
+  q.res_b_dev = p.res_b_dev; q.acc = p.acc; q.acc_last = p.acc_last; q.acc_scale = p.acc_scale;
   return q;
 }
 
@@ -244,8 +270,10 @@ static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_
       q.ldv = q.FVL = (int)F;
       return launch_stream<float, 1, 8, 6, true, FORM_PANEL, EPI>(q, stream);
     case 64:
+      // the device coefficient's load costs the weighted 64-float panel loop one register more than 5 blocks per SM
+      // leave it (48), so that epilogue runs at 4 rather than spill
       q.ldv = q.FVL = (int)(F / 2);
-      return launch_stream<float2, 1, 8, 5, true, FORM_PANEL, EPI>(q, stream);
+      return launch_stream<float2, 1, 8, EPI == EPI_RESID_DEV ? 4 : 5, true, FORM_PANEL, EPI>(q, stream);
     default:
       q.ldv = q.FVL = (int)(F / 4);
       return launch_stream<float4, 1, 4, EPI != EPI_NONE ? 4 : 5, true, FORM_PANEL, EPI>(q, stream);
@@ -257,7 +285,15 @@ static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
   const char *vec = sizeof(VecT) == 16 ? "float4" : "float";
   const char *what = p.val ? "weighted" : "unweighted";
   const int64_t items = (int64_t)p.hub.n_chunks + p.n_rows;
-  if constexpr (EPI == EPI_LABELPROP)
+  if constexpr (EPI == EPI_RESID_DEV)
+    return launch_items(p.val ? spmm_dcoef_kernel<VecT, GROUP, NV, true> : spmm_dcoef_kernel<VecT, GROUP, NV, false>,
+                        p, items, GROUP, stream, "spmm_dcoef",
+                        "cogdl_b200::spmm_dcoef_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
+  else if constexpr (EPI == EPI_ACCUM)
+    return launch_items(p.val ? spmm_accum_kernel<VecT, GROUP, NV, true> : spmm_accum_kernel<VecT, GROUP, NV, false>,
+                        p, items, GROUP, stream, "spmm_accum",
+                        "cogdl_b200::spmm_accum_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
+  else if constexpr (EPI == EPI_LABELPROP)
     return launch_items(p.val ? spmm_labelprop_kernel<VecT, GROUP, NV, true> : spmm_labelprop_kernel<VecT, GROUP, NV, false>,
                         p, items, GROUP, stream, "label_prop",
                         "cogdl_b200::spmm_labelprop_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
@@ -302,16 +338,18 @@ static inline bool overlaps(const float *p, int64_t n, const float *q, int64_t m
 
 // The host side of every fp32 SpMM entry point: argument checks, the parameters, the panel count and the dispatch.
 // X1 (nullptr = X0) serves the columns >= n0 (two-source form); peers are the peer form's shards; Z, row_scale, a and
-// b are the epilogue's (EPI_RESID, EPI_LABELPROP); pin, has_clamp, lo and hi the label-propagation epilogue's.  x_rows,
-// X0's row count, sizes the automatic panel count (panels = 0).  Static, so each object instantiates only the form it
-// calls.
+// b are the epilogue's (EPI_RESID, EPI_LABELPROP); pin, has_clamp, lo and hi the label-propagation epilogue's; b_dev
+// the device coefficient that replaces b (EPI_RESID_DEV); acc, acc_last and acc_scale the accumulating epilogue's
+// (EPI_ACCUM, with Z as ACC's input).  x_rows, X0's row count, sizes the automatic panel count (panels = 0).  Static,
+// so each object instantiates only the form it calls.
 template <int EPI>
 static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X0, int64_t n0,
                       const float *X1, float *Y, int64_t n_rows, int64_t F, const cogdl_b200_hub_plan_t *plan,
                       cogdl_b200_stream_t stream, const char *who, const float *const *peers = nullptr,
                       int n_peers = 0, int peer_shift = 0, int64_t x_rows = 0, int panels = 1,
                       const float *Z = nullptr, const float *row_scale = nullptr, float a = 1.f, float b = 0.f,
-                      const unsigned char *pin = nullptr, int has_clamp = 0, float lo = 0.f, float hi = 0.f) {
+                      const unsigned char *pin = nullptr, int has_clamp = 0, float lo = 0.f, float hi = 0.f,
+                      const float *b_dev = nullptr, float *acc = nullptr, int acc_last = 0, float acc_scale = 1.f) {
   CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
   CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
@@ -325,6 +363,7 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
   p.n_peers = n_peers; p.peer_shift = peer_shift;
   p.Z = Z; p.row_scale = row_scale; p.res_a = a; p.res_b = b;
   p.pin = pin; p.has_clamp = has_clamp; p.clamp_lo = lo; p.clamp_hi = hi;
+  p.res_b_dev = b_dev; p.acc = acc; p.acc_last = acc_last; p.acc_scale = acc_scale;
   bool peers_aligned = true;
   for (int i = 0; i < n_peers; ++i) {
     p.peers[i] = peers[i];
@@ -334,7 +373,7 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
     CB_REQUIRE(p.hub.n_segs > 0 && F % 4 == 0 && F <= 512 && peers_aligned && aligned16(X0) && aligned16(Y),
                "%s: the peer form needs a plan with segments, F %% 4 == 0, F <= 512 and 16-byte aligned buffers", who);
   const bool vec = (F % 4 == 0) && aligned16(X0) && aligned16(p.X1) && aligned16(Y) && aligned16(Z) &&
-                   (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
+                   aligned16(acc) && (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
   if (vec) p.FV = (int)(F / 4);
   const bool panel_form = vec && n_peers == 0 && n0 == INT64_MAX && p.hub.n_segs > 0 && F % 32 == 0;
   if (panels > 1)

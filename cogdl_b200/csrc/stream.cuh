@@ -63,6 +63,15 @@ struct StreamParams {
   const unsigned char *pin = nullptr;
   int has_clamp = 0;
   float clamp_lo = 0.f, clamp_hi = 0.f;
+  // residual epilogue with a device coefficient (gin.cu, EPI_RESID_DEV): the residual epilogue with res_b read from
+  // *res_b_dev (one fp32 value in device memory) instead of res_b.
+  const float *res_b_dev = nullptr;
+  // accumulating epilogue (spmm_accum.cu, EPI_ACCUM): v = fl(row_scale[i] * acc) is stored to Y[i] unless acc_last,
+  // and ACC[i] = fl(Z[i] + v), times acc_scale (fl) when acc_last.  Z is ACC's input: ACC itself (in place) or another
+  // buffer of Y's layout; Y is ACC when acc_last (nothing else is written).
+  float *acc = nullptr;
+  int acc_last = 0;
+  float acc_scale = 1.f;
 };
 
 enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2, MODE_COMP_MULT = 3, MODE_COMP_SUB = 4 };
@@ -78,8 +87,9 @@ enum { SRC_ONE = 0, SRC_TWO = 1, SRC_PEERS = 2 };
 // the multi-head SpMM.
 enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
 // What a store site of the plain SpMM writes: the sum (EPI_NONE), the residual epilogue of spmm_residual.cu
-// (EPI_RESID) or the label-propagation epilogue of label_prop.cu (EPI_LABELPROP).
-enum { EPI_NONE = 0, EPI_RESID = 1, EPI_LABELPROP = 2 };
+// (EPI_RESID), the label-propagation epilogue of label_prop.cu (EPI_LABELPROP), the residual epilogue with its b read
+// on the device (gin.cu, EPI_RESID_DEV) or the accumulating epilogue of spmm_accum.cu (EPI_ACCUM, two stores per row).
+enum { EPI_NONE = 0, EPI_RESID = 1, EPI_LABELPROP = 2, EPI_RESID_DEV = 3, EPI_ACCUM = 4 };
 
 // The residual epilogue of one output element, rounded step by step as the unfused sequence
 // `a * (r * spmm(x)) + b * z` rounds it (no contraction); r and z are used iff has_r / has_z.
@@ -104,6 +114,32 @@ __device__ __forceinline__ VecT residual_out(const P &p, const VecT &acc, int64_
   const float r = hr ? __ldg(p.row_scale + row) : 1.f;
   const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.Z) + o) : vzero<VecT>();
   return residual_rn(acc, z, hr, r, hz, p.res_a, p.res_b);
+}
+
+// The residual epilogue with b = *p.res_b_dev, a coefficient that lives in device memory (GIN's 1 + eps, a trainable
+// parameter), read by the kernel so the host never waits for it.  Only read when Z is given.
+template <typename VecT, typename P>
+__device__ __forceinline__ VecT residual_dev_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
+  const int64_t o = yp - reinterpret_cast<const VecT *>(p.Y);
+  const bool hr = p.row_scale != nullptr, hz = p.Z != nullptr;
+  const float r = hr ? __ldg(p.row_scale + row) : 1.f;
+  const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.Z) + o) : vzero<VecT>();
+  return residual_rn(acc, z, hr, r, hz, p.res_a, hz ? __ldg(p.res_b_dev) : 0.f);
+}
+
+// One element of the accumulating epilogue's running sum: fl(s + v), then times `scale` (fl) on the last hop -- what
+// GRAND's `y.add_(x)` and the closing `y.div_(order + 1.0)` give on CUDA, where a division by a host scalar is a
+// multiply by its fp32 reciprocal.
+__device__ __forceinline__ float accum_rn(float s, float v, bool last, float scale) {
+  const float t = __fadd_rn(s, v);
+  return last ? __fmul_rn(t, scale) : t;
+}
+__device__ __forceinline__ float2 accum_rn(float2 s, float2 v, bool last, float scale) {
+  return make_float2(accum_rn(s.x, v.x, last, scale), accum_rn(s.y, v.y, last, scale));
+}
+__device__ __forceinline__ float4 accum_rn(float4 s, float4 v, bool last, float scale) {
+  return make_float4(accum_rn(s.x, v.x, last, scale), accum_rn(s.y, v.y, last, scale), accum_rn(s.z, v.z, last, scale),
+                     accum_rn(s.w, v.w, last, scale));
 }
 
 // torch.clamp(v, lo, hi) as its CUDA kernel evaluates it: a NaN passes through, otherwise min(max(v, lo), hi) with the
@@ -131,7 +167,36 @@ template <int EPI, typename VecT, typename P>
 __device__ __forceinline__ VecT epilogue_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
   if constexpr (EPI == EPI_RESID) return residual_out(p, acc, row, yp);
   else if constexpr (EPI == EPI_LABELPROP) return label_prop_out(p, acc, row, yp);
+  else if constexpr (EPI == EPI_RESID_DEV) return residual_dev_out(p, acc, row, yp);
   else return acc;
+}
+
+// Pull one vector of ACC_in into the L1 ahead of its accumulating store (EPI_ACCUM).  Each element of ACC_in is read
+// once per launch, by the thread that then writes ACC's element, so a line cached early holds current values for every
+// element that will be read from it.  On a graph as small as Cora the SpMM runs a few dozen warps, each walking its
+// rows one after the other, and the store's dependent load of ACC_in is the step's critical path; from the L1 it is
+// short.
+template <typename VecT>
+__device__ __forceinline__ void prefetch_l1(const VecT *ptr) {
+  asm volatile("prefetch.global.L1 [%0];" ::"l"(ptr));
+}
+
+// Every store site of the plain SpMM: output row `row`'s finished acc, epilogue EPI applied, to yp.  The accumulating
+// epilogue stores twice: the hop's row v = fl(r * acc) to yp (unless the last hop) and ACC's row fl(Z + v) in place.
+// ACC's element is read and written by this thread only, and ACC is never gathered in the launch that writes it, so
+// the plain load and the store cannot race.
+template <int EPI, typename VecT, typename P>
+__device__ __forceinline__ void epilogue_store(const P &p, const VecT &acc, int64_t row, VecT *yp) {
+  if constexpr (EPI == EPI_ACCUM) {
+    const int64_t o = yp - reinterpret_cast<const VecT *>(p.Y);
+    const bool hr = p.row_scale != nullptr;
+    const VecT v = residual_rn(acc, vzero<VecT>(), hr, hr ? __ldg(p.row_scale + row) : 1.f, false, 1.f, 0.f);
+    if (!p.acc_last) st_stream(yp, v);
+    const VecT s = reinterpret_cast<const VecT *>(p.Z)[o];
+    st_stream(reinterpret_cast<VecT *>(p.acc) + o, accum_rn(s, v, p.acc_last != 0, p.acc_scale));
+  } else {
+    st_stream(yp, epilogue_out<EPI>(p, acc, row, yp));
+  }
 }
 
 // Stream the edge range [e, e_end).  ROWS: flush at row ends (segment); otherwise accumulate the
@@ -169,6 +234,14 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
   for (; e < e_end; e += 32) {
     const int cnt = min(32, e_end - e);
     const unsigned endmask = ROWS ? __ballot_sync(FULL, lane < cnt && rid != rnx) : 0u;
+    if constexpr (EPI == EPI_ACCUM && ROWS) {      // ACC_in of the rows that end in this slab, while its gathers run
+      for (unsigned m = endmask; m != 0u; m &= m - 1u) {
+        const int rj = __shfl_sync(FULL, rid, __ffs(m) - 1);
+#pragma unroll
+        for (int k = 0; k < NV; ++k)
+          if (colok[k]) prefetch_l1(reinterpret_cast<const VecT *>(p.Z) + cv + (int64_t)rj * p.ldv + k * 32);
+      }
+    }
     int cn, pn, ridn, rnxn;
     float vn;
     if (PREFETCH) load_slab(e + 32, cn, vn, pn, ridn, rnxn);  // next slab rides behind this slab's gathers
@@ -227,7 +300,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
             for (int k = 0; k < NV; ++k)
               if (colok[k]) {
                 VecT *yp = Y + (int64_t)rj * p.ldv + k * 32;
-                st_stream(yp, epilogue_out<EPI>(p, acc[k], rj, yp));
+                epilogue_store<EPI>(p, acc[k], rj, yp);
                 acc[k] = vzero<VecT>();
               }
           }
@@ -273,7 +346,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
   };
   auto store_row = [&](int rj) {                    // row rj is complete: store it (epilogue applied) and restart
     VecT *yp = Y + (int64_t)rj * p.ldv;
-    st_stream(yp, epilogue_out<EPI>(p, acc, rj, yp));
+    epilogue_store<EPI>(p, acc, rj, yp);
     acc = vzero<VecT>();
   };
   constexpr bool CURSOR = ROWS && PF;               // row ends from rowptr; otherwise (ROWS) from edge_row
@@ -328,6 +401,10 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
     if (CURSOR) endmask = row_ends(e, end);
     else if (ROWS) s_r[lane] = rid;
     __syncwarp();
+    if constexpr (EPI == EPI_ACCUM && ROWS) {      // ACC_in of the rows that end in this slab, while its gathers run
+      for (unsigned m = endmask; m != 0u; m &= m - 1u)
+        if (colok) prefetch_l1(reinterpret_cast<const VecT *>(p.Z) + cv + (int64_t)s_r[__ffs(m) - 1] * p.ldv);
+    }
     if (PF) load_slab(e + 32, pc, pv, pend);        // consumed by the next iteration only (r is already past this slab)
     int j = 0;
 #pragma unroll 1
@@ -429,7 +506,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
         const VecT s = merge_chunks<8>(w.n_row_chunks, [&](int q) { return ld_cg(pp + (int64_t)q * p.ldv); },
                                        [](VecT &a, const VecT &t) { add_rn(a, t); });
         VecT *yp = Y + (int64_t)w.row * p.ldv + cv;
-        st_stream(yp, epilogue_out<EPI>(p, s, w.row, yp));
+        epilogue_store<EPI>(p, s, w.row, yp);
       }
     }
     return;
@@ -459,7 +536,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
           for (int k = 0; k < NV; ++k) {
             if (colok[k]) {
               VecT *yp = Y + (int64_t)(rb + k0) * p.ldv + cv + k * 32;
-              st_stream(yp, epilogue_out<EPI>(p, vzero<VecT>(), rb + k0, yp));
+              epilogue_store<EPI>(p, vzero<VecT>(), rb + k0, yp);
             }
           }
         }
@@ -509,10 +586,36 @@ __global__ void __launch_bounds__(256, MINB) stream_labelprop_kernel(const Strea
   stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_LABELPROP>(p, wid, lane, s_cv, s_r);
 }
 
+// stream_kernel of the plain SpMM (one source) with the device-coefficient residual epilogue (gin.cu) and with the
+// accumulating epilogue (spmm_accum.cu).
+template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
+__global__ void __launch_bounds__(256, MINB) stream_dcoef_kernel(const StreamParams p) {
+  const int lane = threadIdx.x & 31;
+  constexpr bool LEAN = is_lean<MODE, NV>();
+  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
+  __shared__ int s_r_all[LEAN ? 8 : 1][32];
+  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
+  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
+  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_RESID_DEV>(p, wid, lane, s_cv, s_r);
+}
+
+template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
+__global__ void __launch_bounds__(256, MINB) stream_accum_kernel(const StreamParams p) {
+  const int lane = threadIdx.x & 31;
+  constexpr bool LEAN = is_lean<MODE, NV>();
+  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
+  __shared__ int s_r_all[LEAN ? 8 : 1][32];
+  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
+  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
+  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_ACCUM>(p, wid, lane, s_cv, s_r);
+}
+
 // Launch helper: picks the instantiation of FORM for (weighted, perm, source form); U / MINB fixed by the caller.
 // The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.  EPI: the plain
-// or panel form with the residual (stream_residual_kernel) or label-propagation (stream_labelprop_kernel) epilogue,
-// one source.
+// or panel form with the residual (stream_residual_kernel), label-propagation (stream_labelprop_kernel),
+// device-coefficient residual (stream_dcoef_kernel) or accumulating (stream_accum_kernel) epilogue, one source.
 template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN, int EPI = EPI_NONE>
 static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   static_assert(FORM == FORM_PLAIN || NV == 1, "the panel and multi-head forms have one VecT per lane");
@@ -533,7 +636,8 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
     return set_error(COGDL_B200_EINVAL, "stream kernel: the panel, multi-head and epilogue forms read one source");
   const bool drop = FORM == FORM_MULTIHEAD && p.drop_scale > 0.f;
   note_kernel("cogdl_b200::%s<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>",
-              EPI == EPI_RESID ? "stream_residual_kernel" : (EPI == EPI_LABELPROP ? "stream_labelprop_kernel" : "stream_kernel"),
+              EPI == EPI_RESID ? "stream_residual_kernel" : EPI == EPI_LABELPROP ? "stream_labelprop_kernel"
+              : EPI == EPI_RESID_DEV ? "stream_dcoef_kernel" : EPI == EPI_ACCUM ? "stream_accum_kernel" : "stream_kernel",
               sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
               FORM == FORM_MULTIHEAD ? "multihead" : (p.val ? "weighted" : "unweighted"),
               (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "", drop ? "+drop" : "",
@@ -549,6 +653,14 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
     constexpr bool PANEL = FORM == FORM_PANEL;
     if (p.val) stream_labelprop_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
     else stream_labelprop_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if constexpr (EPI == EPI_RESID_DEV) {
+    constexpr bool PANEL = FORM == FORM_PANEL;
+    if (p.val) stream_dcoef_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_dcoef_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if constexpr (EPI == EPI_ACCUM) {
+    constexpr bool PANEL = FORM == FORM_PANEL;
+    if (p.val) stream_accum_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_accum_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
   } else if constexpr (FORM == FORM_MULTIHEAD) {
     if (drop) {
       if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);

@@ -35,6 +35,10 @@ correct_smooth=True rebinds the module globals `outcome_correlation` and `diffus
 the row reset go to cogdl_b200.label_propagate, the p = 1 diffusion steps to cogdl_b200.spmm_residual.  The originals
 stay reachable as `_cogdl_b200_original_outcome_correlation` / `_cogdl_b200_original_diffusion` on that module
 (uninstall_correct_smooth() restores them).
+gin=True rebinds `cogdl.layers.gin_layer.GINLayer.forward` (GIN, InfoGraph, GCC) and `cogdl.layers.gine_layer.GINELayer.forward`
+to gin_forward / gine_forward, which send `(1 + eps) * x + spmm(graph, x)` to cogdl_b200.gin_aggregate (uninstall_gin()).
+grand=True rebinds `cogdl.models.nn.grand.Grand.rand_prop` (GRAND) to grand_rand_prop, which keeps the reference's DropNode
+draw and sends the propagation to cogdl_b200.random_propagate (uninstall_grand()).
 """
 import sys
 
@@ -66,19 +70,19 @@ def genconv_forward(self, graph, x):
     return self.mlp(h)
 
 
-def _rebind_forward(cls, forward, name):
-    """cls.forward = forward, keeping the original at cls._cogdl_b200_original_forward; idempotent."""
-    if getattr(cls.forward, "_cogdl_b200", False):
+def _rebind_forward(cls, forward, name, attr="forward"):
+    """cls.<attr> (forward by default) = forward, keeping the original at cls._cogdl_b200_original_<attr>; idempotent."""
+    if getattr(getattr(cls, attr), "_cogdl_b200", False):
         return []
-    cls._cogdl_b200_original_forward = cls.forward
+    setattr(cls, "_cogdl_b200_original_" + attr, getattr(cls, attr))
     forward._cogdl_b200 = True
-    cls.forward = forward
+    setattr(cls, attr, forward)
     return [name]
 
 
-def _restore_forward(cls):
-    if getattr(cls.forward, "_cogdl_b200", False):
-        cls.forward = cls._cogdl_b200_original_forward
+def _restore_forward(cls, attr="forward"):
+    if getattr(getattr(cls, attr), "_cogdl_b200", False):
+        setattr(cls, attr, getattr(cls, "_cogdl_b200_original_" + attr))
 
 
 def install_genconv():
@@ -348,6 +352,72 @@ def uninstall_correct_smooth():
             setattr(cs, name, getattr(cs, "_cogdl_b200_original_" + name))
 
 
+def _gin_unsupported(self, graph, x):
+    eps = self.eps
+    return (unsupported_operands(graph, x) is not None or not torch.is_tensor(eps) or eps.device != x.device
+            or eps.dtype != torch.float32 or eps.numel() != 1 or x.dim() != 2 or x.shape[0] != graph.num_nodes)
+
+
+def gin_forward(self, graph, x):
+    """GINLayer.forward (cogdl/layers/gin_layer.py:34-38) with `(1 + self.eps) * x + spmm(graph, x)` in one
+    cogdl_b200.gin_aggregate launch (the backward, d eps included, through its autograd Function); apply_func is the
+    layer's own.  CPU or non-fp32 input or eps, and graphs with a dense grb_adj, run the original."""
+    from .operators.gin import gin_aggregate
+
+    if _gin_unsupported(self, graph, x):
+        return type(self)._cogdl_b200_original_forward(self, graph, x)
+    out = gin_aggregate(graph, x, self.eps)
+    return self.apply_func(out) if self.apply_func is not None else out
+
+
+def gine_forward(self, graph, x):
+    """GINELayer.forward (cogdl/layers/gine_layer.py:30-38): `out = spmm(graph, x); out += (1 + self.eps) * x` is the
+    same sum as GIN's (fp32 addition commutes), so it is one cogdl_b200.gin_aggregate launch; the fallbacks are
+    gin_forward's."""
+    return gin_forward(self, graph, x)
+
+
+def install_gin():
+    import cogdl.layers.gin_layer as gl
+    import cogdl.layers.gine_layer as gel
+
+    return (_rebind_forward(gl.GINLayer, gin_forward, "cogdl.layers.gin_layer.GINLayer.forward")
+            + _rebind_forward(gel.GINELayer, gine_forward, "cogdl.layers.gine_layer.GINELayer.forward"))
+
+
+def uninstall_gin():
+    import cogdl.layers.gin_layer as gl
+    import cogdl.layers.gine_layer as gel
+
+    _restore_forward(gl.GINLayer)
+    _restore_forward(gel.GINELayer)
+
+
+def grand_rand_prop(self, graph, x):
+    """Grand.rand_prop (cogdl/models/nn/grand.py:98-104): the reference's own drop_node (the same torch.bernoulli on the
+    CPU generator and `masks.to(device) * x`, so a seeded run draws the same mask; `x * (1 - p)` in eval mode), then the
+    order hops in cogdl_b200.random_propagate, one SpMM launch each with the running sum and the final division in its
+    store.  CPU or non-fp32 features and graphs with a dense grb_adj run the original."""
+    from .operators.grand import random_propagate
+
+    if unsupported_operands(graph, x) is not None or x.dim() != 2 or x.shape[0] != graph.num_nodes:
+        return type(self)._cogdl_b200_original_rand_prop(self, graph, x)
+    x = self.drop_node(x)
+    return random_propagate(graph, x, self.order)
+
+
+def install_grand():
+    import cogdl.models.nn.grand as gm
+
+    return _rebind_forward(gm.Grand, grand_rand_prop, "cogdl.models.nn.grand.Grand.rand_prop", attr="rand_prop")
+
+
+def uninstall_grand():
+    import cogdl.models.nn.grand as gm
+
+    _restore_forward(gm.Grand, attr="rand_prop")
+
+
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
 _spspmm_state = {"stub": None, "rebound": []}
 
@@ -452,7 +522,7 @@ def uninstall_actnn():
 
 
 def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
-            gcnii=False, appnp=False, correct_smooth=False):
+            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -550,4 +620,8 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_appnp()
     if correct_smooth:
         patched += install_correct_smooth()
+    if gin:
+        patched += install_gin()
+    if grand:
+        patched += install_grand()
     return patched

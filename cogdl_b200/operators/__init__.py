@@ -21,3 +21,5 @@ from .comp_aggr import compgcn_aggregate, CompAggrFunction  # noqa: F401
 from .spspmm import spspmm, coo_spmm, SpSpMMFunction  # noqa: F401
 from .spmm_residual import spmm_residual, SpmmResidualFunction  # noqa: F401
 from .label_prop import label_propagate  # noqa: F401
+from .gin import gin_aggregate, GinAggregateFunction  # noqa: F401
+from .grand import random_propagate  # noqa: F401

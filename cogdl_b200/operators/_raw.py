@@ -458,3 +458,40 @@ def comp_aggr_raw(st: CSRStructure, idx2, w, a, b, op):
                    _cabi.COMP_OPS[op], plan, _stream(dev))
         del keep
     return y
+
+
+def spmm_residual_dcoef_raw(st: CSRStructure, val, x, z, a, b_dev, row_scale=None, panels=0):
+    """Y = a * (row_scale[:, None] * (A @ x)) + b * z with b = b_dev[0], a one-element fp32 tensor on x's device that
+    the kernel reads (no host synchronisation); otherwise as spmm_residual_raw.  z may be None (b_dev is then unused)."""
+    dev, val, x, z, row_scale = _epilogue_args(st, val, x, z, row_scale)
+    require_cuda(x, b_dev)
+    b_dev = _f32c(b_dev, "b_dev").view(-1)
+    if b_dev.numel() != 1:
+        raise ValueError(f"b_dev must hold one value, got {b_dev.numel()}")
+    with torch.cuda.device(dev):
+        y, plan, keep = _spmm_out(st, val, x)
+        _cabi.call("cogdl_b200_spmm_residual_dcoef_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x),
+                   x.shape[0], _ptr(z), float(a), _ptr(b_dev), _ptr(row_scale), _ptr(y), st.n_rows, x.shape[1],
+                   int(panels), plan, _stream(dev))
+        del keep
+    return y
+
+
+def spmm_accum_raw(st: CSRStructure, val, x, acc, acc_in=None, row_scale=None, last=False, scale=1.0, xn=None,
+                   panels=0):
+    """One hop of GRAND's propagation: xn = row_scale[:, None] * (A @ x) (not stored when last) and, in place,
+    acc = acc_in + xn (acc_in None: acc itself), then acc * scale when last.  x [n_src, F], acc and acc_in [n_rows, F],
+    row_scale [n_rows], all fp32; scale is rounded to fp32.  xn: a preallocated [n_rows, F] fp32 output, allocated when
+    None and not last.  Returns xn (None when last)."""
+    dev, val, x, acc_in, row_scale = _epilogue_args(st, val, x, acc_in, row_scale)
+    require_cuda(x, acc, xn)
+    for name, t in (("acc", acc), ("xn", xn)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.shape != (st.n_rows, x.shape[1])):
+            raise ValueError(f"{name} must be a contiguous float32 [{st.n_rows}, {x.shape[1]}] tensor")
+    with torch.cuda.device(dev):
+        out, plan, keep = _spmm_out(st, val, x, acc if last else xn)   # acc: nothing to allocate on the last hop
+        _cabi.call("cogdl_b200_spmm_accum_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
+                   _ptr(row_scale), _ptr(acc_in), _ptr(acc), int(bool(last)), float(scale), _ptr(None if last else out),
+                   st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
+        del keep
+    return None if last else out

@@ -176,6 +176,30 @@ COGDL_B200_API int cogdl_b200_label_prop_f32(const int32_t *rowptr, const int32_
                                float *Y, int64_t n_rows, int64_t F, int32_t panels,
                                const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
+/* The residual epilogue of cogdl_b200_spmm_residual_f32 with b read on the device: GIN's `(1 + eps) * x + A @ x`, with
+ * a = 1 and b_dev pointing at fl(1 + eps), and its feature gradient over the adjoint.
+ *   Y[i,:] = fl( fl(a * fl(r[i] * (A @ X)[i,:])) + fl((*b_dev) * Z[i,:]) )
+ * b_dev is one fp32 value in device memory, read by the kernel (no host synchronisation); it is needed iff Z is given
+ * and must not overlap Y.  Everything else -- sums, rounding, x_rows, panels, plan scratch, the alignment rules and the
+ * overlap checks (COGDL_B200_EINVAL) -- is as for cogdl_b200_spmm_residual_f32. */
+COGDL_B200_API int cogdl_b200_spmm_residual_dcoef_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
+                               const float *X, int64_t x_rows, const float *Z, float a, const float *b_dev,
+                               const float *row_scale, float *Y, int64_t n_rows, int64_t F, int32_t panels,
+                               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
+/* One hop of GRAND's random propagation in one launch: the SpMM, the in_norm and the running hop sum.
+ *   Xn[i,:]  = fl(r[i] * (A @ X)[i,:])                       stored unless last != 0 (Xn may then be NULL)
+ *   ACC[i,:] = fl(ACC_in[i,:] + Xn[i,:]), times scale (one fp32 multiply) when last != 0
+ * acc_in may be NULL (ACC is updated in place) or another [n_rows, F] buffer that does not overlap ACC.  For
+ * `y.div_(order + 1.0)` pass scale = fl(1 / (order + 1)): on CUDA torch divides by a host scalar as a multiply by its
+ * fp32 reciprocal.  ACC must not overlap X or row_scale; Xn must not overlap X, ACC, acc_in or row_scale
+ * (COGDL_B200_EINVAL).  Sums, x_rows, panels, plan scratch and the alignment rules (ACC and acc_in with Y) are as for
+ * cogdl_b200_spmm_residual_f32. */
+COGDL_B200_API int cogdl_b200_spmm_accum_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
+                               const float *X, int64_t x_rows, const float *row_scale, const float *acc_in, float *acc,
+                               int32_t last, float scale, float *Xn, int64_t n_rows, int64_t F, int32_t panels,
+                               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
 /* fp16 storage (X, val, Y are IEEE half), fp32 accumulation (the reference accumulates in
  * half, spmm_kernel.cu:222-250,311-368,442-512 -- documented divergence). */
 COGDL_B200_API int cogdl_b200_spmm_csr_f16(const int32_t *rowptr, const int32_t *colind, const void *val,

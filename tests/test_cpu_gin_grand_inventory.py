@@ -1,0 +1,60 @@
+"""Every kernel compiled into gin.o and spmm_accum.o has a row in tests/gin_grand_table.py that the GPU suite runs
+(test_gpu_gin_grand.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The symbols
+are mapped to their recorded names through the residual inventory's note_of(): these kernels take the residual
+kernels' template parameters."""
+from tests.gin_grand_table import TABLE
+from tests.test_cpu_kernel_inventory import canonical, compiled_kernels
+from tests.test_cpu_spmm_residual_inventory import note_of as residual_note_of
+
+_NAMES = (("spmm_dcoef_kernel", "spmm_residual_kernel"), ("stream_dcoef_kernel", "stream_residual_kernel"),
+          ("spmm_accum_kernel", "spmm_residual_kernel"), ("stream_accum_kernel", "stream_residual_kernel"))
+
+
+def note_of(sym):
+    for mine, theirs in _NAMES:
+        if f"cogdl_b200::{mine}<" in sym:
+            return residual_note_of(sym.replace(mine, theirs)).replace(theirs, mine)
+    raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
+
+
+def _check(obj, epi):
+    compiled = {note_of(s): s for s in compiled_kernels((obj,))}
+    assert compiled, f"{obj}.o holds no kernels"
+    assert all(f"_{epi}_kernel<" in n for n in compiled), sorted(compiled)
+    table = {k for c in TABLE if c.epi == epi for k in canonical(c.kernel)}
+    untested = sorted(set(compiled) - table)
+    assert not untested, "compiled kernels without a row in tests/gin_grand_table.py:\n" + "\n".join(
+        f"  {n}   ({compiled[n]})" for n in untested)
+    unknown = sorted(table - set(compiled))
+    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+
+
+def test_gin_table_covers_every_compiled_kernel():
+    _check("gin", "dcoef")
+
+
+def test_accum_table_covers_every_compiled_kernel():
+    _check("spmm_accum", "accum")
+
+
+def test_gin_grand_rows_are_distinct_and_cover_every_epilogue_form():
+    ids = [c.id for c in TABLE]
+    assert len(ids) == len(set(ids))
+    dc = [c for c in TABLE if c.epi == "dcoef"]
+    ac = [c for c in TABLE if c.epi == "accum"]
+    assert {(c.z, c.row_scale) for c in dc} == {(True, True), (True, False), (False, True), (False, False)}
+    assert {(c.last, c.in_place) for c in ac} == {(True, True), (True, False), (False, True), (False, False)}
+    assert {False, True} == {c.row_scale for c in ac}
+    for rows in (dc, ac):
+        assert {1, 7, 16, 40, 47, 64, 128, 256} <= {c.F for c in rows}
+        assert {2, 4} <= {c.panels for c in rows}
+        assert {"none", "chunks", "default"} == {c.plan for c in rows}
+        assert any(not c.aligned for c in rows) and any(c.graph == "bounds" for c in rows)
+
+
+def test_note_of_maps_gin_grand_symbols():
+    assert note_of("void cogdl_b200::stream_accum_kernel<float4, (int)1, (int)1, (int)4, (int)4, (bool)0, (bool)0>"
+                   "(cogdl_b200::StreamParams)") == \
+        "cogdl_b200::stream_accum_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=4>"
+    assert note_of("void cogdl_b200::spmm_dcoef_kernel<float, (int)32, (int)4, (bool)0>(cogdl_b200::SpmmParams)") \
+        == "cogdl_b200::spmm_dcoef_kernel<float,GROUP=32,NV=4,unweighted>"
