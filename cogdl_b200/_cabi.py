@@ -104,7 +104,10 @@ SIGNATURES = {
     "cogdl_b200_comp_aggr_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_comp_aggr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _plan_p,
                                                 _vp]),
-    "cogdl_b200_spgemm_scratch_bytes": (_i64, [_i64, _i64, _i64]),
+    "cogdl_b200_rgcn_aggr_scratch_bytes": (_i64, [_i64, _i64, _i64]),
+    "cogdl_b200_rgcn_aggr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_rgcn_edge_dot_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_spgemm_scratch_bytes":(_i64, [_i64, _i64, _i64]),
     "cogdl_b200_spgemm_count": (ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, ctypes.POINTER(_i64), _vp,
                                                _i64, _vp]),
     "cogdl_b200_spgemm_fill_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp,

@@ -2,7 +2,7 @@
 (cogdl/data/data.py:134-451 Adjacency, :474-959 Graph), for use where the `cogdl` package is not
 importable (the GPU machine) and as the place where device-side structure caches live.
 
-Same names and meaning: row_indptr / col_indices / edge_index / edge_weight / raw_edge_weight /
+Same names and meaning: row_indptr / col_indices / edge_index / edge_weight / raw_edge_weight / edge_attr /
 in_norm / out_norm / is_symmetric / sym_norm / row_norm / col_norm / local_graph /
 add_remaining_self_loops / degrees / num_nodes / num_edges / to(device).  Index tensors are int64
 as in the reference; the kernels' int32 copy, the hub plan and the transpose are cached in
@@ -51,8 +51,9 @@ def _degrees_from_ptr(row_ptr):
 
 
 class Adjacency:
-    def __init__(self, row=None, col=None, row_ptr=None, weight=None, num_nodes=None):
+    def __init__(self, row=None, col=None, row_ptr=None, weight=None, num_nodes=None, attr=None):
         self.row, self.col, self.row_ptr, self.weight = row, col, row_ptr, weight
+        self.attr = attr                   # edge-aligned, reordered with the edges (reference data.py:279-287)
         self.__num_nodes__ = num_nodes
         self.__normed__ = None
         self.__in_norm__ = self.__out_norm__ = None
@@ -84,6 +85,8 @@ class Adjacency:
         self.row, self.col = self.row[reindex], self.col[reindex]
         if self.weight is not None:
             self.weight = self.weight[reindex]
+        if self.attr is not None:
+            self.attr = self.attr[reindex]
         self._structure = None
 
     @property
@@ -193,12 +196,17 @@ class Adjacency:
         self.row = torch.cat([row[mask], loop])
         self.col = torch.cat([col[mask], loop])
         self.weight = torch.cat([w[mask], loop_w])
+        if self.attr is not None:          # a new loop's attribute is 0, an existing loop keeps its own
+            loop_a = torch.zeros((n,) + tuple(self.attr.shape[1:]), dtype=self.attr.dtype, device=self.attr.device)
+            if inv.any():
+                loop_a[row[inv]] = self.attr[inv]
+            self.attr = torch.cat([self.attr[mask], loop_a])
         self.row_ptr = None
         self._to_csr()
 
     # ----------------------------------------------------------------- misc
     def to(self, device):
-        for k in ("row", "col", "row_ptr", "weight", "__in_norm__", "__out_norm__"):
+        for k in ("row", "col", "row_ptr", "weight", "attr", "__in_norm__", "__out_norm__"):
             v = getattr(self, k)
             if torch.is_tensor(v):
                 setattr(self, k, v.to(device))
@@ -214,16 +222,17 @@ class Adjacency:
 
 
 class Graph:
-    def __init__(self, x=None, y=None, edge_index=None, edge_weight=None, row_ptr=None, col=None, num_nodes=None, **kw):
+    def __init__(self, x=None, y=None, edge_index=None, edge_weight=None, row_ptr=None, col=None, num_nodes=None,
+                 edge_attr=None, **kw):
         self.x, self.y = x, y
         self.grb_adj = None
         if num_nodes is None and x is not None:
             num_nodes = x.shape[0]
         if edge_index is not None:
             row, col_ = edge_index
-            self._adj = Adjacency(row=row, col=col_, weight=edge_weight, num_nodes=num_nodes)
+            self._adj = Adjacency(row=row, col=col_, weight=edge_weight, num_nodes=num_nodes, attr=edge_attr)
         else:
-            self._adj = Adjacency(col=col, row_ptr=row_ptr, weight=edge_weight, num_nodes=num_nodes)
+            self._adj = Adjacency(col=col, row_ptr=row_ptr, weight=edge_weight, num_nodes=num_nodes, attr=edge_attr)
         self.__temp_adj_stack__ = []
         for k, v in kw.items():
             setattr(self, k, v)
@@ -273,6 +282,16 @@ class Graph:
     @property
     def raw_edge_weight(self):
         return self._adj.get_weight("raw")
+
+    @property
+    def edge_attr(self):
+        """Edge-aligned attributes (R-GCN / CompGCN edge types), in the graph's current edge order: building the CSR
+        of a graph held as COO reorders them with the edges, as it reorders the weights."""
+        return self._adj.attr
+
+    @edge_attr.setter
+    def edge_attr(self, attr):
+        self._adj.attr = attr
 
     @property
     def in_norm(self):

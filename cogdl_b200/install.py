@@ -39,6 +39,10 @@ gin=True rebinds `cogdl.layers.gin_layer.GINLayer.forward` (GIN, InfoGraph, GCC)
 to gin_forward / gine_forward, which send `(1 + eps) * x + spmm(graph, x)` to cogdl_b200.gin_aggregate (uninstall_gin()).
 grand=True rebinds `cogdl.models.nn.grand.Grand.rand_prop` (GRAND) to grand_rand_prop, which keeps the reference's DropNode
 draw and sends the propagation to cogdl_b200.random_propagate (uninstall_grand()).
+rgcn=True rebinds `cogdl.layers.rgcn_layer.RGCNLayer.forward` (RGCN, LinkPredictRGCN) to rgcn_forward, which computes the
+relational sum with cogdl_b200.rgcn_conv (uninstall_rgcn()).  This deliberately differs from the original for more than
+one relation: the original aggregates every edge with the weight of the first relation that has edges (see
+rgcn_forward).
 """
 import sys
 
@@ -418,6 +422,67 @@ def uninstall_grand():
     _restore_forward(gm.Grand, attr="rand_prop")
 
 
+_RGCN_EYE = {}
+
+
+def rgcn_forward(self, graph, x):
+    """RGCNLayer.forward (cogdl/layers/rgcn_layer.py:99-150) computing the relational sum the reference's loop was
+    written to compute, sum_t spmm(A_t, x W_t) with W_t = sum_b alpha[t, b] weight[b] and A_t the row-normalised graph
+    restricted to the type-t edges, in one cogdl_b200.rgcn_conv (a fan-out aggregation and one GEMM).
+
+    A deliberate divergence from the original: there, `return h_list` sits inside the per-relation loop and the
+    SpMM takes the whole graph, so every edge is aggregated with the W_t of the first relation that has edges, whatever
+    its type.  Both agree when there is one relation.  As in the original: graph.row_norm() is called (so the
+    normalisation runs over all of a row's edges, with the same side effect on the graph), alpha is the identity when
+    num_bases >= num_edge_types, and dropout, layer_norm, bias and the self-loop term follow in its order.  The masked
+    graphs' padding_self_loops() (weight 0.01), which the original builds and never uses, are not reproduced.  Edge
+    types held on the host are moved to x's device (LinkPredictRGCN.loss samples them there).  CPU or
+    non-fp32 input or weights, a dense grb_adj, and a regularizer other than basis run the original, the single-relation
+    computation above."""
+    import torch.nn.functional as F
+
+    from .operators.rgcn import rgcn_conv
+
+    params = [self.weight] + ([self.alpha] if self.alpha is not None else [])
+    if (self.regularizer != "basis" or unsupported_operands(graph, x, *params) is not None or x.dim() != 2
+            or any(p.device != x.device for p in params)):
+        return type(self)._cogdl_b200_original_forward(self, graph, x)
+    if self.num_bases < self.num_edge_types:
+        coef = self.alpha
+    else:
+        key = (self.num_edge_types, x.device)
+        coef = _RGCN_EYE.get(key)
+        if coef is None:
+            coef = _RGCN_EYE[key] = torch.eye(self.num_edge_types, dtype=torch.float32, device=x.device)
+    etype = graph.edge_attr
+    if etype is not None and etype.device != x.device:
+        # LinkPredictRGCN.loss builds its graph with host-side types (sampling_edge_uniform), on which building the
+        # CSR of a graph on the GPU raises in the original; the types go to the features' device once per graph
+        graph.edge_attr = etype.to(x.device)
+    graph.row_norm()
+    h_result = rgcn_conv(graph, x, coef, self.weight)
+    h_result = F.dropout(h_result, p=self.dropout, training=self.training)
+    if self.layer_norm is not None:
+        h_result = self.layer_norm(h_result)
+    if self.bias is not None:
+        h_result = h_result + self.bias
+    if self.self_loop is not None:
+        h_result += F.dropout(torch.matmul(x, self.weight_self_loop), p=self.self_dropout, training=self.training)
+    return h_result
+
+
+def install_rgcn():
+    import cogdl.layers.rgcn_layer as rl
+
+    return _rebind_forward(rl.RGCNLayer, rgcn_forward, "cogdl.layers.rgcn_layer.RGCNLayer.forward")
+
+
+def uninstall_rgcn():
+    import cogdl.layers.rgcn_layer as rl
+
+    _restore_forward(rl.RGCNLayer)
+
+
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
 _spspmm_state = {"stub": None, "rebound": []}
 
@@ -522,7 +587,7 @@ def uninstall_actnn():
 
 
 def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
-            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False):
+            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False, rgcn=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -624,4 +689,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_gin()
     if grand:
         patched += install_grand()
+    if rgcn:
+        patched += install_rgcn()
     return patched

@@ -23,3 +23,4 @@ from .spmm_residual import spmm_residual, SpmmResidualFunction  # noqa: F401
 from .label_prop import label_propagate  # noqa: F401
 from .gin import gin_aggregate, GinAggregateFunction  # noqa: F401
 from .grand import random_propagate  # noqa: F401
+from .rgcn import rgcn_aggregate, rgcn_conv, RgcnAggregateFunction, RgcnConvFunction  # noqa: F401

@@ -495,3 +495,57 @@ def spmm_accum_raw(st: CSRStructure, val, x, acc, acc_in=None, row_scale=None, l
                    st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
         del keep
     return None if last else out
+
+
+def rgcn_aggr_raw(st: CSRStructure, etype, w, coef, x, per_basis=False):
+    """R-GCN fan-out aggregation: y[i, b] = sum over row i's slots q of fl(w[q] * coef[etype[q], b]) * x[colind[q]]
+    (per_basis: x is [*, B, F] and basis b gathers x[colind[q], b]).  etype [nnz] int32 with every type in
+    [0, coef.shape[0]) (the caller's to guarantee), w [nnz] fp32, coef [T, B] fp32, x [*, F] fp32.  Returns y
+    [st.n_rows, B, F]; rows without slots are zero."""
+    dev = require_cuda(x, w, coef, etype)
+    x, w, coef = _f32c(x, "x"), _f32c(w, "w").view(-1), _f32c(coef, "coef")
+    if coef.dim() != 2:
+        raise ValueError(f"coef must be [T, B], got {tuple(coef.shape)}")
+    B = coef.shape[1]
+    if per_basis and (x.dim() != 3 or x.shape[1] != B):
+        raise ValueError(f"x must be [*, {B}, F] for the per-basis form, got {tuple(x.shape)}")
+    if not per_basis and x.dim() != 2:
+        raise ValueError(f"x must be [*, F], got {tuple(x.shape)}")
+    F = x.shape[-1]
+    if F <= 0 or B <= 0:
+        raise ValueError("F and B must be positive")
+    if w.numel() != st.nnz or etype.numel() != st.nnz:
+        raise ValueError(f"per-slot arrays must have {st.nnz} entries")
+    if etype.dtype != torch.int32:
+        raise TypeError(f"etype must be int32, got {etype.dtype}")
+    with torch.cuda.device(dev):
+        if st.nnz == 0:
+            return torch.zeros((st.n_rows, B, F), dtype=torch.float32, device=dev)
+        y = torch.empty((st.n_rows, B, F), dtype=torch.float32, device=dev)
+        need = int(_cabi.load().cogdl_b200_rgcn_aggr_scratch_bytes(st.plan.n_chunks, B, F))
+        plan, keep = st.plan_struct(need)
+        _cabi.call("cogdl_b200_rgcn_aggr_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(etype.contiguous()), _ptr(w),
+                   _ptr(coef), B, _ptr(x), int(bool(per_basis)), _ptr(y), st.n_rows, F, plan, _stream(dev))
+        del keep
+    return y
+
+
+def rgcn_edge_dot_raw(st: CSRStructure, w, g, x):
+    """p[q, b] = fl(w[q] * <g[row_q, b], x[colind[q]]>) for every slot q: g [st.n_rows, B, F], x [*, F], w [nnz], all
+    fp32.  Returns p [nnz, B] in slot order."""
+    dev = require_cuda(w, g, x)
+    w, g, x = _f32c(w, "w").view(-1), _f32c(g, "g"), _f32c(x, "x")
+    if g.dim() != 3 or g.shape[0] != st.n_rows or x.dim() != 2 or x.shape[1] != g.shape[2]:
+        raise ValueError(f"g must be [{st.n_rows}, B, F] and x [*, F], got {tuple(g.shape)} and {tuple(x.shape)}")
+    if w.numel() != st.nnz:
+        raise ValueError(f"w must have {st.nnz} entries")
+    B, F = g.shape[1], g.shape[2]
+    with torch.cuda.device(dev):
+        p = torch.empty((st.nnz, B), dtype=torch.float32, device=dev)
+        if st.nnz == 0:
+            return p
+        plan, keep = st.plan_struct(0)
+        _cabi.call("cogdl_b200_rgcn_edge_dot_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(w), _ptr(g), _ptr(x), _ptr(p),
+                   st.n_rows, B, F, plan, _stream(dev))
+        del keep
+    return p

@@ -349,6 +349,7 @@ def clear_structure_cache():
     _CACHE.clear()
     _COMP_CACHE.clear()
     _COO_CACHE.clear()
+    _RGCN_CACHE.clear()
 
 
 class CompStructure:
@@ -544,3 +545,71 @@ def coo_structure_for(index, n_rows, n_cols):
         cs = CooStructure(index, n_rows, n_cols)
         _COO_CACHE.put(key, (index,), cs)
     return cs
+
+
+class RgcnStructure:
+    """R-GCN's typed CSR: a graph's CSRStructure `st` with its edge types `type` (int32, in CSR slot order), in the
+    form the fan-out aggregation reads.  Built from the types a graph holds once its CSR exists (graph_operands, then
+    edge_attr), so every type stays paired with its edge.  Owns, built on first use:
+      * `transpose()`: the cached transpose of `st`, the types permuted to it and the permutation (the feature gradient);
+      * `by_type(T)`: the CSR with T type rows whose colind is the CSR slot, in slot order (the coefficient gradient
+        reduces per-slot products over it with the SpMM).
+    The types are checked once here (one host sync): a negative type raises ValueError, and `max_type` lets every call
+    check its coefficient table's size on the host."""
+
+    def __init__(self, st, etype):
+        etype = etype.reshape(-1)
+        if etype.numel() != st.nnz:
+            raise ValueError(f"edge_attr holds {etype.numel()} edge types, the graph has {st.nnz} edges")
+        if etype.dtype.is_floating_point or etype.dtype.is_complex or etype.dtype == torch.bool:
+            raise TypeError(f"edge types must be integers, got {etype.dtype}")
+        self.st, self.device, self.nnz = st, st.device, st.nnz
+        etype = etype.to(st.device, torch.int64)
+        self.max_type = -1
+        if st.nnz > 0:
+            lo, hi = (int(v) for v in torch.stack([etype.min(), etype.max()]).tolist())   # one sync per structure
+            if lo < 0:
+                raise ValueError(f"edge type {lo} is negative")
+            if hi >= 2**31:
+                raise ValueError(f"edge type {hi} does not fit int32")
+            self.max_type = hi
+        self.type = etype.to(torch.int32).contiguous()
+        self._transpose = None
+        self._by_type = {}
+
+    def transpose(self):
+        """(CSRStructure of A^T, type in its slot order, perm [nnz] int64: CSR slot of each transpose slot)."""
+        if self._transpose is None:
+            t, perm = self.st.csc()
+            p = perm.long()
+            self._transpose = (t, self.type[p].contiguous(), p)
+        return self._transpose
+
+    def by_type(self, T):
+        """CSRStructure with T rows (types) whose colind lists the CSR slots of that type in slot order."""
+        from .data import coo2csr_index
+
+        st = self._by_type.get(T)
+        if st is None:
+            if self.max_type >= T:
+                raise ValueError(f"edge type {self.max_type} is out of range for {T} relations")
+            rowptr, reindex = coo2csr_index(self.type.long(), T)
+            st = self._by_type[T] = CSRStructure(rowptr.int(), reindex.int(), n_cols=self.nnz)
+        return st
+
+
+# RgcnStructure cache, keyed on the storage identity of the graph structure's int32 CSR and of the edge-type tensor:
+# both layers of a model, and repeated predict() calls on one graph, share one entry.
+rgcn_cache_stats = {"hit": 0, "miss": 0}
+_RGCN_CACHE = IdentityCache(4, rgcn_cache_stats)
+
+
+def rgcn_structure_for(st, etype):
+    keys = (st.rowptr, st.colind, etype)
+    key = tuple((t.data_ptr(), t.numel(), str(t.device), t.dtype) for t in keys)
+    rs = _RGCN_CACHE.get(key)
+    if rs is None or rs.st is not st:
+        rgcn_cache_stats["miss"] += 1
+        rs = RgcnStructure(st, etype)
+        _RGCN_CACHE.put(key, keys, rs)
+    return rs

@@ -502,6 +502,31 @@ COGDL_B200_API int cogdl_b200_comp_aggr_f32(const int32_t *rowptr, const int32_t
                                             const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * R-GCN relational aggregation under a basis decomposition (cogdl/layers/rgcn_layer.py:118-150), without a
+ * per-relation tensor.  Per row i of the CSR (rowptr, colind) with per-slot edge type etype and weight w, and a
+ * coefficient table coef [T, B] (etype < T is the caller's to guarantee):
+ *   cogdl_b200_rgcn_aggr_f32:      Y[i,b,:] = sum_{q in row i} fl(w[q] * coef[etype[q], b]) * X[colind[q], :]
+ *                                  (per_basis != 0: X is [*, B, F] and basis b gathers X[colind[q], b, :])
+ *   cogdl_b200_rgcn_edge_dot_f32:  P[q, b]  = fl(w[q] * <G[i, b, :], X[colind[q], :]>) for every slot q of row i
+ * X [*, F] (or [*, B, F]), Y and G [n_rows, B, F], P [nnz, B], all fp32 row-major.  Degree-0 rows give zeros.  Y[:, b, :]
+ * is accumulated in CSR order with a separate multiply and add and hub rows are merged in chunk order, so it is
+ * bit-identical to cogdl_b200_spmm_csr_f32_ex with values fl(w * coef[etype, b]) on the same plan; both entries are
+ * reproducible run to run (no float atomics).  Needs a hub plan (chunk_edges > 0) with row-stream segments; for the
+ * aggregation plan->partials needs cogdl_b200_rgcn_aggr_scratch_bytes(n_chunks, B, F) bytes.  16-byte vectors when
+ * F % 4 == 0 and the feature buffers (and the partials) are 16-byte aligned.  Rejects F <= 0, B outside [1, 4096] and a
+ * plan whose row counts do not match n_rows.
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_rgcn_aggr_scratch_bytes(int64_t n_chunks, int64_t B, int64_t F);
+COGDL_B200_API int cogdl_b200_rgcn_aggr_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *etype,
+                                            const float *w, const float *coef, int64_t B, const float *X,
+                                            int32_t per_basis, float *Y, int64_t n_rows, int64_t F,
+                                            const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_rgcn_edge_dot_f32(const int32_t *rowptr, const int32_t *colind, const float *w,
+                                                const float *G, const float *X, float *P, int64_t n_rows, int64_t B,
+                                                int64_t F, const cogdl_b200_hub_plan_t *plan,
+                                                cogdl_b200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Sparse x sparse product C = A.B, A [a_rows x a_cols] and B [b_rows x b_cols] int32 CSR with fp32 values, columns
  * ascending and unique inside every row (b_rows must equal a_cols).  C comes out as CSR with ascending, unique columns.
  * Replaces  torch_sparse.spspmm(indexA, valueA, indexB, valueB, m, k, n)   (cuSPARSE SpGEMM), imported at module level
