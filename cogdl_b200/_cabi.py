@@ -96,6 +96,11 @@ SIGNATURES = {
     "cogdl_b200_softmax_aggr_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_softmax_aggr_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _vp, _i64, _i64,
                                                        _plan_p, _vp]),
+    "cogdl_b200_genconv_edge_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _f32, _vp, _vp, _vp, _i64, _i64,
+                                                       _plan_p, _vp]),
+    "cogdl_b200_genconv_edge_dw_scratch_bytes": (_i64, [_i64, _i64]),
+    "cogdl_b200_genconv_edge_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _f32, _vp, _vp, _vp, _vp, _vp,
+                                                       _vp, _i64, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_disen_route_scratch_bytes": (_i64, [_i64, _i64, _i64]),
     "cogdl_b200_disen_route_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _f32,
                                                       _plan_p, _vp]),

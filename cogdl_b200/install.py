@@ -55,8 +55,11 @@ _GENCONV_KERNEL_AGGRS = ("softmax_sg", "softmax", "mean", "sum", "max", "powerme
 
 def genconv_forward(self, graph, x):
     """GENConv.forward (cogdl/layers/deepergcn_layer.py:64-102) with the aggregation in the sm_90a kernels.  The
-    edge encoder, message_norm, residual and MLP are the layer's own.  Cases without a kernel -- CPU or non-fp32
-    input, an aggregation name GENConv does not define, max / powermean with an edge encoder -- run the original."""
+    message_norm, residual and MLP are the layer's own.  A bias-free EdgeEncoder on fp32 CUDA edge features of at
+    most 16 columns that need no gradient is folded into the softmax aggregations (its product with the features is
+    formed inside the kernels, so no [nnz, F] edge tensor exists); any other edge encoder runs as the layer's own
+    module and its output goes in as the edge term.  Cases without a kernel -- CPU or non-fp32 input, an
+    aggregation name GENConv does not define, max / powermean with an edge encoder -- run the original."""
     from .operators.softmax_aggr import genconv_aggregate
 
     original = type(self)._cogdl_b200_original_forward
@@ -65,13 +68,38 @@ def genconv_forward(self, graph, x):
             or (has_edge and self.aggr in ("max", "powermean"))):
         return original(self, graph, x)
     st = graph_operands(graph).st
-    edge_term = self.edge_encoder(graph.edge_attr) if has_edge else None
-    h = genconv_aggregate(st, x, self.aggr, beta=self.beta, eps=self.eps, edge_term=edge_term, p=self.p)
+    edge = {}
+    if has_edge:
+        attr = graph.edge_attr                       # read after graph_operands: in CSR order
+        weight = _fused_edge_encoder_weight(self.edge_encoder, attr, x.shape[1])
+        if weight is not None:
+            edge = {"edge_attr": attr, "edge_weight": weight}
+        else:
+            edge = {"edge_term": self.edge_encoder(attr)}
+    h = genconv_aggregate(st, x, self.aggr, beta=self.beta, eps=self.eps, p=self.p, **edge)
     if self.use_msg_norm:
         h = self.message_norm(x, h)
     if self.residual:
         h = h + x
     return self.mlp(h)
+
+
+def _fused_edge_encoder_weight(encoder, attr, F):
+    """The [F, D] weight of `encoder` when the fused edge-encoder kernels can take it: an EdgeEncoder whose nn.Linear
+    has no bias, fp32 CUDA weight and edge features, features that need no gradient, 1 <= D <= 16.  None otherwise
+    (BondEncoder, wider or trainable features: the encoder runs as a module)."""
+    from cogdl.layers.deepergcn_layer import EdgeEncoder
+
+    from .operators._raw import GENCONV_EDGE_MAX_D
+
+    if type(encoder) is not EdgeEncoder or not isinstance(encoder.nn, torch.nn.Linear) or encoder.nn.bias is not None:
+        return None
+    w = encoder.nn.weight
+    if (attr.dtype != torch.float32 or not attr.is_cuda or attr.requires_grad or attr.dim() != 2
+            or not 1 <= attr.shape[1] <= GENCONV_EDGE_MAX_D or w.dtype != torch.float32 or w.device != attr.device
+            or w.shape != (F, attr.shape[1])):
+        return None
+    return w
 
 
 def _rebind_forward(cls, forward, name, attr="forward"):

@@ -15,7 +15,7 @@ from .edge_softmax import csr_edge_softmax, EdgeSoftmaxFunction  # noqa: F401
 from .mhspmm import csrmhspmm, MHSPMMFunction  # noqa: F401
 from .scatter_max import scatter_max, ScatterMaxFunction  # noqa: F401
 from .fused_gat import fused_gat_func, FusedGATFunction  # noqa: F401
-from .softmax_aggr import genconv_aggregate, SoftmaxAggrFunction  # noqa: F401
+from .softmax_aggr import genconv_aggregate, GenconvEdgeFunction, SoftmaxAggrFunction  # noqa: F401
 from .disen_routing import disen_routing, DisenRouteFunction  # noqa: F401
 from .comp_aggr import compgcn_aggregate, CompAggrFunction  # noqa: F401
 from .spspmm import spspmm, coo_spmm, SpSpMMFunction  # noqa: F401

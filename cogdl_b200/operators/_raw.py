@@ -348,6 +348,71 @@ def softmax_aggr_bwd_raw(st: CSRStructure, x, beta, eps, g, out, lse2, edge_term
     return dx, da
 
 
+GENCONV_EDGE_MAX_D = 16   # widest edge feature of cogdl_b200/csrc/genconv_edge.cu
+
+
+def _ge_check(st, x, attr, w):
+    """Shared argument checks of the edge-encoder aggregation: attr [nnz, D] and w [F, D] fp32 on x's device,
+    1 <= D <= 16.  Returns (attr, w) contiguous."""
+    require_cuda(attr, w)
+    attr, w = _f32c(attr, "edge_attr"), _f32c(w, "edge encoder weight")
+    if attr.dim() != 2 or attr.shape[0] != st.nnz:
+        raise ValueError(f"edge_attr must be [nnz={st.nnz}, D], got {tuple(attr.shape)}")
+    D = attr.shape[1]
+    if not 1 <= D <= GENCONV_EDGE_MAX_D:
+        raise ValueError(f"edge_attr has D = {D} features; the fused edge encoder takes 1 to {GENCONV_EDGE_MAX_D}")
+    if w.shape != (x.shape[1], D):
+        raise ValueError(f"edge encoder weight must be [F={x.shape[1]}, D={D}], got {tuple(w.shape)}")
+    return attr, w
+
+
+def genconv_edge_fwd_raw(st: CSRStructure, x, attr, w, beta, eps, want_lse=False, want_q=False):
+    """softmax_aggr_fwd_raw with the edge term attr @ w.T formed inside the kernel (no [nnz, F] tensor): attr
+    [nnz, D] in CSR order, w [F, D] (nn.Linear layout), 1 <= D <= 16.  Returns (out, lse2, q) as softmax_aggr_fwd_raw."""
+    dev = require_cuda(x)
+    x, beta, _ = _sa_check(st, x, beta, None, st.n_cols)
+    attr, w = _ge_check(st, x, attr, w)
+    F = x.shape[1]
+    with torch.cuda.device(dev):
+        out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+        lse2 = torch.empty_like(out) if want_lse else None
+        q = torch.empty_like(out) if want_q else None
+        plan, keep = st.plan_struct(_sa_scratch(st, F))
+        _cabi.call("cogdl_b200_genconv_edge_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(x), _ptr(attr), _ptr(w),
+                   attr.shape[1], _ptr(beta), float(eps), _ptr(out), _ptr(lse2), _ptr(q), st.n_rows, F, plan,
+                   _stream(dev))
+        del keep
+    return out, lse2, q
+
+
+def genconv_edge_bwd_raw(st: CSRStructure, x, attr, w, beta, eps, g, out, lse2, want_dx=True, want_dw=True):
+    """(dx [n_cols, F] or None, dw [F, D] or None) of genconv_edge_fwd_raw, over the cached transpose of st.  dw is
+    summed in a fixed order without float atomics (bit-identical run to run)."""
+    dev = require_cuda(x, g, out, lse2)
+    x, beta, _ = _sa_check(st, x, beta, None, st.n_cols)
+    attr, w = _ge_check(st, x, attr, w)
+    F, D = x.shape[1], attr.shape[1]
+    g, out, lse2 = _f32c(g, "grad"), _f32c(out, "out"), _f32c(lse2, "lse2")
+    for name, t in (("grad", g), ("out", out), ("lse2", lse2)):
+        if t.shape != (st.n_rows, F):
+            raise ValueError(f"{name} must be [{st.n_rows}, {F}], got {tuple(t.shape)}")
+    if not (want_dx or want_dw):
+        return None, None
+    st_t, perm = st.csc()
+    with torch.cuda.device(dev):
+        dx = torch.empty_like(x) if want_dx else None
+        dw = torch.empty((F, D), dtype=torch.float32, device=dev) if want_dw else None
+        n_scr = int(_cabi.load().cogdl_b200_genconv_edge_dw_scratch_bytes(F, D)) if want_dw else 0
+        scratch = torch.empty(n_scr // 4, dtype=torch.float32, device=dev) if want_dw else None
+        need = st_t.plan.n_chunks * F * 4 if st_t.chunk_edges > 0 and want_dx else 0
+        plan, keep = st_t.plan_struct(need)
+        _cabi.call("cogdl_b200_genconv_edge_bwd_f32", _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(x),
+                   _ptr(attr), _ptr(w), D, _ptr(beta), float(eps), _ptr(g), _ptr(out), _ptr(lse2), _ptr(dx), _ptr(dw),
+                   _ptr(scratch), n_scr, st_t.n_rows, F, plan, _stream(dev))
+        del keep
+    return dx, dw
+
+
 def _dr_scratch(st, F, K):
     if st.chunk_edges <= 0:
         return 0

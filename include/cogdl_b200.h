@@ -447,6 +447,36 @@ COGDL_B200_API int cogdl_b200_softmax_aggr_bwd_f32(const int32_t *colptr, const 
                                     cogdl_b200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * GENConv softmax aggregation with a linear edge encoder (EdgeEncoder, cogdl/layers/deepergcn_layer.py:168-174:
+ * nn.Linear(D, F, bias=False)), the edge term formed in registers instead of read from an [nnz, F] tensor:
+ *   edge_term[e,f] = sum_{d=0..D-1} attr[e,d] W[f,d]   (one fmaf chain, d ascending)
+ * and otherwise the operation of cogdl_b200_softmax_aggr_fwd_f32 / _bwd_f32, with the same work items, hub plan,
+ * chunk-order merge and lse2 / Q outputs.  attr is [nnz, D] fp32 in CSR order, W is [F, D] fp32 (nn.Linear layout),
+ * 1 <= D <= 16 (wider D is rejected).  The forward's plan->partials needs what cogdl_b200_softmax_aggr_scratch_bytes
+ * gives.  When F is a multiple of 4, 16-byte vectors if X, out, lse2, Q (and G, dX, the partials) are aligned.
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int cogdl_b200_genconv_edge_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
+                                                   const float *attr, const float *W, int64_t D, const float *beta,
+                                                   float eps, float *out, float *lse2, float *Q, int64_t n_rows,
+                                                   int64_t F, const cogdl_b200_hub_plan_t *plan,
+                                                   cogdl_b200_stream_t stream);
+/* Backward over the transpose (colptr, rowind, perm; n_cols columns; `plan` is the TRANSPOSE's plan, partials
+ * n_chunks*F*4 bytes when dX is asked for), given G = dL/dout and the forward's out and lse2:
+ *   dX[j]    = sum_{e: c_e = j} dpre_e             (as cogdl_b200_softmax_aggr_bwd_f32; NULL: not computed)
+ *   dW[f,d]  = sum_e dpre_e[f] attr[e,d]           ([F, D]; NULL: not computed)
+ * dW is summed without float atomics: per warp over a fixed, static assignment of work items, then per block in warp
+ * order into dw_scratch, then over the blocks in block order, so it is bit-identical run to run on one device.
+ * dw_scratch must hold cogdl_b200_genconv_edge_dw_scratch_bytes(F, D) bytes (a bound independent of nnz).  At least
+ * one of dX, dW.  d beta = sum G (Q - out^2) is left to the caller. */
+COGDL_B200_API int64_t cogdl_b200_genconv_edge_dw_scratch_bytes(int64_t F, int64_t D);
+COGDL_B200_API int cogdl_b200_genconv_edge_bwd_f32(const int32_t *colptr, const int32_t *rowind, const int32_t *perm,
+                                                   const float *X, const float *attr, const float *W, int64_t D,
+                                                   const float *beta, float eps, const float *G, const float *out,
+                                                   const float *lse2, float *dX, float *dW, float *dw_scratch,
+                                                   int64_t dw_scratch_bytes, int64_t n_cols, int64_t F,
+                                                   const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * DisenGCN neighbourhood routing, one step (cogdl/layers/disengcn_layer.py:40-91) without per-edge feature
  * tensors.  Rows of F = K*d floats are K channels of d (channel k = columns [k*d, (k+1)*d)).  c holds the
  * per-(node, channel) normalised features, q the current routing state ([n, F] each).  Per row i, channel k,

@@ -1,0 +1,51 @@
+"""Every kernel compiled into genconv_edge.o has a row in tests/genconv_edge_table.py that the GPU suite runs
+(test_gpu_genconv_edge.py), and every kernel the table names is compiled, checked on a machine without a GPU."""
+import re
+
+from tests.genconv_edge_table import DS, FS, MAX_D, TABLE
+from tests.test_cpu_kernel_inventory import canonical, compiled_kernels
+
+
+def note_of(sym):
+    """The name cogdl_b200_last_kernel() records for a demangled genconv_edge.o kernel symbol."""
+    if re.match(r"cogdl_b200::genconv_edge_dw_reduce_kernel\(", sym):
+        return "cogdl_b200::genconv_edge_dw_reduce_kernel"
+    m = re.match(r"void cogdl_b200::genconv_edge_(fwd|bwd)_kernel<\(int\)([14]), \(int\)(\d+)(?:, \(bool\)([01]))?>", sym)
+    assert m, f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table"
+    op, w, dm, q = m.groups()
+    v = "float4" if w == "4" else "float"
+    if op == "fwd":
+        return f"cogdl_b200::genconv_edge_fwd_kernel<{v},DM={dm},{'Q' if q == '1' else 'no_Q'}>"
+    return f"cogdl_b200::genconv_edge_bwd_kernel<{v},DM={dm}>"
+
+
+def test_genconv_edge_table_covers_every_compiled_kernel():
+    compiled = {note_of(s): s for s in compiled_kernels(("genconv_edge",))}
+    assert compiled, "genconv_edge.o holds no kernels"
+    table = {k for c in TABLE for k in canonical(c.kernel)}
+    untested = sorted(set(compiled) - table)
+    assert not untested, "compiled kernels without a row in tests/genconv_edge_table.py:\n" + "\n".join(
+        f"  {n}   ({compiled[n]})" for n in untested)
+    unknown = sorted(table - set(compiled))
+    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+
+
+def test_genconv_edge_rows_are_distinct_and_cover_the_shapes():
+    ids = [c.id for c in TABLE]
+    assert len(ids) == len(set(ids))
+    for op in ("fwd", "bwd"):
+        rows = [c for c in TABLE if c.op == op]
+        assert set(FS) <= {c.F for c in rows} and set(DS) <= {c.D for c in rows}
+        assert {1, MAX_D} <= {c.D for c in rows}
+        assert {"hub", "two_hubs", "ragged", "rect", "empty_graph"} <= {c.graph for c in rows}
+        assert any(not c.aligned for c in rows) and any(c.F > 128 for c in rows)
+    assert {c.want for c in TABLE if c.op == "bwd"} == {"dx_dw", "dx", "dw"}
+
+
+def test_note_of_maps_genconv_edge_symbols():
+    assert note_of("void cogdl_b200::genconv_edge_fwd_kernel<(int)4, (int)8, (bool)1>(cogdl_b200::GeFwdParams)") == \
+        "cogdl_b200::genconv_edge_fwd_kernel<float4,DM=8,Q>"
+    assert note_of("void cogdl_b200::genconv_edge_bwd_kernel<(int)1, (int)16>(cogdl_b200::GeBwdParams)") == \
+        "cogdl_b200::genconv_edge_bwd_kernel<float,DM=16>"
+    assert note_of("cogdl_b200::genconv_edge_dw_reduce_kernel(const float *, int, long, float *)") == \
+        "cogdl_b200::genconv_edge_dw_reduce_kernel"
