@@ -112,6 +112,11 @@ SIGNATURES = {
     "cogdl_b200_rgcn_aggr_scratch_bytes": (_i64, [_i64, _i64, _i64]),
     "cogdl_b200_rgcn_aggr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_rgcn_edge_dot_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_hgn_max_table": (_i64, []),
+    "cogdl_b200_hgn_attn_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _f32, ctypes.c_uint64, ctypes.c_uint64,
+                                               _f32, _vp, _f32, _vp, _vp, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_hgn_attn_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _vp, _vp, _i64,
+                                                   _i64, _plan_p, _vp]),
     "cogdl_b200_spgemm_scratch_bytes":(_i64, [_i64, _i64, _i64]),
     "cogdl_b200_spgemm_count": (ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, ctypes.POINTER(_i64), _vp,
                                                _i64, _vp]),

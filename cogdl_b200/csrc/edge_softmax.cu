@@ -5,7 +5,8 @@
 // one block of 32 x H threads per row, three passes over the row with lanes striding H floats apart
 // -- <= 1/H sector efficiency -- and exp() evaluated twice) and, in MODE 2 / 3, the
 // `leakyrelu(h_l[row] + h_r[col])` gathers + LeakyReLU + edge_softmax chain of
-// cogdl/layers/gat_layer.py:73-74 and its autograd backward.
+// cogdl/layers/gat_layer.py:73-74 and its autograd backward.  The kernel bodies live in edge_softmax.cuh, which
+// simple_hgn.cu instantiates with Simple-HGN's edge-type term and residual attention.
 //
 // Key layout fact: in CSR order the [deg, H] logits of row i are ONE contiguous block of deg*H floats
 // at rowptr[i]*H, and consecutive rows are consecutive blocks.  With H a power of two <= 32, the
@@ -44,595 +45,35 @@
 // (edge, head) here instead of in the gather loops.  MODE 3 reads y = |att| and g = (sign bit ? 0 : d att * scale),
 // the gradient of the softmax before the dropout.  The bit is tested, never `att < 0`: a dropped softmax that
 // underflowed to 0 is -0.0.
-#include "common.cuh"
-#include "rng.cuh"
-
-#include <math_constants.h>
-
-#include <cfloat>
-#include <cstdio>
-#include <cstdlib>
+#include "edge_softmax.cuh"
 
 namespace cogdl_b200 {
 
-struct EsParams {
-  const int *rowptr;
-  const float *a;
-  const float *b;
-  float *out;
-  int64_t n_rows;
-  int H;
-  int lgH;
-  const int *colind;      // MODE 2, 3
-  float slope;            // MODE 2, 3
-  const float *hl;        // MODE 3: h_l [N,H]
-  const float *hr;        // MODE 3: h_r [N,H]
-  float *grow;            // MODE 3: [N,H] row sums of the output
-  HubView hub;            // chunks / segments / edge_row / counters
-  float2 *stats;          // per chunk slot x head: (max, sum) -- the row's merged value sits in its first slot
-  float *part;            // MODE 3: per chunk slot x head partial row sums
-  bool bulk;              // tiles may be moved with cp.async.bulk (alignment checked on the host)
-  uint64_t seed;          // DROP: attention-dropout mask (see the header comment)
-  uint64_t drop_below;
-  float scale;            // DROP, MODE 3: 1 / (1 - p_drop), the factor a kept attention was multiplied by
-};
-
-// DROP, MODE 2: the attention a (>= 0) of CSR edge `edge`, head `head`, with the sign bit set if the pair is dropped
-template <bool DROP>
-__device__ __forceinline__ float es_mark(const EsParams &p, int64_t edge, int head, float a) {
-  if (DROP && draw(p.seed, edge, head) < p.drop_below) a = __uint_as_float(__float_as_uint(a) | 0x80000000u);
-  return a;
-}
-// DROP, MODE 3: (y, g) = (saved attention, d attention after dropout) -> (softmax, d softmax)
-template <bool DROP>
-__device__ __forceinline__ void es_unmark(const EsParams &p, float &y, float &g) {
-  if (DROP) {
-    g = (__float_as_uint(y) >> 31) ? 0.f : __fmul_rn(g, p.scale);
-    y = fabsf(y);
-  }
-}
-
-// exp for the plan-based kernels: arguments are x - max <= 0.  ex2.approx(x * log2 e): 2 ulp from the MUFU plus
-// |x| * 2^-24 from the scaling product, i.e. <= ~2e-6 relative for logits within 30 of the row maximum and an
-// absolute error far below 1e-5 of the row's largest term beyond that (parity bar: 1e-5).  FMUL + MUFU.EX2
-// instead of the ~12-instruction expf(): these kernels are issue-bound, not memory-bound.
-__device__ __forceinline__ float es_exp(float x) { return __expf(x); }
-
-// reduce across lanes that share lane % H  (strides 16 .. H)
-__device__ __forceinline__ float head_max(float v, int H) {
-  for (int s = 16; s >= H; s >>= 1) v = fmaxf(v, __shfl_xor_sync(FULL, v, s));
-  return v;
-}
-__device__ __forceinline__ float head_sum(float v, int H) {
-  for (int s = 16; s >= H; s >>= 1) v += __shfl_xor_sync(FULL, v, s);
-  return v;
-}
-
-// Forward input of element t of the row whose block starts at edge lb (head = t % H).
-template <int MODE>
-__device__ __forceinline__ float es_in(const EsParams &p, int lb, int64_t t, int head, float hl) {
-  if (MODE == 2) {
-    const int c = __ldg(p.colind + lb + (int)(t >> p.lgH));
-    const float z = hl + __ldg(p.b + (int64_t)c * p.H + head);
-    return z > 0.f ? z : z * p.slope;
-  }
-  return __ldg(p.a + (int64_t)lb * p.H + t);
-}
-// MODE 3: derivative of the LeakyReLU at the pre-activation of element t
-__device__ __forceinline__ float es_dact(const EsParams &p, int lb, int64_t t, int head, float hlrow) {
-  const int c = __ldg(p.colind + lb + (int)(t >> p.lgH));
-  const float z = hlrow + __ldg(p.hr + (int64_t)c * p.H + head);
-  return z > 0.f ? 1.f : p.slope;
-}
-
-// One row handled by a team of NT threads striding the row's elements (tid = index inside the
-// team, NT % H == 0).  reduce(v, is_max) must return the team-wide per-head reduction.
-template <int MODE, int NT, bool DROP, typename Reduce>
-__device__ __forceinline__ void es_row(const EsParams &p, int64_t row, int lb, int64_t n, int tid, Reduce reduce) {
-  const int head = tid & (p.H - 1);
-  float *o = p.out + (int64_t)lb * p.H;
-  if (MODE == 1 || MODE == 3) {
-    const float *y = p.a + (int64_t)lb * p.H, *g = p.b + (int64_t)lb * p.H;
-    auto yg = [&](int64_t t) {
-      float yv = __ldg(y + t), gv = __ldg(g + t);
-      es_unmark<DROP>(p, yv, gv);
-      return make_float2(yv, gv);
-    };
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    int64_t t = tid;
-    for (; t + 3 * NT < n; t += 4 * NT) {
-      float2 v = yg(t);
-      s0 = fmaf(v.x, v.y, s0);
-      v = yg(t + NT);
-      s1 = fmaf(v.x, v.y, s1);
-      v = yg(t + 2 * NT);
-      s2 = fmaf(v.x, v.y, s2);
-      v = yg(t + 3 * NT);
-      s3 = fmaf(v.x, v.y, s3);
-    }
-    for (; t < n; t += NT) { const float2 v = yg(t); s0 = fmaf(v.x, v.y, s0); }
-    const float s = reduce((s0 + s1) + (s2 + s3), false);
-    t = tid;
-    if (MODE == 1) {
-#pragma unroll 4
-      for (; t < n; t += NT) st_stream(o + t, __ldg(y + t) * (__ldg(g + t) - s));
-    } else {
-      const float hlrow = __ldg(p.hl + row * p.H + head);
-      float acc = 0.f;
-      for (; t < n; t += NT) {
-        const float2 w = yg(t);
-        const float v = w.x * (w.y - s) * es_dact(p, lb, t, head, hlrow);
-        st_stream(o + t, v);
-        acc += v;
-      }
-      acc = reduce(acc, false);
-      if (tid < p.H) p.grow[row * p.H + head] = acc;
-    }
-    return;
-  }
-  const float hl = (MODE == 2) ? __ldg(p.a + row * p.H + head) : 0.f;
-  float m0 = -CUDART_INF_F, m1 = m0, m2 = m0, m3 = m0;
-  int64_t t = tid;
-  for (; t + 3 * NT < n; t += 4 * NT) {
-    const float x0 = es_in<MODE>(p, lb, t, head, hl), x1 = es_in<MODE>(p, lb, t + NT, head, hl);
-    const float x2 = es_in<MODE>(p, lb, t + 2 * NT, head, hl), x3 = es_in<MODE>(p, lb, t + 3 * NT, head, hl);
-    m0 = fmaxf(m0, x0); m1 = fmaxf(m1, x1); m2 = fmaxf(m2, x2); m3 = fmaxf(m3, x3);
-  }
-  for (; t < n; t += NT) m0 = fmaxf(m0, es_in<MODE>(p, lb, t, head, hl));
-  const float m = reduce(fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)), true);
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-  t = tid;
-  for (; t + 3 * NT < n; t += 4 * NT) {
-    const float x0 = es_in<MODE>(p, lb, t, head, hl), x1 = es_in<MODE>(p, lb, t + NT, head, hl);
-    const float x2 = es_in<MODE>(p, lb, t + 2 * NT, head, hl), x3 = es_in<MODE>(p, lb, t + 3 * NT, head, hl);
-    s0 += expf(x0 - m); s1 += expf(x1 - m); s2 += expf(x2 - m); s3 += expf(x3 - m);
-  }
-  for (; t < n; t += NT) s0 += expf(es_in<MODE>(p, lb, t, head, hl) - m);
-  const float s = reduce((s0 + s1) + (s2 + s3), false);
-  t = tid;
-  for (; t + 3 * NT < n; t += 4 * NT) {
-    const float x0 = es_in<MODE>(p, lb, t, head, hl), x1 = es_in<MODE>(p, lb, t + NT, head, hl);
-    const float x2 = es_in<MODE>(p, lb, t + 2 * NT, head, hl), x3 = es_in<MODE>(p, lb, t + 3 * NT, head, hl);
-    const int64_t e = lb + (t >> p.lgH), de = NT >> p.lgH;     // CSR edge of element t (DROP)
-    st_stream(o + t, es_mark<DROP>(p, e, head, expf(x0 - m) / s));
-    st_stream(o + t + NT, es_mark<DROP>(p, e + de, head, expf(x1 - m) / s));
-    st_stream(o + t + 2 * NT, es_mark<DROP>(p, e + 2 * de, head, expf(x2 - m) / s));
-    st_stream(o + t + 3 * NT, es_mark<DROP>(p, e + 3 * de, head, expf(x3 - m) / s));
-  }
-  for (; t < n; t += NT)
-    st_stream(o + t, es_mark<DROP>(p, lb + (t >> p.lgH), head, expf(es_in<MODE>(p, lb, t, head, hl) - m) / s));
-}
-
-// ---------------------------------------------------------------- warp per row (no plan)
+// The kernels: the bodies of edge_softmax.cuh without the type term or the residual blend.
 template <int MODE, bool DROP>
 __global__ void __launch_bounds__(256) es_warp_kernel(const EsParams p) {
-  const int lane = threadIdx.x & 31;
-  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (row >= p.n_rows) return;  // whole warp
-  const int lb = __ldg(p.rowptr + row), hb = __ldg(p.rowptr + row + 1);
-  const int64_t n = (int64_t)(hb - lb) * p.H;
-  const int H = p.H;
-  if (n == 0) {
-    if (MODE == 3 && lane < H) p.grow[row * H + lane] = 0.f;
-    return;
-  }
-  es_row<MODE, 32, DROP>(p, row, lb, n, lane, [H](float v, bool is_max) { return is_max ? head_max(v, H) : head_sum(v, H); });
+  es_warp_body<MODE, DROP, false, false>(p, nullptr);
 }
 
-// ---------------------------------------------------------------- hub chunks, pass 1: statistics
-// One warp per chunk slot.  Forward / attention: (max, sum exp(x - max)) per head; backward: sum y*g.
-// The last chunk of the row to arrive merges the chunks' values in chunk order into stats[first].
 template <int MODE, bool DROP>
 __global__ void __launch_bounds__(256) es_stats_kernel(const EsParams p) {
-  // programmatic dependent launch: the main kernel may start as soon as every CTA of this grid is running; its
-  // segment items need nothing from us, its chunk items wait (griddepcontrol.wait) for this grid to finish
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  const int lane = threadIdx.x & 31;
-  const int64_t item = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (item >= p.hub.n_chunks) return;
-  const WorkItem w = decode_item(item, 0, p.rowptr, p.hub);
-  const int H = p.H, head = lane & (H - 1);
-  const int n = (w.hb - w.lb) * H;
-  float m = -CUDART_INF_F, s = 0.f;
-  if (MODE == 1 || MODE == 3) {
-    const float *y = p.a + (int64_t)w.lb * H, *g = p.b + (int64_t)w.lb * H;
-    for (int t = lane; t < n; t += 32) {
-      float yv = __ldg(y + t), gv = __ldg(g + t);
-      es_unmark<DROP>(p, yv, gv);
-      s = fmaf(yv, gv, s);
-    }
-    s = head_sum(s, H);
-  } else {
-    const float hl = (MODE == 2) ? __ldg(p.a + (int64_t)w.row * H + head) : 0.f;
-    for (int t = lane; t < n; t += 32) m = fmaxf(m, es_in<MODE>(p, w.lb, t, head, hl));
-    m = head_max(m, H);
-    for (int t = lane; t < n; t += 32) s += es_exp(es_in<MODE>(p, w.lb, t, head, hl) - m);   // second read hits L1
-    s = head_sum(s, H);
-  }
-  if (lane < H) {
-    float2 *dst = p.stats + (int64_t)w.slot * H + lane;
-    asm volatile("st.global.cg.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(m), "f"(s) : "memory");
-  }
-  if (hub_arrive_last<32>(w, p.hub, lane)) {
-    // lanes sharing a head split the chunks between them, then merge across the head's lanes
-    const int grp = lane >> p.lgH, ngrp = 32 >> p.lgH;
-    float M = -CUDART_INF_F, S = 0.f;
-    const float2 *sb = p.stats + (int64_t)w.first * H + head;
-    for (int q0 = grp; q0 < w.n_row_chunks; q0 += 4 * ngrp) {
-      float2 c[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {        // four independent L2 loads in flight (the 22 K-edge hub merges 354 chunks)
-        const int q = q0 + u * ngrp;
-        c[u] = (q < w.n_row_chunks) ? __ldcg(sb + (int64_t)q * H) : make_float2(-CUDART_INF_F, 0.f);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        if (MODE == 1 || MODE == 3) {
-          S += c[u].y;
-        } else if (c[u].x != -CUDART_INF_F) {
-          const float nm = fmaxf(M, c[u].x);
-          S = S * es_exp(M - nm) + c[u].y * es_exp(c[u].x - nm);   // exp(-inf) = 0 on the first chunk
-          M = nm;
-        }
-      }
-    }
-    for (int st = 16; st >= H; st >>= 1) {
-      const float oM = __shfl_xor_sync(FULL, M, st), oS = __shfl_xor_sync(FULL, S, st);
-      if (MODE == 1 || MODE == 3) {
-        S += oS;
-      } else {
-        const float nm = fmaxf(M, oM);
-        const float a = (M == -CUDART_INF_F) ? 0.f : S * es_exp(M - nm);
-        const float b = (oM == -CUDART_INF_F) ? 0.f : oS * es_exp(oM - nm);
-        S = a + b;
-        M = nm;
-      }
-    }
-    __syncwarp();
-    if (lane < H) {
-      float2 *dst = p.stats + (int64_t)w.first * H + lane;
-      asm volatile("st.global.cg.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(M), "f"(S) : "memory");
-    }
-  }
+  es_stats_body<MODE, DROP, false>(p, nullptr);
 }
 
-// ---------------------------------------------------------------- hub chunk, pass 2 (shared by both main kernels)
-// normalise the chunk's elements with its row's merged statistics (stats[first slot])
-template <int MODE, bool DROP>
-__device__ __forceinline__ void es_chunk_item(const EsParams &p, int64_t item, int lane) {
-  constexpr bool TWO = (MODE == 1 || MODE == 3);
-  const int H = p.H;
-
-    const WorkItem w = decode_item(item, 0, p.rowptr, p.hub);
-    const int head = lane & (H - 1);
-    const int n = (w.hb - w.lb) * H;
-    const float2 rs = __ldcg(p.stats + (int64_t)w.first * H + head);
-    float *o = p.out + (int64_t)w.lb * H;
-    if (TWO) {
-      const float *y = p.a + (int64_t)w.lb * H, *g = p.b + (int64_t)w.lb * H;
-      if (MODE == 1) {
-#pragma unroll 4
-        for (int t = lane; t < n; t += 32) st_stream(o + t, __ldg(y + t) * (__ldg(g + t) - rs.y));
-      } else {
-        const float hlrow = __ldg(p.hl + (int64_t)w.row * H + head);
-        float acc = 0.f;
-        for (int t = lane; t < n; t += 32) {
-          float yv = __ldg(y + t), gv = __ldg(g + t);
-          es_unmark<DROP>(p, yv, gv);
-          const float v = yv * (gv - rs.y) * es_dact(p, w.lb, t, head, hlrow);
-          st_stream(o + t, v);
-          acc += v;
-        }
-        acc = head_sum(acc, H);
-        if (lane < H) st_cg(p.part + (int64_t)w.slot * H + lane, acc);
-        if (hub_arrive_last<32>(w, p.hub, lane)) {      // row sum of the hub row: chunk partials in chunk order
-          if (lane < H) {
-            float tot = 0.f;
-            for (int q = 0; q < w.n_row_chunks; ++q) tot += ld_cg(p.part + (int64_t)(w.first + q) * H + lane);
-            p.grow[(int64_t)w.row * H + lane] = tot;
-          }
-        }
-      }
-    } else {
-      const float hl = (MODE == 2) ? __ldg(p.a + (int64_t)w.row * H + head) : 0.f;
-      const float inv = 1.f / rs.y;
-#pragma unroll 4
-      for (int t = lane; t < n; t += 32)
-        st_stream(o + t, es_mark<DROP>(p, w.lb + (t >> p.lgH), head, es_exp(es_in<MODE>(p, w.lb, t, head, hl) - rs.x) * inv));
-    }
-    }
-
-// ---------------------------------------------------------------- bulk-copy helpers (TMA 1-D)
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// global -> shared, completion counted in bytes on the mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-// shared -> global, tracked by the bulk async-group of the issuing thread
-__device__ __forceinline__ void bulk_s2g(void *dst, const void *src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ---------------------------------------------------------------- main kernel: chunks + segments
-// Shared memory per warp: CAP floats (+ CAP for the backward's second operand) + 33 row offsets.
 template <int MODE, int CAP, int WARPS, bool DROP>
 __global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
-  constexpr bool TWO = (MODE == 1 || MODE == 3);
-  extern __shared__ __align__(128) unsigned char es_smem[];
-  float *tiles = reinterpret_cast<float *>(es_smem);
-  int *rps = reinterpret_cast<int *>(es_smem + (size_t)WARPS * CAP * 4 * (TWO ? 2 : 1));
-  uint64_t *bars = reinterpret_cast<uint64_t *>(rps + WARPS * 34);
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int64_t item = (int64_t)blockIdx.x * WARPS + wib;
-  const int H = p.H;
-
-  // ------------------------------------------------ hub chunk (LAST in the grid): normalise with the row's merged
-  // statistics, which the statistics kernel -- possibly still running: programmatic dependent launch -- produces
-  if (item >= p.hub.n_segs) {
-    if (item - p.hub.n_segs < p.hub.n_chunks) {
-      asm volatile("griddepcontrol.wait;" ::: "memory");
-      es_chunk_item<MODE, DROP>(p, item - p.hub.n_segs, lane);
-    }
-    return;
-  }
-
-  // ------------------------------------------------ segment of short rows
-  const int64_t seg = item;
-  const int2 rr = __ldg(p.hub.segs + seg);
-  float *T = tiles + (size_t)wib * CAP * (TWO ? 2 : 1);
-  float *T2 = T + CAP;
-  int *RP = rps + wib * 34;
-  uint64_t *bar = bars + wib;
-  const bool bulk = p.bulk && MODE != 2;
-  if (bulk) {
-    if (lane == 0) {
-      mbar_init(bar, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-  }
-  uint32_t phase = 0;
-  int rw = rr.x;
-  while (rw < rr.y) {
-    // window of <= 32 rows starting at rw; keep the longest prefix that fits the tile
-    const int row = rw + lane;
-    const int base = __ldg(p.rowptr + rw);
-    int endl = 0x7fffffff;
-    if (row < rr.y) endl = __ldg(p.rowptr + row + 1);
-    const unsigned fit = __ballot_sync(FULL, row < rr.y && (int64_t)(endl - base) * H <= CAP);
-    const int m = __popc(fit);                 // fit is a prefix mask (row ends are monotone)
-    if (m == 0) {                              // cannot happen when chunk_edges * H <= CAP (host check)
-      rw += 1;
-      continue;
-    }
-    const int e_end = __shfl_sync(FULL, endl, m - 1);
-    const int n = (e_end - base) * H;
-    // ---- stage (issue the bulk copy first, do the index work while it flies)
-    if (bulk && n > 0) {
-      if (lane == 0) {
-        mbar_expect_tx(bar, (uint32_t)n * 4u * (TWO ? 2u : 1u));
-        bulk_g2s(T, p.a + (int64_t)base * H, (uint32_t)n * 4u, bar);
-        if (TWO) bulk_g2s(T2, p.b + (int64_t)base * H, (uint32_t)n * 4u, bar);
-      }
-    }
-    const int startl = __shfl_up_sync(FULL, endl, 1);
-    const int sl = (lane == 0) ? base : startl;          // start edge of my row
-    if (lane < m) RP[lane + 1] = endl - base;
-    if (lane == 0) RP[0] = 0;
-    // degree-sorted visiting order of the window's rows (ascending): key = degree << 5 | row slot
-    unsigned key = (lane < m) ? (((unsigned)(endl - sl) << 5) | (unsigned)lane) : 0xffffffffu;
-#pragma unroll
-    for (int k = 2; k <= 32; k <<= 1) {
-#pragma unroll
-      for (int j = k >> 1; j > 0; j >>= 1) {
-        const unsigned o = __shfl_xor_sync(FULL, key, j);
-        const bool up = (lane & k) == 0, lower = (lane & j) == 0;
-        key = (lower == up) ? min(key, o) : max(key, o);
-      }
-    }
-    if (!bulk) {
-      if (MODE == 2) {
-#pragma unroll 4
-        for (int t = lane; t < n; t += 32) {
-          const int pe = base + (t >> p.lgH), h = t & (H - 1);
-          const int r = __ldg(p.hub.edge_row + pe);
-          const int c = __ldg(p.colind + pe);
-          const float z = __ldg(p.a + (int64_t)r * H + h) + __ldg(p.b + (int64_t)c * H + h);
-          T[t] = z > 0.f ? z : z * p.slope;
-        }
-      } else {
-        const float *src = p.a + (int64_t)base * H;
-#pragma unroll 4
-        for (int t = lane; t < n; t += 32) T[t] = ld_stream(src + t);
-        if (TWO) {
-          const float *src2 = p.b + (int64_t)base * H;
-#pragma unroll 4
-          for (int t = lane; t < n; t += 32) T2[t] = ld_stream(src2 + t);
-        }
-      }
-    }
-    __syncwarp();
-    if (bulk && n > 0) {
-      mbar_wait(bar, phase);
-      phase ^= 1u;
-    }
-    // ---- (row, head) pairs, rows in degree-sorted order (warp-uniform trip count: the shuffle needs all lanes)
-    const int pairs = m * H;
-    for (int q0 = 0; q0 < pairs; q0 += 32) {
-      const int q = q0 + lane;
-      const int rl = (int)(__shfl_sync(FULL, key, min(q >> p.lgH, 31)) & 31u);
-      if (q < pairs) {
-        const int h = q & (H - 1);
-        const int k0 = RP[rl], k1 = RP[rl + 1];
-        if (TWO) {
-          float s = 0.f;
-          for (int k = k0; k < k1; ++k) {
-            float yv = T[k * H + h], gv = T2[k * H + h];
-            es_unmark<DROP>(p, yv, gv);
-            s = fmaf(yv, gv, s);
-          }
-          if (MODE == 1) {
-            for (int k = k0; k < k1; ++k) T[k * H + h] = T[k * H + h] * (T2[k * H + h] - s);
-          } else {
-            const int grow_row = rw + rl;
-            const float hlrow = __ldg(p.hl + (int64_t)grow_row * H + h);
-            float acc = 0.f;
-            for (int k = k0; k < k1; ++k) {
-              const int c = __ldg(p.colind + base + k);
-              const float z = hlrow + __ldg(p.hr + (int64_t)c * H + h);
-              float yv = T[k * H + h], gv = T2[k * H + h];
-              es_unmark<DROP>(p, yv, gv);
-              const float v = yv * (gv - s) * (z > 0.f ? 1.f : p.slope);
-              T[k * H + h] = v;
-              acc += v;
-            }
-            p.grow[(int64_t)grow_row * H + h] = acc;     // also the (empty-row) zero
-          }
-        } else {
-          // online max / sum (one pass, one exp per element: e = exp(-|x - m|) is the rescale factor of the running
-          // sum when x is a new maximum and the new term otherwise), then one normalising pass: 2 LDS + 1 STS and
-          // 2 MUFU per element instead of 3 LDS + 2 STS -- the kernel is issue-bound.  The running max starts at
-          // -FLT_MAX, not -inf: a leading -inf logit then gives d = -inf and e = 0 instead of -inf - -inf = NaN, and
-          // a (row, head) whose logits are all -inf still ends in 0 * (1 / 0) = NaN, as the softmax does.
-          float mx = -FLT_MAX, sm = 0.f;
-          for (int k = k0; k < k1; ++k) {
-            const float x = T[k * H + h];
-            const float d = x - mx;
-            const float e = es_exp(-fabsf(d));
-            sm = (d > 0.f) ? fmaf(sm, e, 1.f) : sm + e;
-            mx = fmaxf(mx, x);
-          }
-          const float inv = 1.f / sm;
-          for (int k = k0; k < k1; ++k) T[k * H + h] = es_mark<DROP>(p, (int64_t)base + k, h, es_exp(T[k * H + h] - mx) * inv);
-        }
-      }
-    }
-    __syncwarp();
-    // ---- write back
-    float *dst = p.out + (int64_t)base * H;
-    if (bulk && n > 0) {
-      fence_async_smem();                      // my generic-proxy writes to T -> visible to the async proxy
-      __syncwarp();
-      if (lane == 0) {
-        bulk_s2g(dst, T, (uint32_t)n * 4u);
-        bulk_commit();
-        bulk_wait_read0();                     // T may be overwritten (next window) / freed (exit) after this
-      }
-      __syncwarp();
-    } else {
-      for (int t = lane; t < n; t += 32) st_stream(dst + t, T[t]);
-      __syncwarp();
-    }
-    rw += m;
-  }
+  es_main_body<MODE, CAP, WARPS, DROP, false, false>(p, nullptr);
 }
 
-// ---------------------------------------------------------------- generic H: warp per row, loop over heads
 template <int MODE, bool DROP>
 __global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
-  const int lane = threadIdx.x & 31;
-  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (row >= p.n_rows) return;
-  const int lb = __ldg(p.rowptr + row), hb = __ldg(p.rowptr + row + 1);
-  for (int h = 0; h < p.H; ++h) {
-    if (MODE == 1 || MODE == 3) {
-      float s = 0.f;
-      for (int e = lb + lane; e < hb; e += 32) {
-        float yv = __ldg(p.a + (int64_t)e * p.H + h), gv = __ldg(p.b + (int64_t)e * p.H + h);
-        es_unmark<DROP>(p, yv, gv);
-        s = fmaf(yv, gv, s);
-      }
-      s = head_sum(s, 1);
-      const float hlrow = (MODE == 3) ? __ldg(p.hl + row * p.H + h) : 0.f;
-      float acc = 0.f;
-      for (int e = lb + lane; e < hb; e += 32) {
-        const int64_t k = (int64_t)e * p.H + h;
-        float yv = __ldg(p.a + k), gv = __ldg(p.b + k);
-        es_unmark<DROP>(p, yv, gv);
-        float v = yv * (gv - s);
-        if (MODE == 3) {
-          const float z = hlrow + __ldg(p.hr + (int64_t)__ldg(p.colind + e) * p.H + h);
-          v *= (z > 0.f ? 1.f : p.slope);
-          acc += v;
-        }
-        p.out[k] = v;
-      }
-      if (MODE == 3) {
-        acc = head_sum(acc, 1);
-        if (lane == 0) p.grow[row * p.H + h] = acc;
-      }
-    } else {
-      const float hl = (MODE == 2) ? __ldg(p.a + row * p.H + h) : 0.f;
-      auto in = [&](int e) {
-        if (MODE == 2) {
-          const float z = hl + __ldg(p.b + (int64_t)__ldg(p.colind + e) * p.H + h);
-          return z > 0.f ? z : z * p.slope;
-        }
-        return __ldg(p.a + (int64_t)e * p.H + h);
-      };
-      float m = -CUDART_INF_F;
-      for (int e = lb + lane; e < hb; e += 32) m = fmaxf(m, in(e));
-      m = head_max(m, 1);
-      float s = 0.f;
-      for (int e = lb + lane; e < hb; e += 32) s += expf(in(e) - m);
-      s = head_sum(s, 1);
-      for (int e = lb + lane; e < hb; e += 32) p.out[(int64_t)e * p.H + h] = es_mark<DROP>(p, e, h, expf(in(e) - m) / s);
-    }
-  }
+  es_generic_body<MODE, DROP, false, false>(p, nullptr);
 }
-
-// Warps per block of the main kernel.  For the 512-float tile this is a launch parameter only (2 and 4 warps give
-// bit-identical outputs); a block's shared memory and warp slots are released when its slowest warp retires, and 8
-// is the shape the whole GPU suite is validated with.
-constexpr int ES_WARPS = 8;
 
 template <int MODE, int CAP, bool DROP>
 static int launch_main(const EsParams &p, cudaStream_t s) {
-  constexpr int WARPS = ES_WARPS;
-  constexpr bool TWO = (MODE == 1 || MODE == 3);
-  constexpr size_t smem = (size_t)WARPS * CAP * 4 * (TWO ? 2 : 1) + (size_t)WARPS * 34 * 4 + (size_t)WARPS * 8;
   static unsigned long long attr_done = 0;
-  int dev = 0;
-  if (first_use_on_device(attr_done, &dev))
-    CB_CUDA(cudaFuncSetAttribute(es_main_kernel<MODE, CAP, WARPS, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int64_t items = (int64_t)p.hub.n_chunks + p.hub.n_segs;
-  const int64_t blocks = ceil_div(items, WARPS);
-  if (blocks == 0) return COGDL_B200_OK;
-  CB_REQUIRE(blocks <= 0x7fffffffLL, "edge_softmax: problem too large for one launch");
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)blocks);
-  cfg.blockDim = dim3(WARPS * 32);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;     // overlap with the statistics kernel (see es_stats_kernel)
-  cfg.attrs = attr;
-  cfg.numAttrs = p.hub.n_chunks > 0 ? 1 : 0;
-  CB_CUDA(cudaLaunchKernelEx(&cfg, es_main_kernel<MODE, CAP, WARPS, DROP>, p));
-  count_launch();
-  return COGDL_B200_OK;
+  return es_launch_main(es_main_kernel<MODE, CAP, ES_WARPS, DROP>, es_main_smem<MODE, CAP>(), attr_done, p, s);
 }
 
 // Launch plan (see the header comment).  DROP only with MODE 2 / 3.
@@ -640,42 +81,29 @@ template <int MODE, bool DROP = false>
 static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t s, const char *who) {
   static_assert(!DROP || MODE == 2 || MODE == 3, "attention dropout is a mode of the GAT attention and its backward");
   const char *drop_note = DROP ? ",DROP" : "";
-  const bool pow2 = p.H <= 32 && (p.H & (p.H - 1)) == 0;
   const int64_t row_blocks = ceil_div(p.n_rows * 32, 256);
   CB_REQUIRE(row_blocks <= 0x7fffffffLL, "%s: problem too large for one launch", who);
-  p.lgH = 0;
-  while ((1 << p.lgH) < p.H) ++p.lgH;
-  p.hub = hub_view(nullptr);
-  p.stats = nullptr; p.part = nullptr; p.bulk = false;
-  if (!pow2) {
+  EsForm form;
+  int chosen;
+  int rc = es_plan<MODE>(p, plan, &form, &chosen);
+  if (rc) return rc;
+  if (form == EsForm::GENERIC) {
     note_kernel("cogdl_b200::es_generic_kernel<MODE=%d%s>", MODE, drop_note);
     es_generic_kernel<MODE, DROP><<<(unsigned)row_blocks, 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
     return COGDL_B200_OK;
   }
-  const int64_t cap_need = plan ? (int64_t)plan->chunk_edges * p.H : 0;
-  const bool segs = plan && plan->chunk_edges > 0 && plan->segs && plan->edge_row && plan->n_segs > 0 && cap_need <= 2048;
-  if (!segs) {   // no plan: every row through the warp kernel (hubs serialise on one warp)
+  if (form == EsForm::WARP) {
     note_kernel("cogdl_b200::es_warp_kernel<MODE=%d%s>", MODE, drop_note);
     es_warp_kernel<MODE, DROP><<<(unsigned)row_blocks, 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
     return COGDL_B200_OK;
   }
-  p.hub = hub_view(plan);
-  // scratch: (max, sum) per chunk slot and head, + (MODE 3) one partial row sum per slot and head
-  const int64_t need = (int64_t)p.hub.n_chunks * p.H * (int64_t)(sizeof(float2) + (MODE == 3 ? sizeof(float) : 0));
-  int rc = check_plan(plan, need);
-  if (rc) return rc;
-  p.stats = reinterpret_cast<float2 *>(plan->partials);
-  p.part = reinterpret_cast<float *>(p.stats + (int64_t)p.hub.n_chunks * p.H);
-  // 1-D TMA needs 16-byte aligned global addresses and sizes: rows start at multiples of H floats
-  p.bulk = (p.H % 4 == 0) && aligned16(p.a) && aligned16(p.out) && (MODE == 0 || aligned16(p.b));
   if (p.hub.n_chunks > 0) {
     // the attention's statistics come before the dropout: MODE 2 shares the kernel without DROP
     es_stats_kernel<MODE, DROP && MODE == 3><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
     CB_LAUNCH_CHECK();
   }
-  const int chosen = cap_need <= 512 ? 512 : (cap_need <= 1024 ? 1024 : 2048);   // smallest tile (floats per warp) that fits
   // both launches, in launch order, when the statistics kernel ran
   char stats_note[64] = "";
   if (p.hub.n_chunks > 0)

@@ -43,6 +43,9 @@ rgcn=True rebinds `cogdl.layers.rgcn_layer.RGCNLayer.forward` (RGCN, LinkPredict
 relational sum with cogdl_b200.rgcn_conv (uninstall_rgcn()).  This deliberately differs from the original for more than
 one relation: the original aggregates every edge with the weight of the first relation that has edges (see
 rgcn_forward).
+The Simple-HGN example's layer (examples/simple_hgn/conv.py, myGATConv) is not part of the cogdl package, so it has no
+install() flag: install_simple_hgn(conv_cls) rebinds the class the caller passes to simple_hgn_forward, which sends the
+attention to cogdl_b200.hgn_attention (uninstall_simple_hgn(conv_cls)).
 """
 import sys
 
@@ -509,6 +512,60 @@ def uninstall_rgcn():
     import cogdl.layers.rgcn_layer as rl
 
     _restore_forward(rl.RGCNLayer)
+
+
+def simple_hgn_forward(self, graph, x, res_attn=None):
+    """myGATConv.forward of CogDL's Simple-HGN example (examples/simple_hgn/conv.py) with the attention, its dropout,
+    the residual-attention blend and the aggregation in cogdl_b200.hgn_attention.  The layer's own feat_drop, x @ W,
+    NaN zeroing, h_l / h_r, type table h_e = (a_e * (edge_emb @ W_e)).sum(-1), residual Linear and activation are used,
+    so autograd carries d h_e to a_e, W_e and edge_emb.  The attention dropout is self.dropout.p when training.
+    Returns (out, attention.detach()), the attention in the graph's CSR edge order.
+
+    Edge types come from graph.edge_type, an attribute that building the CSR does not reorder.  They are read with
+    edge_index on entry; when building the CSR reorders the edges (a stable sort by row), the types -- and a given
+    res_attn -- are put through the same sort and graph.edge_type is reassigned, so this and every later call sees
+    each edge with its own type.  CPU or non-fp32 input or weights, and a dropout of 1, run the original."""
+    from .operators.simple_hgn import hgn_attention
+
+    original = type(self)._cogdl_b200_original_forward
+    p = self.dropout.p if self.training else 0.0
+    weights = (self.W, self.W_e, self.edge_emb, self.a_l, self.a_r, self.a_e)
+    if unsupported_operands(graph, x, res_attn, *weights) is not None or p >= 1.0:
+        return original(self, graph, x, res_attn)
+    row0 = graph.edge_index[0]
+    etype = graph.edge_type
+    graph_operands(graph)                       # builds the CSR if the graph has none yet
+    if graph.edge_index[0] is not row0:
+        order = torch.sort(row0, stable=True).indices
+        etype = etype[order.to(etype.device)]
+        graph.edge_type = etype
+        if res_attn is not None:
+            res_attn = res_attn[order]
+    x = self.feat_drop(x)
+    h = torch.matmul(x, self.W).view(-1, self.nhead, self.out_features)
+    h[torch.isnan(h)] = 0.0
+    e = torch.matmul(self.edge_emb, self.W_e).view(-1, self.nhead, self.edge_feats)
+    h_l = (self.a_l * h).sum(dim=-1)
+    h_r = (self.a_r * h).sum(dim=-1)
+    h_e = (self.a_e * e).sum(dim=-1)
+    out, attention = hgn_attention(graph, h, h_l, h_r, h_e, etype, self.leakyrelu.negative_slope, p, res_attn,
+                                   self.alpha)
+    out = out.view(out.shape[0], -1)
+    if self.residual is not None:
+        out = out + self.residual(x)
+    if self.act is not None:
+        out = self.act(out)
+    return out, attention.detach()
+
+
+def install_simple_hgn(conv_cls):
+    """Rebind conv_cls.forward (the Simple-HGN example's myGATConv, which is not part of the cogdl package, so the
+    caller passes the class) to simple_hgn_forward; the original stays at conv_cls._cogdl_b200_original_forward."""
+    return _rebind_forward(conv_cls, simple_hgn_forward, f"{conv_cls.__module__}.{conv_cls.__qualname__}.forward")
+
+
+def uninstall_simple_hgn(conv_cls):
+    _restore_forward(conv_cls)
 
 
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")

@@ -24,3 +24,4 @@ from .label_prop import label_propagate  # noqa: F401
 from .gin import gin_aggregate, GinAggregateFunction  # noqa: F401
 from .grand import random_propagate  # noqa: F401
 from .rgcn import rgcn_aggregate, rgcn_conv, RgcnAggregateFunction, RgcnConvFunction  # noqa: F401
+from .simple_hgn import hgn_attention, HgnAttentionFunction  # noqa: F401

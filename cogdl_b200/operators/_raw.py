@@ -614,3 +614,64 @@ def rgcn_edge_dot_raw(st: CSRStructure, w, g, x):
                    st.n_rows, B, F, plan, _stream(dev))
         del keep
     return p
+
+
+def hgn_max_table():
+    """The largest T * H of a Simple-HGN type table (h_e is staged in shared memory by the kernels)."""
+    return int(_cabi.load().cogdl_b200_hgn_max_table())
+
+
+def _hgn_table(st, etype, h_e, H):
+    """The type operands of the Simple-HGN kernels, checked: etype [nnz] int32, h_e [T, H] fp32 with T * H within the
+    kernels' table.  Types in [0, T) are the caller's to guarantee (RgcnStructure checks them)."""
+    h_e = _f32c(h_e, "h_e")
+    if h_e.dim() != 2 or h_e.shape[1] != H:
+        raise ValueError(f"h_e must be [T, H={H}], got {tuple(h_e.shape)}")
+    if h_e.shape[0] * H > hgn_max_table() or h_e.shape[0] < 1:
+        raise ValueError(f"h_e is [T={h_e.shape[0]}, H={H}]; the fused attention takes T * H from 1 to {hgn_max_table()}")
+    if etype.dtype != torch.int32 or etype.numel() != st.nnz:
+        raise ValueError(f"etype must be int32 [nnz={st.nnz}], got {etype.dtype} {tuple(etype.shape)}")
+    return etype.contiguous(), h_e
+
+
+def hgn_attn_raw(st: CSRStructure, etype, h_l, h_r, h_e, slope, want_att, drop=None, res_attn=None, alpha=0.0):
+    """Simple-HGN attention stage: (mix [nnz, H], att [nnz, H] or None).  a = softmax_row(leakyrelu(h_l[row] + h_r[col]
+    + h_e[etype])); att is a with the sign bit set on the dropped entries (when want_att); mix = (1 - alpha) * (dropped
+    ? 0 : a * scale) + alpha * res_attn (res_attn None: no blend).  drop = (seed, drop_below, scale) as for
+    gat_fwd_raw, None for no dropout."""
+    dev = require_cuda(h_l, h_r, h_e, etype, res_attn)
+    h_l, h_r = _f32c(h_l, "h_l"), _f32c(h_r, "h_r")
+    H = h_l.shape[1]
+    etype, h_e = _hgn_table(st, etype, h_e, H)
+    if res_attn is not None:
+        res_attn = _f32c(res_attn, "res_attn")
+        if res_attn.shape != (st.nnz, H):
+            raise ValueError(f"res_attn must be [nnz={st.nnz}, H={H}], got {tuple(res_attn.shape)}")
+    seed, drop_below, scale = (0, 0, 1.0) if drop is None else drop
+    with torch.cuda.device(dev):
+        mix = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)
+        att = torch.empty_like(mix) if want_att else None
+        plan, keep = st.plan_struct(_es_scratch(st, H))
+        _cabi.call("cogdl_b200_hgn_attn_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(etype), _ptr(h_l), _ptr(h_r),
+                   _ptr(h_e), h_e.shape[0], float(slope), int(seed), int(drop_below), float(scale), _ptr(res_attn),
+                   float(alpha), _ptr(att), _ptr(mix), st.n_rows, H, plan, _stream(dev))
+        del keep
+    return mix, att
+
+
+def hgn_attn_bwd_raw(st: CSRStructure, etype, att, d_mix, h_l, h_r, h_e, slope, grad_scale):
+    """(d_edge [nnz, H], g_row [n_rows, H]) of hgn_attn_raw: the softmax backward on |att| with g = kept ? d_mix *
+    grad_scale : 0, times the typed LeakyReLU', and its row sums, in one pass."""
+    dev = require_cuda(att, d_mix, h_l, h_r, h_e, etype)
+    att, d_mix, h_l, h_r = _f32c(att, "att"), _f32c(d_mix, "d_mix"), _f32c(h_l, "h_l"), _f32c(h_r, "h_r")
+    H = att.shape[1]
+    etype, h_e = _hgn_table(st, etype, h_e, H)
+    with torch.cuda.device(dev):
+        d_edge = torch.empty_like(att)
+        g_row = torch.empty((st.n_rows, H), dtype=torch.float32, device=dev)
+        plan, keep = st.plan_struct(_es_scratch(st, H))
+        _cabi.call("cogdl_b200_hgn_attn_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(etype), _ptr(att),
+                   _ptr(d_mix), _ptr(h_l), _ptr(h_r), _ptr(h_e), h_e.shape[0], float(slope), float(grad_scale),
+                   _ptr(d_edge), _ptr(g_row), st.n_rows, H, plan, _stream(dev))
+        del keep
+    return d_edge, g_row

@@ -557,6 +557,37 @@ COGDL_B200_API int cogdl_b200_rgcn_edge_dot_f32(const int32_t *rowptr, const int
                                                 cogdl_b200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Simple-HGN attention (myGATConv, CogDL examples/simple_hgn/conv.py): the GAT attention stage with an edge-type
+ * term and the residual attention blend.  Per CSR edge p = (i, j) of type t = etype[p] (int32, in [0, T): the
+ * caller's to guarantee) and head h, with h_e [T, H]:
+ *   a[p,h]        = softmax over row i of leakyrelu(h_l[i,h] + h_r[j,h] + h_e[t,h])
+ *   att_out[p,h]  = a with the sign bit set when dropped (optional: NULL when no gradient is needed)
+ *   mix_out[p,h]  = (1 - alpha) * (dropped ? 0 : a * scale) + alpha * res_attn[p,h]   (res_attn NULL: no blend)
+ * Dropout, seed and keep rule are those of cogdl_b200_gat_fwd_dropout_f32 (drop_below = 0 keeps everything; scale
+ * finite and > 0).  mix_out is what the layer aggregates (cogdl_b200_mhspmm_f32) and returns.
+ * cogdl_b200_hgn_attn_bwd_f32, given att (att_out of the forward) and d_mix = mhsddmm(d out, feat), writes
+ *   d_edge[p,h] = |a| * (g - sum_row |a| * g) * leakyrelu'(h_l[i,h] + h_r[j,h] + h_e[t,h])   [nnz, H]
+ *   g_row[i,h]  = sum_{p in row i} d_edge[p,h]                                                [n_rows, H]
+ * with g = (sign bit of att) ? 0 : d_mix * grad_scale, grad_scale = (1 - alpha) / (1 - p_drop).
+ * T * H must be in [1, cogdl_b200_hgn_max_table()] (h_e is staged in shared memory), else COGDL_B200_EINVAL before
+ * any launch.  Any H; scratch in plan->partials as for the edge softmax.  cogdl_b200_last_kernel() names every
+ * launch (hgn_warp_kernel / hgn_generic_kernel / [hgn_stats_kernel +] hgn_main_kernel).
+ * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_hgn_max_table(void);
+COGDL_B200_API int cogdl_b200_hgn_attn_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *etype,
+                                           const float *h_l, const float *h_r, const float *h_e, int64_t T,
+                                           float negative_slope, uint64_t seed, uint64_t drop_below, float scale,
+                                           const float *res_attn, float alpha, float *att_out, float *mix_out,
+                                           int64_t n_rows, int64_t H, const cogdl_b200_hub_plan_t *plan,
+                                           cogdl_b200_stream_t stream);
+COGDL_B200_API int cogdl_b200_hgn_attn_bwd_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *etype,
+                                               const float *att, const float *d_mix, const float *h_l,
+                                               const float *h_r, const float *h_e, int64_t T, float negative_slope,
+                                               float grad_scale, float *d_edge, float *g_row, int64_t n_rows,
+                                               int64_t H, const cogdl_b200_hub_plan_t *plan,
+                                               cogdl_b200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Sparse x sparse product C = A.B, A [a_rows x a_cols] and B [b_rows x b_cols] int32 CSR with fp32 values, columns
  * ascending and unique inside every row (b_rows must equal a_cols).  C comes out as CSR with ascending, unique columns.
  * Replaces  torch_sparse.spspmm(indexA, valueA, indexB, valueB, m, k, n)   (cuSPARSE SpGEMM), imported at module level

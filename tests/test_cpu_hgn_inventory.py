@@ -1,0 +1,57 @@
+"""Every kernel compiled into simple_hgn.o has a row in tests/hgn_table.py that the GPU suite runs
+(test_gpu_simple_hgn.py), and every kernel the table names is compiled, checked on a machine without a GPU."""
+import re
+
+from tests.hgn_table import MAX_TABLE, TABLE
+from tests.test_cpu_kernel_inventory import compiled_kernels
+
+
+def note_of(sym):
+    """The name cogdl_b200_last_kernel() records for a demangled simple_hgn.o kernel symbol."""
+    m = re.fullmatch(r"void cogdl_b200::(hgn_\w+_kernel)<(.*)>\(cogdl_b200::EsParams\)", sym)
+    assert m, f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table"
+    name, args = m.group(1), [re.sub(r"^\(int\)", "", a.strip()) for a in m.group(2).split(",")]
+    mode = int(args[0])
+    if name == "hgn_stats_kernel":
+        return f"cogdl_b200::hgn_stats_kernel<MODE={mode}>"
+    cap = f",CAP={args[1]}" if name == "hgn_main_kernel" else ""
+    drop, mix = (a == "(bool)1" for a in args[-2:])
+    return f"cogdl_b200::{name}<MODE={mode}{cap}{',DROP' if drop else ''}{',MIX' if mix else ''}>"
+
+
+def table_kernels():
+    names = set()
+    for c in TABLE:
+        for mode in (2, 3):
+            names.add(c.kernel(mode))
+            if c.stats(mode):
+                names.add(c.stats(mode))
+    return names
+
+
+def test_hgn_table_covers_every_compiled_kernel():
+    compiled = {note_of(s): s for s in compiled_kernels(("simple_hgn",))}
+    assert compiled, "simple_hgn.o holds no kernels"
+    table = table_kernels()
+    untested = sorted(set(compiled) - table)
+    assert not untested, "compiled kernels without a row in tests/hgn_table.py:\n" + "\n".join(
+        f"  {n}   ({compiled[n]})" for n in untested)
+    unknown = sorted(table - set(compiled))
+    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+
+
+def test_hgn_rows_are_distinct_and_cover_the_shapes():
+    ids = [c.id for c in TABLE]
+    assert len(ids) == len(set(ids))
+    assert {1, 2, 8} <= {c.H for c in TABLE}
+    assert {1, 5} <= {c.T for c in TABLE} and any(c.T * c.H == MAX_TABLE for c in TABLE)
+    assert {"tiny", "empty_graph", "ragged", "hub", "two_hubs", "rect", "bounds"} <= {c.graph for c in TABLE}
+    assert {(r, p) for c in TABLE for r, p in [(c.res, c.p)]} == {(False, 0.0), (False, 0.5), (True, 0.0), (True, 0.5)}
+
+
+def test_note_of_maps_hgn_symbols():
+    assert note_of("void cogdl_b200::hgn_main_kernel<(int)2, (int)512, (bool)1, (bool)0>(cogdl_b200::EsParams)") == \
+        "cogdl_b200::hgn_main_kernel<MODE=2,CAP=512,DROP>"
+    assert note_of("void cogdl_b200::hgn_warp_kernel<(int)2, (bool)0, (bool)1>(cogdl_b200::EsParams)") == \
+        "cogdl_b200::hgn_warp_kernel<MODE=2,MIX>"
+    assert note_of("void cogdl_b200::hgn_stats_kernel<(int)3>(cogdl_b200::EsParams)") == "cogdl_b200::hgn_stats_kernel<MODE=3>"
