@@ -2,7 +2,7 @@
 (test_gpu_simple_hgn.py), and every kernel the table names is compiled, checked on a machine without a GPU."""
 import re
 
-from tests.hgn_table import MAX_TABLE, TABLE
+from tests.hgn_table import MAX_TABLE, TABLE, form_key
 from tests.test_cpu_kernel_inventory import compiled_kernels
 
 
@@ -45,8 +45,22 @@ def test_hgn_rows_are_distinct_and_cover_the_shapes():
     assert len(ids) == len(set(ids))
     assert {1, 2, 8} <= {c.H for c in TABLE}
     assert {1, 5} <= {c.T for c in TABLE} and any(c.T * c.H == MAX_TABLE for c in TABLE)
-    assert {"tiny", "empty_graph", "ragged", "hub", "two_hubs", "rect", "bounds"} <= {c.graph for c in TABLE}
+    graphs = {"tiny", "empty_graph", "ragged", "hub", "two_hubs", "rect", "bounds", "bounds_t"}
+    assert graphs <= {c.graph for c in TABLE}
     assert {(r, p) for c in TABLE for r, p in [(c.res, c.p)]} == {(False, 0.0), (False, 0.5), (True, 0.0), (True, 0.5)}
+
+
+def test_hgn_rows_cover_every_launch_form():
+    """Every launch form (the main kernel at each tile, the warp and the generic kernel) has rows, so its forward also
+    runs without the attention output (test_row_against_fp64 repeats every row's forward that way), and one row whose
+    backward walks boundary-degree columns (bounds_t); one row blends with alpha = 1.  Removing any bounds_t row fails
+    here."""
+    forms = {form_key(c) for c in TABLE}
+    assert forms == {"main-512", "main-1024", "main-2048", "warp", "generic"}, forms
+    bounds_t = sorted(form_key(c) for c in TABLE if c.graph == "bounds_t")
+    assert bounds_t == sorted(["main-512", "main-512", "main-1024", "main-2048", "warp", "generic"]), bounds_t
+    assert {1, 8, 16, 3} <= {c.H for c in TABLE if c.graph == "bounds_t"}
+    assert any(c.alpha == 1.0 and c.res for c in TABLE)
 
 
 def test_note_of_maps_hgn_symbols():

@@ -7,7 +7,9 @@ a GPU.
 
 Objects left out on purpose, none of which picks a kernel by size and all of which are checked bit for bit: actnn.o
 (against the numpy restatement, test_gpu_actnn.py), sampler.o (against the oracle, test_gpu_sampler.py) and
-csr_tools.o (integer and permutation kernels, checked exactly by the structure tests).
+csr_tools.o (its integer and permutation kernels checked exactly by the structure tests; its one float reduction,
+cogdl_b200_edge_colsum_f32, per element against fp64 with its column-degree bound by every row of
+test_gpu_simple_hgn.py::test_row_against_fp64, as d h_r, hub columns on the boundary degrees and no plan included).
 
 The kernel entry points are read from the objects with cuobjdump and demangled with cu++filt; each instantiation
 is mapped to the string its launcher records for cogdl_b200_last_kernel()."""

@@ -81,11 +81,17 @@ def csr64(rp, ci, vals, n_cols):
     return sp.csr_matrix((np.array(vals, np.float64), ci.copy(), rp.copy()), shape=(rp.shape[0] - 1, n_cols))
 
 
+RATIOS = {}
+
+
 def assert_within(got, ref, bound, what):
+    """|got - ref| <= bound element-wise (NaN anywhere fails); records the worst err / bound under `what`."""
     err = np.abs(np.asarray(got, np.float64) - ref)
     bad = np.argwhere(~(err <= bound))
     assert bad.size == 0, (f"{what}: {len(bad)} elements outside the bound, first at {tuple(bad[0])}: "
                            f"got {got[tuple(bad[0])]!r}, ref {ref[tuple(bad[0])]!r}, bound {bound[tuple(bad[0])]!r}")
+    if err.size:
+        RATIOS[what] = float(np.max(err / np.maximum(bound, 1e-300)))
 
 
 def split_rows(rp, st):

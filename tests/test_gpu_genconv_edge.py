@@ -1,17 +1,43 @@
 """GENConv edge-encoder kernels (cogdl_b200/csrc/genconv_edge.cu) and genconv_aggregate(edge_attr=, edge_weight=)
 against the fp64 restatement of tests/genconv_ref.py with edge_term = attr @ W.T, against the edge-term kernels bit
-for bit where the product is exact, and the reference DeeperGCN with an EdgeEncoder through install(genconv=True)."""
+for bit where the product is exact, and the reference DeeperGCN with an EdgeEncoder through install(genconv=True).
+
+Every row of tests/genconv_edge_table.py is checked per element (test_table_row), with u = 2^-24:
+- The kernel forms the edge term as one fmaf chain of D steps from 0, A32 = fl(attr @ W.T).  In the exact family
+  (attr in {-2..2}, W a power of two times multiples of 1/8) every partial sum is exact, so A32 = attr @ W.T and the
+  bounds of the edge-term kernel (tests/test_gpu_dispatch_message.py: sa_fwd64 for out, lse2 and Q, run_sa_bwd's
+  terms for dX) apply unchanged to the fp32 m = relu(x[c] + A32) + eps.  For one edge per column (columns not a
+  multiple of 7, whose x rows are 0) x[c] = -A_e, so that edge's pre-activation is exactly 0 and it adds nothing to dX
+  or dW (ReLU'(0) = 0).  x spreads beta m over at least 60 in every row; beta in {0, 0.5, 4, 20, -2}.
+- In the general family (attr ~ U[0, 1), W ~ N(0, 1/D)) the reference takes A = fl(attr @ W.T in fp64); the kernel's A
+  is within dA = (D + 1) u sum_d |attr W| of it, its pre-activation within dpre = dA + 2u (|pre| + dA) (two adds
+  rounded apart), its m within dm = dpre + 2u (m + dpre), and dm = 0 where pre <= -dpre (both sides give m = eps).
+  With Dm the row's largest dm, each logit moves by at most |beta| log2(e) Dm in base 2, each normalised weight by
+  k = 2 |beta| Dm relative (once its own, once the normaliser): out gains k (out64 + Dm) + Dm, Q gains
+  k Q' + (Q' - Q64) with Q' = Q64 + 2 Dm out64 + Dm^2, lse2 gains |beta| log2(e) Dm.  Backward: the weight
+  2^(z - lse2) and the factor 1 + beta (m - out) each move by |beta| dm, so dpre_e gains |beta| dm (mag_e + w_e |g_i|);
+  an edge whose pre-activation is within dpre of 0 may change sides of the ReLU and counts its whole magnitude.
+- dW[f, d] = sum_e dpre_e[f] attr[e, d]: each term carries the dpre bound times |attr|, and the fp32 sum has a depth of
+  L + 8 + B + 2 (u times sum |dpre attr|), not nnz: B = min(ceil(items / 8), 264) blocks summed in block order, 8
+  warps in warp order, and one lane's fmaf chain of at most L = ceil(items / (8 B)) x (edges of one item) products,
+  items = the transpose's hub chunks + its columns.  The wide graph has more items than the grid has warps (every
+  warp carries its dW partial into a second item); its dX and dW must also be bit-identical run to run.
+The worst error / bound ratio of every check is printed."""
 import json
 import os
 import subprocess
 import sys
+from types import SimpleNamespace
 
+import numpy as np
 import pytest
 import torch
 
 from tests import graphs
-from tests.genconv_edge_table import TABLE
+from tests.genconv_edge_table import GE_BWD_BLOCKS, GE_WARPS, TABLE, wide_csr
 from tests.genconv_ref import genconv_aggregate_fp64
+from tests.test_gpu_dispatch_message import (EPS, LN2, LOG2E, RATIOS, TINY, U32, assert_within, check_counters,
+                                             col_sum, edge_rows, misaligned, sa_fwd64, sa_inputs, sa_m, seg_reduce)
 from tests.test_gpu_genconv import err, structure
 
 pytestmark = pytest.mark.gpu
@@ -164,48 +190,194 @@ def test_forward_backward_bitwise_reproducible(dev, name):
     assert all(torch.equal(u, v) for u, v in zip(first, second))
 
 
-def _row_operands(c, dev):
-    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES
+def _row_graph(c):
+    if c.graph == "bounds":
+        return graphs.boundary_csr(c.chunk)
+    if c.graph == "bounds_t":
+        return graphs.boundary_csc(c.chunk)
+    if c.graph == "wide":
+        return wide_csr()
+    return graphs.case(c.graph)
 
-    st, *_ = structure(c.graph, dev, c.chunk or DEFAULT_CHUNK_EDGES)
-    x, attr, w = operands(st, c.F, c.D, dev, seed=c.F * 17 + c.D)
-    if not c.aligned:    # 4 bytes off 16-byte alignment: the scalar kernel
-        x = torch.empty(st.n_cols * c.F + 1, device=dev)[1:].view(st.n_cols, c.F).copy_(x)
-    return st, x, attr, w
+
+def _row_inputs(c, rp, ci, n_cols):
+    """x [n_cols, F], attr [nnz, D], W [F, D] (fp32 numpy) of the row's input family, the reference edge term A (fp32)
+    and the bound dA of the kernel's A against it (0 in the exact family)."""
+    rng = np.random.default_rng(c.F * 17 + c.D + (7919 if c.family == "exact" else 0))
+    x, _ = sa_inputs(SimpleNamespace(F=c.F, beta=abs(c.beta), edge_term=False), rp, ci, n_cols, rng)
+    nnz = ci.size
+    if c.family == "exact":
+        top = 3.0 if c.beta == 0 else max(3.0, 70.0 / abs(c.beta))
+        s = 2.0 ** np.floor(np.log2(max(top / (2 * c.D ** 0.5), 1.0)))   # A spreads about as x does
+        attr = rng.integers(-2, 3, (nnz, c.D)).astype(np.float32)
+        w = (rng.integers(-8, 9, (c.F, c.D)) * (s / 8)).astype(np.float32)
+        A = (attr.astype(np.float64) @ w.astype(np.float64).T).astype(np.float32)
+        cols, first = np.unique(ci, return_index=True)
+        pick = cols % 7 != 0
+        x[cols[pick]] = -A[first[pick]]                   # that edge's pre-activation is exactly 0
+        return x, attr, w, A, np.zeros_like(A, np.float64)
+    attr = rng.random((nnz, c.D)).astype(np.float32)
+    w = (rng.standard_normal((c.F, c.D)) / c.D ** 0.5).astype(np.float32)
+    a64, w64 = attr.astype(np.float64), w.astype(np.float64)
+    return x, attr, w, (a64 @ w64.T).astype(np.float32), (c.D + 1) * U32 * (np.abs(a64) @ np.abs(w64).T)
+
+
+def _m_error(pre, m, dA):
+    """Per-edge bound on |m_kernel - m| from the edge term's dA (module docstring), and the edges that may change
+    sides of the ReLU."""
+    dpre = dA + 2 * U32 * (np.abs(pre) + dA)
+    dm = np.where((pre <= -dpre) | (dA == 0), 0.0, dpre + 2 * U32 * (m + dpre))
+    return dm, (np.abs(pre) <= dpre) & (dA > 0)
+
+
+def _fwd_call(c, st, xd, attr, w, beta_d, dev):
+    """The forward through genconv_edge_fwd_raw, or with c.partials_offset straight through the C entry point with the
+    plan's partial scratch shifted off 16-byte alignment (as test_gpu_dispatch_message.sa_fwd_call does)."""
+    from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import _sa_scratch, genconv_edge_fwd_raw
+    from cogdl_b200.structure import _ptr, _stream
+
+    if not c.partials_offset:
+        return genconv_edge_fwd_raw(st, xd, attr, w, beta_d, EPS, want_lse=True, want_q=c.want_q)
+    assert st.plan.n_chunks > 0, f"{c.id}: the partials offset only matters with hub chunks"
+    out = torch.empty((st.n_rows, c.F), device=dev)
+    lse2, q = torch.empty_like(out), (torch.empty_like(out) if c.want_q else None)
+    plan, keep = st.plan_struct(_sa_scratch(st, c.F) + 16)
+    keep[0].partials += c.partials_offset
+    keep[0].partials_bytes -= c.partials_offset
+    _cabi.call("cogdl_b200_genconv_edge_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(xd), _ptr(attr), _ptr(w),
+               c.D, _ptr(beta_d), float(EPS), _ptr(out), _ptr(lse2), _ptr(q), st.n_rows, c.F, plan, _stream(dev))
+    torch.cuda.synchronize(dev)
+    del keep
+    return out, lse2, q
+
+
+def _bwd_call(c, st, xd, attr, w, beta_d, g, out, lse2, dev):
+    from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import genconv_edge_bwd_raw
+    from cogdl_b200.structure import _ptr, _stream
+
+    if not c.partials_offset:
+        return genconv_edge_bwd_raw(st, xd, attr, w, beta_d, EPS, g, out, lse2, want_dx="dx" in c.want,
+                                    want_dw="dw" in c.want)
+    assert c.want == "dx", "the plan's partial scratch is used by dX only"
+    st_t, perm = st.csc()
+    assert st_t.plan.n_chunks > 0, f"{c.id}: the partials offset only matters with hub chunks"
+    dx = torch.empty_like(xd)
+    plan, keep = st_t.plan_struct(st_t.plan.n_chunks * c.F * 4 + 16)
+    keep[0].partials += c.partials_offset
+    keep[0].partials_bytes -= c.partials_offset
+    _cabi.call("cogdl_b200_genconv_edge_bwd_f32", _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(xd),
+               _ptr(attr), _ptr(w), c.D, _ptr(beta_d), float(EPS), _ptr(g), _ptr(out), _ptr(lse2), _ptr(dx), None,
+               None, 0, st_t.n_rows, c.F, plan, _stream(dev))
+    torch.cuda.synchronize(dev)
+    del keep
+    return dx, None
+
+
+def _check_fwd(c, rp, out, lse2, q, m, dm):
+    out64, lse64, Q64, E, deg = sa_fwd64(rp, m, c.beta)
+    Dm = seg_reduce(np.maximum, dm, rp)
+    k = 2.01 * abs(c.beta) * Dm
+    assert_within(out.cpu().numpy(), out64, out64 * (2 * E + (2 * deg + 1) * U32) + k * (out64 + Dm) + Dm + TINY,
+                  f"{c.id} out")
+    assert_within(lse2.cpu().numpy(), lse64, (E + deg * U32) * LOG2E + 2.0 ** -21 + 2 * U32 * np.abs(lse64)
+                  + abs(c.beta) * LOG2E * Dm, f"{c.id} lse2")
+    if c.want_q:
+        Qp = Q64 + 2 * Dm * out64 + Dm ** 2
+        assert_within(q.cpu().numpy(), Q64, Q64 * (2 * E + (2 * deg + 3) * U32) + k * Qp + (Qp - Q64) + TINY,
+                      f"{c.id} Q")
+    else:
+        assert q is None
+    empty = np.diff(rp) == 0
+    assert np.all(out.cpu().numpy()[empty] == 0) and np.all(lse2.cpu().numpy()[empty] == 0)
+
+
+def _check_bwd(c, st, rp, ci, n, attr, g, out, lse2, dx, dw, pre, m, dm, flip):
+    """dX and dW against fp64 on the kernel's out and lse2 (run_sa_bwd's terms, plus the edge term's and dW's)."""
+    beta = c.beta
+    rows = edge_rows(rp)
+    o32, l32 = out.cpu().numpy().astype(np.float64), lse2.cpu().numpy().astype(np.float64)
+    z = beta * LOG2E * m.astype(np.float64)
+    arg = z - l32[rows]
+    wgt = np.exp2(arg)
+    dev_m = np.abs(m - o32[rows])
+    live = pre > 0
+    dpre = np.where(live, wgt * g[rows] * (1 + beta * (m - o32[rows])), 0.0)
+    full = wgt * np.abs(g[rows]) * (1 + abs(beta) * dev_m)
+    mag = np.where(live, full, 0.0)
+    eb = mag * (2.0 ** -22 + LN2 * U32 * (3 * np.abs(z) + np.abs(arg)) + 4 * U32)
+    eb = eb + np.where(live, 1.01 * abs(beta) * dm * (mag + wgt * np.abs(g[rows])), 0.0)
+    eb = eb + np.where(flip, 1.01 * full * (1 + abs(beta) * dm) + dm, 0.0)
+    coldeg = np.bincount(ci, minlength=n).astype(np.float64)[:, None]
+    if "dx" in c.want:
+        assert_within(dx.cpu().numpy(), col_sum(dpre, ci, n),
+                      col_sum(eb, ci, n) + coldeg * U32 * col_sum(mag, ci, n) + TINY, f"{c.id} dX")
+    else:
+        assert dx is None
+    if "dw" in c.want:
+        st_t, _ = st.csc()
+        n_chunks = st_t.plan.n_chunks if st_t.chunk_edges > 0 else 0
+        items = n_chunks + n
+        B = min(-(-items // GE_WARPS), GE_BWD_BLOCKS)
+        per_item = st_t.chunk_edges if st_t.chunk_edges > 0 else int(coldeg.max(initial=0))
+        L = -(-items // (GE_WARPS * B)) * per_item
+        a64 = np.abs(attr.astype(np.float64))
+        assert_within(dw.cpu().numpy(), dpre.T @ attr.astype(np.float64),
+                      eb.T @ a64 + (L + GE_WARPS + B + 2) * U32 * (mag.T @ a64) + TINY, f"{c.id} dW")
+    else:
+        assert dw is None
 
 
 @pytest.mark.parametrize("c", TABLE, ids=[c.id for c in TABLE])
 def test_table_row(dev, c):
-    """Every compiled instantiation: records its name, and matches fp64 (forward 1e-5, gradients 1e-4)."""
+    """Every row: records its instantiation's name, every output element lies within the bound of the module
+    docstring, and the hub plans' arrival counters are back at zero."""
     from cogdl_b200 import _cabi
-    from cogdl_b200.operators._raw import genconv_edge_bwd_raw, genconv_edge_fwd_raw
+    from cogdl_b200.operators._raw import genconv_edge_fwd_raw
+    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES, CSRStructure
 
-    st, x, attr, w = _row_operands(c, dev)
-    beta = torch.full((1,), 1.3, device=dev)
-    out, lse2, q = genconv_edge_fwd_raw(st, x, attr, w, beta, 1e-7, want_lse=True, want_q=c.want_q)
+    RATIOS.clear()
+    rp, ci, n = _row_graph(c)
+    x, attr, w, A, dA = _row_inputs(c, rp, ci, n)
+    st = CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n,
+                      chunk_edges=(c.chunk or DEFAULT_CHUNK_EDGES) if c.plan else 0)
+    xd = torch.from_numpy(x).to(dev)
+    if not c.aligned:    # 4 bytes off 16-byte alignment: the scalar kernel
+        xd = misaligned(xd)
+    attr_d, w_d = torch.from_numpy(attr).to(dev), torch.from_numpy(w).to(dev)
+    beta_d = torch.tensor([c.beta], dtype=torch.float32, device=dev)
+    pre, m = sa_m(x, A, ci)
+    if c.family == "exact":
+        cols, first = np.unique(ci, return_index=True)
+        assert np.all(pre[first[cols % 7 != 0]] == 0)
+    dm, flip = _m_error(pre, m, dA)
     if c.op == "fwd":
+        out, lse2, q = _fwd_call(c, st, xd, attr_d, w_d, beta_d, dev)
         if st.n_rows and c.F:
             assert _cabi.last_kernel() == c.kernel
-        want = fp64(st, x, attr, w, "softmax_sg", beta)
-        assert err(out, want) <= 1e-5
-        if c.want_q:
-            assert err(q, q_fp64(st, x, attr, w, float(beta))) <= 1e-5
-        return
-    r = torch.randn(st.n_rows, c.F, device=dev, generator=torch.Generator(device=dev).manual_seed(3))
-    dx, dw = genconv_edge_bwd_raw(st, x, attr, w, beta, 1e-7, r, out, lse2, want_dx="dx" in c.want,
-                                  want_dw="dw" in c.want)
-    if st.n_cols and c.F:
-        assert _cabi.last_kernel() == c.kernel
-    x64, w64 = x.double().requires_grad_(True), w.double().requires_grad_(True)
-    (fp64(st, x64, attr, w64, "softmax_sg", beta) * r.double()).sum().backward()
-    if "dx" in c.want:
-        assert err(dx, x64.grad) <= 1e-4
+        if c.graph.startswith("bounds") or c.partials_offset:
+            assert st.plan.n_chunks > 0
+        _check_fwd(c, rp, out, lse2, q, m, dm)
+        check_counters(c, st)
     else:
-        assert dx is None
-    if "dw" in c.want:
-        assert err(dw, w64.grad) <= 1e-4
-    else:
-        assert dw is None
+        out, lse2, _ = genconv_edge_fwd_raw(st, xd, attr_d, w_d, beta_d, EPS, want_lse=True)
+        g = np.random.default_rng(3 + c.F).standard_normal((st.n_rows, c.F)).astype(np.float32)
+        gd = torch.from_numpy(g).to(dev)
+        dx, dw = _bwd_call(c, st, xd, attr_d, w_d, beta_d, gd, out, lse2, dev)
+        if st.n_cols and c.F:
+            assert _cabi.last_kernel() == c.kernel
+        st_t, _ = st.csc()
+        if c.graph.startswith("bounds") or c.graph == "wide" or c.partials_offset:
+            assert st_t.plan.n_chunks > 0
+        if c.graph == "wide":
+            assert st_t.plan.n_chunks + n > GE_WARPS * GE_BWD_BLOCKS
+            again = _bwd_call(c, st, xd, attr_d, w_d, beta_d, gd, out, lse2, dev)
+            for a, b in zip((dx, dw), again):
+                assert (a is None and b is None) or torch.equal(a, b), f"{c.id}: not reproducible"
+        _check_bwd(c, st, rp, ci, n, attr, g, out, lse2, dx, dw, pre, m, dm, flip)
+        check_counters(c, st, st_t)
+    print(" ".join(f"[{k}: worst err/bound {v:.3g}]" for k, v in RATIOS.items()))
 
 
 def test_no_edge_sized_tensor(dev):
