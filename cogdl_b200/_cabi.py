@@ -9,7 +9,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libcogdl_b200.so")
-MAX_PANELS = 8   # COGDL_B200_MAX_PANELS: a hub plan holds n_chunks * MAX_PANELS arrival counters
+MAX_PANELS = 8   # COGDL_B200_MAX_PANELS: a hub plan holds MAX_PANELS arrival counters per chunk
 COMP_OPS = {"mult": 0, "sub": 1, "copy": 2}   # COGDL_B200_COMP_MULT / _SUB / _COPY of cogdl_b200_comp_aggr_f32
 
 OK, EINVAL, ECUDA, EDEVICE, ESCRATCH = 0, -1, -2, -3, -4
@@ -56,6 +56,7 @@ SIGNATURES = {
     "cogdl_b200_hub_plan_count": (ctypes.c_int, [_vp, _i64, _i32, _i32, _vp, _vp]),
     "cogdl_b200_hub_plan_fill": (ctypes.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "cogdl_b200_edge_rows": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp]),
+    "cogdl_b200_spmm_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_spmm_csr_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_spmm_csr_f32_ex": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _plan_p, _vp]),
     "cogdl_b200_spmm_residual_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _f32, _f32, _vp, _vp, _i64, _i64, _i32,
@@ -75,13 +76,17 @@ SIGNATURES = {
     "cogdl_b200_gather_rows_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _vp]),
     "cogdl_b200_edge_softmax_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_gat_attn_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_edge_colsum_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_edge_colsum_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_edge_softmax_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_edge_softmax_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_mhspmm_scratch_bytes": (_i64, [_i64, _i64, _i64]),
     "cogdl_b200_mhspmm_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_mhsddmm_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_scatter_max_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_scatter_max_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_scatter_max_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "cogdl_b200_gat_fwd_scratch_bytes": (_i64, [_i64, _i64, _i64]),
     "cogdl_b200_gat_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_gat_fwd_dropout_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, ctypes.c_uint64, ctypes.c_uint64, _f32,
                                                       _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
@@ -89,16 +94,20 @@ SIGNATURES = {
     "cogdl_b200_gat_attn_bwd_dropout_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _f32, _vp, _vp, _i64, _i64,
                                                            _plan_p, _vp]),
     "cogdl_b200_gcn_fused_supported": (ctypes.c_int, [_i64, _i64]),
+    "cogdl_b200_gcn_fused_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_gcn_fused_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _plan_p, _vp]),
+    "cogdl_b200_sage_fused_scratch_bytes": (_i64, [_i64, _i64, _i32]),
     "cogdl_b200_sage_fused_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32,
                                                  _plan_p, _vp]),
     "cogdl_b200_softmax_aggr_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_softmax_aggr_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
+    "cogdl_b200_softmax_aggr_bwd_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_softmax_aggr_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _vp, _i64, _i64,
                                                        _plan_p, _vp]),
     "cogdl_b200_genconv_edge_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _f32, _vp, _vp, _vp, _i64, _i64,
                                                        _plan_p, _vp]),
     "cogdl_b200_genconv_edge_dw_scratch_bytes": (_i64, [_i64, _i64]),
+    "cogdl_b200_genconv_edge_bwd_scratch_bytes": (_i64, [_i64, _i64, _i32]),
     "cogdl_b200_genconv_edge_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _f32, _vp, _vp, _vp, _vp, _vp,
                                                        _vp, _i64, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_disen_route_scratch_bytes": (_i64, [_i64, _i64, _i64]),

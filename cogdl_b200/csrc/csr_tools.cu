@@ -194,6 +194,10 @@ extern "C" int cogdl_b200_gather_rows_f32(const int32_t *perm, const float *in, 
   return COGDL_B200_OK;
 }
 
+extern "C" int64_t cogdl_b200_edge_colsum_scratch_bytes(int64_t n_chunks, int64_t H) {
+  return n_chunks > 0 && H > 0 ? n_chunks * H * (int64_t)sizeof(float) : 0;
+}
+
 extern "C" int cogdl_b200_edge_colsum_f32(const int32_t *colptr, const int32_t *perm, const float *e, float *out,
                                           int64_t n_cols, int64_t H, const cogdl_b200_hub_plan_t *plan,
                                           cogdl_b200_stream_t stream) {
@@ -205,7 +209,7 @@ extern "C" int cogdl_b200_edge_colsum_f32(const int32_t *colptr, const int32_t *
   p.colptr = colptr; p.perm = perm; p.e = e; p.out = out; p.n_cols = n_cols; p.H = (int)H;
   p.hub = hub_view(plan);
   p.hub.n_segs = 0;
-  int rc = check_plan(plan, (int64_t)p.hub.n_chunks * H * (int64_t)sizeof(float));
+  int rc = check_plan(plan, cogdl_b200_edge_colsum_scratch_bytes(p.hub.n_chunks, H));
   if (rc) return rc;
   p.part = reinterpret_cast<float *>(p.hub.partials);
   cudaStream_t s = (cudaStream_t)stream;

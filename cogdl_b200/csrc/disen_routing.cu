@@ -580,9 +580,9 @@ extern "C" int cogdl_b200_disen_route_bwd_f32(const int32_t *rowptr, const int32
              "%s: null pointer", who);
   const int64_t n_chunks = plan && plan->chunk_edges > 0 ? plan->n_chunks : 0;
   const int64_t n_chunks_t = plan_t && plan_t->chunk_edges > 0 ? plan_t->n_chunks : 0;
-  rc = check_plan(plan, n_chunks * (2 * F + K) * 4);
+  rc = check_plan(plan, cogdl_b200_disen_route_scratch_bytes(n_chunks, F, K));
   if (rc) return rc;
-  rc = check_plan(plan_t, n_chunks_t * F * 4);
+  rc = check_plan(plan_t, cogdl_b200_disen_route_scratch_bytes(n_chunks_t, F, K));
   if (rc) return rc;
   const bool vec = d % 4 == 0 && aligned16(q) && aligned16(c) && aligned16(G) && aligned16(out) && aligned16(g_u) &&
                    aligned16(dq) && aligned16(dc) && (n_chunks == 0 || aligned16(plan->partials)) &&

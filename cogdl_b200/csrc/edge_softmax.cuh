@@ -678,9 +678,8 @@ static int es_plan(EsParams &p, const cogdl_b200_hub_plan_t *plan, EsForm *form,
     return COGDL_B200_OK;
   }
   p.hub = hub_view(plan);
-  // scratch: (max, sum) per chunk slot and head, + (MODE 3) one partial row sum per slot and head
-  const int64_t need = (int64_t)p.hub.n_chunks * p.H * (int64_t)(sizeof(float2) + (MODE == 3 ? sizeof(float) : 0));
-  int rc = check_plan(plan, need);
+  // scratch: (max, sum) per chunk slot and head, then (MODE 3) one partial row sum per slot and head
+  int rc = check_plan(plan, cogdl_b200_edge_softmax_scratch_bytes(p.hub.n_chunks, p.H));
   if (rc) return rc;
   p.stats = reinterpret_cast<float2 *>(plan->partials);
   p.part = reinterpret_cast<float *>(p.stats + (int64_t)p.hub.n_chunks * p.H);

@@ -506,6 +506,16 @@ using namespace cogdl_b200;
 
 extern "C" int cogdl_b200_gcn_fused_supported(int64_t K, int64_t Fout) { return (K == fg::KDIM && Fout >= 1 && Fout <= 128) ? 1 : 0; }
 
+// The partials are those of the hub-row pre-pass: the SpMM's, or scatter_max's for the max aggregation.
+extern "C" int64_t cogdl_b200_gcn_fused_scratch_bytes(int64_t n_chunks, int64_t K) {
+  return cogdl_b200_spmm_scratch_bytes(n_chunks, K);
+}
+
+extern "C" int64_t cogdl_b200_sage_fused_scratch_bytes(int64_t n_chunks, int64_t K, int32_t aggr) {
+  return aggr == COGDL_B200_AGGR_MAX ? cogdl_b200_scatter_max_scratch_bytes(n_chunks, K)
+                                     : cogdl_b200_spmm_scratch_bytes(n_chunks, K);
+}
+
 extern "C" int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X,
                                         const float *W, const float *bias, const float *rowsum, float *out, float *hub_agg,
                                         int64_t n_rows,
@@ -520,7 +530,7 @@ extern "C" int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t *co
   CB_REQUIRE(n_rows < 0x7fffff00LL, "%s: n_rows must fit int32", who);
   CB_REQUIRE(plan && plan->chunk_edges > 0 && plan->edge_row, "%s: needs a hub plan with edge_row (row-stream form)", who);
   CB_REQUIRE(aligned16(X) && aligned16(W) && aligned16(out), "%s: X, W and out must be 16-byte aligned", who);
-  int rc = check_plan(plan, (int64_t)plan->n_chunks * K * (int64_t)sizeof(float));
+  int rc = check_plan(plan, cogdl_b200_gcn_fused_scratch_bytes(plan->n_chunks, K));
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (plan->n_chunks > 0) {
@@ -556,8 +566,7 @@ extern "C" int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_t *c
   CB_REQUIRE(plan && plan->chunk_edges > 0 && plan->edge_row, "%s: needs a hub plan with edge_row (row-stream form)", who);
   CB_REQUIRE(aligned16(X) && aligned16(W_neigh) && aligned16(S) && aligned16(out), "%s: X, W_neigh, S and out must be 16-byte aligned",
              who);
-  const int64_t elem = aggr == COGDL_B200_AGGR_MAX ? 8 : 4;       // max partials carry (value, argmax)
-  int rc = check_plan(plan, (int64_t)plan->n_chunks * K * elem);
+  int rc = check_plan(plan, cogdl_b200_sage_fused_scratch_bytes(plan->n_chunks, K, aggr));
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (plan->n_chunks > 0) {

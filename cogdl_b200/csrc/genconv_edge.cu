@@ -335,6 +335,11 @@ extern "C" int64_t cogdl_b200_genconv_edge_dw_scratch_bytes(int64_t F, int64_t D
   return F > 0 && D > 0 ? (int64_t)GE_BWD_BLOCKS * F * D * 4 : 0;
 }
 
+// only dX's hub columns use the partials
+extern "C" int64_t cogdl_b200_genconv_edge_bwd_scratch_bytes(int64_t n_chunks, int64_t F, int32_t want_dx) {
+  return want_dx ? cogdl_b200_softmax_aggr_bwd_scratch_bytes(n_chunks, F) : 0;
+}
+
 extern "C" int cogdl_b200_genconv_edge_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
                                                const float *attr, const float *W, int64_t D, const float *beta,
                                                float eps, float *out, float *lse2, float *Q, int64_t n_rows, int64_t F,
@@ -346,7 +351,7 @@ extern "C" int cogdl_b200_genconv_edge_fwd_f32(const int32_t *rowptr, const int3
   CB_REQUIRE(rowptr && colind && X && attr && W && beta && out, "cogdl_b200_genconv_edge_fwd_f32: null pointer");
   CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "cogdl_b200_genconv_edge_fwd_f32: sizes must fit int32");
   const int64_t n_chunks = plan && plan->chunk_edges > 0 ? plan->n_chunks : 0;
-  int rc = check_plan(plan, n_chunks * F * (Q ? 16 : 12));
+  int rc = check_plan(plan, cogdl_b200_softmax_aggr_scratch_bytes(n_chunks, F));
   if (rc) return rc;
   GeFwdParams p;
   SaFwdParams &s = p.sa;
@@ -390,7 +395,7 @@ extern "C" int cogdl_b200_genconv_edge_bwd_f32(const int32_t *colptr, const int3
              "cogdl_b200_genconv_edge_bwd_f32: null pointer");
   CB_REQUIRE(n_cols < 0x7fffffffLL && F < 0x7fffffffLL, "cogdl_b200_genconv_edge_bwd_f32: sizes must fit int32");
   const int64_t n_chunks = plan && plan->chunk_edges > 0 ? plan->n_chunks : 0;
-  int rc = check_plan(plan, dX ? n_chunks * F * 4 : 0);
+  int rc = check_plan(plan, cogdl_b200_genconv_edge_bwd_scratch_bytes(n_chunks, F, dX != nullptr));
   if (rc) return rc;
   GeBwdParams p;
   p.colptr = colptr; p.rowind = rowind; p.perm = perm; p.X = X; p.attr = attr; p.Wt = W; p.beta = beta; p.eps = eps;

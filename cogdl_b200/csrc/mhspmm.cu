@@ -183,6 +183,10 @@ static int mhspmm_run(const int32_t *rowptr, const int32_t *colind, const int32_
 
 using namespace cogdl_b200;
 
+extern "C" int64_t cogdl_b200_mhspmm_scratch_bytes(int64_t n_chunks, int64_t H, int64_t F) {
+  return n_chunks > 0 && H > 0 && F > 0 ? n_chunks * H * F * (int64_t)sizeof(float) : 0;
+}
+
 static int mhspmm_entry(const int32_t *rowptr, const int32_t *colind, const int32_t *perm, const float *att,
                         const float *feat, float *out, int64_t n_rows, int64_t H, int64_t F,
                         const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream, float drop_scale,
@@ -191,7 +195,7 @@ static int mhspmm_entry(const int32_t *rowptr, const int32_t *colind, const int3
   if (n_rows == 0 || H == 0 || F == 0) return COGDL_B200_OK;
   CB_REQUIRE(rowptr && colind && att && feat && out, "%s: null pointer", who);
   CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "%s: sizes must fit int32", who);
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
+  int rc = check_plan(plan, cogdl_b200_mhspmm_scratch_bytes(plan ? plan->n_chunks : 0, H, F));
   if (rc) return rc;
   return mhspmm_run(rowptr, colind, perm, att, feat, out, n_rows, H, F, plan, stream, drop_scale);
 }
@@ -235,6 +239,13 @@ int gat_attention(const int32_t *rowptr, const int32_t *colind, const float *h_l
                   bool drop, uint64_t seed, uint64_t drop_below);
 }
 
+// The attention stage and the aggregation use the same partials one after the other.
+extern "C" int64_t cogdl_b200_gat_fwd_scratch_bytes(int64_t n_chunks, int64_t H, int64_t F) {
+  const int64_t att = cogdl_b200_edge_softmax_scratch_bytes(n_chunks, H);
+  const int64_t agg = cogdl_b200_mhspmm_scratch_bytes(n_chunks, H, F);
+  return att > agg ? att : agg;
+}
+
 // drop: attention dropout (seed, drop_below, scale) -- see cogdl_b200_gat_fwd_dropout_f32
 static int gat_fwd(const int32_t *rowptr, const int32_t *colind, const float *h_l, const float *h_r, const float *feat,
                    float negative_slope, bool drop, uint64_t seed, uint64_t drop_below, float scale, float *out,
@@ -245,7 +256,7 @@ static int gat_fwd(const int32_t *rowptr, const int32_t *colind, const float *h_
   CB_REQUIRE(rowptr && colind && h_l && h_r && feat && out, "%s: null pointer", who);
   CB_REQUIRE(att_out, "%s: att_out ([nnz,H] attention, also scratch) is required", who);
   CB_REQUIRE(n_rows < 0x7fffffffLL && H * F < 0x7fffffffLL, "%s: sizes must fit int32", who);
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * H * F * (int64_t)sizeof(float));
+  int rc = check_plan(plan, cogdl_b200_gat_fwd_scratch_bytes(plan ? plan->n_chunks : 0, H, F));
   if (rc) return rc;
   rc = gat_attention(rowptr, colind, h_l, h_r, negative_slope, att_out, n_rows, H, plan, (cudaStream_t)stream, drop,
                      seed, drop_below);

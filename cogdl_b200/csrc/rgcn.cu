@@ -240,9 +240,9 @@ static int launch_rgcn(K kernel, const RgcnParams &p, cudaStream_t stream, const
   return COGDL_B200_OK;
 }
 
-// The checks both entries share; fills p's structure, plan and sizes.  `need` = partial bytes the plan must hold.
+// The checks both entries share; fills p's structure, plan and sizes.
 static int rgcn_setup(const char *who, RgcnParams &p, const int32_t *rowptr, const int32_t *colind, const float *w,
-                      int64_t n_rows, int64_t B, int64_t F, const cogdl_b200_hub_plan_t *plan, int64_t need) {
+                      int64_t n_rows, int64_t B, int64_t F, const cogdl_b200_hub_plan_t *plan) {
   CB_REQUIRE(F > 0 && F < 0x7fffffffLL, "%s: F must be in [1, 2^31), got %lld", who, (long long)F);
   CB_REQUIRE(B > 0 && B <= 4096, "%s: B must be in [1, 4096], got %lld", who, (long long)B);
   CB_REQUIRE(n_rows >= 0 && n_rows < 0x7fffffffLL, "%s: bad row count", who);
@@ -251,8 +251,6 @@ static int rgcn_setup(const char *who, RgcnParams &p, const int32_t *rowptr, con
   CB_REQUIRE(plan->n_hub_rows <= n_rows && (plan->n_segs > 0 || plan->n_hub_rows == n_rows),
              "%s: the plan does not match the structure's %lld rows (%d hub rows, %d segments)", who,
              (long long)n_rows, plan->n_hub_rows, plan->n_segs);
-  int rc = check_plan(plan, need);
-  if (rc) return rc;
   p.rowptr = rowptr; p.colind = colind; p.w = w; p.B = (int)B;
   p.hub = hub_view(plan);
   return COGDL_B200_OK;
@@ -273,8 +271,9 @@ extern "C" int cogdl_b200_rgcn_aggr_f32(const int32_t *rowptr, const int32_t *co
   const char *who = "cogdl_b200_rgcn_aggr_f32";
   RgcnParams p = {};
   if (n_rows == 0) return COGDL_B200_OK;
-  int rc = rgcn_setup(who, p, rowptr, colind, w, n_rows, B, F, plan,
-                      cogdl_b200_rgcn_aggr_scratch_bytes(plan ? plan->n_chunks : 0, B, F));
+  int rc = rgcn_setup(who, p, rowptr, colind, w, n_rows, B, F, plan);
+  if (rc) return rc;
+  rc = check_plan(plan, cogdl_b200_rgcn_aggr_scratch_bytes(plan->n_chunks, B, F));
   if (rc) return rc;
   CB_REQUIRE(etype && coef && X && Y, "%s: null pointer", who);
   p.etype = etype; p.coef = coef; p.X = X; p.Y = Y;
@@ -295,7 +294,9 @@ extern "C" int cogdl_b200_rgcn_edge_dot_f32(const int32_t *rowptr, const int32_t
   const char *who = "cogdl_b200_rgcn_edge_dot_f32";
   RgcnParams p = {};
   if (n_rows == 0) return COGDL_B200_OK;
-  int rc = rgcn_setup(who, p, rowptr, colind, w, n_rows, B, F, plan, 0);
+  int rc = rgcn_setup(who, p, rowptr, colind, w, n_rows, B, F, plan);
+  if (rc) return rc;
+  rc = check_plan(plan, 0);
   if (rc) return rc;
   CB_REQUIRE(G && X && P, "%s: null pointer", who);
   p.G = G; p.X = X; p.P = P;

@@ -334,7 +334,7 @@ static int dispatch_smax(const SmaxParams &p, cudaStream_t s) {
 // Only the hub rows (degree > plan chunk) of the max values, no argmax: the hub-chunk items of the row-stream
 // kernel with their in-order combine, no segments.  Used by the fused
 // SAGE layer (fused_gcn.cu), which aggregates every other row straight into shared memory.  F == 128, 16-byte
-// aligned X / Y; plan->partials n_chunks * F * 8 bytes.
+// aligned X / Y; plan->partials cogdl_b200_scatter_max_scratch_bytes(n_chunks, F) bytes.
 int smax_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float *X, float *Y, int64_t F,
                        const cogdl_b200_hub_plan_t *plan, cudaStream_t stream) {
   SmaxParams p;
@@ -366,6 +366,11 @@ __global__ void __launch_bounds__(256) scatter_max_bwd_kernel(const float *__res
 
 using namespace cogdl_b200;
 
+// (value, argmax) per chunk and column
+extern "C" int64_t cogdl_b200_scatter_max_scratch_bytes(int64_t n_chunks, int64_t F) {
+  return n_chunks > 0 && F > 0 ? n_chunks * F * 8 : 0;
+}
+
 extern "C" int cogdl_b200_scatter_max_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
                                               float *out, int32_t *argmax, int64_t n_rows, int64_t F,
                                               const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream) {
@@ -373,7 +378,7 @@ extern "C" int cogdl_b200_scatter_max_fwd_f32(const int32_t *rowptr, const int32
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
   CB_REQUIRE(rowptr && colind && X && out && argmax, "cogdl_b200_scatter_max_fwd_f32: null pointer");
   CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "cogdl_b200_scatter_max_fwd_f32: sizes must fit int32");
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * F * 8);
+  int rc = check_plan(plan, cogdl_b200_scatter_max_scratch_bytes(plan ? plan->n_chunks : 0, F));
   if (rc) return rc;
   SmaxParams p;
   p.rowptr = rowptr; p.colind = colind; p.X = X; p.out = out; p.argmax = argmax; p.n_rows = n_rows;

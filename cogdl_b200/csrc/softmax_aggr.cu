@@ -226,6 +226,10 @@ extern "C" int64_t cogdl_b200_softmax_aggr_scratch_bytes(int64_t n_chunks, int64
   return n_chunks > 0 && F > 0 ? n_chunks * F * 16 : 0;
 }
 
+extern "C" int64_t cogdl_b200_softmax_aggr_bwd_scratch_bytes(int64_t n_chunks, int64_t F) {
+  return n_chunks > 0 && F > 0 ? n_chunks * F * 4 : 0;
+}
+
 extern "C" int cogdl_b200_softmax_aggr_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
                                                const float *edge_term, const float *beta, float eps, float *out,
                                                float *lse2, float *Q, int64_t n_rows, int64_t F,
@@ -235,7 +239,7 @@ extern "C" int cogdl_b200_softmax_aggr_fwd_f32(const int32_t *rowptr, const int3
   CB_REQUIRE(rowptr && colind && X && beta && out, "cogdl_b200_softmax_aggr_fwd_f32: null pointer");
   CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "cogdl_b200_softmax_aggr_fwd_f32: sizes must fit int32");
   const int64_t n_chunks = plan && plan->chunk_edges > 0 ? plan->n_chunks : 0;
-  int rc = check_plan(plan, n_chunks * F * (Q ? 16 : 12));
+  int rc = check_plan(plan, cogdl_b200_softmax_aggr_scratch_bytes(n_chunks, F));
   if (rc) return rc;
   SaFwdParams p;
   p.rowptr = rowptr; p.colind = colind; p.X = X; p.A = edge_term; p.beta = beta; p.eps = eps;
@@ -272,7 +276,7 @@ extern "C" int cogdl_b200_softmax_aggr_bwd_f32(const int32_t *colptr, const int3
   CB_REQUIRE(!d_edge_term || edge_term, "cogdl_b200_softmax_aggr_bwd_f32: d_edge_term without an edge term");
   CB_REQUIRE(n_cols < 0x7fffffffLL && F < 0x7fffffffLL, "cogdl_b200_softmax_aggr_bwd_f32: sizes must fit int32");
   const int64_t n_chunks = plan && plan->chunk_edges > 0 ? plan->n_chunks : 0;
-  int rc = check_plan(plan, n_chunks * F * 4);
+  int rc = check_plan(plan, cogdl_b200_softmax_aggr_bwd_scratch_bytes(n_chunks, F));
   if (rc) return rc;
   SaBwdParams p;
   p.colptr = colptr; p.rowind = rowind; p.perm = perm; p.X = X; p.A = edge_term; p.beta = beta; p.eps = eps;

@@ -141,6 +141,10 @@ int spmm_hub_rows_only(const int32_t *rowptr, const int32_t *colind, const float
 
 using namespace cogdl_b200;
 
+extern "C" int64_t cogdl_b200_spmm_scratch_bytes(int64_t n_chunks, int64_t F) {
+  return n_chunks > 0 && F > 0 ? n_chunks * F * (int64_t)sizeof(float) : 0;
+}
+
 extern "C" int cogdl_b200_spmm_csr_f32_ex(const int32_t *rowptr, const int32_t *colind, const float *val,
                                           const float *X, int64_t x_rows, float *Y, int64_t n_rows, int64_t F,
                                           int32_t panels, const cogdl_b200_hub_plan_t *plan,
@@ -172,7 +176,7 @@ extern "C" int cogdl_b200_spmm_csr_f16(const int32_t *rowptr, const int32_t *col
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
   CB_REQUIRE(rowptr && colind && X && Y, "cogdl_b200_spmm_csr_f16: null pointer");
   CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "cogdl_b200_spmm_csr_f16: sizes must fit int32");
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * F * (int64_t)sizeof(float));
+  int rc = check_plan(plan, cogdl_b200_spmm_scratch_bytes(plan ? plan->n_chunks : 0, F));
   if (rc) return rc;
   SpmmHalfParams p;
   p.rowptr = rowptr; p.colind = colind; p.val = (const __half *)val; p.X = (const __half *)X;

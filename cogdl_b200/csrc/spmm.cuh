@@ -355,7 +355,7 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
   CB_REQUIRE(rowptr && colind && X0 && Y, "%s: null pointer", who);
   CB_REQUIRE(n_rows < 0x7fffffffLL && F < 0x7fffffffLL, "%s: n_rows / F must fit int32", who);
-  int rc = check_plan(plan, (plan ? (int64_t)plan->n_chunks : 0) * F * (int64_t)sizeof(float));
+  int rc = check_plan(plan, cogdl_b200_spmm_scratch_bytes(plan ? plan->n_chunks : 0, F));
   if (rc) return rc;
   SpmmParams p;
   p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X0; p.X1 = X1 ? X1 : X0; p.n0 = n0;

@@ -201,19 +201,16 @@ class PartitionedSpMM:
         """Y_local from the features currently in the symmetric shards (barrier, then ONE kernel)."""
         import ctypes
 
-        from . import _cabi
-        from .operators._raw import _spmm_out
-        from .structure import _ptr, _stream
+        from .operators._raw import _launch, _scratch, _spmm_out
+        from .structure import _ptr
 
         buf, hdl, ptrs = self._symm
         hdl.barrier()   # every rank's shard is written before anyone gathers from it
-        dev = self.device
-        with torch.cuda.device(dev):
-            y, plan, keep = _spmm_out(self.st, self.val, buf)
-            _cabi.call("cogdl_b200_spmm_csr_f32_peers", _ptr(self.st.rowptr), _ptr(self.st.colind), _ptr(self.val),
-                       _ptr(buf), self.n_local, ctypes.cast(ptrs, ctypes.c_void_p), self.world, self.part.peer_shift,
-                       _ptr(y), self.st.n_rows, buf.shape[1], plan, _stream(dev))
-            del keep
+        st = self.st
+        y = _spmm_out(st, self.val, buf)
+        _launch("cogdl_b200_spmm_csr_f32_peers", st, _scratch("spmm", st, buf.shape[1]), _ptr(st.rowptr),
+                _ptr(st.colind), _ptr(self.val), _ptr(buf), self.n_local, ctypes.cast(ptrs, ctypes.c_void_p), self.world,
+                self.part.peer_shift, _ptr(y), st.n_rows, buf.shape[1])
         return y
 
     # ------------------------------------------------------------------ nccl (halo) form: three stages

@@ -12,21 +12,30 @@ def _f32c(t, name):
     return t.contiguous()
 
 
-def _spmm_scratch(st: CSRStructure, F):
-    """Bytes of plan scratch an SpMM of width F needs: one fp32 partial row per hub chunk."""
-    return st.plan.n_chunks * F * 4 if st.chunk_edges > 0 else 0
+def _scratch(family, st: CSRStructure, *shape):
+    """Bytes of plan scratch an entry of `family` needs on st's hub plan, as the library's
+    cogdl_b200_<family>_scratch_bytes(n_chunks, *shape) gives it; 0 when st has no plan."""
+    if st.chunk_edges <= 0:
+        return 0
+    return int(getattr(_cabi.load(), f"cogdl_b200_{family}_scratch_bytes")(st.plan.n_chunks, *shape))
+
+
+def _launch(symbol, st: CSRStructure, partial_bytes, *args):
+    """symbol(*args, plan, stream) on st's device: plan is st's hub plan with partial_bytes of scratch, which stays
+    alive until the call returns; stream is the device's current stream."""
+    with torch.cuda.device(st.device):
+        plan, keep = st.plan_struct(partial_bytes)
+        _cabi.call(symbol, *args, plan, _stream(st.device))
 
 
 def _spmm_out(st: CSRStructure, val, x, out=None):
-    """What every SpMM wrapper shares: checks val against the nnz and x for being 2-D, allocates Y [n_rows, F] in x's
-    dtype (unless given `out`) and takes the plan with the SpMM's scratch.  Returns (y, plan, keepalive)."""
+    """What every SpMM wrapper shares: checks val against the nnz and x for being 2-D and allocates Y [n_rows, F] in
+    x's dtype (unless given `out`).  Returns y."""
     if x.dim() != 2:
         raise ValueError("x must be [n_src, F]")
     if val is not None and val.numel() != st.nnz:
         raise ValueError(f"edge values have {val.numel()} entries, CSR has {st.nnz}")
-    y = torch.empty((st.n_rows, x.shape[1]), dtype=x.dtype, device=x.device) if out is None else out
-    plan, keep = st.plan_struct(_spmm_scratch(st, x.shape[1]))
-    return y, plan, keep
+    return torch.empty((st.n_rows, x.shape[1]), dtype=x.dtype, device=x.device) if out is None else out
 
 
 def _epilogue_args(st: CSRStructure, val, x, z, row_scale):
@@ -49,12 +58,10 @@ def _epilogue_args(st: CSRStructure, val, x, z, row_scale):
 def _spmm_epilogue_raw(symbol, st: CSRStructure, val, x, z, a, b, row_scale, extra=(), panels=0, out=None):
     """One launch of an SpMM-epilogue entry: symbol(rowptr, colind, val, x, n_src, z, a, b, row_scale, *extra, y,
     n_rows, F, panels, plan, stream), with the operands of _epilogue_args.  Returns y (`out` when given)."""
-    dev, val, x, z, row_scale = _epilogue_args(st, val, x, z, row_scale)
-    with torch.cuda.device(dev):
-        y, plan, keep = _spmm_out(st, val, x, out)
-        _cabi.call(symbol, _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0], _ptr(z), float(a),
-                   float(b), _ptr(row_scale), *extra, _ptr(y), st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
-        del keep
+    _, val, x, z, row_scale = _epilogue_args(st, val, x, z, row_scale)
+    y = _spmm_out(st, val, x, out)
+    _launch(symbol, st, _scratch("spmm", st, x.shape[1]), _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x),
+            x.shape[0], _ptr(z), float(a), float(b), _ptr(row_scale), *extra, _ptr(y), st.n_rows, x.shape[1], int(panels))
     return y
 
 
@@ -62,40 +69,37 @@ def spmm_raw(st: CSRStructure, val, x, panels=0):
     """Y = A @ X with A = (st, val).  x: [n_src, F] fp32 or fp16; val: [nnz] or None.
     panels: column panels of X for the fp32 kernel (0 = chosen from X's size against the L2; the output
     does not depend on it)."""
-    dev = require_cuda(x, val)
+    require_cuda(x, val)
     x = x.contiguous()
     val = None if val is None else val.contiguous().view(-1)
-    with torch.cuda.device(dev):
-        y, plan, keep = _spmm_out(st, val, x)
-        if x.dtype == torch.float32:
-            if val is not None and val.dtype != torch.float32:
-                val = val.float()
-            _cabi.call("cogdl_b200_spmm_csr_f32_ex", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
-                       _ptr(y), st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
-        elif x.dtype == torch.float16:
-            if val is not None and val.dtype != torch.float16:
-                val = val.half()
-            _cabi.call("cogdl_b200_spmm_csr_f16", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), _ptr(y),
-                       st.n_rows, x.shape[1], plan, _stream(dev))
-        else:
-            raise TypeError(f"spmm supports float32 / float16 features, got {x.dtype}")
-        del keep
+    y = _spmm_out(st, val, x)
+    need = _scratch("spmm", st, x.shape[1])
+    if x.dtype == torch.float32:
+        if val is not None and val.dtype != torch.float32:
+            val = val.float()
+        _launch("cogdl_b200_spmm_csr_f32_ex", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x),
+                x.shape[0], _ptr(y), st.n_rows, x.shape[1], int(panels))
+    elif x.dtype == torch.float16:
+        if val is not None and val.dtype != torch.float16:
+            val = val.half()
+        _launch("cogdl_b200_spmm_csr_f16", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), _ptr(y),
+                st.n_rows, x.shape[1])
+    else:
+        raise TypeError(f"spmm supports float32 / float16 features, got {x.dtype}")
     return y
 
 
 def spmm_2src_raw(st: CSRStructure, val, x0, x1):
     """Partitioned SpMM: columns < x0.shape[0] read x0, the others read x1 (halo rows)."""
-    dev = require_cuda(x0, x1, val)
+    require_cuda(x0, x1, val)
     x0, x1 = _f32c(x0, "x0"), _f32c(x1, "x1")
     if x1.shape[1] != x0.shape[1]:
         raise ValueError("x0 / x1 feature widths differ")
     val = None if val is None else _f32c(val, "val").view(-1)
-    with torch.cuda.device(dev):
-        y, plan, keep = _spmm_out(st, val, x0)
-        x1p = x1 if x1.numel() > 0 else x0
-        _cabi.call("cogdl_b200_spmm_csr_f32_2src", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x0),
-                   x0.shape[0], _ptr(x1p), _ptr(y), st.n_rows, x0.shape[1], plan, _stream(dev))
-        del keep
+    y = _spmm_out(st, val, x0)
+    x1p = x1 if x1.numel() > 0 else x0
+    _launch("cogdl_b200_spmm_csr_f32_2src", st, _scratch("spmm", st, x0.shape[1]), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(val), _ptr(x0), x0.shape[0], _ptr(x1p), _ptr(y), st.n_rows, x0.shape[1])
     return y
 
 
@@ -121,13 +125,9 @@ def spmm_adjoint_raw(st: CSRStructure, val, g, sym, a=None):
 def sddmm_raw(st: CSRStructure, d1, d2):
     dev = require_cuda(d1, d2)
     d1, d2 = _f32c(d1, "d1"), _f32c(d2, "d2")
-    F = d1.shape[1]
-    with torch.cuda.device(dev):
-        out = torch.empty(st.nnz, dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(0)
-        _cabi.call("cogdl_b200_sddmm_csr_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(d1), _ptr(d2), _ptr(out),
-                   st.n_rows, F, plan, _stream(dev))
-        del keep
+    out = torch.empty(st.nnz, dtype=torch.float32, device=dev)
+    _launch("cogdl_b200_sddmm_csr_f32", st, 0, _ptr(st.rowptr), _ptr(st.colind), _ptr(d1), _ptr(d2), _ptr(out),
+            st.n_rows, d1.shape[1])
     return out
 
 
@@ -141,34 +141,23 @@ def gather_rows_raw(perm, x):
     return out
 
 
-def _es_scratch(st, H):
-    """Bytes of plan scratch the split-row softmax needs (per hub chunk and head: (max, sum) + a partial)."""
-    return st.plan.n_chunks * H * 12 if st.chunk_edges > 0 else 0
-
-
 def edge_softmax_fwd_raw(st: CSRStructure, e):
-    dev = require_cuda(e)
+    require_cuda(e)
     e = _f32c(e, "edge values")
     if e.dim() != 2 or e.shape[0] != st.nnz:
         raise ValueError(f"edge values must be [nnz={st.nnz}, H], got {tuple(e.shape)}")
-    with torch.cuda.device(dev):
-        out = torch.empty_like(e)
-        plan, keep = st.plan_struct(_es_scratch(st, e.shape[1]))
-        _cabi.call("cogdl_b200_edge_softmax_fwd_f32", _ptr(st.rowptr), _ptr(e), _ptr(out), st.n_rows, e.shape[1],
-                   plan, _stream(dev))
-        del keep
+    out = torch.empty_like(e)
+    _launch("cogdl_b200_edge_softmax_fwd_f32", st, _scratch("edge_softmax", st, e.shape[1]), _ptr(st.rowptr), _ptr(e),
+            _ptr(out), st.n_rows, e.shape[1])
     return out
 
 
 def edge_softmax_bwd_raw(st: CSRStructure, y, g):
-    dev = require_cuda(y, g)
+    require_cuda(y, g)
     y, g = _f32c(y, "y"), _f32c(g, "g")
-    with torch.cuda.device(dev):
-        out = torch.empty_like(y)
-        plan, keep = st.plan_struct(_es_scratch(st, y.shape[1]))
-        _cabi.call("cogdl_b200_edge_softmax_bwd_f32", _ptr(st.rowptr), _ptr(y), _ptr(g), _ptr(out), st.n_rows,
-                   y.shape[1], plan, _stream(dev))
-        del keep
+    out = torch.empty_like(y)
+    _launch("cogdl_b200_edge_softmax_bwd_f32", st, _scratch("edge_softmax", st, y.shape[1]), _ptr(st.rowptr), _ptr(y),
+            _ptr(g), _ptr(out), st.n_rows, y.shape[1])
     return out
 
 
@@ -183,16 +172,14 @@ def mhspmm_raw(st: CSRStructure, att, feat, perm=None, drop_scale=None):
     H, F = feat.shape[1], feat.shape[2]
     if att.shape != (st.nnz, H):
         raise ValueError(f"attention must be [nnz={st.nnz}, H={H}], got {tuple(att.shape)}")
-    with torch.cuda.device(dev):
-        out = torch.empty((st.n_rows, H, F), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(st.plan.n_chunks * H * F * 4 if st.chunk_edges > 0 else 0)
-        if drop_scale is None:
-            _cabi.call("cogdl_b200_mhspmm_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att), _ptr(feat),
-                       _ptr(out), st.n_rows, H, F, plan, _stream(dev))
-        else:
-            _cabi.call("cogdl_b200_mhspmm_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att),
-                       _ptr(feat), float(drop_scale), _ptr(out), st.n_rows, H, F, plan, _stream(dev))
-        del keep
+    out = torch.empty((st.n_rows, H, F), dtype=torch.float32, device=dev)
+    need = _scratch("mhspmm", st, H, F)
+    if drop_scale is None:
+        _launch("cogdl_b200_mhspmm_f32", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att), _ptr(feat),
+                _ptr(out), st.n_rows, H, F)
+    else:
+        _launch("cogdl_b200_mhspmm_dropout_f32", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(perm), _ptr(att),
+                _ptr(feat), float(drop_scale), _ptr(out), st.n_rows, H, F)
     return out
 
 
@@ -200,12 +187,9 @@ def mhsddmm_raw(st: CSRStructure, grad, feat):
     dev = require_cuda(grad, feat)
     grad, feat = _f32c(grad, "grad"), _f32c(feat, "feat")
     H, F = feat.shape[1], feat.shape[2]
-    with torch.cuda.device(dev):
-        out = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(0)
-        _cabi.call("cogdl_b200_mhsddmm_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(grad), _ptr(feat), _ptr(out),
-                   st.n_rows, H, F, plan, _stream(dev))
-        del keep
+    out = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)
+    _launch("cogdl_b200_mhsddmm_f32", st, 0, _ptr(st.rowptr), _ptr(st.colind), _ptr(grad), _ptr(feat), _ptr(out),
+            st.n_rows, H, F)
     return out
 
 
@@ -213,13 +197,10 @@ def scatter_max_fwd_raw(st: CSRStructure, x):
     dev = require_cuda(x)
     x = _f32c(x, "feat")
     F = x.shape[1]
-    with torch.cuda.device(dev):
-        out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
-        arg = torch.empty((st.n_rows, F), dtype=torch.int32, device=dev)
-        plan, keep = st.plan_struct(st.plan.n_chunks * F * 8 if st.chunk_edges > 0 else 0)
-        _cabi.call("cogdl_b200_scatter_max_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(x), _ptr(out),
-                   _ptr(arg), st.n_rows, F, plan, _stream(dev))
-        del keep
+    out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+    arg = torch.empty((st.n_rows, F), dtype=torch.int32, device=dev)
+    _launch("cogdl_b200_scatter_max_fwd_f32", st, _scratch("scatter_max", st, F), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(x), _ptr(out), _ptr(arg), st.n_rows, F)
     return out, arg
 
 
@@ -248,19 +229,17 @@ def gat_fwd_raw(st: CSRStructure, h_l, h_r, feat, slope, want_att, drop=None):
     dev = require_cuda(h_l, h_r, feat)
     h_l, h_r, feat = _f32c(h_l, "attn_row"), _f32c(h_r, "attn_col"), _f32c(feat, "in_feat")
     H, F = feat.shape[1], feat.shape[2]
-    with torch.cuda.device(dev):
-        out = torch.empty((st.n_rows, H, F), dtype=torch.float32, device=dev)
-        att = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)   # output for training, scratch otherwise
-        plan, keep = st.plan_struct(max(st.plan.n_chunks * H * F * 4, _es_scratch(st, H)) if st.chunk_edges > 0 else 0)
-        if drop is None:
-            _cabi.call("cogdl_b200_gat_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r), _ptr(feat),
-                       float(slope), _ptr(out), _ptr(att), st.n_rows, H, F, plan, _stream(dev))
-        else:
-            seed, drop_below, scale = drop
-            _cabi.call("cogdl_b200_gat_fwd_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r),
-                       _ptr(feat), float(slope), int(seed), int(drop_below), float(scale), _ptr(out), _ptr(att),
-                       st.n_rows, H, F, plan, _stream(dev))
-        del keep
+    out = torch.empty((st.n_rows, H, F), dtype=torch.float32, device=dev)
+    att = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)   # output for training, scratch otherwise
+    need = _scratch("gat_fwd", st, H, F)
+    if drop is None:
+        _launch("cogdl_b200_gat_fwd_f32", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r), _ptr(feat),
+                float(slope), _ptr(out), _ptr(att), st.n_rows, H, F)
+    else:
+        seed, drop_below, scale = drop
+        _launch("cogdl_b200_gat_fwd_dropout_f32", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r),
+                _ptr(feat), float(slope), int(seed), int(drop_below), float(scale), _ptr(out), _ptr(att), st.n_rows, H,
+                F)
     return out, att
 
 
@@ -270,25 +249,22 @@ def gat_attn_bwd_raw(st: CSRStructure, att, d_att, h_l, h_r, slope, drop_scale=N
     dev = require_cuda(att, d_att, h_l, h_r)
     att, d_att, h_l, h_r = _f32c(att, "att"), _f32c(d_att, "d_att"), _f32c(h_l, "attn_row"), _f32c(h_r, "attn_col")
     H = att.shape[1]
-    with torch.cuda.device(dev):
-        d_edge = torch.empty_like(att)
-        g_row = torch.empty((st.n_rows, H), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(_es_scratch(st, H))
-        if drop_scale is None:
-            _cabi.call("cogdl_b200_gat_attn_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(att), _ptr(d_att),
-                       _ptr(h_l), _ptr(h_r), float(slope), _ptr(d_edge), _ptr(g_row), st.n_rows, H, plan, _stream(dev))
-        else:
-            _cabi.call("cogdl_b200_gat_attn_bwd_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(att), _ptr(d_att),
-                       _ptr(h_l), _ptr(h_r), float(slope), float(drop_scale), _ptr(d_edge), _ptr(g_row), st.n_rows,
-                       H, plan, _stream(dev))
-        del keep
+    d_edge = torch.empty_like(att)
+    g_row = torch.empty((st.n_rows, H), dtype=torch.float32, device=dev)
+    need = _scratch("edge_softmax", st, H)
+    if drop_scale is None:
+        _launch("cogdl_b200_gat_attn_bwd_f32", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(att), _ptr(d_att),
+                _ptr(h_l), _ptr(h_r), float(slope), _ptr(d_edge), _ptr(g_row), st.n_rows, H)
+    else:
+        _launch("cogdl_b200_gat_attn_bwd_dropout_f32", st, need, _ptr(st.rowptr), _ptr(st.colind), _ptr(att),
+                _ptr(d_att), _ptr(h_l), _ptr(h_r), float(slope), float(drop_scale), _ptr(d_edge), _ptr(g_row),
+                st.n_rows, H)
     return d_edge, g_row
 
 
 def _sa_scratch(st, F):
-    if st.chunk_edges <= 0:
-        return 0
-    return int(_cabi.load().cogdl_b200_softmax_aggr_scratch_bytes(st.plan.n_chunks, F))
+    """Plan scratch of the softmax aggregation's forward, which the GENConv edge encoder's forward shares."""
+    return _scratch("softmax_aggr", st, F)
 
 
 def _sa_check(st, x, beta, edge_term, n_x_rows):
@@ -316,14 +292,11 @@ def softmax_aggr_fwd_raw(st: CSRStructure, x, beta, eps, edge_term=None, want_ls
     dev = require_cuda(x)
     x, beta, edge_term = _sa_check(st, x, beta, edge_term, st.n_cols)
     F = x.shape[1]
-    with torch.cuda.device(dev):
-        out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
-        lse2 = torch.empty_like(out) if want_lse else None
-        q = torch.empty_like(out) if want_q else None
-        plan, keep = st.plan_struct(_sa_scratch(st, F))
-        _cabi.call("cogdl_b200_softmax_aggr_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(x), _ptr(edge_term),
-                   _ptr(beta), float(eps), _ptr(out), _ptr(lse2), _ptr(q), st.n_rows, F, plan, _stream(dev))
-        del keep
+    out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+    lse2 = torch.empty_like(out) if want_lse else None
+    q = torch.empty_like(out) if want_q else None
+    _launch("cogdl_b200_softmax_aggr_fwd_f32", st, _sa_scratch(st, F), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(x), _ptr(edge_term), _ptr(beta), float(eps), _ptr(out), _ptr(lse2), _ptr(q), st.n_rows, F)
     return out, lse2, q
 
 
@@ -337,14 +310,11 @@ def softmax_aggr_bwd_raw(st: CSRStructure, x, beta, eps, g, out, lse2, edge_term
         if t.shape != (st.n_rows, F):
             raise ValueError(f"{name} must be [{st.n_rows}, {F}], got {tuple(t.shape)}")
     st_t, perm = st.csc()
-    with torch.cuda.device(dev):
-        dx = torch.empty_like(x)
-        da = torch.empty_like(edge_term) if edge_term is not None and want_edge_grad else None
-        plan, keep = st_t.plan_struct(st_t.plan.n_chunks * F * 4 if st_t.chunk_edges > 0 else 0)
-        _cabi.call("cogdl_b200_softmax_aggr_bwd_f32", _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(x),
-                   _ptr(edge_term), _ptr(beta), float(eps), _ptr(g), _ptr(out), _ptr(lse2), _ptr(dx), _ptr(da),
-                   st_t.n_rows, F, plan, _stream(dev))
-        del keep
+    dx = torch.empty_like(x)
+    da = torch.empty_like(edge_term) if edge_term is not None and want_edge_grad else None
+    _launch("cogdl_b200_softmax_aggr_bwd_f32", st_t, _scratch("softmax_aggr_bwd", st_t, F), _ptr(st_t.rowptr),
+            _ptr(st_t.colind), _ptr(perm), _ptr(x), _ptr(edge_term), _ptr(beta), float(eps), _ptr(g), _ptr(out),
+            _ptr(lse2), _ptr(dx), _ptr(da), st_t.n_rows, F)
     return dx, da
 
 
@@ -373,15 +343,12 @@ def genconv_edge_fwd_raw(st: CSRStructure, x, attr, w, beta, eps, want_lse=False
     x, beta, _ = _sa_check(st, x, beta, None, st.n_cols)
     attr, w = _ge_check(st, x, attr, w)
     F = x.shape[1]
-    with torch.cuda.device(dev):
-        out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
-        lse2 = torch.empty_like(out) if want_lse else None
-        q = torch.empty_like(out) if want_q else None
-        plan, keep = st.plan_struct(_sa_scratch(st, F))
-        _cabi.call("cogdl_b200_genconv_edge_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(x), _ptr(attr), _ptr(w),
-                   attr.shape[1], _ptr(beta), float(eps), _ptr(out), _ptr(lse2), _ptr(q), st.n_rows, F, plan,
-                   _stream(dev))
-        del keep
+    out = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+    lse2 = torch.empty_like(out) if want_lse else None
+    q = torch.empty_like(out) if want_q else None
+    _launch("cogdl_b200_genconv_edge_fwd_f32", st, _sa_scratch(st, F), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(x), _ptr(attr), _ptr(w), attr.shape[1], _ptr(beta), float(eps), _ptr(out), _ptr(lse2), _ptr(q),
+            st.n_rows, F)
     return out, lse2, q
 
 
@@ -399,24 +366,14 @@ def genconv_edge_bwd_raw(st: CSRStructure, x, attr, w, beta, eps, g, out, lse2, 
     if not (want_dx or want_dw):
         return None, None
     st_t, perm = st.csc()
-    with torch.cuda.device(dev):
-        dx = torch.empty_like(x) if want_dx else None
-        dw = torch.empty((F, D), dtype=torch.float32, device=dev) if want_dw else None
-        n_scr = int(_cabi.load().cogdl_b200_genconv_edge_dw_scratch_bytes(F, D)) if want_dw else 0
-        scratch = torch.empty(n_scr // 4, dtype=torch.float32, device=dev) if want_dw else None
-        need = st_t.plan.n_chunks * F * 4 if st_t.chunk_edges > 0 and want_dx else 0
-        plan, keep = st_t.plan_struct(need)
-        _cabi.call("cogdl_b200_genconv_edge_bwd_f32", _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(x),
-                   _ptr(attr), _ptr(w), D, _ptr(beta), float(eps), _ptr(g), _ptr(out), _ptr(lse2), _ptr(dx), _ptr(dw),
-                   _ptr(scratch), n_scr, st_t.n_rows, F, plan, _stream(dev))
-        del keep
+    dx = torch.empty_like(x) if want_dx else None
+    dw = torch.empty((F, D), dtype=torch.float32, device=dev) if want_dw else None
+    n_scr = int(_cabi.load().cogdl_b200_genconv_edge_dw_scratch_bytes(F, D)) if want_dw else 0
+    scratch = torch.empty(n_scr // 4, dtype=torch.float32, device=dev) if want_dw else None
+    _launch("cogdl_b200_genconv_edge_bwd_f32", st_t, _scratch("genconv_edge_bwd", st_t, F, int(bool(want_dx))),
+            _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(x), _ptr(attr), _ptr(w), D, _ptr(beta), float(eps),
+            _ptr(g), _ptr(out), _ptr(lse2), _ptr(dx), _ptr(dw), _ptr(scratch), n_scr, st_t.n_rows, F)
     return dx, dw
-
-
-def _dr_scratch(st, F, K):
-    if st.chunk_edges <= 0:
-        return 0
-    return int(_cabi.load().cogdl_b200_disen_route_scratch_bytes(st.plan.n_chunks, F, K))
 
 
 def _dr_check(st, K, **feats):
@@ -443,14 +400,11 @@ def disen_route_fwd_raw(st: CSRStructure, q, c, K, tau, want_saved=False):
     dev = require_cuda(q, c)
     (q, c), F = _dr_check(st, K, q=q, c=c)
     n = st.n_rows
-    with torch.cuda.device(dev):
-        out = torch.empty((n, F), dtype=torch.float32, device=dev)
-        lse2 = torch.empty((n, K), dtype=torch.float32, device=dev) if want_saved else None
-        r = torch.empty_like(lse2) if want_saved else None
-        plan, keep = st.plan_struct(_dr_scratch(st, F, K))
-        _cabi.call("cogdl_b200_disen_route_fwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(q), _ptr(c), _ptr(out),
-                   _ptr(lse2), _ptr(r), n, st.n_cols, F, K, float(tau), plan, _stream(dev))
-        del keep
+    out = torch.empty((n, F), dtype=torch.float32, device=dev)
+    lse2 = torch.empty((n, K), dtype=torch.float32, device=dev) if want_saved else None
+    r = torch.empty_like(lse2) if want_saved else None
+    _launch("cogdl_b200_disen_route_fwd_f32", st, _scratch("disen_route", st, F, K), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(q), _ptr(c), _ptr(out), _ptr(lse2), _ptr(r), n, st.n_cols, F, K, float(tau))
     return out, lse2, r
 
 
@@ -468,8 +422,8 @@ def disen_route_bwd_raw(st: CSRStructure, q, c, K, tau, g, out, lse2, r):
     with torch.cuda.device(dev):
         dq, dc, gu = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
         D = torch.empty_like(lse2)
-        plan, keep = st.plan_struct(_dr_scratch(st, F, K))
-        plan_t, keep_t = st_t.plan_struct(_dr_scratch(st_t, F, K))
+        plan, keep = st.plan_struct(_scratch("disen_route", st, F, K))
+        plan_t, keep_t = st_t.plan_struct(_scratch("disen_route", st_t, F, K))
         _cabi.call("cogdl_b200_disen_route_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), plan, _ptr(st_t.rowptr),
                    _ptr(st_t.colind), plan_t, _ptr(q), _ptr(c), _ptr(g), _ptr(out), _ptr(lse2), _ptr(r), _ptr(gu),
                    _ptr(D), _ptr(dq), _ptr(dc), n, st.n_cols, F, K, float(tau), _stream(dev))
@@ -482,12 +436,9 @@ def edge_colsum_raw(st_t: CSRStructure, perm, e):
     dev = require_cuda(perm, e)
     e = _f32c(e, "edge values")
     H = e.shape[1]
-    with torch.cuda.device(dev):
-        out = torch.empty((st_t.n_rows, H), dtype=torch.float32, device=dev)
-        plan, keep = st_t.plan_struct(st_t.plan.n_chunks * H * 4 if st_t.chunk_edges > 0 else 0)
-        _cabi.call("cogdl_b200_edge_colsum_f32", _ptr(st_t.rowptr), _ptr(perm), _ptr(e), _ptr(out), st_t.n_rows, H, plan,
-                   _stream(dev))
-        del keep
+    out = torch.empty((st_t.n_rows, H), dtype=torch.float32, device=dev)
+    _launch("cogdl_b200_edge_colsum_f32", st_t, _scratch("edge_colsum", st_t, H), _ptr(st_t.rowptr), _ptr(perm), _ptr(e),
+            _ptr(out), st_t.n_rows, H)
     return out
 
 
@@ -512,33 +463,27 @@ def comp_aggr_raw(st: CSRStructure, idx2, w, a, b, op):
         raise ValueError(f"per-slot arrays must have {st.nnz} entries")
     if two and idx2.dtype != torch.int32:
         raise TypeError(f"idx2 must be int32, got {idx2.dtype}")
-    with torch.cuda.device(dev):
-        if st.nnz == 0:
-            return torch.zeros((st.n_rows, F), dtype=torch.float32, device=dev)
-        y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
-        need = int(_cabi.load().cogdl_b200_comp_aggr_scratch_bytes(st.plan.n_chunks, F))
-        plan, keep = st.plan_struct(need)
-        _cabi.call("cogdl_b200_comp_aggr_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(idx2.contiguous() if two else None),
-                   _ptr(w), _ptr(a), a.shape[0], _ptr(b), b.shape[0] if two else 0, _ptr(y), st.n_rows, F,
-                   _cabi.COMP_OPS[op], plan, _stream(dev))
-        del keep
+    if st.nnz == 0:
+        return torch.zeros((st.n_rows, F), dtype=torch.float32, device=dev)
+    y = torch.empty((st.n_rows, F), dtype=torch.float32, device=dev)
+    _launch("cogdl_b200_comp_aggr_f32", st, _scratch("comp_aggr", st, F), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(idx2.contiguous() if two else None), _ptr(w), _ptr(a), a.shape[0], _ptr(b), b.shape[0] if two else 0,
+            _ptr(y), st.n_rows, F, _cabi.COMP_OPS[op])
     return y
 
 
 def spmm_residual_dcoef_raw(st: CSRStructure, val, x, z, a, b_dev, row_scale=None, panels=0):
     """Y = a * (row_scale[:, None] * (A @ x)) + b * z with b = b_dev[0], a one-element fp32 tensor on x's device that
     the kernel reads (no host synchronisation); otherwise as spmm_residual_raw.  z may be None (b_dev is then unused)."""
-    dev, val, x, z, row_scale = _epilogue_args(st, val, x, z, row_scale)
+    _, val, x, z, row_scale = _epilogue_args(st, val, x, z, row_scale)
     require_cuda(x, b_dev)
     b_dev = _f32c(b_dev, "b_dev").view(-1)
     if b_dev.numel() != 1:
         raise ValueError(f"b_dev must hold one value, got {b_dev.numel()}")
-    with torch.cuda.device(dev):
-        y, plan, keep = _spmm_out(st, val, x)
-        _cabi.call("cogdl_b200_spmm_residual_dcoef_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x),
-                   x.shape[0], _ptr(z), float(a), _ptr(b_dev), _ptr(row_scale), _ptr(y), st.n_rows, x.shape[1],
-                   int(panels), plan, _stream(dev))
-        del keep
+    y = _spmm_out(st, val, x)
+    _launch("cogdl_b200_spmm_residual_dcoef_f32", st, _scratch("spmm", st, x.shape[1]), _ptr(st.rowptr),
+            _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0], _ptr(z), float(a), _ptr(b_dev), _ptr(row_scale), _ptr(y),
+            st.n_rows, x.shape[1], int(panels))
     return y
 
 
@@ -548,17 +493,15 @@ def spmm_accum_raw(st: CSRStructure, val, x, acc, acc_in=None, row_scale=None, l
     acc = acc_in + xn (acc_in None: acc itself), then acc * scale when last.  x [n_src, F], acc and acc_in [n_rows, F],
     row_scale [n_rows], all fp32; scale is rounded to fp32.  xn: a preallocated [n_rows, F] fp32 output, allocated when
     None and not last.  Returns xn (None when last)."""
-    dev, val, x, acc_in, row_scale = _epilogue_args(st, val, x, acc_in, row_scale)
+    _, val, x, acc_in, row_scale = _epilogue_args(st, val, x, acc_in, row_scale)
     require_cuda(x, acc, xn)
     for name, t in (("acc", acc), ("xn", xn)):
         if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.shape != (st.n_rows, x.shape[1])):
             raise ValueError(f"{name} must be a contiguous float32 [{st.n_rows}, {x.shape[1]}] tensor")
-    with torch.cuda.device(dev):
-        out, plan, keep = _spmm_out(st, val, x, acc if last else xn)   # acc: nothing to allocate on the last hop
-        _cabi.call("cogdl_b200_spmm_accum_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), x.shape[0],
-                   _ptr(row_scale), _ptr(acc_in), _ptr(acc), int(bool(last)), float(scale), _ptr(None if last else out),
-                   st.n_rows, x.shape[1], int(panels), plan, _stream(dev))
-        del keep
+    out = _spmm_out(st, val, x, acc if last else xn)   # acc: nothing to allocate on the last hop
+    _launch("cogdl_b200_spmm_accum_f32", st, _scratch("spmm", st, x.shape[1]), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(val), _ptr(x), x.shape[0], _ptr(row_scale), _ptr(acc_in), _ptr(acc), int(bool(last)), float(scale),
+            _ptr(None if last else out), st.n_rows, x.shape[1], int(panels))
     return None if last else out
 
 
@@ -583,15 +526,11 @@ def rgcn_aggr_raw(st: CSRStructure, etype, w, coef, x, per_basis=False):
         raise ValueError(f"per-slot arrays must have {st.nnz} entries")
     if etype.dtype != torch.int32:
         raise TypeError(f"etype must be int32, got {etype.dtype}")
-    with torch.cuda.device(dev):
-        if st.nnz == 0:
-            return torch.zeros((st.n_rows, B, F), dtype=torch.float32, device=dev)
-        y = torch.empty((st.n_rows, B, F), dtype=torch.float32, device=dev)
-        need = int(_cabi.load().cogdl_b200_rgcn_aggr_scratch_bytes(st.plan.n_chunks, B, F))
-        plan, keep = st.plan_struct(need)
-        _cabi.call("cogdl_b200_rgcn_aggr_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(etype.contiguous()), _ptr(w),
-                   _ptr(coef), B, _ptr(x), int(bool(per_basis)), _ptr(y), st.n_rows, F, plan, _stream(dev))
-        del keep
+    if st.nnz == 0:
+        return torch.zeros((st.n_rows, B, F), dtype=torch.float32, device=dev)
+    y = torch.empty((st.n_rows, B, F), dtype=torch.float32, device=dev)
+    _launch("cogdl_b200_rgcn_aggr_f32", st, _scratch("rgcn_aggr", st, B, F), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(etype.contiguous()), _ptr(w), _ptr(coef), B, _ptr(x), int(bool(per_basis)), _ptr(y), st.n_rows, F)
     return y
 
 
@@ -605,14 +544,11 @@ def rgcn_edge_dot_raw(st: CSRStructure, w, g, x):
     if w.numel() != st.nnz:
         raise ValueError(f"w must have {st.nnz} entries")
     B, F = g.shape[1], g.shape[2]
-    with torch.cuda.device(dev):
-        p = torch.empty((st.nnz, B), dtype=torch.float32, device=dev)
-        if st.nnz == 0:
-            return p
-        plan, keep = st.plan_struct(0)
-        _cabi.call("cogdl_b200_rgcn_edge_dot_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(w), _ptr(g), _ptr(x), _ptr(p),
-                   st.n_rows, B, F, plan, _stream(dev))
-        del keep
+    p = torch.empty((st.nnz, B), dtype=torch.float32, device=dev)
+    if st.nnz == 0:
+        return p
+    _launch("cogdl_b200_rgcn_edge_dot_f32", st, 0, _ptr(st.rowptr), _ptr(st.colind), _ptr(w), _ptr(g), _ptr(x), _ptr(p),
+            st.n_rows, B, F)
     return p
 
 
@@ -648,14 +584,11 @@ def hgn_attn_raw(st: CSRStructure, etype, h_l, h_r, h_e, slope, want_att, drop=N
         if res_attn.shape != (st.nnz, H):
             raise ValueError(f"res_attn must be [nnz={st.nnz}, H={H}], got {tuple(res_attn.shape)}")
     seed, drop_below, scale = (0, 0, 1.0) if drop is None else drop
-    with torch.cuda.device(dev):
-        mix = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)
-        att = torch.empty_like(mix) if want_att else None
-        plan, keep = st.plan_struct(_es_scratch(st, H))
-        _cabi.call("cogdl_b200_hgn_attn_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(etype), _ptr(h_l), _ptr(h_r),
-                   _ptr(h_e), h_e.shape[0], float(slope), int(seed), int(drop_below), float(scale), _ptr(res_attn),
-                   float(alpha), _ptr(att), _ptr(mix), st.n_rows, H, plan, _stream(dev))
-        del keep
+    mix = torch.empty((st.nnz, H), dtype=torch.float32, device=dev)
+    att = torch.empty_like(mix) if want_att else None
+    _launch("cogdl_b200_hgn_attn_f32", st, _scratch("edge_softmax", st, H), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(etype), _ptr(h_l), _ptr(h_r), _ptr(h_e), h_e.shape[0], float(slope), int(seed), int(drop_below),
+            float(scale), _ptr(res_attn), float(alpha), _ptr(att), _ptr(mix), st.n_rows, H)
     return mix, att
 
 
@@ -666,12 +599,9 @@ def hgn_attn_bwd_raw(st: CSRStructure, etype, att, d_mix, h_l, h_r, h_e, slope, 
     att, d_mix, h_l, h_r = _f32c(att, "att"), _f32c(d_mix, "d_mix"), _f32c(h_l, "h_l"), _f32c(h_r, "h_r")
     H = att.shape[1]
     etype, h_e = _hgn_table(st, etype, h_e, H)
-    with torch.cuda.device(dev):
-        d_edge = torch.empty_like(att)
-        g_row = torch.empty((st.n_rows, H), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(_es_scratch(st, H))
-        _cabi.call("cogdl_b200_hgn_attn_bwd_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(etype), _ptr(att),
-                   _ptr(d_mix), _ptr(h_l), _ptr(h_r), _ptr(h_e), h_e.shape[0], float(slope), float(grad_scale),
-                   _ptr(d_edge), _ptr(g_row), st.n_rows, H, plan, _stream(dev))
-        del keep
+    d_edge = torch.empty_like(att)
+    g_row = torch.empty((st.n_rows, H), dtype=torch.float32, device=dev)
+    _launch("cogdl_b200_hgn_attn_bwd_f32", st, _scratch("edge_softmax", st, H), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(etype), _ptr(att), _ptr(d_mix), _ptr(h_l), _ptr(h_r), _ptr(h_e), h_e.shape[0], float(slope),
+            float(grad_scale), _ptr(d_edge), _ptr(g_row), st.n_rows, H)
     return d_edge, g_row

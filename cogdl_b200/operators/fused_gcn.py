@@ -8,8 +8,8 @@ against an fp64 evaluation instead of being bit-matched.  Kernel: cogdl_b200/csr
 import torch
 
 from .. import _cabi
-from ..structure import CSRStructure, _ptr, _stream, graph_operands, require_cuda
-from ._raw import _spmm_scratch, spmm_adjoint_raw, spmm_raw
+from ..structure import CSRStructure, _ptr, graph_operands, require_cuda
+from ._raw import _launch, _scratch, spmm_adjoint_raw, spmm_raw
 
 
 def supported(K, Fout):
@@ -46,14 +46,11 @@ def fused_gcn_raw(st: CSRStructure, val, x, weight, bias=None, relu=False, cache
     bias = None if bias is None else bias.contiguous().float()
     if st.nnz == 0:        # no edge anywhere: A = 0, so (A.X).W^T + (A.1) b^T = 0 and act(0) = 0 for ReLU / identity
         return torch.zeros((st.n_rows, Fout), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        out = torch.empty((st.n_rows, Fout), dtype=torch.float32, device=dev)
-        plan, keep = st.plan_struct(_spmm_scratch(st, K))
-        hub = torch.empty((st.n_rows, K), dtype=torch.float32, device=dev) if st.plan.n_chunks > 0 else None
-        rowsum = cached_rowsum(st, val) if (cache_rowsum and val is not None and bias is not None) else None
-        _cabi.call("cogdl_b200_gcn_fused_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(x), _ptr(weight), _ptr(bias),
-                   _ptr(rowsum), _ptr(out), _ptr(hub), st.n_rows, K, Fout, int(bool(relu)), plan, _stream(dev))
-        del keep, hub
+    out = torch.empty((st.n_rows, Fout), dtype=torch.float32, device=dev)
+    hub = torch.empty((st.n_rows, K), dtype=torch.float32, device=dev) if st.plan.n_chunks > 0 else None
+    rowsum = cached_rowsum(st, val) if (cache_rowsum and val is not None and bias is not None) else None
+    _launch("cogdl_b200_gcn_fused_f32", st, _scratch("gcn_fused", st, K), _ptr(st.rowptr), _ptr(st.colind), _ptr(val),
+            _ptr(x), _ptr(weight), _ptr(bias), _ptr(rowsum), _ptr(out), _ptr(hub), st.n_rows, K, Fout, int(bool(relu)))
     return out
 
 

@@ -11,9 +11,8 @@ aggregation, only the GEMM rounds differently (bf16x3 split, ~1e-7 of the row sc
 import torch
 import torch.nn.functional as F
 
-from .. import _cabi
-from ..structure import CSRStructure, _ptr, _stream, graph_operands, require_cuda
-from ._raw import scatter_max_bwd_raw, scatter_max_fwd_raw, spmm_adjoint_raw, spmm_raw
+from ..structure import CSRStructure, _ptr, graph_operands, require_cuda
+from ._raw import _launch, _scratch, scatter_max_bwd_raw, scatter_max_fwd_raw, spmm_adjoint_raw, spmm_raw
 from .fused_gcn import supported
 
 AGGR = {"sum": 0, "max": 1}     # COGDL_B200_AGGR_SUM / _MAX; mean is "sum" with row-normalised weights or row_scale
@@ -49,14 +48,11 @@ def fused_sage_raw(st: CSRStructure, val, row_scale, x, weight, bias=None, aggr=
     if st.nnz == 0:          # no edge anywhere: agg = 0 for sum and max
         return torch.relu(S) if relu else S
     w_neigh = weight[:, K:].contiguous()
-    with torch.cuda.device(dev):
-        out = torch.empty((n, Fout), dtype=torch.float32, device=dev)
-        elem = 8 if aggr == "max" else 4                              # max partials carry (value, argmax)
-        plan, keep = st.plan_struct(st.plan.n_chunks * K * elem)
-        hub = torch.empty((n, K), dtype=torch.float32, device=dev) if st.plan.n_chunks > 0 else None
-        _cabi.call("cogdl_b200_sage_fused_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(val), _ptr(row_scale), _ptr(x),
-                   _ptr(w_neigh), _ptr(S), _ptr(out), _ptr(hub), n, K, Fout, AGGR[aggr], int(bool(relu)), plan, _stream(dev))
-        del keep, hub
+    out = torch.empty((n, Fout), dtype=torch.float32, device=dev)
+    hub = torch.empty((n, K), dtype=torch.float32, device=dev) if st.plan.n_chunks > 0 else None
+    _launch("cogdl_b200_sage_fused_f32", st, _scratch("sage_fused", st, K, AGGR[aggr]), _ptr(st.rowptr), _ptr(st.colind),
+            _ptr(val), _ptr(row_scale), _ptr(x), _ptr(w_neigh), _ptr(S), _ptr(out), _ptr(hub), n, K, Fout, AGGR[aggr],
+            int(bool(relu)))
     return out
 
 

@@ -14,7 +14,7 @@ import torch
 
 from .. import _cabi
 from ..structure import _ptr, _stream, graph_operands, require_cuda, unsupported_operands
-from ._raw import _epilogue_args, _spmm_epilogue_raw, _spmm_out
+from ._raw import _epilogue_args, _scratch, _spmm_epilogue_raw, _spmm_out
 
 
 def label_prop_raw(st, val, x, z, a, b, row_scale=None, pin=None, clamp=None, panels=0, out=None):
@@ -70,7 +70,8 @@ def label_propagate(graph, labels, alpha, nprop, lower=None, upper=None, pinned=
     n, F = labels.shape
     step = _cabi.load().cogdl_b200_label_prop_f32
     with torch.cuda.device(dev):
-        y, plan, keep = _spmm_out(st, val, labels)
+        y = _spmm_out(st, val, labels)
+        plan, keep = st.plan_struct(_scratch("spmm", st, F))
         bufs = (y, torch.empty_like(y))
         stream = _stream(dev)
         x = labels

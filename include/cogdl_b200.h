@@ -73,8 +73,8 @@ COGDL_B200_API const char *cogdl_b200_last_kernel(void);
  *                               zero on entry; left zero on exit (arrival counters; the panel form of
  *                               the SpMM keeps one set of n_chunks per column panel)
  *   partials                    scratch for per-chunk partial results; `partials_bytes` capacity.
- *                               needs n_chunks*F*4 bytes (SpMM, mh-SpMM: F := H*F) or
- *                               n_chunks*F*8 bytes (scatter_max: value + argmax).
+ *                               Each entry point below names the cogdl_b200_*_scratch_bytes query
+ *                               that gives its need (COGDL_B200_ESCRATCH when it is not met).
  * counters/partials are per-stream scratch: do not share one plan between concurrent streams.
  * Partial results of a hub row are combined in chunk order by the last chunk to finish, so
  * results are deterministic run to run.
@@ -134,7 +134,10 @@ COGDL_B200_API int cogdl_b200_edge_rows(const int32_t *rowptr, int64_t n_rows, i
  * X is [n_src, F], Y is [n_rows, F]; colind values index rows of X.  Rows not split by a hub
  * plan are accumulated in CSR order with separate fp32 multiply and add, i.e. bit-identical
  * to the reference CPU SpMM (spmm_cpu.cpp:24-36).
+ * Every SpMM entry below (fp32, fp16, residual, label propagation, device coefficient, accumulating,
+ * two-source and peer forms) needs cogdl_b200_spmm_scratch_bytes(plan->n_chunks, F) bytes of plan->partials.
  * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_spmm_scratch_bytes(int64_t n_chunks, int64_t F);
 COGDL_B200_API int cogdl_b200_spmm_csr_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
                             const float *X, float *Y, int64_t n_rows, int64_t F,
                             const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
@@ -266,9 +269,7 @@ COGDL_B200_API int cogdl_b200_gather_rows_f32(const int32_t *perm, const float *
  * fwd: out = exp(in - max_row) / sum_row exp(in - max_row).  bwd: gin = y * (g - sum_row y*g).
  * Degree-0 rows own no entries, so nothing is written for them.
  * ------------------------------------------------------------------------------------- */
-/* With a hub plan that has hub rows, the calls below (and the GAT attention stages) need per-call scratch
- * in plan->partials: at least cogdl_b200_edge_softmax_scratch_bytes(plan->n_chunks, H) bytes (per hub
- * chunk and head: a (max, sum) pair for the two-pass split-row softmax + one partial row sum). */
+/* The calls below need cogdl_b200_edge_softmax_scratch_bytes(plan->n_chunks, H) bytes of plan->partials. */
 COGDL_B200_API int64_t cogdl_b200_edge_softmax_scratch_bytes(int64_t n_chunks, int64_t H);
 COGDL_B200_API int cogdl_b200_edge_softmax_fwd_f32(const int32_t *rowptr, const float *in, float *out,
                                     int64_t n_rows, int64_t H,
@@ -283,7 +284,9 @@ COGDL_B200_API int cogdl_b200_edge_softmax_bwd_f32(const int32_t *rowptr, const 
  *           (kernels mhspmmSimple / mhspmm_1           .../spmm/multiheadSpmm.cu:6-51)
  * feat/out are [n, H, F]; att is [nnz, H].  `perm` fuses the backward's mhtranspose
  * (mhspmm.py:60-61) into the CSC pass.  Accumulation order/rounding as for SpMM.
+ * plan->partials: cogdl_b200_mhspmm_scratch_bytes(plan->n_chunks, H, F) bytes (also for _dropout_f32).
  * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_mhspmm_scratch_bytes(int64_t n_chunks, int64_t H, int64_t F);
 COGDL_B200_API int cogdl_b200_mhspmm_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *perm,
                           const float *att, const float *feat, float *out, int64_t n_rows,
                           int64_t H, int64_t F, const cogdl_b200_hub_plan_t *plan,
@@ -307,7 +310,9 @@ COGDL_B200_API int cogdl_b200_mhsddmm_f32(const int32_t *rowptr, const int32_t *
  *      reference whenever every row has a neighbour value > FLT_MIN.
  * bwd: gx[argmax[i,f], f] += g[i,f]; gx [n_src, F] is zero-filled by the call (the reference
  *      forgets to, scatter_max.cu:70); argmax < 0 is skipped.
+ * fwd plan->partials: cogdl_b200_scatter_max_scratch_bytes(plan->n_chunks, F) bytes.
  * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_scatter_max_scratch_bytes(int64_t n_chunks, int64_t F);
 COGDL_B200_API int cogdl_b200_scatter_max_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
                                    float *out, int32_t *argmax, int64_t n_rows, int64_t F,
                                    const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
@@ -324,7 +329,9 @@ COGDL_B200_API int cogdl_b200_scatter_max_bwd_f32(const float *g, const int32_t 
  * saved tensor of the backward and the operand of the row-stream multi-head SpMM that follows).
  * Replaces the unfused chain cogdl/layers/gat_layer.py:73-77 and the stale dgNN binding
  * cogdl/operators/fused_gat.py:17-19.
+ * plan->partials: cogdl_b200_gat_fwd_scratch_bytes(plan->n_chunks, H, F) bytes (also for _dropout_f32).
  * ------------------------------------------------------------------------------------- */
+COGDL_B200_API int64_t cogdl_b200_gat_fwd_scratch_bytes(int64_t n_chunks, int64_t H, int64_t F);
 COGDL_B200_API int cogdl_b200_gat_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *h_l,
                            const float *h_r, const float *feat, float negative_slope, float *out,
                            float *att_out, int64_t n_rows, int64_t H, int64_t F,
@@ -336,15 +343,17 @@ COGDL_B200_API int cogdl_b200_gat_fwd_f32(const int32_t *rowptr, const int32_t *
  *   d_edge[p,h] = att*(d_att - sum_row att*d_att) * leakyrelu'(h_l[row,h] + h_r[col,h])   [nnz,H]
  *   g_row[i,h]  = sum_{p in row i} d_edge[p,h]                                            [n_rows,H]
  * d_att is the multi-head SDDMM of (d out, feat).  g_col = cogdl_b200_edge_colsum_f32 over the transpose.
- * Scratch in plan->partials as for the edge softmax. */
+ * plan->partials: cogdl_b200_edge_softmax_scratch_bytes(plan->n_chunks, H) bytes (also for _dropout_f32). */
 COGDL_B200_API int cogdl_b200_gat_attn_bwd_f32(const int32_t *rowptr, const int32_t *colind, const float *att,
                                 const float *d_att, const float *h_l, const float *h_r, float negative_slope,
                                 float *d_edge, float *g_row, int64_t n_rows, int64_t H,
                                 const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream);
 /* out[j,h] = sum_{q in column j of the transpose} e[perm[q], h]: column sums of an edge-aligned [nnz,H]
- * tensor through the cached CSC (colptr, perm).  Deterministic (no atomics; hub columns via the plan's chunks). */
+ * tensor through the cached CSC (colptr, perm).  Deterministic (no atomics; hub columns via the plan's chunks).
+ * plan is the transpose's; its partials need cogdl_b200_edge_colsum_scratch_bytes(plan->n_chunks, H) bytes. */
+COGDL_B200_API int64_t cogdl_b200_edge_colsum_scratch_bytes(int64_t n_chunks, int64_t H);
 COGDL_B200_API int cogdl_b200_edge_colsum_f32(const int32_t *colptr, const int32_t *perm, const float *e, float *out,
-                               int64_t n_cols, int64_t H, const cogdl_b200_hub_plan_t *plan /* of the transpose; scratch n_chunks*H*4 B */,
+                               int64_t n_cols, int64_t H, const cogdl_b200_hub_plan_t *plan,
                                cogdl_b200_stream_t stream);
 
 /* GAT with attention dropout (the nn.Dropout between edge_softmax and mh_spmm in cogdl/layers/gat_layer.py:73-77).
@@ -381,11 +390,12 @@ COGDL_B200_API int cogdl_b200_gat_attn_bwd_dropout_f32(const int32_t *rowptr, co
  * scale.  X [n_src,K], W [Fout,K] (torch.nn.Linear.weight layout), bias [Fout] or NULL, out [n_rows,Fout].
  * Needs K == 128, Fout <= 128 (cogdl_b200_gcn_fused_supported), a hub plan with edge_row, 16-byte aligned
  * X / W / out.  hub_agg: scratch [n_rows, K] fp32, required iff the plan has hub rows (only those rows are
- * written); plan->partials as for cogdl_b200_spmm_csr_f32 (n_chunks*K*4 bytes).  rowsum: optional [n_rows]
+ * written); plan->partials: cogdl_b200_gcn_fused_scratch_bytes(n_chunks, K) bytes.  rowsum: optional [n_rows]
  * = A.1 (sum of each row's edge values), worth caching when the edge weights are fixed (GCN); NULL =>
  * the kernel sums the weights itself (one warp per hub row: slow on 10^4-edge hubs).
  * ------------------------------------------------------------------------------------- */
 COGDL_B200_API int cogdl_b200_gcn_fused_supported(int64_t K, int64_t Fout);
+COGDL_B200_API int64_t cogdl_b200_gcn_fused_scratch_bytes(int64_t n_chunks, int64_t K);
 COGDL_B200_API int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X,
                              const float *W, const float *bias, const float *rowsum, float *out, float *hub_agg, int64_t n_rows,
                              int64_t K, int64_t Fout, int32_t relu, const cogdl_b200_hub_plan_t *plan,
@@ -406,11 +416,12 @@ COGDL_B200_API int cogdl_b200_gcn_fused_f32(const int32_t *rowptr, const int32_t
  * The dense product is the bf16x3 wgmma of cogdl_b200_gcn_fused_f32 (~1e-7 of the row scale vs fp64).
  * X [n_src,K], W_neigh [Fout,K] contiguous, S and out [n_rows,Fout]; constraints as cogdl_b200_gcn_fused_f32
  * (cogdl_b200_gcn_fused_supported, hub plan with edge_row, 16-byte aligned X / W_neigh / S / out).
- * hub_agg: scratch [n_rows, K] fp32, required iff the plan has hub rows.  plan->partials: n_chunks*K*4
- * bytes for sum, n_chunks*K*8 for max.
+ * hub_agg: scratch [n_rows, K] fp32, required iff the plan has hub rows.  plan->partials:
+ * cogdl_b200_sage_fused_scratch_bytes(n_chunks, K, aggr) bytes.
  * ------------------------------------------------------------------------------------- */
 #define COGDL_B200_AGGR_SUM 0
 #define COGDL_B200_AGGR_MAX 1
+COGDL_B200_API int64_t cogdl_b200_sage_fused_scratch_bytes(int64_t n_chunks, int64_t K, int32_t aggr);
 COGDL_B200_API int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_t *colind, const float *val,
                               const float *row_scale, const float *X, const float *W_neigh, const float *S, float *out,
                               float *hub_agg, int64_t n_rows, int64_t K, int64_t Fout, int32_t aggr, int32_t relu,
@@ -427,7 +438,7 @@ COGDL_B200_API int cogdl_b200_sage_fused_f32(const int32_t *rowptr, const int32_
  *   Q[i,f]    = sum_e w_e m_e^2                   (d out / d beta = Q - out^2)
  * Any F >= 1; 16-byte vectors when F % 4 == 0 and every buffer is 16-byte aligned.  Hub rows are cut into the
  * plan's chunks and merged in chunk order (no float atomics: bit-reproducible).  plan->partials needs
- * n_chunks*F*12 bytes (16 with Q); cogdl_b200_softmax_aggr_scratch_bytes covers both directions.
+ * cogdl_b200_softmax_aggr_scratch_bytes(n_chunks, F) bytes.
  * ------------------------------------------------------------------------------------- */
 COGDL_B200_API int64_t cogdl_b200_softmax_aggr_scratch_bytes(int64_t n_chunks, int64_t F);
 COGDL_B200_API int cogdl_b200_softmax_aggr_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
@@ -438,8 +449,10 @@ COGDL_B200_API int cogdl_b200_softmax_aggr_fwd_f32(const int32_t *rowptr, const 
  * the forward's out and lse2:
  *   dpre_e = G[i] w_e (1 + beta (m_e - out[i])) [X[j] + edge_term[e] > 0]
  *   dX[j] = sum_{e: c_e = j} dpre_e  (transpose order; hub columns through `plan`, the TRANSPOSE's plan, whose
- *           partials need n_chunks*F*4 bytes)            d_edge_term[e] = dpre_e  (optional, needs edge_term)
+ *           partials need cogdl_b200_softmax_aggr_bwd_scratch_bytes(n_chunks, F) bytes)
+ *   d_edge_term[e] = dpre_e  (optional, needs edge_term)
  * perm is needed only with an edge term.  d beta = sum G (Q - out^2) is left to the caller. */
+COGDL_B200_API int64_t cogdl_b200_softmax_aggr_bwd_scratch_bytes(int64_t n_chunks, int64_t F);
 COGDL_B200_API int cogdl_b200_softmax_aggr_bwd_f32(const int32_t *colptr, const int32_t *rowind, const int32_t *perm,
                                     const float *X, const float *edge_term, const float *beta, float eps,
                                     const float *G, const float *out, const float *lse2, float *dX,
@@ -452,8 +465,8 @@ COGDL_B200_API int cogdl_b200_softmax_aggr_bwd_f32(const int32_t *colptr, const 
  *   edge_term[e,f] = sum_{d=0..D-1} attr[e,d] W[f,d]   (one fmaf chain, d ascending)
  * and otherwise the operation of cogdl_b200_softmax_aggr_fwd_f32 / _bwd_f32, with the same work items, hub plan,
  * chunk-order merge and lse2 / Q outputs.  attr is [nnz, D] fp32 in CSR order, W is [F, D] fp32 (nn.Linear layout),
- * 1 <= D <= 16 (wider D is rejected).  The forward's plan->partials needs what cogdl_b200_softmax_aggr_scratch_bytes
- * gives.  When F is a multiple of 4, 16-byte vectors if X, out, lse2, Q (and G, dX, the partials) are aligned.
+ * 1 <= D <= 16 (wider D is rejected).  The forward's plan->partials needs cogdl_b200_softmax_aggr_scratch_bytes(n_chunks,
+ * F) bytes.  When F is a multiple of 4, 16-byte vectors if X, out, lse2, Q (and G, dX, the partials) are aligned.
  * ------------------------------------------------------------------------------------- */
 COGDL_B200_API int cogdl_b200_genconv_edge_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *X,
                                                    const float *attr, const float *W, int64_t D, const float *beta,
@@ -461,7 +474,8 @@ COGDL_B200_API int cogdl_b200_genconv_edge_fwd_f32(const int32_t *rowptr, const 
                                                    int64_t F, const cogdl_b200_hub_plan_t *plan,
                                                    cogdl_b200_stream_t stream);
 /* Backward over the transpose (colptr, rowind, perm; n_cols columns; `plan` is the TRANSPOSE's plan, partials
- * n_chunks*F*4 bytes when dX is asked for), given G = dL/dout and the forward's out and lse2:
+ * cogdl_b200_genconv_edge_bwd_scratch_bytes(n_chunks, F, dX != NULL) bytes), given G = dL/dout and the forward's out
+ * and lse2:
  *   dX[j]    = sum_{e: c_e = j} dpre_e             (as cogdl_b200_softmax_aggr_bwd_f32; NULL: not computed)
  *   dW[f,d]  = sum_e dpre_e[f] attr[e,d]           ([F, D]; NULL: not computed)
  * dW is summed without float atomics: per warp over a fixed, static assignment of work items, then per block in warp
@@ -469,6 +483,7 @@ COGDL_B200_API int cogdl_b200_genconv_edge_fwd_f32(const int32_t *rowptr, const 
  * dw_scratch must hold cogdl_b200_genconv_edge_dw_scratch_bytes(F, D) bytes (a bound independent of nnz).  At least
  * one of dX, dW.  d beta = sum G (Q - out^2) is left to the caller. */
 COGDL_B200_API int64_t cogdl_b200_genconv_edge_dw_scratch_bytes(int64_t F, int64_t D);
+COGDL_B200_API int64_t cogdl_b200_genconv_edge_bwd_scratch_bytes(int64_t n_chunks, int64_t F, int32_t want_dx);
 COGDL_B200_API int cogdl_b200_genconv_edge_bwd_f32(const int32_t *colptr, const int32_t *rowind, const int32_t *perm,
                                                    const float *X, const float *attr, const float *W, int64_t D,
                                                    const float *beta, float eps, const float *G, const float *out,
@@ -488,7 +503,7 @@ COGDL_B200_API int cogdl_b200_genconv_edge_bwd_f32(const int32_t *colptr, const 
  * The structure must be square (n_rows == n_cols); F % K == 0; d = F/K a power of two from 1 to 32; tau > 0.
  * 16-byte vectors when d % 4 == 0 and every feature buffer is 16-byte aligned.  Hub rows are cut into the plan's
  * chunks and merged in chunk order (no float atomics: bit-reproducible).  plan->partials needs
- * cogdl_b200_disen_route_scratch_bytes(n_chunks, F, K) bytes, which also covers the backward.
+ * cogdl_b200_disen_route_scratch_bytes(n_chunks, F, K) bytes.
  * ------------------------------------------------------------------------------------- */
 COGDL_B200_API int64_t cogdl_b200_disen_route_scratch_bytes(int64_t n_chunks, int64_t F, int64_t K);
 COGDL_B200_API int cogdl_b200_disen_route_fwd_f32(const int32_t *rowptr, const int32_t *colind, const float *q,
@@ -501,8 +516,8 @@ COGDL_B200_API int cogdl_b200_disen_route_fwd_f32(const int32_t *rowptr, const i
  *     dq[i] = sum_e w_e (t_e - D[i]) c[j] / tau
  *   column kernel (transpose colptr/rowind of cogdl_b200_csr2csc, ITS plan `plan_t`):
  *     dc[j] = g_u[j] + sum_{e=(i,j)} [w_e g_u[i] + w_e (t_e - D[i]) q[i] / tau]
- * w_e is recomputed from lse2.  plan's partials need n_chunks*(2F+K)*4 bytes, plan_t's n_chunks*F*4 (both within
- * cogdl_b200_disen_route_scratch_bytes); hub rows / columns are merged in chunk order.  dq and dc are overwritten. */
+ * w_e is recomputed from lse2.  plan and plan_t each need cogdl_b200_disen_route_scratch_bytes(n_chunks, F, K) bytes of
+ * partials, with that plan's n_chunks; hub rows / columns are merged in chunk order.  dq and dc are overwritten. */
 COGDL_B200_API int cogdl_b200_disen_route_bwd_f32(const int32_t *rowptr, const int32_t *colind,
                                    const cogdl_b200_hub_plan_t *plan, const int32_t *colptr,
                                    const int32_t *rowind, const cogdl_b200_hub_plan_t *plan_t, const float *q,
@@ -570,8 +585,9 @@ COGDL_B200_API int cogdl_b200_rgcn_edge_dot_f32(const int32_t *rowptr, const int
  *   g_row[i,h]  = sum_{p in row i} d_edge[p,h]                                                [n_rows, H]
  * with g = (sign bit of att) ? 0 : d_mix * grad_scale, grad_scale = (1 - alpha) / (1 - p_drop).
  * T * H must be in [1, cogdl_b200_hgn_max_table()] (h_e is staged in shared memory), else COGDL_B200_EINVAL before
- * any launch.  Any H; scratch in plan->partials as for the edge softmax.  cogdl_b200_last_kernel() names every
- * launch (hgn_warp_kernel / hgn_generic_kernel / [hgn_stats_kernel +] hgn_main_kernel).
+ * any launch.  Any H; plan->partials needs cogdl_b200_edge_softmax_scratch_bytes(plan->n_chunks, H) bytes.
+ * cogdl_b200_last_kernel() names every launch (hgn_warp_kernel / hgn_generic_kernel / [hgn_stats_kernel +]
+ * hgn_main_kernel).
  * ------------------------------------------------------------------------------------- */
 COGDL_B200_API int64_t cogdl_b200_hgn_max_table(void);
 COGDL_B200_API int cogdl_b200_hgn_attn_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *etype,

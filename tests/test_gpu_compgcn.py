@@ -230,6 +230,7 @@ def test_errors_raise_before_launch(dev):
         compgcn_aggregate((row.cpu(), col.cpu()), typ.cpu(), x.cpu(), rel.cpu(), "sub")
     assert lib.cogdl_b200_launch_count() == n0
     # the C entry point's own checks
+    from cogdl_b200.operators._raw import _scratch
     from cogdl_b200.structure import CompStructure, _ptr, _stream
 
     # the type-grouped structure of the hub graph: its 3 rows are all hubs, so its plan has no segments and only
@@ -238,7 +239,7 @@ def test_errors_raise_before_launch(dev):
     x = torch.randn(N, 8, device=dev)
     st, tcol, tw = CompStructure(row, col, typ, N).by_type(3)
     assert st.plan.n_hub_rows == 3 and st.plan.n_segs == 0
-    plan, keep = st.plan_struct(st.plan.n_chunks * 8 * 4)
+    plan, keep = st.plan_struct(_scratch("comp_aggr", st, 8))
     g = torch.empty(2 * N, 8, device=dev)
     y = torch.empty(4, 8, device=dev)
     n0 = lib.cogdl_b200_launch_count()

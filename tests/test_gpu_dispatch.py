@@ -110,6 +110,7 @@ def check_kernel(c):
 def _peer_call(dev, c, rp, ci, n_cols, val_d, X):
     """cogdl_b200_spmm_csr_f32_peers with three shards on this GPU: [0,400) local, [400,700) owner 1, [700,n) owner 2."""
     from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import _scratch
     from cogdl_b200.structure import _ptr, _stream
 
     bounds, shift = [0, 400, 700, n_cols], 9
@@ -121,7 +122,7 @@ def _peer_call(dev, c, rp, ci, n_cols, val_d, X):
     shards = [T(X[bounds[o]:bounds[o + 1]], dev) for o in range(3)]
     ptrs = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in shards])
     y = torch.empty((rp.shape[0] - 1, c.F), device=dev)
-    plan, keep = st.plan_struct(st.plan.n_chunks * c.F * 4 + 16)
+    plan, keep = st.plan_struct(_scratch("spmm", st, c.F) + 16)
     if c.partials_offset:
         assert st.plan.n_chunks > 0, "the partials offset only matters with hub chunks"
         keep[0].partials += c.partials_offset

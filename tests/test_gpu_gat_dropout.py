@@ -239,13 +239,14 @@ def test_kernel_names_list_every_launch_with_the_dropout_flag(dev):
 def test_bad_arguments_raise_the_library_error(dev):
     import cogdl_b200
     from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import _scratch
     from cogdl_b200.structure import _ptr, _stream
 
     rp, ci, n, h_l, h_r, feat = inputs("tiny", 8, 16, dev)
     st = structure(rp, ci, n, dev, 256)
     out = torch.empty(n, 8, 16, device=dev)
     att = torch.empty(ci.size, 8, device=dev)
-    plan, keep = st.plan_struct(st.plan.n_chunks * 8 * 16 * 4)
+    plan, keep = st.plan_struct(_scratch("gat_fwd", st, 8, 16))
     fwd = ("cogdl_b200_gat_fwd_dropout_f32", _ptr(st.rowptr), _ptr(st.colind), _ptr(h_l), _ptr(h_r), _ptr(feat), 0.2,
            1, 2 ** 63)
     for scale in (0.0, -1.0, float("inf"), float("nan")):

@@ -254,7 +254,7 @@ def _fwd_call(c, st, xd, attr, w, beta_d, dev):
 
 def _bwd_call(c, st, xd, attr, w, beta_d, g, out, lse2, dev):
     from cogdl_b200 import _cabi
-    from cogdl_b200.operators._raw import genconv_edge_bwd_raw
+    from cogdl_b200.operators._raw import _scratch, genconv_edge_bwd_raw
     from cogdl_b200.structure import _ptr, _stream
 
     if not c.partials_offset:
@@ -264,7 +264,7 @@ def _bwd_call(c, st, xd, attr, w, beta_d, g, out, lse2, dev):
     st_t, perm = st.csc()
     assert st_t.plan.n_chunks > 0, f"{c.id}: the partials offset only matters with hub chunks"
     dx = torch.empty_like(xd)
-    plan, keep = st_t.plan_struct(st_t.plan.n_chunks * c.F * 4 + 16)
+    plan, keep = st_t.plan_struct(_scratch("genconv_edge_bwd", st_t, c.F, 1) + 16)
     keep[0].partials += c.partials_offset
     keep[0].partials_bytes -= c.partials_offset
     _cabi.call("cogdl_b200_genconv_edge_bwd_f32", _ptr(st_t.rowptr), _ptr(st_t.colind), _ptr(perm), _ptr(xd),

@@ -162,12 +162,13 @@ def test_edge_cases_match_torch(dev, F):
 
 def test_rejects_aliasing_and_pins_without_z(dev):
     from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import _scratch
     from cogdl_b200.structure import _ptr, _stream
 
     rp, ci, n, st, X, Z = special_inputs(dev, 32)
     pin = torch.ones(n, dtype=torch.uint8, device=dev)
     Y = torch.empty_like(Z)
-    plan, keep = st.plan_struct(st.plan.n_chunks * 32 * 4)
+    plan, keep = st.plan_struct(_scratch("spmm", st, 32))
     for Ya, Za, P in ((X, Z, None), (Z, Z, None), (Y, None, pin)):
         with pytest.raises(_cabi.CogdlB200Error) as e:
             _cabi.call("cogdl_b200_label_prop_f32", _ptr(st.rowptr), _ptr(st.colind), None, _ptr(X), n, _ptr(Za), 0.5,

@@ -119,6 +119,7 @@ def test_spmm_peer_form_single_gpu(dev, F):
     import ctypes
 
     from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import _scratch
     from cogdl_b200.structure import _ptr, _stream
 
     rp, ci, n_cols = case("two_hubs")
@@ -138,7 +139,7 @@ def test_spmm_peer_form_single_gpu(dev, F):
     st = structure(rp, enc, n_cols, dev)
     ptrs = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in shards])
     y = torch.empty((n, F), device=dev)
-    plan, keep = st.plan_struct(st.plan.n_chunks * F * 4)
+    plan, keep = st.plan_struct(_scratch("spmm", st, F))
     _cabi.call("cogdl_b200_spmm_csr_f32_peers", _ptr(st.rowptr), _ptr(st.colind), _ptr(T(val, dev)), _ptr(shards[0]),
                bounds[1], ctypes.cast(ptrs, ctypes.c_void_p), 3, shift, _ptr(y), n, F, plan, _stream(dev))
     torch.cuda.synchronize()

@@ -149,13 +149,14 @@ def test_symmetric_backward_runs_over_the_matrix_itself(dev):
 
 def test_aliased_output_is_rejected(dev):
     from cogdl_b200 import _cabi
+    from cogdl_b200.operators._raw import _scratch
     from cogdl_b200.structure import _ptr, _stream
 
     rp, ci, n = boundary_csr(64)
     st = structure(rp, ci, n, dev, type("C", (), {"plan": "default", "chunk": 64})())
     X = torch.randn(n, 32, device=dev)
     Z = torch.randn(n, 32, device=dev)
-    plan, keep = st.plan_struct(st.plan.n_chunks * 32 * 4)
+    plan, keep = st.plan_struct(_scratch("spmm", st, 32))
     Xbig = torch.randn(2 * n, 32, device=dev)
     Y = torch.empty(n, 32, device=dev)
     # (Y, X, x_rows, Z, row_scale): Y is X; Y is Z; Y starts one row into X; Y ends inside Z; Y starts inside X at an
