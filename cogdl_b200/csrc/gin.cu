@@ -9,8 +9,8 @@
 // behind whatever computes 1 + eps without the host waiting.  Rounding and store sites are the residual epilogue's
 // (fp32 addition commutes, so with a = 1 the forward is bit-identical to the reference expression on this package's
 // spmm); the backward's d x = A^T (r g) + (1 + eps) g is the same launch over the adjoint.  The kernels and their
-// dispatch are the SpMM's (spmm.cuh, stream.cuh) with EPI_RESID_DEV; this file holds their instantiations and the
-// entry point.
+// dispatch are the SpMM's: the row and row-stream kernels (spmm.cuh, stream.cuh) with EPI = EPI_RESID_DEV, only that
+// form instantiated here, behind the entry point.
 #include "spmm.cuh"
 
 using namespace cogdl_b200;
@@ -21,15 +21,16 @@ extern "C" int cogdl_b200_spmm_residual_dcoef_f32(const int32_t *rowptr, const i
                                                   int64_t F, int32_t panels, const cogdl_b200_hub_plan_t *plan,
                                                   cogdl_b200_stream_t stream) {
   const char *who = "cogdl_b200_spmm_residual_dcoef_f32";
-  // as cogdl_b200_spmm_residual_f32: X, Z, row_scale and b_dev are read (read-only cache path) while finished Y rows
-  // are written, so Y may overlap none of them.  The coefficient multiplies Z, so Z needs it.
+  // b_dev is read (read-only cache path) as X, Z and row_scale are, so Y may not overlap it either.  The coefficient
+  // multiplies Z, so Z needs it.
   if (n_rows > 0 && F > 0) {
-    CB_REQUIRE(Y != X && !overlaps(Y, n_rows * F, X, x_rows * F), "%s: Y overlaps X", who);
-    CB_REQUIRE(!Z || !overlaps(Y, n_rows * F, Z, n_rows * F), "%s: Y overlaps Z", who);
-    CB_REQUIRE(!row_scale || !overlaps(Y, n_rows * F, row_scale, n_rows), "%s: Y overlaps row_scale", who);
+    const int rc = check_output_apart(who, "Y", Y, n_rows, F, X, x_rows, Z, row_scale);
+    if (rc) return rc;
     CB_REQUIRE(!Z || b_dev, "%s: Z needs the coefficient b_dev", who);
     CB_REQUIRE(!b_dev || !overlaps(Y, n_rows * F, b_dev, 1), "%s: Y overlaps b_dev", who);
   }
+  SpmmEpilogue epi;
+  epi.Z = Z; epi.row_scale = row_scale; epi.res_a = a; epi.res_b_dev = b_dev;
   return spmm_entry<EPI_RESID_DEV>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream, who, nullptr,
-                                   0, 0, x_rows, panels, Z, row_scale, a, 0.f, nullptr, 0, 0.f, 0.f, b_dev);
+                                   0, 0, x_rows, panels, epi);
 }

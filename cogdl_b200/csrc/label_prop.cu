@@ -12,8 +12,8 @@
 // matches torch for -0.0 and lo > hi.  A pinned row stores Z's row bit for bit, whatever its sum, which is what the
 // row reset leaves behind.  The store sites are the residual epilogue's: the row kernel's row and hub-merge stores,
 // the row-stream loops' row ends (general, lean one-pass and lean panel), their hub merge and the empty-row fill.  The
-// kernels and their dispatch are the SpMM's (spmm.cuh, stream.cuh) with EPI_LABELPROP; this file holds their
-// instantiations and the entry point.
+// kernels and their dispatch are the SpMM's: the row and row-stream kernels (spmm.cuh, stream.cuh) with
+// EPI = EPI_LABELPROP, only that form instantiated here, behind the entry point.
 #include "spmm.cuh"
 
 using namespace cogdl_b200;
@@ -24,14 +24,15 @@ extern "C" int cogdl_b200_label_prop_f32(const int32_t *rowptr, const int32_t *c
                                          int64_t n_rows, int64_t F, int32_t panels, const cogdl_b200_hub_plan_t *plan,
                                          cogdl_b200_stream_t stream) {
   const char *who = "cogdl_b200_label_prop_f32";
-  // as cogdl_b200_spmm_residual_f32: X, Z and row_scale are read (read-only cache path) while finished Y rows are
-  // written, so Y may overlap none of them.  A pinned row is Z's row, so pin needs Z.
+  // a pinned row is Z's row, so pin needs Z
   if (n_rows > 0 && F > 0) {
-    CB_REQUIRE(Y != X && !overlaps(Y, n_rows * F, X, x_rows * F), "%s: Y overlaps X", who);
-    CB_REQUIRE(!Z || !overlaps(Y, n_rows * F, Z, n_rows * F), "%s: Y overlaps Z", who);
-    CB_REQUIRE(!row_scale || !overlaps(Y, n_rows * F, row_scale, n_rows), "%s: Y overlaps row_scale", who);
+    const int rc = check_output_apart(who, "Y", Y, n_rows, F, X, x_rows, Z, row_scale);
+    if (rc) return rc;
     CB_REQUIRE(!pin || Z, "%s: pinned rows need Z", who);
   }
+  SpmmEpilogue epi;
+  epi.Z = Z; epi.row_scale = row_scale; epi.res_a = a; epi.res_b = b;
+  epi.pin = pin; epi.has_clamp = has_clamp != 0; epi.clamp_lo = lo; epi.clamp_hi = hi;
   return spmm_entry<EPI_LABELPROP>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream, who, nullptr,
-                                   0, 0, x_rows, panels, Z, row_scale, a, b, pin, has_clamp != 0, lo, hi);
+                                   0, 0, x_rows, panels, epi);
 }

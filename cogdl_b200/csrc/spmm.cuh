@@ -1,8 +1,9 @@
 // spmm.cuh -- the fp32 SpMM's sub-warp row kernel, its dispatch by width, alignment, plan form and panel count, and
 // the host entry in front of it, shared by the plain SpMM (spmm.cu), the SpMM with a residual epilogue
 // (spmm_residual.cu), the label-propagation step (label_prop.cu), the GIN aggregation (gin.cu) and GRAND's propagation
-// hop (spmm_accum.cu).  EPI selects the epilogue: every finished row is written by epilogue_store<EPI> (stream.cuh) --
-// acc itself for EPI_NONE.  Design notes: spmm.cu.
+// hop (spmm_accum.cu).  EPI, the last template argument of the row kernel and of stream_kernel, selects the epilogue:
+// every finished row is written by epilogue_store<EPI> (stream.cuh) -- acc itself for EPI_NONE -- with the operands in
+// SpmmEpilogue.  Design notes: spmm.cu.
 #pragma once
 #include "common.cuh"
 #include "stream.cuh"
@@ -23,19 +24,7 @@ struct SpmmParams {
   int64_t n_rows;
   int FV;      // feature row length in VecT units
   HubView hub;
-  // residual epilogue (EPI_RESID, EPI_LABELPROP): see StreamParams
-  const float *Z = nullptr;
-  const float *row_scale = nullptr;
-  float res_a = 1.f, res_b = 0.f;
-  // label-propagation epilogue (EPI_LABELPROP): see StreamParams
-  const unsigned char *pin = nullptr;
-  int has_clamp = 0;
-  float clamp_lo = 0.f, clamp_hi = 0.f;
-  // device-coefficient residual epilogue (EPI_RESID_DEV) and accumulating epilogue (EPI_ACCUM): see StreamParams
-  const float *res_b_dev = nullptr;
-  float *acc = nullptr;
-  int acc_last = 0;
-  float acc_scale = 1.f;
+  SpmmEpilogue epi;   // the store epilogue (stream.cuh)
 };
 
 template <typename VecT, int GROUP, int NV, bool HAS_VAL, int EPI>
@@ -72,7 +61,7 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
       if (!w.is_chunk && w.active) {
 #pragma unroll
         for (int k = 0; k < NV; ++k)
-          if (colok[k]) prefetch_l1(reinterpret_cast<const VecT *>(p.Z) + (int64_t)w.row * p.FV + cv + k * GROUP);
+          if (colok[k]) prefetch_l1(reinterpret_cast<const VecT *>(p.epi.Z) + (int64_t)w.row * p.FV + cv + k * GROUP);
       }
     }
 
@@ -157,34 +146,12 @@ __device__ __forceinline__ void spmm_rows(const SpmmParams &p) {
   }
 }
 
-template <typename VecT, int GROUP, int NV, bool HAS_VAL>
-__global__ void __launch_bounds__(256) spmm_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_NONE>(p);
-}
-
-// at least 3 blocks per SM: left to itself ptxas fits the GROUP=4 float4 weighted instantiation in 64 registers
-// and spills; 80 registers hold every instantiation without spilling
-template <typename VecT, int GROUP, int NV, bool HAS_VAL>
-__global__ void __launch_bounds__(256, 3) spmm_residual_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_RESID>(p);
-}
-
-// the row kernel with the label-propagation epilogue (label_prop.cu); 3 blocks per SM as for the residual form
-template <typename VecT, int GROUP, int NV, bool HAS_VAL>
-__global__ void __launch_bounds__(256, 3) spmm_labelprop_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_LABELPROP>(p);
-}
-
-// the row kernel with the device-coefficient residual epilogue (gin.cu) and with the accumulating epilogue
-// (spmm_accum.cu); 3 blocks per SM as for the residual form
-template <typename VecT, int GROUP, int NV, bool HAS_VAL>
-__global__ void __launch_bounds__(256, 3) spmm_dcoef_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_RESID_DEV>(p);
-}
-
-template <typename VecT, int GROUP, int NV, bool HAS_VAL>
-__global__ void __launch_bounds__(256, 3) spmm_accum_kernel(const SpmmParams p) {
-  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI_ACCUM>(p);
+// EPI_NONE leaves the register budget to ptxas.  The epilogues ask for at least 3 blocks per SM: left to itself ptxas
+// fits the GROUP=4 float4 weighted residual instantiation in 64 registers and spills; 80 registers hold every
+// instantiation without spilling.
+template <typename VecT, int GROUP, int NV, bool HAS_VAL, int EPI>
+__global__ void __launch_bounds__(256, EPI == EPI_NONE ? 0 : 3) spmm_kernel(const SpmmParams p) {
+  spmm_rows<VecT, GROUP, NV, HAS_VAL, EPI>(p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -198,9 +165,7 @@ static StreamParams to_stream(const SpmmParams &p) {
   q.hub = p.hub;
   q.n_peers = p.n_peers; q.peer_shift = p.peer_shift;
   for (int i = 0; i < 8; ++i) q.peers[i] = p.peers[i];
-  q.Z = p.Z; q.row_scale = p.row_scale; q.res_a = p.res_a; q.res_b = p.res_b;
-  q.pin = p.pin; q.has_clamp = p.has_clamp; q.clamp_lo = p.clamp_lo; q.clamp_hi = p.clamp_hi;
-  q.res_b_dev = p.res_b_dev; q.acc = p.acc; q.acc_last = p.acc_last; q.acc_scale = p.acc_scale;
+  q.epi = p.epi;
   return q;
 }
 
@@ -280,30 +245,15 @@ static int launch_spmm_panels(const SpmmParams &p, int64_t F, int P, cudaStream_
   }
 }
 
+// the row kernel's name in its launch errors, per epilogue
+constexpr const char *EPI_WHO[] = {"spmm", "spmm_residual", "label_prop", "spmm_dcoef", "spmm_accum"};
+
 template <typename VecT, int GROUP, int NV, int EPI>
 static int launch_spmm(const SpmmParams &p, cudaStream_t stream) {
-  const char *vec = sizeof(VecT) == 16 ? "float4" : "float";
-  const char *what = p.val ? "weighted" : "unweighted";
-  const int64_t items = (int64_t)p.hub.n_chunks + p.n_rows;
-  if constexpr (EPI == EPI_RESID_DEV)
-    return launch_items(p.val ? spmm_dcoef_kernel<VecT, GROUP, NV, true> : spmm_dcoef_kernel<VecT, GROUP, NV, false>,
-                        p, items, GROUP, stream, "spmm_dcoef",
-                        "cogdl_b200::spmm_dcoef_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
-  else if constexpr (EPI == EPI_ACCUM)
-    return launch_items(p.val ? spmm_accum_kernel<VecT, GROUP, NV, true> : spmm_accum_kernel<VecT, GROUP, NV, false>,
-                        p, items, GROUP, stream, "spmm_accum",
-                        "cogdl_b200::spmm_accum_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
-  else if constexpr (EPI == EPI_LABELPROP)
-    return launch_items(p.val ? spmm_labelprop_kernel<VecT, GROUP, NV, true> : spmm_labelprop_kernel<VecT, GROUP, NV, false>,
-                        p, items, GROUP, stream, "label_prop",
-                        "cogdl_b200::spmm_labelprop_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
-  else if constexpr (EPI == EPI_RESID)
-    return launch_items(p.val ? spmm_residual_kernel<VecT, GROUP, NV, true> : spmm_residual_kernel<VecT, GROUP, NV, false>,
-                        p, items, GROUP, stream, "spmm_residual",
-                        "cogdl_b200::spmm_residual_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
-  else
-    return launch_items(p.val ? spmm_kernel<VecT, GROUP, NV, true> : spmm_kernel<VecT, GROUP, NV, false>, p, items,
-                        GROUP, stream, "spmm", "cogdl_b200::spmm_kernel<%s,GROUP=%d,NV=%d,%s>", vec, GROUP, NV, what);
+  return launch_items(p.val ? spmm_kernel<VecT, GROUP, NV, true, EPI> : spmm_kernel<VecT, GROUP, NV, false, EPI>, p,
+                      (int64_t)p.hub.n_chunks + p.n_rows, GROUP, stream, EPI_WHO[EPI],
+                      "cogdl_b200::spmm%s_kernel<%s,GROUP=%d,NV=%d,%s>", EPI_TAG[EPI],
+                      sizeof(VecT) == 16 ? "float4" : "float", GROUP, NV, p.val ? "weighted" : "unweighted");
 }
 
 // narrow rows (F = 40 -> 10 float4): the lean row-stream form with the idle lanes masked beats the sub-warp
@@ -330,26 +280,35 @@ static int dispatch_spmm(const SpmmParams &p, cudaStream_t s) {
   return stream ? launch_spmm_stream<VecT, 2, EPI>(p, s) : launch_spmm<VecT, 32, 2, EPI>(p, s);
 }
 
-// [p, p + n) and [q, q + m) share a byte: the epilogue entries' output overlap checks
+// [p, p + n) and [q, q + m) share a byte
 static inline bool overlaps(const float *p, int64_t n, const float *q, int64_t m) {
   const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
   return a < b + (uintptr_t)m * sizeof(float) && b < a + (uintptr_t)n * sizeof(float);
 }
 
+// The output checks of the epilogue entries, for a non-empty output `out` ([n_rows, F], `name` in the messages): the
+// kernels read X, Z and row_scale (read-only cache path) while other warps write finished rows of out, so out may
+// overlap none of them.  X holds x_rows rows (colind < x_rows), so an empty X can only coincide with out.  Z and
+// row_scale are optional.
+static int check_output_apart(const char *who, const char *name, const float *out, int64_t n_rows, int64_t F,
+                              const float *X, int64_t x_rows, const float *Z, const float *row_scale) {
+  const int64_t nf = n_rows * F;
+  CB_REQUIRE(out != X && !overlaps(out, nf, X, x_rows * F), "%s: %s overlaps X", who, name);
+  CB_REQUIRE(!Z || !overlaps(out, nf, Z, nf), "%s: %s overlaps Z", who, name);
+  CB_REQUIRE(!row_scale || !overlaps(out, nf, row_scale, n_rows), "%s: %s overlaps row_scale", who, name);
+  return COGDL_B200_OK;
+}
+
 // The host side of every fp32 SpMM entry point: argument checks, the parameters, the panel count and the dispatch.
-// X1 (nullptr = X0) serves the columns >= n0 (two-source form); peers are the peer form's shards; Z, row_scale, a and
-// b are the epilogue's (EPI_RESID, EPI_LABELPROP); pin, has_clamp, lo and hi the label-propagation epilogue's; b_dev
-// the device coefficient that replaces b (EPI_RESID_DEV); acc, acc_last and acc_scale the accumulating epilogue's
-// (EPI_ACCUM, with Z as ACC's input).  x_rows, X0's row count, sizes the automatic panel count (panels = 0).  Static,
-// so each object instantiates only the form it calls.
+// X1 (nullptr = X0) serves the columns >= n0 (two-source form); peers are the peer form's shards; epi holds the
+// operands of the epilogue EPI (stream.cuh).  x_rows, X0's row count, sizes the automatic panel count (panels = 0).
+// Static, so each object instantiates only the form it calls.
 template <int EPI>
 static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float *val, const float *X0, int64_t n0,
                       const float *X1, float *Y, int64_t n_rows, int64_t F, const cogdl_b200_hub_plan_t *plan,
                       cogdl_b200_stream_t stream, const char *who, const float *const *peers = nullptr,
                       int n_peers = 0, int peer_shift = 0, int64_t x_rows = 0, int panels = 1,
-                      const float *Z = nullptr, const float *row_scale = nullptr, float a = 1.f, float b = 0.f,
-                      const unsigned char *pin = nullptr, int has_clamp = 0, float lo = 0.f, float hi = 0.f,
-                      const float *b_dev = nullptr, float *acc = nullptr, int acc_last = 0, float acc_scale = 1.f) {
+                      const SpmmEpilogue &epi = {}) {
   CB_REQUIRE(n_rows >= 0 && F >= 0, "%s: negative size (n_rows=%lld, F=%lld)", who, (long long)n_rows, (long long)F);
   CB_REQUIRE(x_rows >= 0 && panels >= 0, "%s: negative x_rows / panels", who);
   if (n_rows == 0 || F == 0) return COGDL_B200_OK;
@@ -361,9 +320,7 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
   p.rowptr = rowptr; p.colind = colind; p.val = val; p.X0 = X0; p.X1 = X1 ? X1 : X0; p.n0 = n0;
   p.Y = Y; p.n_rows = n_rows; p.hub = hub_view(plan);
   p.n_peers = n_peers; p.peer_shift = peer_shift;
-  p.Z = Z; p.row_scale = row_scale; p.res_a = a; p.res_b = b;
-  p.pin = pin; p.has_clamp = has_clamp; p.clamp_lo = lo; p.clamp_hi = hi;
-  p.res_b_dev = b_dev; p.acc = acc; p.acc_last = acc_last; p.acc_scale = acc_scale;
+  p.epi = epi;
   bool peers_aligned = true;
   for (int i = 0; i < n_peers; ++i) {
     p.peers[i] = peers[i];
@@ -372,8 +329,8 @@ static int spmm_entry(const int32_t *rowptr, const int32_t *colind, const float 
   if (n_peers > 0)
     CB_REQUIRE(p.hub.n_segs > 0 && F % 4 == 0 && F <= 512 && peers_aligned && aligned16(X0) && aligned16(Y),
                "%s: the peer form needs a plan with segments, F %% 4 == 0, F <= 512 and 16-byte aligned buffers", who);
-  const bool vec = (F % 4 == 0) && aligned16(X0) && aligned16(p.X1) && aligned16(Y) && aligned16(Z) &&
-                   aligned16(acc) && (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
+  const bool vec = (F % 4 == 0) && aligned16(X0) && aligned16(p.X1) && aligned16(Y) && aligned16(epi.Z) &&
+                   aligned16(epi.acc) && (p.hub.n_chunks == 0 || aligned16(p.hub.partials));
   if (vec) p.FV = (int)(F / 4);
   const bool panel_form = vec && n_peers == 0 && n0 == INT64_MAX && p.hub.n_segs > 0 && F % 32 == 0;
   if (panels > 1)

@@ -13,8 +13,8 @@
 // element by the same thread are race-free; ACC_in (NULL: ACC itself) lets the first hop read the hop-0 features
 // without a copy.  The store sites are the residual epilogue's: the row kernel's row and hub-merge stores, the
 // row-stream loops' row ends (general, lean one-pass and lean panel), their hub merge and the empty-row fill.  The
-// kernels and their dispatch are the SpMM's (spmm.cuh, stream.cuh) with EPI_ACCUM; this file holds their
-// instantiations and the entry point.
+// kernels and their dispatch are the SpMM's: the row and row-stream kernels (spmm.cuh, stream.cuh) with
+// EPI = EPI_ACCUM, only that form instantiated here, behind the entry point.
 #include "spmm.cuh"
 
 using namespace cogdl_b200;
@@ -26,25 +26,25 @@ extern "C" int cogdl_b200_spmm_accum_f32(const int32_t *rowptr, const int32_t *c
                                          cogdl_b200_stream_t stream) {
   const char *who = "cogdl_b200_spmm_accum_f32";
   const float *in = acc_in ? acc_in : acc;
-  // X is gathered and row_scale read (read-only cache path) while finished rows of Xn and ACC are written, so neither
-  // output may overlap them, nor each other.  ACC_in is read by the thread that writes the same element of ACC: it is
-  // ACC itself or lies apart from it.
+  // Neither output, Xn nor ACC, may overlap X or row_scale, nor each other.  ACC_in is read by the thread that writes
+  // the same element of ACC: it is ACC itself or lies apart from it.
   if (n_rows > 0 && F > 0) {
     const int64_t nf = n_rows * F;
     CB_REQUIRE(acc, "%s: null ACC", who);
     CB_REQUIRE(last || Xn, "%s: Xn may be NULL on the last hop only", who);
-    CB_REQUIRE(acc != X && !overlaps(acc, nf, X, x_rows * F), "%s: ACC overlaps X", who);
+    int rc = check_output_apart(who, "ACC", acc, n_rows, F, X, x_rows, nullptr, row_scale);
+    if (rc) return rc;
     CB_REQUIRE(in == acc || !overlaps(acc, nf, in, nf), "%s: ACC_in overlaps ACC without being it", who);
-    CB_REQUIRE(!row_scale || !overlaps(acc, nf, row_scale, n_rows), "%s: ACC overlaps row_scale", who);
     if (!last) {
-      CB_REQUIRE(Xn != X && !overlaps(Xn, nf, X, x_rows * F), "%s: Xn overlaps X", who);
+      rc = check_output_apart(who, "Xn", Xn, n_rows, F, X, x_rows, nullptr, row_scale);
+      if (rc) return rc;
       CB_REQUIRE(!overlaps(Xn, nf, acc, nf), "%s: Xn overlaps ACC", who);
       CB_REQUIRE(!overlaps(Xn, nf, in, nf), "%s: Xn overlaps ACC_in", who);
-      CB_REQUIRE(!row_scale || !overlaps(Xn, nf, row_scale, n_rows), "%s: Xn overlaps row_scale", who);
     }
   }
+  SpmmEpilogue epi;
+  epi.Z = in; epi.row_scale = row_scale; epi.acc = acc; epi.acc_last = last != 0; epi.acc_scale = scale;
   // on the last hop nothing but ACC is written: it stands in as Y, the base the store sites index from
   return spmm_entry<EPI_ACCUM>(rowptr, colind, val, X, INT64_MAX, nullptr, last ? acc : Xn, n_rows, F, plan, stream, who,
-                               nullptr, 0, 0, x_rows, panels, in, row_scale, 1.f, 0.f, nullptr, 0, 0.f, 0.f, nullptr,
-                               acc, last != 0, scale);
+                               nullptr, 0, 0, x_rows, panels, epi);
 }

@@ -8,8 +8,9 @@
 // applied there: the row kernel's row and hub-merge stores, the row-stream loops' row ends (general, lean one-pass and
 // lean panel), their hub merge and the empty-row zero fill (an empty row is the epilogue of a zero sum).  A (A @ X)
 // is the plain SpMM's, in its accumulation order, and each epilogue step is one fp32 multiply or add in the unfused
-// sequence's order, so Y is bit-identical to that sequence.  The kernels and their dispatch are the SpMM's (spmm.cuh,
-// stream.cuh) with EPI_RESID; this file holds their instantiations and the entry point.
+// sequence's order, so Y is bit-identical to that sequence.  The kernels and their dispatch are the SpMM's: the row and
+// row-stream kernels (spmm.cuh, stream.cuh) with EPI = EPI_RESID, only that form instantiated here, behind the entry
+// point.
 #include "spmm.cuh"
 
 using namespace cogdl_b200;
@@ -20,13 +21,12 @@ extern "C" int cogdl_b200_spmm_residual_f32(const int32_t *rowptr, const int32_t
                                             int32_t panels, const cogdl_b200_hub_plan_t *plan,
                                             cogdl_b200_stream_t stream) {
   const char *who = "cogdl_b200_spmm_residual_f32";
-  // the kernels read X, Z and row_scale (read-only cache path) while other warps write finished Y rows; X holds
-  // x_rows rows (colind < x_rows), so an empty X can only coincide with Y.  An empty Y is written by no one.
-  if (n_rows > 0 && F > 0) {
-    CB_REQUIRE(Y != X && !overlaps(Y, n_rows * F, X, x_rows * F), "%s: Y overlaps X", who);
-    CB_REQUIRE(!Z || !overlaps(Y, n_rows * F, Z, n_rows * F), "%s: Y overlaps Z", who);
-    CB_REQUIRE(!row_scale || !overlaps(Y, n_rows * F, row_scale, n_rows), "%s: Y overlaps row_scale", who);
+  if (n_rows > 0 && F > 0) {     // an empty Y is written by no one
+    const int rc = check_output_apart(who, "Y", Y, n_rows, F, X, x_rows, Z, row_scale);
+    if (rc) return rc;
   }
+  SpmmEpilogue epi;
+  epi.Z = Z; epi.row_scale = row_scale; epi.res_a = a; epi.res_b = b;
   return spmm_entry<EPI_RESID>(rowptr, colind, val, X, INT64_MAX, nullptr, Y, n_rows, F, plan, stream, who, nullptr, 0, 0,
-                          x_rows, panels, Z, row_scale, a, b);
+                               x_rows, panels, epi);
 }

@@ -1,5 +1,5 @@
-// stream.cuh -- the row-stream gather kernel shared by the SpMM, the multi-head SpMM and the CompGCN composition
-// aggregation (sm_90a).
+// stream.cuh -- the row-stream gather kernel shared by the SpMM (with each of its store epilogues), the multi-head SpMM
+// and the CompGCN composition aggregation (sm_90a).
 //
 // Work items, in grid order:
 //   [0, n_chunks)                 hub chunks: <= chunk_edges edges of ONE hub row -> partial sum in
@@ -22,6 +22,30 @@
 #include "common.cuh"
 
 namespace cogdl_b200 {
+
+// The operands of the plain SpMM's store epilogue (EPI below), a member of StreamParams and of SpmmParams (spmm.cuh).
+struct SpmmEpilogue {
+  // residual epilogue (spmm_residual.cu, EPI_RESID): every finished row i is written as
+  // fl(fl(res_a * fl(row_scale[i] * acc)) + fl(res_b * Z[i])); row_scale and Z are optional ([n_rows], [n_rows, ldv]).
+  const float *Z = nullptr;
+  const float *row_scale = nullptr;
+  float res_a = 1.f, res_b = 0.f;
+  // label-propagation epilogue (label_prop.cu, EPI_LABELPROP): the residual epilogue's value, clamped to
+  // [clamp_lo, clamp_hi] as torch.clamp does when has_clamp; a row i with pin[i] != 0 stores Z[i] instead.  pin
+  // ([n_rows] bytes) is optional and needs Z.
+  const unsigned char *pin = nullptr;
+  int has_clamp = 0;
+  float clamp_lo = 0.f, clamp_hi = 0.f;
+  // residual epilogue with a device coefficient (gin.cu, EPI_RESID_DEV): the residual epilogue with res_b read from
+  // *res_b_dev (one fp32 value in device memory) instead of res_b.
+  const float *res_b_dev = nullptr;
+  // accumulating epilogue (spmm_accum.cu, EPI_ACCUM): v = fl(row_scale[i] * acc) is stored to Y[i] unless acc_last,
+  // and ACC[i] = fl(Z[i] + v), times acc_scale (fl) when acc_last.  Z is ACC's input: ACC itself (in place) or another
+  // buffer of Y's layout; Y is ACC when acc_last (nothing else is written).
+  float *acc = nullptr;
+  int acc_last = 0;
+  float acc_scale = 1.f;
+};
 
 struct StreamParams {
   const int *rowptr;
@@ -52,26 +76,7 @@ struct StreamParams {
   // MODE 2); a kept entry is read as att * drop_scale, a dropped one as 0 (drop_att, common.cuh).  Read only by
   // the multi-head form, which takes the DROP instantiation iff drop_scale > 0.
   float drop_scale;
-  // residual epilogue (spmm_residual.cu, EPI_RESID): every finished row i is written as
-  // fl(fl(res_a * fl(row_scale[i] * acc)) + fl(res_b * Z[i])); row_scale and Z are optional ([n_rows], [n_rows, ldv]).
-  const float *Z = nullptr;
-  const float *row_scale = nullptr;
-  float res_a = 1.f, res_b = 0.f;
-  // label-propagation epilogue (label_prop.cu, EPI_LABELPROP): the residual epilogue's value, clamped to
-  // [clamp_lo, clamp_hi] as torch.clamp does when has_clamp; a row i with pin[i] != 0 stores Z[i] instead.  pin
-  // ([n_rows] bytes) is optional and needs Z.
-  const unsigned char *pin = nullptr;
-  int has_clamp = 0;
-  float clamp_lo = 0.f, clamp_hi = 0.f;
-  // residual epilogue with a device coefficient (gin.cu, EPI_RESID_DEV): the residual epilogue with res_b read from
-  // *res_b_dev (one fp32 value in device memory) instead of res_b.
-  const float *res_b_dev = nullptr;
-  // accumulating epilogue (spmm_accum.cu, EPI_ACCUM): v = fl(row_scale[i] * acc) is stored to Y[i] unless acc_last,
-  // and ACC[i] = fl(Z[i] + v), times acc_scale (fl) when acc_last.  Z is ACC's input: ACC itself (in place) or another
-  // buffer of Y's layout; Y is ACC when acc_last (nothing else is written).
-  float *acc = nullptr;
-  int acc_last = 0;
-  float acc_scale = 1.f;
+  SpmmEpilogue epi;   // the plain SpMM's store epilogue
 };
 
 enum { MODE_UNWEIGHTED = 0, MODE_WEIGHTED = 1, MODE_MULTIHEAD = 2, MODE_COMP_MULT = 3, MODE_COMP_SUB = 4 };
@@ -90,6 +95,9 @@ enum { FORM_PLAIN = 0, FORM_PANEL = 1, FORM_MULTIHEAD = 2 };
 // (EPI_RESID), the label-propagation epilogue of label_prop.cu (EPI_LABELPROP), the residual epilogue with its b read
 // on the device (gin.cu, EPI_RESID_DEV) or the accumulating epilogue of spmm_accum.cu (EPI_ACCUM, two stores per row).
 enum { EPI_NONE = 0, EPI_RESID = 1, EPI_LABELPROP = 2, EPI_RESID_DEV = 3, EPI_ACCUM = 4 };
+// EPI is the last template argument of the row kernel (spmm.cuh) and of stream_kernel.  cogdl_b200_last_kernel() names
+// their instantiations spmm<tag>_kernel<...> and stream<tag>_kernel<...>, with the tag of their epilogue.
+constexpr const char *EPI_TAG[] = {"", "_residual", "_labelprop", "_dcoef", "_accum"};
 
 // The residual epilogue of one output element, rounded step by step as the unfused sequence
 // `a * (r * spmm(x)) + b * z` rounds it (no contraction); r and z are used iff has_r / has_z.
@@ -110,21 +118,21 @@ __device__ __forceinline__ float4 residual_rn(float4 acc, float4 z, bool hr, flo
 template <typename VecT, typename P>
 __device__ __forceinline__ VecT residual_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
   const int64_t o = yp - reinterpret_cast<const VecT *>(p.Y);
-  const bool hr = p.row_scale != nullptr, hz = p.Z != nullptr;
-  const float r = hr ? __ldg(p.row_scale + row) : 1.f;
-  const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.Z) + o) : vzero<VecT>();
-  return residual_rn(acc, z, hr, r, hz, p.res_a, p.res_b);
+  const bool hr = p.epi.row_scale != nullptr, hz = p.epi.Z != nullptr;
+  const float r = hr ? __ldg(p.epi.row_scale + row) : 1.f;
+  const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.epi.Z) + o) : vzero<VecT>();
+  return residual_rn(acc, z, hr, r, hz, p.epi.res_a, p.epi.res_b);
 }
 
-// The residual epilogue with b = *p.res_b_dev, a coefficient that lives in device memory (GIN's 1 + eps, a trainable
+// The residual epilogue with b = *res_b_dev, a coefficient that lives in device memory (GIN's 1 + eps, a trainable
 // parameter), read by the kernel so the host never waits for it.  Only read when Z is given.
 template <typename VecT, typename P>
 __device__ __forceinline__ VecT residual_dev_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
   const int64_t o = yp - reinterpret_cast<const VecT *>(p.Y);
-  const bool hr = p.row_scale != nullptr, hz = p.Z != nullptr;
-  const float r = hr ? __ldg(p.row_scale + row) : 1.f;
-  const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.Z) + o) : vzero<VecT>();
-  return residual_rn(acc, z, hr, r, hz, p.res_a, hz ? __ldg(p.res_b_dev) : 0.f);
+  const bool hr = p.epi.row_scale != nullptr, hz = p.epi.Z != nullptr;
+  const float r = hr ? __ldg(p.epi.row_scale + row) : 1.f;
+  const VecT z = hz ? __ldg(reinterpret_cast<const VecT *>(p.epi.Z) + o) : vzero<VecT>();
+  return residual_rn(acc, z, hr, r, hz, p.epi.res_a, hz ? __ldg(p.epi.res_b_dev) : 0.f);
 }
 
 // One element of the accumulating epilogue's running sum: fl(s + v), then times `scale` (fl) on the last hop -- what
@@ -153,13 +161,13 @@ __device__ __forceinline__ float4 clamp_torch(float4 v, float lo, float hi) {
 }
 
 // The label-propagation epilogue of one output element: Z's element for a pinned row (the row reset of Correct &
-// Smooth's fixed_post), else the residual epilogue, clamped when p.has_clamp (autoscale_post).
+// Smooth's fixed_post), else the residual epilogue, clamped when p.epi.has_clamp (autoscale_post).
 template <typename VecT, typename P>
 __device__ __forceinline__ VecT label_prop_out(const P &p, const VecT &acc, int64_t row, const VecT *yp) {
-  if (p.pin != nullptr && __ldg(p.pin + row) != 0)
-    return __ldg(reinterpret_cast<const VecT *>(p.Z) + (yp - reinterpret_cast<const VecT *>(p.Y)));
+  if (p.epi.pin != nullptr && __ldg(p.epi.pin + row) != 0)
+    return __ldg(reinterpret_cast<const VecT *>(p.epi.Z) + (yp - reinterpret_cast<const VecT *>(p.Y)));
   const VecT v = residual_out(p, acc, row, yp);
-  return p.has_clamp ? clamp_torch(v, p.clamp_lo, p.clamp_hi) : v;
+  return p.epi.has_clamp ? clamp_torch(v, p.epi.clamp_lo, p.epi.clamp_hi) : v;
 }
 
 // acc of output row `row`, to be stored at yp, with the epilogue EPI applied.
@@ -189,11 +197,11 @@ template <int EPI, typename VecT, typename P>
 __device__ __forceinline__ void epilogue_store(const P &p, const VecT &acc, int64_t row, VecT *yp) {
   if constexpr (EPI == EPI_ACCUM) {
     const int64_t o = yp - reinterpret_cast<const VecT *>(p.Y);
-    const bool hr = p.row_scale != nullptr;
-    const VecT v = residual_rn(acc, vzero<VecT>(), hr, hr ? __ldg(p.row_scale + row) : 1.f, false, 1.f, 0.f);
-    if (!p.acc_last) st_stream(yp, v);
-    const VecT s = reinterpret_cast<const VecT *>(p.Z)[o];
-    st_stream(reinterpret_cast<VecT *>(p.acc) + o, accum_rn(s, v, p.acc_last != 0, p.acc_scale));
+    const bool hr = p.epi.row_scale != nullptr;
+    const VecT v = residual_rn(acc, vzero<VecT>(), hr, hr ? __ldg(p.epi.row_scale + row) : 1.f, false, 1.f, 0.f);
+    if (!p.epi.acc_last) st_stream(yp, v);
+    const VecT s = reinterpret_cast<const VecT *>(p.epi.Z)[o];
+    st_stream(reinterpret_cast<VecT *>(p.epi.acc) + o, accum_rn(s, v, p.epi.acc_last != 0, p.epi.acc_scale));
   } else {
     st_stream(yp, epilogue_out<EPI>(p, acc, row, yp));
   }
@@ -239,7 +247,7 @@ __device__ __forceinline__ void stream_range(const StreamParams &p, int e, const
         const int rj = __shfl_sync(FULL, rid, __ffs(m) - 1);
 #pragma unroll
         for (int k = 0; k < NV; ++k)
-          if (colok[k]) prefetch_l1(reinterpret_cast<const VecT *>(p.Z) + cv + (int64_t)rj * p.ldv + k * 32);
+          if (colok[k]) prefetch_l1(reinterpret_cast<const VecT *>(p.epi.Z) + cv + (int64_t)rj * p.ldv + k * 32);
       }
     }
     int cn, pn, ridn, rnxn;
@@ -403,7 +411,7 @@ __device__ __forceinline__ void stream_range_lean(const StreamParams &p, int e, 
     __syncwarp();
     if constexpr (EPI == EPI_ACCUM && ROWS) {      // ACC_in of the rows that end in this slab, while its gathers run
       for (unsigned m = endmask; m != 0u; m &= m - 1u)
-        if (colok) prefetch_l1(reinterpret_cast<const VecT *>(p.Z) + cv + (int64_t)s_r[__ffs(m) - 1] * p.ldv);
+        if (colok) prefetch_l1(reinterpret_cast<const VecT *>(p.epi.Z) + cv + (int64_t)s_r[__ffs(m) - 1] * p.ldv);
     }
     if (PF) load_slab(e + 32, pc, pv, pend);        // consumed by the next iteration only (r is already past this slab)
     int j = 0;
@@ -548,7 +556,7 @@ __device__ __forceinline__ void stream_item(const StreamParams &p, const int64_t
 }
 
 template <typename VecT, int NV, int MODE, bool HAS_PERM, int SRC, int U, int MINB, bool PREFETCH, bool PANEL = false,
-          bool DROP = false>
+          bool DROP = false, int EPI = EPI_NONE>
 __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p) {
   const int lane = threadIdx.x & 31;
   constexpr bool LEAN = is_lean<MODE, NV>();
@@ -557,65 +565,12 @@ __global__ void __launch_bounds__(256, MINB) stream_kernel(const StreamParams p)
   int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
   int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, PANEL, DROP>(p, wid, lane, s_cv, s_r);
-}
-
-// stream_kernel of the plain SpMM (one source) with the residual epilogue (spmm_residual.cu).
-template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
-__global__ void __launch_bounds__(256, MINB) stream_residual_kernel(const StreamParams p) {
-  const int lane = threadIdx.x & 31;
-  constexpr bool LEAN = is_lean<MODE, NV>();
-  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
-  __shared__ int s_r_all[LEAN ? 8 : 1][32];
-  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
-  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
-  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_RESID>(p, wid, lane, s_cv, s_r);
-}
-
-// stream_kernel of the plain SpMM (one source) with the label-propagation epilogue (label_prop.cu).
-template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
-__global__ void __launch_bounds__(256, MINB) stream_labelprop_kernel(const StreamParams p) {
-  const int lane = threadIdx.x & 31;
-  constexpr bool LEAN = is_lean<MODE, NV>();
-  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
-  __shared__ int s_r_all[LEAN ? 8 : 1][32];
-  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
-  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
-  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_LABELPROP>(p, wid, lane, s_cv, s_r);
-}
-
-// stream_kernel of the plain SpMM (one source) with the device-coefficient residual epilogue (gin.cu) and with the
-// accumulating epilogue (spmm_accum.cu).
-template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
-__global__ void __launch_bounds__(256, MINB) stream_dcoef_kernel(const StreamParams p) {
-  const int lane = threadIdx.x & 31;
-  constexpr bool LEAN = is_lean<MODE, NV>();
-  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
-  __shared__ int s_r_all[LEAN ? 8 : 1][32];
-  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
-  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
-  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_RESID_DEV>(p, wid, lane, s_cv, s_r);
-}
-
-template <typename VecT, int NV, int MODE, int U, int MINB, bool PREFETCH, bool PANEL>
-__global__ void __launch_bounds__(256, MINB) stream_accum_kernel(const StreamParams p) {
-  const int lane = threadIdx.x & 31;
-  constexpr bool LEAN = is_lean<MODE, NV>();
-  __shared__ int2 s_cv_all[LEAN ? 8 : 1][32];
-  __shared__ int s_r_all[LEAN ? 8 : 1][32];
-  int2 *s_cv = s_cv_all[LEAN ? (threadIdx.x >> 5) : 0];
-  int *s_r = s_r_all[LEAN ? (threadIdx.x >> 5) : 0];
-  const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  stream_item<VecT, NV, MODE, false, SRC_ONE, U, PREFETCH, PANEL, false, EPI_ACCUM>(p, wid, lane, s_cv, s_r);
+  stream_item<VecT, NV, MODE, HAS_PERM, SRC, U, PREFETCH, PANEL, DROP, EPI>(p, wid, lane, s_cv, s_r);
 }
 
 // Launch helper: picks the instantiation of FORM for (weighted, perm, source form); U / MINB fixed by the caller.
-// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.  EPI: the plain
-// or panel form with the residual (stream_residual_kernel), label-propagation (stream_labelprop_kernel),
-// device-coefficient residual (stream_dcoef_kernel) or accumulating (stream_accum_kernel) epilogue, one source.
+// The panel form has p.S panels of 32 VecT each (grid.y); the multi-head form p.S slices per item.  EPI: the store
+// epilogue of the plain or panel form, which then reads one source.
 template <typename VecT, int NV, int U, int MINB, bool PREFETCH = true, int FORM = FORM_PLAIN, int EPI = EPI_NONE>
 static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   static_assert(FORM == FORM_PLAIN || NV == 1, "the panel and multi-head forms have one VecT per lane");
@@ -635,9 +590,7 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
   if ((FORM != FORM_PLAIN || EPI != EPI_NONE) && src != SRC_ONE)
     return set_error(COGDL_B200_EINVAL, "stream kernel: the panel, multi-head and epilogue forms read one source");
   const bool drop = FORM == FORM_MULTIHEAD && p.drop_scale > 0.f;
-  note_kernel("cogdl_b200::%s<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>",
-              EPI == EPI_RESID ? "stream_residual_kernel" : EPI == EPI_LABELPROP ? "stream_labelprop_kernel"
-              : EPI == EPI_RESID_DEV ? "stream_dcoef_kernel" : EPI == EPI_ACCUM ? "stream_accum_kernel" : "stream_kernel",
+  note_kernel("cogdl_b200::stream%s_kernel<%s,NV=%d,%s%s%s,%s,U=%d,MINB=%d%s>", EPI_TAG[EPI],
               sizeof(VecT) == 16 ? "float4" : (sizeof(VecT) == 8 ? "float2" : "float"), NV,
               FORM == FORM_MULTIHEAD ? "multihead" : (p.val ? "weighted" : "unweighted"),
               (FORM == FORM_MULTIHEAD && p.perm) ? "+perm" : "", drop ? "+drop" : "",
@@ -645,23 +598,7 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
               PREFETCH ? ",prefetch" : "");
   if (FORM == FORM_PANEL && p.S > 1) append_kernel_note(",panels=%d", p.S);
   append_kernel_note(" block=%d", STREAM_BLOCK);
-  if constexpr (EPI == EPI_RESID) {
-    constexpr bool PANEL = FORM == FORM_PANEL;
-    if (p.val) stream_residual_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_residual_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-  } else if constexpr (EPI == EPI_LABELPROP) {
-    constexpr bool PANEL = FORM == FORM_PANEL;
-    if (p.val) stream_labelprop_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_labelprop_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-  } else if constexpr (EPI == EPI_RESID_DEV) {
-    constexpr bool PANEL = FORM == FORM_PANEL;
-    if (p.val) stream_dcoef_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_dcoef_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-  } else if constexpr (EPI == EPI_ACCUM) {
-    constexpr bool PANEL = FORM == FORM_PANEL;
-    if (p.val) stream_accum_kernel<VecT, NV, MODE_WEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_accum_kernel<VecT, NV, MODE_UNWEIGHTED, U, MINB, PREFETCH, PANEL><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-  } else if constexpr (FORM == FORM_MULTIHEAD) {
+  if constexpr (FORM == FORM_MULTIHEAD) {
     if (drop) {
       if (p.perm) stream_kernel<VecT, 1, MODE_MULTIHEAD, true, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
       else stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH, false, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
@@ -671,16 +608,19 @@ static int launch_stream(const StreamParams &p, cudaStream_t stream) {
       stream_kernel<VecT, 1, MODE_MULTIHEAD, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
     }
   } else if constexpr (FORM == FORM_PANEL) {
-    if (p.val) stream_kernel<VecT, 1, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_kernel<VecT, 1, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-  } else if (p.val) {
-    if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else if (src == SRC_TWO) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_TWO, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-  } else {
-    if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else if (src == SRC_TWO) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_TWO, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
-    else stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    if (p.val) stream_kernel<VecT, 1, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true, false, EPI><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_kernel<VecT, 1, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, true, false, EPI><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if (src == SRC_ONE) {
+    if (p.val) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, false, false, EPI><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    else stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_ONE, U, MINB, PREFETCH, false, false, EPI><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+  } else if constexpr (EPI == EPI_NONE) {       // the two-source and peer forms have no epilogue (turned away above)
+    if (p.val) {
+      if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+      else stream_kernel<VecT, NV, MODE_WEIGHTED, false, SRC_TWO, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    } else {
+      if (src == SRC_PEERS) stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_PEERS, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+      else stream_kernel<VecT, NV, MODE_UNWEIGHTED, false, SRC_TWO, U, MINB, PREFETCH><<<grid, STREAM_BLOCK, 0, stream>>>(p);
+    }
   }
   CB_LAUNCH_CHECK();
   return COGDL_B200_OK;

@@ -1,20 +1,8 @@
 """Every kernel compiled into gin.o and spmm_accum.o has a row in tests/gin_grand_table.py that the GPU suite runs
 (test_gpu_gin_grand.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The symbols
-are mapped to their recorded names through the residual inventory's note_of(): these kernels take the residual
-kernels' template parameters."""
+are mapped to their recorded names by test_cpu_kernel_inventory.py's note_of()."""
 from tests.gin_grand_table import TABLE
-from tests.test_cpu_kernel_inventory import canonical, compiled_kernels
-from tests.test_cpu_spmm_residual_inventory import note_of as residual_note_of
-
-_NAMES = (("spmm_dcoef_kernel", "spmm_residual_kernel"), ("stream_dcoef_kernel", "stream_residual_kernel"),
-          ("spmm_accum_kernel", "spmm_residual_kernel"), ("stream_accum_kernel", "stream_residual_kernel"))
-
-
-def note_of(sym):
-    for mine, theirs in _NAMES:
-        if f"cogdl_b200::{mine}<" in sym:
-            return residual_note_of(sym.replace(mine, theirs)).replace(theirs, mine)
-    raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
+from tests.test_cpu_kernel_inventory import canonical, compiled_kernels, note_of
 
 
 def _check(obj, epi):
@@ -53,8 +41,8 @@ def test_gin_grand_rows_are_distinct_and_cover_every_epilogue_form():
 
 
 def test_note_of_maps_gin_grand_symbols():
-    assert note_of("void cogdl_b200::stream_accum_kernel<float4, (int)1, (int)1, (int)4, (int)4, (bool)0, (bool)0>"
-                   "(cogdl_b200::StreamParams)") == \
+    assert note_of("void cogdl_b200::stream_kernel<float4, (int)1, (int)1, (bool)0, (int)0, (int)4, (int)4, (bool)0, "
+                   "(bool)0, (bool)0, (int)4>(cogdl_b200::StreamParams)") == \
         "cogdl_b200::stream_accum_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=4>"
-    assert note_of("void cogdl_b200::spmm_dcoef_kernel<float, (int)32, (int)4, (bool)0>(cogdl_b200::SpmmParams)") \
+    assert note_of("void cogdl_b200::spmm_kernel<float, (int)32, (int)4, (bool)0, (int)3>(cogdl_b200::SpmmParams)") \
         == "cogdl_b200::spmm_dcoef_kernel<float,GROUP=32,NV=4,unweighted>"

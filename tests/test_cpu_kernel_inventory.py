@@ -62,6 +62,8 @@ def compiled_kernels(objects=OBJECTS):
 
 
 _SRC = {0: "SRC_ONE", 1: "SRC_TWO", 2: "SRC_PEERS"}
+# the SpMM row and row-stream kernels are recorded as spmm<tag>_kernel / stream<tag>_kernel, by their epilogue argument
+_EPI_TAG = {0: "", 1: "_residual", 2: "_labelprop", 3: "_dcoef", 4: "_accum"}
 
 
 def _args(sig):
@@ -85,17 +87,18 @@ def note_of(sym):
     a = _args(m.group(2)) if m.group(2) else []
     w = lambda b: "weighted" if b else "unweighted"  # noqa: E731
     if name == "spmm_kernel":
-        vec, group, nv, has_val = a
-        return f"cogdl_b200::spmm_kernel<{vec},GROUP={group},NV={nv},{w(has_val)}>"
+        vec, group, nv, has_val, epi = a
+        return f"cogdl_b200::spmm{_EPI_TAG[epi]}_kernel<{vec},GROUP={group},NV={nv},{w(has_val)}>"
     if name == "spmm_half_kernel":
         has_val, vec = a
         return f"cogdl_b200::spmm_half_kernel<{w(has_val)},{'vec' if vec else 'scalar'}>"
     if name == "stream_kernel":
-        vec, nv, mode, perm, src, u, minb, prefetch, panel, drop = a
+        vec, nv, mode, perm, src, u, minb, prefetch, panel, drop, epi = a
         what = {0: "unweighted", 1: "weighted", 2: "multihead", 3: "comp_mult", 4: "comp_sub"}[mode]
         if mode == 2:
             what += ("+perm" if perm else "") + ("+drop" if drop else "")
-        s = f"cogdl_b200::stream_kernel<{vec},NV={nv},{what},{_SRC[src]},U={u},MINB={minb}{',prefetch' if prefetch else ''}>"
+        s = (f"cogdl_b200::stream{_EPI_TAG[epi]}_kernel<{vec},NV={nv},{what},{_SRC[src]},U={u},MINB={minb}"
+             f"{',prefetch' if prefetch else ''}>")
         return s + (",panels" if panel else "")
     if name == "sddmm_kernel":
         vec, group, sub, nv = a
@@ -159,10 +162,10 @@ def canonical(note):
 
 
 def test_note_of_maps_known_symbols():
-    assert note_of("void cogdl_b200::spmm_kernel<float, (int)32, (int)4, (bool)1>(cogdl_b200::SpmmParams)") == \
+    assert note_of("void cogdl_b200::spmm_kernel<float, (int)32, (int)4, (bool)1, (int)0>(cogdl_b200::SpmmParams)") == \
         "cogdl_b200::spmm_kernel<float,GROUP=32,NV=4,weighted>"
     assert note_of("void cogdl_b200::stream_kernel<float2, (int)1, (int)0, (bool)0, (int)0, (int)8, (int)5, (bool)1, "
-                   "(bool)1, (bool)0>(cogdl_b200::StreamParams)") == \
+                   "(bool)1, (bool)0, (int)0>(cogdl_b200::StreamParams)") == \
         "cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"
     assert canonical("cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels=4 block=128") \
         == ["cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"]
@@ -181,7 +184,7 @@ def test_note_of_maps_known_symbols():
         "cogdl_b200::stream_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=5>",
         "cogdl_b200::fg::fused_layer_kernel<sage-sum, 2 groups x tile 64xN, K=128, bf16x3 split, wgmma m64n32k16>"]
     assert note_of("void cogdl_b200::stream_kernel<float, (int)2, (int)4, (bool)0, (int)0, (int)2, (int)1, (bool)1, "
-                   "(bool)0, (bool)0>(cogdl_b200::StreamParams)") == \
+                   "(bool)0, (bool)0, (int)0>(cogdl_b200::StreamParams)") == \
         "cogdl_b200::stream_kernel<float,NV=2,comp_sub,SRC_ONE,U=2,MINB=1,prefetch>"
     assert note_of("void cogdl_b200::softmax_aggr_fwd_kernel<(int)4, (bool)1, (bool)0>(cogdl_b200::SaFwdParams)") == \
         "cogdl_b200::softmax_aggr_fwd_kernel<float4,edge_term,no_Q>"

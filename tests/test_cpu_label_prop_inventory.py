@@ -1,19 +1,8 @@
 """Every kernel compiled into label_prop.o has a row in tests/label_prop_table.py that the GPU suite runs
 (test_gpu_label_prop.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The
-symbols are mapped to their recorded names through the residual inventory's note_of(): the label-propagation kernels
-take the residual kernels' template parameters."""
+symbols are mapped to their recorded names by test_cpu_kernel_inventory.py's note_of()."""
 from tests.label_prop_table import TABLE
-from tests.test_cpu_kernel_inventory import canonical, compiled_kernels
-from tests.test_cpu_spmm_residual_inventory import note_of as residual_note_of
-
-_NAMES = (("spmm_labelprop_kernel", "spmm_residual_kernel"), ("stream_labelprop_kernel", "stream_residual_kernel"))
-
-
-def note_of(sym):
-    for mine, theirs in _NAMES:
-        if f"cogdl_b200::{mine}<" in sym:
-            return residual_note_of(sym.replace(mine, theirs)).replace(theirs, mine)
-    raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
+from tests.test_cpu_kernel_inventory import canonical, compiled_kernels, note_of
 
 
 def test_label_prop_table_covers_every_compiled_kernel():
@@ -45,8 +34,8 @@ def test_label_prop_rows_are_distinct_and_cover_every_epilogue():
 
 
 def test_note_of_maps_label_prop_symbols():
-    assert note_of("void cogdl_b200::stream_labelprop_kernel<float4, (int)1, (int)1, (int)4, (int)4, (bool)0, (bool)0>"
-                   "(cogdl_b200::StreamParams)") == \
+    assert note_of("void cogdl_b200::stream_kernel<float4, (int)1, (int)1, (bool)0, (int)0, (int)4, (int)4, (bool)0, "
+                   "(bool)0, (bool)0, (int)2>(cogdl_b200::StreamParams)") == \
         "cogdl_b200::stream_labelprop_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=4>"
-    assert note_of("void cogdl_b200::spmm_labelprop_kernel<float, (int)32, (int)4, (bool)0>(cogdl_b200::SpmmParams)") \
+    assert note_of("void cogdl_b200::spmm_kernel<float, (int)32, (int)4, (bool)0, (int)2>(cogdl_b200::SpmmParams)") \
         == "cogdl_b200::spmm_labelprop_kernel<float,GROUP=32,NV=4,unweighted>"

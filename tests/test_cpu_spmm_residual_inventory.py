@@ -1,27 +1,9 @@
 """Every kernel compiled into spmm_residual.o has a row in tests/spmm_residual_table.py that the GPU suite runs
 (test_gpu_spmm_residual.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The
-kernel entry points are read from the object as in test_cpu_kernel_inventory.py and mapped to the string their
-launchers record for cogdl_b200_last_kernel()."""
-import re
-
+kernel entry points are read from the object and mapped to the string their launchers record for
+cogdl_b200_last_kernel() by test_cpu_kernel_inventory.py."""
 from tests.spmm_residual_table import TABLE
-from tests.test_cpu_kernel_inventory import _SRC, _args, canonical, compiled_kernels
-
-
-def note_of(sym):
-    m = re.fullmatch(r"void cogdl_b200::(\w+)(<.*>)\(.*\)", sym)
-    assert m, f"unexpected symbol {sym!r}"
-    name, a = m.group(1), _args(m.group(2))
-    w = lambda b: "weighted" if b else "unweighted"  # noqa: E731
-    if name == "spmm_residual_kernel":
-        vec, group, nv, has_val = a
-        return f"cogdl_b200::spmm_residual_kernel<{vec},GROUP={group},NV={nv},{w(has_val)}>"
-    if name == "stream_residual_kernel":
-        vec, nv, mode, u, minb, prefetch, panel = a
-        s = (f"cogdl_b200::stream_residual_kernel<{vec},NV={nv},{w(mode == 1)},{_SRC[0]},U={u},MINB={minb}"
-             f"{',prefetch' if prefetch else ''}>")
-        return s + (",panels" if panel else "")
-    raise AssertionError(f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table")
+from tests.test_cpu_kernel_inventory import canonical, compiled_kernels, note_of
 
 
 def test_residual_table_covers_every_compiled_kernel():
@@ -48,8 +30,8 @@ def test_residual_rows_are_distinct_and_cover_both_epilogue_inputs():
 
 
 def test_note_of_maps_residual_symbols():
-    assert note_of("void cogdl_b200::stream_residual_kernel<float4, (int)1, (int)1, (int)4, (int)4, (bool)0, (bool)0>"
-                   "(cogdl_b200::StreamParams)") == \
+    assert note_of("void cogdl_b200::stream_kernel<float4, (int)1, (int)1, (bool)0, (int)0, (int)4, (int)4, (bool)0, "
+                   "(bool)0, (bool)0, (int)1>(cogdl_b200::StreamParams)") == \
         "cogdl_b200::stream_residual_kernel<float4,NV=1,weighted,SRC_ONE,U=4,MINB=4>"
-    assert note_of("void cogdl_b200::spmm_residual_kernel<float, (int)32, (int)4, (bool)0>(cogdl_b200::SpmmParams)") \
+    assert note_of("void cogdl_b200::spmm_kernel<float, (int)32, (int)4, (bool)0, (int)1>(cogdl_b200::SpmmParams)") \
         == "cogdl_b200::spmm_residual_kernel<float,GROUP=32,NV=4,unweighted>"
