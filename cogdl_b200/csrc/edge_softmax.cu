@@ -5,8 +5,8 @@
 // one block of 32 x H threads per row, three passes over the row with lanes striding H floats apart
 // -- <= 1/H sector efficiency -- and exp() evaluated twice) and, in MODE 2 / 3, the
 // `leakyrelu(h_l[row] + h_r[col])` gathers + LeakyReLU + edge_softmax chain of
-// cogdl/layers/gat_layer.py:73-74 and its autograd backward.  The kernel bodies live in edge_softmax.cuh, which
-// simple_hgn.cu instantiates with Simple-HGN's edge-type term and residual attention.
+// cogdl/layers/gat_layer.py:73-74 and its autograd backward.  The kernels and their launch plan live in
+// edge_softmax.cuh, which simple_hgn.cu launches with Simple-HGN's edge-type term and residual attention.
 //
 // Key layout fact: in CSR order the [deg, H] logits of row i are ONE contiguous block of deg*H floats
 // at rowptr[i]*H, and consecutive rows are consecutive blocks.  With H a power of two <= 32, the
@@ -49,73 +49,6 @@
 
 namespace cogdl_b200 {
 
-// The kernels: the bodies of edge_softmax.cuh without the type term or the residual blend.
-template <int MODE, bool DROP>
-__global__ void __launch_bounds__(256) es_warp_kernel(const EsParams p) {
-  es_warp_body<MODE, DROP, false, false>(p, nullptr);
-}
-
-template <int MODE, bool DROP>
-__global__ void __launch_bounds__(256) es_stats_kernel(const EsParams p) {
-  es_stats_body<MODE, DROP, false>(p, nullptr);
-}
-
-template <int MODE, int CAP, int WARPS, bool DROP>
-__global__ void __launch_bounds__(WARPS * 32) es_main_kernel(const EsParams p) {
-  es_main_body<MODE, CAP, WARPS, DROP, false, false>(p, nullptr);
-}
-
-template <int MODE, bool DROP>
-__global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
-  es_generic_body<MODE, DROP, false, false>(p, nullptr);
-}
-
-template <int MODE, int CAP, bool DROP>
-static int launch_main(const EsParams &p, cudaStream_t s) {
-  static unsigned long long attr_done = 0;
-  return es_launch_main(es_main_kernel<MODE, CAP, ES_WARPS, DROP>, es_main_smem<MODE, CAP>(), attr_done, p, s);
-}
-
-// Launch plan (see the header comment).  DROP only with MODE 2 / 3.
-template <int MODE, bool DROP = false>
-static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t s, const char *who) {
-  static_assert(!DROP || MODE == 2 || MODE == 3, "attention dropout is a mode of the GAT attention and its backward");
-  const char *drop_note = DROP ? ",DROP" : "";
-  const int64_t row_blocks = ceil_div(p.n_rows * 32, 256);
-  CB_REQUIRE(row_blocks <= 0x7fffffffLL, "%s: problem too large for one launch", who);
-  EsForm form;
-  int chosen;
-  int rc = es_plan<MODE>(p, plan, &form, &chosen);
-  if (rc) return rc;
-  if (form == EsForm::GENERIC) {
-    note_kernel("cogdl_b200::es_generic_kernel<MODE=%d%s>", MODE, drop_note);
-    es_generic_kernel<MODE, DROP><<<(unsigned)row_blocks, 256, 0, s>>>(p);
-    CB_LAUNCH_CHECK();
-    return COGDL_B200_OK;
-  }
-  if (form == EsForm::WARP) {
-    note_kernel("cogdl_b200::es_warp_kernel<MODE=%d%s>", MODE, drop_note);
-    es_warp_kernel<MODE, DROP><<<(unsigned)row_blocks, 256, 0, s>>>(p);
-    CB_LAUNCH_CHECK();
-    return COGDL_B200_OK;
-  }
-  if (p.hub.n_chunks > 0) {
-    // the attention's statistics come before the dropout: MODE 2 shares the kernel without DROP
-    es_stats_kernel<MODE, DROP && MODE == 3><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
-    CB_LAUNCH_CHECK();
-  }
-  // both launches, in launch order, when the statistics kernel ran
-  char stats_note[64] = "";
-  if (p.hub.n_chunks > 0)
-    snprintf(stats_note, sizeof(stats_note), "cogdl_b200::es_stats_kernel<MODE=%d%s> + ", MODE,
-             (DROP && MODE == 3) ? ",DROP" : "");
-  note_kernel("%scogdl_b200::es_main_kernel<MODE=%d,CAP=%d,WARPS=%d%s>%s", stats_note, MODE, chosen, ES_WARPS,
-              drop_note, (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
-  if (chosen == 512) return launch_main<MODE, 512, DROP>(p, s);
-  if (chosen == 1024) return launch_main<MODE, 1024, DROP>(p, s);
-  return launch_main<MODE, 2048, DROP>(p, s);
-}
-
 template <int MODE>
 static int es_entry(const int32_t *rowptr, const float *a, const float *b, float *out, int64_t n_rows,
                     int64_t H, const cogdl_b200_hub_plan_t *plan, cogdl_b200_stream_t stream,
@@ -126,9 +59,7 @@ static int es_entry(const int32_t *rowptr, const float *a, const float *b, float
   CB_REQUIRE(n_rows < 0x7fffffffLL && H < 0x7fffffffLL, "%s: sizes must fit int32", who);
   EsParams p;
   p.rowptr = rowptr; p.a = a; p.b = b; p.out = out; p.n_rows = n_rows; p.H = (int)H;
-  p.colind = nullptr; p.slope = 0.f; p.hl = nullptr; p.hr = nullptr; p.grow = nullptr;
-  p.seed = 0; p.drop_below = 0; p.scale = 1.f;
-  return es_launch<MODE>(p, plan, (cudaStream_t)stream, who);
+  return es_launch<MODE, false, false, false>(p, plan, (cudaStream_t)stream, who);
 }
 
 // GAT attention (used by cogdl_b200_gat_fwd_f32 / _dropout_f32, mhspmm.cu): att = softmax_row(leakyrelu(h_l[row] +
@@ -138,10 +69,9 @@ int gat_attention(const int32_t *rowptr, const int32_t *colind, const float *h_l
                   bool drop, uint64_t seed, uint64_t drop_below) {
   EsParams p;
   p.rowptr = rowptr; p.a = h_l; p.b = h_r; p.out = att; p.n_rows = n_rows; p.H = (int)H;
-  p.colind = colind; p.slope = slope; p.hl = nullptr; p.hr = nullptr; p.grow = nullptr;
-  p.seed = seed; p.drop_below = drop_below; p.scale = 1.f;
-  if (drop) return es_launch<2, true>(p, plan, s, "cogdl_b200_gat_fwd_dropout_f32");
-  return es_launch<2>(p, plan, s, "cogdl_b200_gat_fwd_f32");
+  p.colind = colind; p.slope = slope; p.seed = seed; p.drop_below = drop_below;
+  if (drop) return es_launch<2, true, false, false>(p, plan, s, "cogdl_b200_gat_fwd_dropout_f32");
+  return es_launch<2, false, false, false>(p, plan, s, "cogdl_b200_gat_fwd_f32");
 }
 
 }  // namespace cogdl_b200
@@ -179,9 +109,8 @@ static int gat_attn_bwd(const int32_t *rowptr, const int32_t *colind, const floa
   CB_REQUIRE(n_rows < 0x7fffffffLL && H < 0x7fffffffLL, "%s: sizes must fit int32", who);
   EsParams p;
   p.rowptr = rowptr; p.a = att; p.b = d_att; p.out = d_edge; p.n_rows = n_rows; p.H = (int)H;
-  p.colind = colind; p.slope = negative_slope; p.hl = h_l; p.hr = h_r; p.grow = g_row;
-  p.seed = 0; p.drop_below = 0; p.scale = scale;
-  return es_launch<3, DROP>(p, plan, (cudaStream_t)stream, who);
+  p.colind = colind; p.slope = negative_slope; p.hl = h_l; p.hr = h_r; p.grow = g_row; p.scale = scale;
+  return es_launch<3, DROP, false, false>(p, plan, (cudaStream_t)stream, who);
 }
 
 extern "C" int cogdl_b200_gat_attn_bwd_f32(const int32_t *rowptr, const int32_t *colind, const float *att,

@@ -1,12 +1,11 @@
-// edge_softmax.cuh -- the per-row softmax machinery of edge_softmax.cu (MODES 0-3, see its header comment), shared
-// with simple_hgn.cu, which instantiates the attention forms with two more flags:
+// edge_softmax.cuh -- the per-row softmax kernels of edge_softmax.cu (MODES 0-3, see its header comment) and their
+// launch plan, es_launch.  simple_hgn.cu launches the attention forms with two more flags:
 //   TYPED (MODES 2, 3): the logit gains a per-edge-type term, leakyrelu(h_l[row,h] + h_r[col,h] + h_e[type[p],h]),
 //          h_e [T, H] staged in shared memory by the kernel (`tab`), type [nnz] int32 in CSR slot order;
 //   MIX   (MODE 2, TYPED only): besides the signed softmax (out, nullable), the kernel writes the attention the layer
 //          returns, mix = (1 - alpha) * (dropped ? 0 : a * keep_scale) + alpha * res[p,h]; without MIX it is
 //          (dropped ? 0 : a * keep_scale).
-// The kernels of edge_softmax.cu are thin wrappers that instantiate the bodies below with TYPED = MIX = false and
-// tab = nullptr, so their names and work are those of the code before the split.
+// edge_softmax.cu launches them with TYPED = MIX = false.
 #pragma once
 #include "common.cuh"
 #include "rng.cuh"
@@ -27,18 +26,18 @@ struct EsParams {
   int64_t n_rows;
   int H;
   int lgH;
-  const int *colind;      // MODE 2, 3
-  float slope;            // MODE 2, 3
-  const float *hl;        // MODE 3: h_l [N,H]
-  const float *hr;        // MODE 3: h_r [N,H]
-  float *grow;            // MODE 3: [N,H] row sums of the output
+  const int *colind = nullptr;  // MODE 2, 3
+  float slope = 0.f;            // MODE 2, 3
+  const float *hl = nullptr;    // MODE 3: h_l [N,H]
+  const float *hr = nullptr;    // MODE 3: h_r [N,H]
+  float *grow = nullptr;        // MODE 3: [N,H] row sums of the output
   HubView hub;            // chunks / segments / edge_row / counters
   float2 *stats;          // per chunk slot x head: (max, sum) -- the row's merged value sits in its first slot
   float *part;            // MODE 3: per chunk slot x head partial row sums
   bool bulk;              // tiles may be moved with cp.async.bulk (alignment checked on the host)
-  uint64_t seed;          // DROP: attention-dropout mask (see the header comment of edge_softmax.cu)
-  uint64_t drop_below;
-  float scale;            // DROP, MODE 3: the factor d att is multiplied by on a kept entry
+  uint64_t seed = 0;            // DROP: attention-dropout mask (see the header comment of edge_softmax.cu)
+  uint64_t drop_below = 0;
+  float scale = 1.f;            // DROP, MODE 3: the factor d att is multiplied by on a kept entry
   // TYPED / MIX (simple_hgn.cu)
   const int *etype = nullptr;   // TYPED: edge type of each CSR slot, in [0, T)
   const float *he = nullptr;    // TYPED: h_e [T, H], copied to `tab` by the kernel
@@ -85,13 +84,17 @@ __device__ __forceinline__ float es_typed(const EsParams &p, const float *tab, i
   return z;
 }
 
-// TYPED: copy h_e into the block's table (every thread of the block calls this before any early exit)
-template <bool TYPED>
-__device__ __forceinline__ void es_stage_table(const EsParams &p, float *tab) {
-  if (TYPED) {
-    for (int i = threadIdx.x; i < p.n_table; i += blockDim.x) tab[i] = __ldg(p.he + i);
+constexpr int HGN_MAX_TABLE = 1024;   // the largest T * H: the floats of a kernel's static shared table for h_e
+
+// TAB (the kernel reads the type term): copy h_e into the block's table, declared table[TAB ? HGN_MAX_TABLE : 1], and
+// return it; else return null.  Every thread of the block calls this before any early exit.
+template <bool TAB>
+__device__ __forceinline__ const float *es_stage_table(const EsParams &p, float *table) {
+  if (TAB) {
+    for (int i = threadIdx.x; i < p.n_table; i += blockDim.x) table[i] = __ldg(p.he + i);
     __syncthreads();
   }
+  return TAB ? table : nullptr;
 }
 
 // exp for the plan-based kernels: arguments are x - max <= 0.  ex2.approx(x * log2 e): 2 ulp from the MUFU plus
@@ -209,7 +212,9 @@ __device__ __forceinline__ void es_row(const EsParams &p, const float *tab, int6
 
 // ---------------------------------------------------------------- warp per row (no plan)
 template <int MODE, bool DROP, bool TYPED, bool MIX>
-__device__ __forceinline__ void es_warp_body(const EsParams &p, const float *tab) {
+__global__ void __launch_bounds__(256) es_warp_kernel(const EsParams p) {
+  __shared__ float table[TYPED ? HGN_MAX_TABLE : 1];
+  const float *tab = es_stage_table<TYPED>(p, table);
   const int lane = threadIdx.x & 31;
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (row >= p.n_rows) return;  // whole warp
@@ -226,9 +231,13 @@ __device__ __forceinline__ void es_warp_body(const EsParams &p, const float *tab
 
 // ---------------------------------------------------------------- hub chunks, pass 1: statistics
 // One warp per chunk slot.  Forward / attention: (max, sum exp(x - max)) per head; backward: sum y*g.
-// The last chunk of the row to arrive merges the chunks' values in chunk order into stats[first].
+// The last chunk of the row to arrive merges the chunks' values in chunk order into stats[first].  A typed MODE 3
+// sums a * g and forms no logit, so of the typed forms only MODE 2 reads the type table.
 template <int MODE, bool DROP, bool TYPED>
-__device__ __forceinline__ void es_stats_body(const EsParams &p, const float *tab) {
+__global__ void __launch_bounds__(256) es_stats_kernel(const EsParams p) {
+  constexpr bool TAB = TYPED && MODE == 2;
+  __shared__ float table[TAB ? HGN_MAX_TABLE : 1];
+  const float *tab = es_stage_table<TAB>(p, table);
   // programmatic dependent launch: the main kernel may start as soon as every CTA of this grid is running; its
   // segment items need nothing from us, its chunk items wait (griddepcontrol.wait) for this grid to finish
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -249,9 +258,9 @@ __device__ __forceinline__ void es_stats_body(const EsParams &p, const float *ta
     s = head_sum(s, H);
   } else {
     const float hl = (MODE == 2) ? __ldg(p.a + (int64_t)w.row * H + head) : 0.f;
-    for (int t = lane; t < n; t += 32) m = fmaxf(m, es_in<MODE, TYPED>(p, tab, w.lb, t, head, hl));
+    for (int t = lane; t < n; t += 32) m = fmaxf(m, es_in<MODE, TAB>(p, tab, w.lb, t, head, hl));
     m = head_max(m, H);
-    for (int t = lane; t < n; t += 32) s += es_exp(es_in<MODE, TYPED>(p, tab, w.lb, t, head, hl) - m);   // L1 hits
+    for (int t = lane; t < n; t += 32) s += es_exp(es_in<MODE, TAB>(p, tab, w.lb, t, head, hl) - m);   // L1 hits
     s = head_sum(s, H);
   }
   if (lane < H) {
@@ -301,7 +310,7 @@ __device__ __forceinline__ void es_stats_body(const EsParams &p, const float *ta
   }
 }
 
-// ---------------------------------------------------------------- hub chunk, pass 2 (shared by both main kernels)
+// ---------------------------------------------------------------- hub chunk, pass 2 (a chunk item of the main kernel)
 // normalise the chunk's elements with its row's merged statistics (stats[first slot])
 template <int MODE, bool DROP, bool TYPED, bool MIX>
 __device__ __forceinline__ void es_chunk_item(const EsParams &p, const float *tab, int64_t item, int lane) {
@@ -382,16 +391,23 @@ __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------- main kernel: chunks + segments
-// Shared memory per warp: CAP floats (+ CAP for the backward's second operand) + 33 row offsets.
-template <int MODE, int CAP, int WARPS, bool DROP, bool TYPED, bool MIX>
-__device__ __forceinline__ void es_main_body(const EsParams &p, const float *tab) {
+// Warps per block of the main kernel.  For the 512-float tile this is a launch parameter only (2 and 4 warps give
+// bit-identical outputs); a block's shared memory and warp slots are released when its slowest warp retires, and 8
+// is the shape the whole GPU suite is validated with.
+constexpr int ES_WARPS = 8;
+
+// Dynamic shared memory per warp: CAP floats (+ CAP for the backward's second operand) + 33 row offsets.
+template <int MODE, int CAP, bool DROP, bool TYPED, bool MIX>
+__global__ void __launch_bounds__(ES_WARPS * 32) es_main_kernel(const EsParams p) {
+  __shared__ float table[TYPED ? HGN_MAX_TABLE : 1];
+  const float *tab = es_stage_table<TYPED>(p, table);
   constexpr bool TWO = (MODE == 1 || MODE == 3);
   extern __shared__ __align__(128) unsigned char es_smem[];
   float *tiles = reinterpret_cast<float *>(es_smem);
-  int *rps = reinterpret_cast<int *>(es_smem + (size_t)WARPS * CAP * 4 * (TWO ? 2 : 1));
-  uint64_t *bars = reinterpret_cast<uint64_t *>(rps + WARPS * 34);
+  int *rps = reinterpret_cast<int *>(es_smem + (size_t)ES_WARPS * CAP * 4 * (TWO ? 2 : 1));
+  uint64_t *bars = reinterpret_cast<uint64_t *>(rps + ES_WARPS * 34);
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int64_t item = (int64_t)blockIdx.x * WARPS + wib;
+  const int64_t item = (int64_t)blockIdx.x * ES_WARPS + wib;
   const int H = p.H;
 
   // ------------------------------------------------ hub chunk (LAST in the grid): normalise with the row's merged
@@ -560,7 +576,9 @@ __device__ __forceinline__ void es_main_body(const EsParams &p, const float *tab
 
 // ---------------------------------------------------------------- generic H: warp per row, loop over heads
 template <int MODE, bool DROP, bool TYPED, bool MIX>
-__device__ __forceinline__ void es_generic_body(const EsParams &p, const float *tab) {
+__global__ void __launch_bounds__(256) es_generic_kernel(const EsParams p) {
+  __shared__ float table[TYPED ? HGN_MAX_TABLE : 1];
+  const float *tab = es_stage_table<TYPED>(p, table);
   const int lane = threadIdx.x & 31;
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (row >= p.n_rows) return;
@@ -616,21 +634,14 @@ __device__ __forceinline__ void es_generic_body(const EsParams &p, const float *
   }
 }
 
-// Warps per block of the main kernel.  For the 512-float tile this is a launch parameter only (2 and 4 warps give
-// bit-identical outputs); a block's shared memory and warp slots are released when its slowest warp retires, and 8
-// is the shape the whole GPU suite is validated with.
-constexpr int ES_WARPS = 8;
-
-// Dynamic shared memory of the main kernel with a CAP-float tile.
-template <int MODE, int CAP>
-constexpr size_t es_main_smem() {
-  return (size_t)ES_WARPS * CAP * 4 * ((MODE == 1 || MODE == 3) ? 2 : 1) + (size_t)ES_WARPS * 34 * 4 + (size_t)ES_WARPS * 8;
-}
-
-// Launch one main kernel (segments first, hub chunks last) on the items of p's plan; attr_done is the kernel's own
-// per-device record of its shared-memory attribute.
-template <typename Kernel>
-static int es_launch_main(Kernel kernel, size_t smem, unsigned long long &attr_done, const EsParams &p, cudaStream_t s) {
+// Launch the main kernel (segments first, hub chunks last) on the items of p's plan.
+template <int MODE, int CAP, bool DROP, bool TYPED, bool MIX>
+static int es_launch_main(const EsParams &p, cudaStream_t s) {
+  const auto kernel = es_main_kernel<MODE, CAP, DROP, TYPED, MIX>;
+  // per warp: the tile(s), the row offsets and the mbarrier
+  constexpr size_t smem = (size_t)ES_WARPS * CAP * 4 * ((MODE == 1 || MODE == 3) ? 2 : 1) + (size_t)ES_WARPS * 34 * 4 +
+                          (size_t)ES_WARPS * 8;
+  static unsigned long long attr_done = 0;   // the kernel's per-device record of its shared-memory attribute
   int dev = 0;
   if (first_use_on_device(attr_done, &dev))
     CB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -645,7 +656,7 @@ static int es_launch_main(Kernel kernel, size_t smem, unsigned long long &attr_d
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;     // overlap with the statistics kernel (see es_stats_body)
+  attr[0].val.programmaticStreamSerializationAllowed = 1;   // overlap with the statistics kernel (see es_stats_kernel)
   cfg.attrs = attr;
   cfg.numAttrs = p.hub.n_chunks > 0 ? 1 : 0;
   CB_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
@@ -688,6 +699,54 @@ static int es_plan(EsParams &p, const cogdl_b200_hub_plan_t *plan, EsForm *form,
   *form = EsForm::MAIN;
   *cap = cap_need <= 512 ? 512 : (cap_need <= 1024 ? 1024 : 2048);
   return COGDL_B200_OK;
+}
+
+// The launch plan (see the header comment of edge_softmax.cu).  The typed MODE 3 always reads the signed attention
+// (DROP): its gradient scale applies with or without dropout.  cogdl_b200_last_kernel() records the launches as
+// es_*_kernel, or hgn_*_kernel when TYPED; of the two name formats only the es_ one names the main kernel's warps per
+// block, and the DROP of the MODE-3 statistics kernel.
+template <int MODE, bool DROP, bool TYPED, bool MIX>
+static int es_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t s, const char *who) {
+  static_assert(!DROP || MODE == 2 || MODE == 3, "attention dropout is a mode of the GAT attention and its backward");
+  static_assert(TYPED ? MODE == 2 || (MODE == 3 && DROP && !MIX) : !MIX,
+                "the typed kernels are the attention and its backward, and only the typed attention blends");
+  const char *fam = TYPED ? "hgn" : "es";
+  const char *flags = DROP ? (MIX ? ",DROP,MIX" : ",DROP") : (MIX ? ",MIX" : "");
+  const int64_t row_blocks = ceil_div(p.n_rows * 32, 256);
+  CB_REQUIRE(row_blocks <= 0x7fffffffLL, "%s: problem too large for one launch", who);
+  EsForm form;
+  int chosen;
+  int rc = es_plan<MODE>(p, plan, &form, &chosen);
+  if (rc) return rc;
+  if (form == EsForm::GENERIC) {
+    note_kernel("cogdl_b200::%s_generic_kernel<MODE=%d%s>", fam, MODE, flags);
+    es_generic_kernel<MODE, DROP, TYPED, MIX><<<(unsigned)row_blocks, 256, 0, s>>>(p);
+    CB_LAUNCH_CHECK();
+    return COGDL_B200_OK;
+  }
+  if (form == EsForm::WARP) {
+    note_kernel("cogdl_b200::%s_warp_kernel<MODE=%d%s>", fam, MODE, flags);
+    es_warp_kernel<MODE, DROP, TYPED, MIX><<<(unsigned)row_blocks, 256, 0, s>>>(p);
+    CB_LAUNCH_CHECK();
+    return COGDL_B200_OK;
+  }
+  // both launches, in launch order, when the statistics kernel runs
+  char stats_note[64] = "";
+  if (p.hub.n_chunks > 0) {
+    // the attention's statistics come before the dropout: MODE 2 shares the kernel without DROP
+    constexpr bool SDROP = DROP && MODE == 3;
+    es_stats_kernel<MODE, SDROP, TYPED><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
+    CB_LAUNCH_CHECK();
+    snprintf(stats_note, sizeof(stats_note), "cogdl_b200::%s_stats_kernel<MODE=%d%s> + ", fam, MODE,
+             (SDROP && !TYPED) ? ",DROP" : "");
+  }
+  char warps[16] = "";
+  if (!TYPED) snprintf(warps, sizeof(warps), ",WARPS=%d", ES_WARPS);
+  note_kernel("%scogdl_b200::%s_main_kernel<MODE=%d,CAP=%d%s%s>%s", stats_note, fam, MODE, chosen, warps, flags,
+              (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
+  if (chosen == 512) return es_launch_main<MODE, 512, DROP, TYPED, MIX>(p, s);
+  if (chosen == 1024) return es_launch_main<MODE, 1024, DROP, TYPED, MIX>(p, s);
+  return es_launch_main<MODE, 2048, DROP, TYPED, MIX>(p, s);
 }
 
 }  // namespace cogdl_b200

@@ -15,85 +15,12 @@
 // with gscale = (1 - alpha) / (1 - p_drop), in one pass.  The rest of the backward is existing code: the CSC
 // mh-SpMM over mix for d h, edge_colsum for d h_r and the SpMM over the type-grouped slots for d h_e.
 //
+// The kernels and their launch plan are edge_softmax.cuh's, launched with TYPED (and MIX when res is given).
 // h_e [T, H] is staged in a static shared-memory table of HGN_MAX_TABLE floats per block (4 KB: no kernel loses
 // occupancy to it); larger tables are rejected before any launch.
 #include "edge_softmax.cuh"
 
 namespace cogdl_b200 {
-
-constexpr int HGN_MAX_TABLE = 1024;   // T * H
-
-template <int MODE, bool DROP, bool MIX>
-__global__ void __launch_bounds__(256) hgn_warp_kernel(const EsParams p) {
-  __shared__ float tab[HGN_MAX_TABLE];
-  es_stage_table<true>(p, tab);
-  es_warp_body<MODE, DROP, true, MIX>(p, tab);
-}
-
-template <int MODE, bool DROP, bool MIX>
-__global__ void __launch_bounds__(256) hgn_generic_kernel(const EsParams p) {
-  __shared__ float tab[HGN_MAX_TABLE];
-  es_stage_table<true>(p, tab);
-  es_generic_body<MODE, DROP, true, MIX>(p, tab);
-}
-
-// Hub-chunk statistics: MODE 2 forms the typed logits; MODE 3 (sum of a * g over the chunk) reads no logit.
-template <int MODE>
-__global__ void __launch_bounds__(256) hgn_stats_kernel(const EsParams p) {
-  __shared__ float tab[MODE == 2 ? HGN_MAX_TABLE : 1];
-  es_stage_table<MODE == 2>(p, tab);
-  es_stats_body<MODE, MODE == 3, MODE == 2>(p, tab);
-}
-
-template <int MODE, int CAP, bool DROP, bool MIX>
-__global__ void __launch_bounds__(ES_WARPS * 32) hgn_main_kernel(const EsParams p) {
-  __shared__ float tab[HGN_MAX_TABLE];
-  es_stage_table<true>(p, tab);
-  es_main_body<MODE, CAP, ES_WARPS, DROP, true, MIX>(p, tab);
-}
-
-template <int MODE, int CAP, bool DROP, bool MIX>
-static int hgn_launch_main(const EsParams &p, cudaStream_t s) {
-  static unsigned long long attr_done = 0;
-  return es_launch_main(hgn_main_kernel<MODE, CAP, DROP, MIX>, es_main_smem<MODE, CAP>(), attr_done, p, s);
-}
-
-// The launch plan of es_launch (edge_softmax.cu) over the hgn kernels.  MODE 3 always reads the signed attention
-// (DROP): its gradient scale applies with or without dropout.
-template <int MODE, bool DROP, bool MIX>
-static int hgn_launch(EsParams p, const cogdl_b200_hub_plan_t *plan, cudaStream_t s, const char *who) {
-  static_assert(MODE == 2 || (MODE == 3 && DROP && !MIX), "the hgn kernels are the attention and its backward");
-  const char *flags = DROP ? (MIX ? ",DROP,MIX" : ",DROP") : (MIX ? ",MIX" : "");
-  const int64_t row_blocks = ceil_div(p.n_rows * 32, 256);
-  CB_REQUIRE(row_blocks <= 0x7fffffffLL, "%s: problem too large for one launch", who);
-  EsForm form;
-  int chosen;
-  int rc = es_plan<MODE>(p, plan, &form, &chosen);
-  if (rc) return rc;
-  if (form == EsForm::GENERIC) {
-    note_kernel("cogdl_b200::hgn_generic_kernel<MODE=%d%s>", MODE, flags);
-    hgn_generic_kernel<MODE, DROP, MIX><<<(unsigned)row_blocks, 256, 0, s>>>(p);
-    CB_LAUNCH_CHECK();
-    return COGDL_B200_OK;
-  }
-  if (form == EsForm::WARP) {
-    note_kernel("cogdl_b200::hgn_warp_kernel<MODE=%d%s>", MODE, flags);
-    hgn_warp_kernel<MODE, DROP, MIX><<<(unsigned)row_blocks, 256, 0, s>>>(p);
-    CB_LAUNCH_CHECK();
-    return COGDL_B200_OK;
-  }
-  char stats_note[64] = "";
-  if (p.hub.n_chunks > 0) {
-    hgn_stats_kernel<MODE><<<(unsigned)ceil_div((int64_t)p.hub.n_chunks * 32, 256), 256, 0, s>>>(p);
-    CB_LAUNCH_CHECK();
-    snprintf(stats_note, sizeof(stats_note), "cogdl_b200::hgn_stats_kernel<MODE=%d> + ", MODE);
-  }
-  note_kernel("%scogdl_b200::hgn_main_kernel<MODE=%d,CAP=%d%s>%s", stats_note, MODE, chosen, flags,
-              (p.bulk && MODE != 2) ? " cp.async.bulk tiles" : "");
-  if (chosen == 512) return hgn_launch_main<MODE, 512, DROP, MIX>(p, s);
-  if (chosen == 1024) return hgn_launch_main<MODE, 1024, DROP, MIX>(p, s);
-  return hgn_launch_main<MODE, 2048, DROP, MIX>(p, s);
-}
 
 static int hgn_check(int64_t n_rows, int64_t H, int64_t T, const char *who) {
   CB_REQUIRE(n_rows >= 0 && H >= 0, "%s: negative size", who);
@@ -124,14 +51,14 @@ extern "C" int cogdl_b200_hgn_attn_f32(const int32_t *rowptr, const int32_t *col
   CB_REQUIRE(rowptr && colind && etype && h_l && h_r && h_e && mix_out, "%s: null pointer", who);
   EsParams p;
   p.rowptr = rowptr; p.a = h_l; p.b = h_r; p.out = att_out; p.n_rows = n_rows; p.H = (int)H;
-  p.colind = colind; p.slope = negative_slope; p.hl = nullptr; p.hr = nullptr; p.grow = nullptr;
-  p.seed = seed; p.drop_below = drop_below; p.scale = 1.f;
+  p.colind = colind; p.slope = negative_slope; p.seed = seed; p.drop_below = drop_below;
   p.etype = etype; p.he = h_e; p.n_table = (int)(T * H); p.mix = mix_out; p.res = res_attn;
   p.alpha = alpha; p.keep = 1.f - alpha; p.keep_scale = scale;
   cudaStream_t s = (cudaStream_t)stream;
   const bool drop = drop_below > 0, mix = res_attn != nullptr;
-  if (drop) return mix ? hgn_launch<2, true, true>(p, plan, s, who) : hgn_launch<2, true, false>(p, plan, s, who);
-  return mix ? hgn_launch<2, false, true>(p, plan, s, who) : hgn_launch<2, false, false>(p, plan, s, who);
+  if (drop)
+    return mix ? es_launch<2, true, true, true>(p, plan, s, who) : es_launch<2, true, true, false>(p, plan, s, who);
+  return mix ? es_launch<2, false, true, true>(p, plan, s, who) : es_launch<2, false, true, false>(p, plan, s, who);
 }
 
 extern "C" int cogdl_b200_hgn_attn_bwd_f32(const int32_t *rowptr, const int32_t *colind, const int32_t *etype,
@@ -147,8 +74,7 @@ extern "C" int cogdl_b200_hgn_attn_bwd_f32(const int32_t *rowptr, const int32_t 
   CB_REQUIRE(rowptr && colind && etype && att && d_mix && h_l && h_r && h_e && d_edge && g_row, "%s: null pointer", who);
   EsParams p;
   p.rowptr = rowptr; p.a = att; p.b = d_mix; p.out = d_edge; p.n_rows = n_rows; p.H = (int)H;
-  p.colind = colind; p.slope = negative_slope; p.hl = h_l; p.hr = h_r; p.grow = g_row;
-  p.seed = 0; p.drop_below = 0; p.scale = grad_scale;
+  p.colind = colind; p.slope = negative_slope; p.hl = h_l; p.hr = h_r; p.grow = g_row; p.scale = grad_scale;
   p.etype = etype; p.he = h_e; p.n_table = (int)(T * H);
-  return hgn_launch<3, true, false>(p, plan, (cudaStream_t)stream, who);
+  return es_launch<3, true, true, false>(p, plan, (cudaStream_t)stream, who);
 }

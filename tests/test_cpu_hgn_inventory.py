@@ -1,22 +1,8 @@
 """Every kernel compiled into simple_hgn.o has a row in tests/hgn_table.py that the GPU suite runs
-(test_gpu_simple_hgn.py), and every kernel the table names is compiled, checked on a machine without a GPU."""
-import re
-
+(test_gpu_simple_hgn.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The symbols
+are mapped to their recorded names by test_cpu_kernel_inventory.py's note_of()."""
 from tests.hgn_table import MAX_TABLE, TABLE, form_key
-from tests.test_cpu_kernel_inventory import compiled_kernels
-
-
-def note_of(sym):
-    """The name cogdl_b200_last_kernel() records for a demangled simple_hgn.o kernel symbol."""
-    m = re.fullmatch(r"void cogdl_b200::(hgn_\w+_kernel)<(.*)>\(cogdl_b200::EsParams\)", sym)
-    assert m, f"no last_kernel() name is known for {sym!r}: add it to note_of() and a row to the table"
-    name, args = m.group(1), [re.sub(r"^\(int\)", "", a.strip()) for a in m.group(2).split(",")]
-    mode = int(args[0])
-    if name == "hgn_stats_kernel":
-        return f"cogdl_b200::hgn_stats_kernel<MODE={mode}>"
-    cap = f",CAP={args[1]}" if name == "hgn_main_kernel" else ""
-    drop, mix = (a == "(bool)1" for a in args[-2:])
-    return f"cogdl_b200::{name}<MODE={mode}{cap}{',DROP' if drop else ''}{',MIX' if mix else ''}>"
+from tests.test_cpu_kernel_inventory import compiled_kernels, note_of
 
 
 def table_kernels():
@@ -29,9 +15,10 @@ def table_kernels():
     return names
 
 
-def test_hgn_table_covers_every_compiled_kernel():
+def test_hgn_table_covers_every_typed_kernel():
     compiled = {note_of(s): s for s in compiled_kernels(("simple_hgn",))}
     assert compiled, "simple_hgn.o holds no kernels"
+    assert all(n.startswith("cogdl_b200::hgn_") for n in compiled), sorted(compiled)
     table = table_kernels()
     untested = sorted(set(compiled) - table)
     assert not untested, "compiled kernels without a row in tests/hgn_table.py:\n" + "\n".join(
@@ -64,8 +51,9 @@ def test_hgn_rows_cover_every_launch_form():
 
 
 def test_note_of_maps_hgn_symbols():
-    assert note_of("void cogdl_b200::hgn_main_kernel<(int)2, (int)512, (bool)1, (bool)0>(cogdl_b200::EsParams)") == \
-        "cogdl_b200::hgn_main_kernel<MODE=2,CAP=512,DROP>"
-    assert note_of("void cogdl_b200::hgn_warp_kernel<(int)2, (bool)0, (bool)1>(cogdl_b200::EsParams)") == \
+    assert note_of("void cogdl_b200::es_main_kernel<(int)2, (int)512, (bool)1, (bool)1, (bool)0>(cogdl_b200::EsParams)") \
+        == "cogdl_b200::hgn_main_kernel<MODE=2,CAP=512,DROP>"
+    assert note_of("void cogdl_b200::es_warp_kernel<(int)2, (bool)0, (bool)1, (bool)1>(cogdl_b200::EsParams)") == \
         "cogdl_b200::hgn_warp_kernel<MODE=2,MIX>"
-    assert note_of("void cogdl_b200::hgn_stats_kernel<(int)3>(cogdl_b200::EsParams)") == "cogdl_b200::hgn_stats_kernel<MODE=3>"
+    assert note_of("void cogdl_b200::es_stats_kernel<(int)3, (bool)1, (bool)1>(cogdl_b200::EsParams)") == \
+        "cogdl_b200::hgn_stats_kernel<MODE=3>"

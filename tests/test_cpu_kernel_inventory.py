@@ -117,12 +117,16 @@ def note_of(sym):
         return f"cogdl_b200::scatter_max_stream_kernel<NV={nv},U={u}{'' if argmax else ',values_only'}>"
     if name == "scatter_max_bwd_kernel":
         return "cogdl_b200::scatter_max_bwd_kernel"
-    if name == "es_main_kernel":
-        mode, cap, warps, drop = a
-        return f"cogdl_b200::es_main_kernel<MODE={mode},CAP={cap},WARPS={warps}{',DROP' if drop else ''}>"
-    if name in ("es_stats_kernel", "es_warp_kernel", "es_generic_kernel"):
-        mode, drop = a
-        return f"cogdl_b200::{name}<MODE={mode}{',DROP' if drop else ''}>"
+    # edge softmax: TYPED kernels (Simple-HGN) are recorded as hgn_*_kernel, without the es_ names' WARPS and their
+    # statistics kernel's DROP
+    if name == "es_stats_kernel":
+        mode, drop, typed = a
+        return f"cogdl_b200::{'hgn' if typed else 'es'}_stats_kernel<MODE={mode}{',DROP' * (drop and not typed)}>"
+    if name in ("es_main_kernel", "es_warp_kernel", "es_generic_kernel"):
+        mode, drop, typed, mix = [a[0]] + a[-3:]
+        cap = f",CAP={a[1]}{'' if typed else ',WARPS=8'}" if name == "es_main_kernel" else ""
+        return (f"cogdl_b200::{name.replace('es_', 'hgn_', 1) if typed else name}<MODE={mode}{cap}"
+                f"{',DROP' if drop else ''}{',MIX' if mix else ''}>")
     if name == "softmax_aggr_fwd_kernel":
         w_, has_a, want_q = a
         return (f"cogdl_b200::softmax_aggr_fwd_kernel<{'float4' if w_ == 4 else 'float'},"
@@ -169,10 +173,12 @@ def test_note_of_maps_known_symbols():
         "cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"
     assert canonical("cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels=4 block=128") \
         == ["cogdl_b200::stream_kernel<float2,NV=1,unweighted,SRC_ONE,U=8,MINB=5,prefetch>,panels"]
-    assert note_of("void cogdl_b200::es_main_kernel<(int)3, (int)512, (int)8, (bool)1>(cogdl_b200::EsParams)") == \
-        "cogdl_b200::es_main_kernel<MODE=3,CAP=512,WARPS=8,DROP>"
-    assert note_of("void cogdl_b200::es_stats_kernel<(int)2, (bool)0>(cogdl_b200::EsParams)") == \
+    assert note_of("void cogdl_b200::es_main_kernel<(int)3, (int)512, (bool)1, (bool)0, (bool)0>(cogdl_b200::EsParams)") \
+        == "cogdl_b200::es_main_kernel<MODE=3,CAP=512,WARPS=8,DROP>"
+    assert note_of("void cogdl_b200::es_stats_kernel<(int)2, (bool)0, (bool)0>(cogdl_b200::EsParams)") == \
         "cogdl_b200::es_stats_kernel<MODE=2>"
+    assert note_of("void cogdl_b200::es_stats_kernel<(int)3, (bool)1, (bool)0>(cogdl_b200::EsParams)") == \
+        "cogdl_b200::es_stats_kernel<MODE=3,DROP>"
     assert canonical("cogdl_b200::es_stats_kernel<MODE=0> + cogdl_b200::es_main_kernel<MODE=0,CAP=512,WARPS=8> "
                      "cp.async.bulk tiles") == ["cogdl_b200::es_stats_kernel<MODE=0>",
                                                 "cogdl_b200::es_main_kernel<MODE=0,CAP=512,WARPS=8>"]
@@ -198,7 +204,7 @@ def test_note_of_maps_known_symbols():
                                                                                   "cogdl_b200::spg_dB_kernel"]
 
 
-def test_table_covers_every_compiled_kernel():
+def test_dispatch_table_covers_every_compiled_kernel():
     compiled = {}
     for sym in compiled_kernels():
         compiled.setdefault(note_of(sym), sym)
@@ -259,12 +265,12 @@ def required_es_forms():
         if not m:
             continue
         name, a = m.group(1), _args("<" + m.group(2) + ">")
-        mode, drop = a[0], a[-1]
+        mode, drop = a[0], a[2 if name == "es_main_kernel" else 1]
         op = _ES_OP[mode]
         dn = ",DROP" if drop else ""
         if name == "es_main_kernel":
-            cap, warps = a[1], a[2]
-            main = f"cogdl_b200::es_main_kernel<MODE={mode},CAP={cap},WARPS={warps}{dn}>"
+            cap = a[1]
+            main = note_of(sym)
             st = f"cogdl_b200::es_stats_kernel<MODE={mode}{dn if mode == 3 else ''}> + "
             bulk = " cp.async.bulk tiles" if mode != 2 else ""
             forms.add((op, drop, st + main + bulk, (True, False, True)))
@@ -279,14 +285,14 @@ def required_es_forms():
                     forms.add((op, drop, st + main + bulk, (False, False, False)))
         elif name == "es_warp_kernel":
             for route in ("none", "default"):
-                forms.add((op, drop, f"cogdl_b200::es_warp_kernel<MODE={mode}{dn}>", route))
+                forms.add((op, drop, note_of(sym), route))
         elif name == "es_generic_kernel":
             for H in (3, 6, 64):
-                forms.add((op, drop, f"cogdl_b200::es_generic_kernel<MODE={mode}{dn}>", H))
+                forms.add((op, drop, note_of(sym), H))
     return forms
 
 
-def test_edge_softmax_rows_cover_every_launch_form():
+def test_edge_softmax_and_gat_rows_cover_every_launch_form():
     """Every launch form has a row and every row is the only one of its form, so removing any edge-softmax row fails
     here."""
     rows = [es_form(c) for c in TABLE if c.op in ES_OPS]
