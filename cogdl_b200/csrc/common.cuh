@@ -110,6 +110,9 @@ static int launch_items(void (*kernel)(P), const P &p, int64_t items, int group,
 
 constexpr unsigned FULL = 0xffffffffu;
 
+// ReLU as torch.relu gives it: a NaN passes through (fmaxf(NaN, 0) would return 0 and hide a diverged value).
+__device__ __forceinline__ float relu_nan(float v) { return v < 0.f ? 0.f : v; }
+
 // Streaming (read-once) index/value loads: keep them out of L1 so the gathered feature rows
 // own it.  ld.global.nc.L1::no_allocate.
 __device__ __forceinline__ int ld_stream(const int *p) {

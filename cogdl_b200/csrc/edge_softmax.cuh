@@ -546,7 +546,9 @@ __global__ void __launch_bounds__(ES_WARPS * 32) es_main_kernel(const EsParams p
             sm = (d > 0.f) ? fmaf(sm, e, 1.f) : sm + e;
             mx = fmaxf(mx, x);
           }
-          const float inv = 1.f / sm;
+          // a +Inf logit became the max and counted as exp(0) = 1, but the softmax has exp(Inf - Inf) = NaN there:
+          // the whole (row, head) is NaN, as it is on the unsegmented and chunked paths
+          const float inv = mx < CUDART_INF_F ? 1.f / sm : CUDART_NAN_F;
           for (int k = k0; k < k1; ++k) T[k * H + h] = es_mark<DROP>(p, (int64_t)base + k, h, es_exp(T[k * H + h] - mx) * inv);
         }
       }

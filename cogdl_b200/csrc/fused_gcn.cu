@@ -155,10 +155,13 @@ __device__ __forceinline__ uint32_t sw128_offset(int r, int k, int slab_bytes) {
   return (uint32_t)(slab * slab_bytes + (r >> 3) * 1024 + (r & 7) * 128 + chunk * 16 + (kk & 7) * 2);
 }
 
-// a = a1 + a2 + a3 (bf16 each, round to nearest even; the residuals are exact in fp32)
+// a = a1 + a2 + a3 (bf16 each, round to nearest even; the residuals are exact in fp32).  A finite a that rounds to
+// a bf16 infinity (|a| >= 0x1.fefp127) is rounded toward zero instead, so its residual stays finite; a non-finite a
+// goes whole into a1 with zero residuals (a - bf16(a) would be Inf - Inf = NaN).
 __device__ __forceinline__ void split3(float a, __nv_bfloat16 &a1, __nv_bfloat16 &a2, __nv_bfloat16 &a3) {
   a1 = __float2bfloat16_rn(a);
-  const float r1 = a - __bfloat162float(a1);
+  if (__hisinf(a1) && isfinite(a)) a1 = __float2bfloat16_rz(a);
+  const float r1 = isfinite(a) ? a - __bfloat162float(a1) : 0.f;
   a2 = __float2bfloat16_rn(r1);
   const float r2 = r1 - __bfloat162float(a2);
   a3 = __float2bfloat16_rn(r2);
@@ -465,7 +468,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) fused_layer_kernel(const Params
               }
               y = make_float2(d[4 * j + 2 * i] + sv.x, d[4 * j + 2 * i + 1] + sv.y);
             }
-            if (p.relu) { y.x = fmaxf(y.x, 0.f); y.y = fmaxf(y.y, 0.f); }
+            if (p.relu) { y.x = relu_nan(y.x); y.y = relu_nan(y.y); }
             if (vec && c + 1 < p.Fout) {
               __stcs(reinterpret_cast<float2 *>(o + c), y);
             } else {

@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(256, 1) genconv_edge_fwd_kernel(const GeFwdPar
             unpack(xv[u], xf);
             ge_edge_term<W, DM>(sa + (j + u) * D, D, wr, af);
 #pragma unroll
-            for (int k = 0; k < W; ++k) sa_step<WANT_Q>(fmaxf(xf[k] + af[k], 0.f) + p.eps, b2, M[k], S[k], T[k], Q[k]);
+            for (int k = 0; k < W; ++k) sa_step<WANT_Q>(relu_nan(xf[k] + af[k]) + p.eps, b2, M[k], S[k], T[k], Q[k]);
           }
         }
       }
@@ -243,10 +243,10 @@ __global__ void __launch_bounds__(256, 1) genconv_edge_bwd_kernel(const GeBwdPar
 #pragma unroll
             for (int k = 0; k < W; ++k) {
               const float pre = xj[k] + af[k];
-              const float m = fmaxf(pre, 0.f) + p.eps;
+              const float m = relu_nan(pre) + p.eps;
               const float wgt = exp2f(fmaf(m, b2, -lf[k]));
               const float dm = wgt * gf[k] * fmaf(beta, m - of[k], 1.f);
-              da[k] = pre > 0.f ? dm : 0.f;
+              da[k] = pre <= 0.f ? 0.f : dm;          // torch's relu backward: a NaN pre passes its gradient
               acc[k] += da[k];
             }
             if (want_dw) {

@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(256) softmax_aggr_fwd_kernel(const SaFwdParams
 #pragma unroll
             for (int k = 0; k < W; ++k) {
               const float pre = HAS_A ? xf[k] + af[k] : xf[k];
-              sa_step<WANT_Q>(fmaxf(pre, 0.f) + p.eps, b2, M[k], S[k], T[k], Q[k]);
+              sa_step<WANT_Q>(relu_nan(pre) + p.eps, b2, M[k], S[k], T[k], Q[k]);
             }
           }
         }
@@ -181,10 +181,10 @@ __global__ void __launch_bounds__(256) softmax_aggr_bwd_kernel(const SaBwdParams
 #pragma unroll
             for (int k = 0; k < W; ++k) {
               const float pre = HAS_A ? xj[k] + af[k] : xj[k];
-              const float m = fmaxf(pre, 0.f) + p.eps;
+              const float m = relu_nan(pre) + p.eps;
               const float wgt = exp2f(fmaf(m, b2, -lf[k]));
               const float dm = wgt * gf[k] * fmaf(beta, m - of[k], 1.f);
-              da[k] = pre > 0.f ? dm : 0.f;
+              da[k] = pre <= 0.f ? 0.f : dm;          // torch's relu backward: a NaN pre passes its gradient
               acc[k] += da[k];
             }
             if (HAS_A && dA) __stcs(dA + (int64_t)pj[u] * FV + cv, pack(da));

@@ -75,10 +75,13 @@ __device__ __forceinline__ void sa_finish(const SaFwdParams &p, int64_t off, con
   float o[W], l[W], q[W];
 #pragma unroll
   for (int k = 0; k < W; ++k) {
-    const bool any = S[k] > 0.f;           // degree-0 rows: out = 0 (a scatter_add of nothing)
-    o[k] = any ? T[k] / S[k] : 0.f;
-    l[k] = any ? M[k] + log2f(S[k]) : 0.f;
-    q[k] = any ? Q[k] / S[k] : 0.f;
+    const bool any = S[k] != 0.f;          // degree-0 rows: out = 0 (a scatter_add of nothing); a NaN S is not one
+    // a +Inf logit is its row's max, and exp(z - max) = exp(Inf - Inf) is NaN in the softmax this restates: the
+    // online state counted it as 1, so the row's sums are replaced by NaN here
+    const float s = M[k] < CUDART_INF_F ? S[k] : CUDART_NAN_F;
+    o[k] = any ? T[k] / s : 0.f;
+    l[k] = any ? M[k] + log2f(s) : 0.f;
+    q[k] = any ? Q[k] / s : 0.f;
   }
   st_stream(reinterpret_cast<VecT *>(p.out) + off, pack(o));
   if (p.lse2) st_stream(reinterpret_cast<VecT *>(p.lse2) + off, pack(l));
