@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests import correct_smooth_ref as ref
+from tests.gpu_util import rel
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "correct_smooth.npz")
 CASES = [(a, cn, sn) for a in (False, True) for cn in ("sym", "row") for sn in ("row", "col")]
@@ -17,10 +18,6 @@ NPROP, CORRECT_ALPHA, SMOOTH_ALPHA = 20, 1.0, 0.8
 def softmax(z):
     e = np.exp(z - z.max(axis=1, keepdims=True))
     return e / e.sum(axis=1, keepdims=True)
-
-
-def rel(a, b):
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
 @pytest.mark.parametrize("autoscale,correct_norm,smooth_norm", CASES)

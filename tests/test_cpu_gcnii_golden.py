@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from tests import gcnii_ref
+from tests.gpu_util import rel
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gcnii_appnp.npz")
 CASES = [(m, g) for m in ("gcnii_res0", "gcnii_res1", "appnp") for g in ("csr", "coo")]
@@ -25,10 +26,6 @@ def restated(d, model, built_from):
         y = gcnii_ref.gcnii_fp64(params, A, in_norm, out_norm, x, 8, 0.1, 0.5, model == "gcnii_res1")
     (y * torch.from_numpy(d["G"]).double()).sum().backward()
     return y.detach().numpy(), {k: p.grad.numpy() for k, p in params.items()}
-
-
-def rel(a, b):
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
 @pytest.mark.parametrize("model,built_from", CASES)

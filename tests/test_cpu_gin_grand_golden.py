@@ -9,14 +9,12 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+from tests.gpu_util import rel
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gin_grand.npz")
 GIN_CASES = (("gin", 0.1, True), ("gin_fixed", -1.0, False), ("gine", -0.3, True))
 ORDERS = (0, 1, 2, 8)
 DROPNODE, SEED = 0.5, 123
-
-
-def rel(a, b):
-    return float(np.abs(np.asarray(a, np.float64) - b).max() / max(np.abs(b).max(), 1e-30))
 
 
 def gin_fp64(row, col, n, x, g, eps):

@@ -2,19 +2,13 @@
 (test_gpu_gin_grand.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The symbols
 are mapped to their recorded names by test_cpu_kernel_inventory.py's note_of()."""
 from tests.gin_grand_table import TABLE
-from tests.test_cpu_kernel_inventory import canonical, compiled_kernels, note_of
+from tests.test_cpu_kernel_inventory import assert_table_covers, canonical, note_of
 
 
 def _check(obj, epi):
-    compiled = {note_of(s): s for s in compiled_kernels((obj,))}
-    assert compiled, f"{obj}.o holds no kernels"
-    assert all(f"_{epi}_kernel<" in n for n in compiled), sorted(compiled)
     table = {k for c in TABLE if c.epi == epi for k in canonical(c.kernel)}
-    untested = sorted(set(compiled) - table)
-    assert not untested, "compiled kernels without a row in tests/gin_grand_table.py:\n" + "\n".join(
-        f"  {n}   ({compiled[n]})" for n in untested)
-    unknown = sorted(table - set(compiled))
-    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+    compiled = assert_table_covers(obj, note_of, table, "tests/gin_grand_table.py")
+    assert all(f"_{epi}_kernel<" in n for n in compiled), sorted(compiled)
 
 
 def test_gin_table_covers_every_compiled_kernel():

@@ -2,7 +2,7 @@
 (test_gpu_simple_hgn.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The symbols
 are mapped to their recorded names by test_cpu_kernel_inventory.py's note_of()."""
 from tests.hgn_table import MAX_TABLE, TABLE, form_key
-from tests.test_cpu_kernel_inventory import compiled_kernels, note_of
+from tests.test_cpu_kernel_inventory import assert_table_covers, note_of
 
 
 def table_kernels():
@@ -16,15 +16,8 @@ def table_kernels():
 
 
 def test_hgn_table_covers_every_typed_kernel():
-    compiled = {note_of(s): s for s in compiled_kernels(("simple_hgn",))}
-    assert compiled, "simple_hgn.o holds no kernels"
+    compiled = assert_table_covers("simple_hgn", note_of, table_kernels(), "tests/hgn_table.py")
     assert all(n.startswith("cogdl_b200::hgn_") for n in compiled), sorted(compiled)
-    table = table_kernels()
-    untested = sorted(set(compiled) - table)
-    assert not untested, "compiled kernels without a row in tests/hgn_table.py:\n" + "\n".join(
-        f"  {n}   ({compiled[n]})" for n in untested)
-    unknown = sorted(table - set(compiled))
-    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
 
 
 def test_hgn_rows_are_distinct_and_cover_the_shapes():

@@ -61,6 +61,20 @@ def compiled_kernels(objects=OBJECTS):
     return [ln.strip() for ln in out.splitlines() if ln.strip()]
 
 
+def assert_table_covers(obj, note_of, table_kernels, table_file):
+    """Every kernel compiled into <obj>.o has a row in table_file, and every kernel the table names is compiled.
+    note_of maps a demangled symbol to the name cogdl_b200_last_kernel() records, table_kernels is the set of names the
+    table's rows record.  Returns {recorded name: symbol} of the object."""
+    compiled = {note_of(s): s for s in compiled_kernels((obj,))}
+    assert compiled, f"{obj}.o holds no kernels"
+    untested = sorted(set(compiled) - table_kernels)
+    assert not untested, f"compiled kernels without a row in {table_file}:\n" + "\n".join(
+        f"  {n}   ({compiled[n]})" for n in untested)
+    unknown = sorted(table_kernels - set(compiled))
+    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+    return compiled
+
+
 _SRC = {0: "SRC_ONE", 1: "SRC_TWO", 2: "SRC_PEERS"}
 # the SpMM row and row-stream kernels are recorded as spmm<tag>_kernel / stream<tag>_kernel, by their epilogue argument
 _EPI_TAG = {0: "", 1: "_residual", 2: "_labelprop", 3: "_dcoef", 4: "_accum"}

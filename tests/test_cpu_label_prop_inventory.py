@@ -2,18 +2,12 @@
 (test_gpu_label_prop.py), and every kernel the table names is compiled, checked on a machine without a GPU.  The
 symbols are mapped to their recorded names by test_cpu_kernel_inventory.py's note_of()."""
 from tests.label_prop_table import TABLE
-from tests.test_cpu_kernel_inventory import canonical, compiled_kernels, note_of
+from tests.test_cpu_kernel_inventory import assert_table_covers, canonical, note_of
 
 
 def test_label_prop_table_covers_every_compiled_kernel():
-    compiled = {note_of(s): s for s in compiled_kernels(("label_prop",))}
-    assert compiled, "label_prop.o holds no kernels"
     table = {k for c in TABLE for k in canonical(c.kernel)}
-    untested = sorted(set(compiled) - table)
-    assert not untested, "compiled kernels without a row in tests/label_prop_table.py:\n" + "\n".join(
-        f"  {n}   ({compiled[n]})" for n in untested)
-    unknown = sorted(table - set(compiled))
-    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+    assert_table_covers("label_prop", note_of, table, "tests/label_prop_table.py")
 
 
 def test_label_prop_rows_are_distinct_and_cover_every_epilogue():

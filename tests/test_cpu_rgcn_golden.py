@@ -10,14 +10,10 @@ import os
 import numpy as np
 import torch
 
+from tests.gpu_util import rel
 from tests.rgcn_ref import first_present, layer_post, relational_sum, row_norm_weights, type_weights
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "rgcn.npz")
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
 def load():

@@ -3,7 +3,7 @@ every kernel the table names is compiled, checked on a machine without a GPU."""
 import re
 
 from tests.rgcn_table import BASIS_TILE, BS, FS, TABLE, TS
-from tests.test_cpu_kernel_inventory import compiled_kernels
+from tests.test_cpu_kernel_inventory import assert_table_covers
 
 
 def note_of(sym):
@@ -15,14 +15,7 @@ def note_of(sym):
 
 
 def test_rgcn_table_covers_every_compiled_kernel():
-    compiled = {note_of(s): s for s in compiled_kernels(("rgcn",))}
-    assert compiled, "rgcn.o holds no kernels"
-    table = {c.kernel for c in TABLE}
-    untested = sorted(set(compiled) - table)
-    assert not untested, "compiled kernels without a row in tests/rgcn_table.py:\n" + "\n".join(
-        f"  {n}   ({compiled[n]})" for n in untested)
-    unknown = sorted(table - set(compiled))
-    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+    assert_table_covers("rgcn", note_of, {c.kernel for c in TABLE}, "tests/rgcn_table.py")
 
 
 def test_rgcn_rows_are_distinct_and_cover_the_shapes():

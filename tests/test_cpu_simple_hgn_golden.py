@@ -9,16 +9,12 @@ import os
 import numpy as np
 import torch
 
+from tests.gpu_util import rel
 from tests.simple_hgn_ref import conv_fp64
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "simple_hgn.npz")
 SLOPE, ALPHA = 0.2, 0.05
 HEADS = (8, 8, 1)
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
 def load():

@@ -3,17 +3,12 @@
 kernel entry points are read from the object and mapped to the string their launchers record for
 cogdl_b200_last_kernel() by test_cpu_kernel_inventory.py."""
 from tests.spmm_residual_table import TABLE
-from tests.test_cpu_kernel_inventory import canonical, compiled_kernels, note_of
+from tests.test_cpu_kernel_inventory import assert_table_covers, canonical, note_of
 
 
 def test_residual_table_covers_every_compiled_kernel():
-    compiled = {note_of(s): s for s in compiled_kernels(("spmm_residual",))}
     table = {k for c in TABLE for k in canonical(c.kernel)}
-    untested = sorted(set(compiled) - table)
-    assert not untested, "compiled kernels without a row in tests/spmm_residual_table.py:\n" + "\n".join(
-        f"  {n}   ({compiled[n]})" for n in untested)
-    unknown = sorted(table - set(compiled))
-    assert not unknown, "table rows name kernels that are not compiled:\n" + "\n".join(f"  {n}" for n in unknown)
+    assert_table_covers("spmm_residual", note_of, table, "tests/spmm_residual_table.py")
 
 
 def test_residual_rows_are_distinct_and_cover_both_epilogue_inputs():

@@ -7,14 +7,10 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gpu_util import rel
 from tests import spspmm_models_ref as R
 
 GOLDEN = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gtn_srgcn.npz"))
-
-
-def rel(got, want):
-    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
-    return float(np.abs(got - want).max() / max(np.abs(want).max(), 1e-30))
 
 
 def params(tag):

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import T, dev, rel
 from tests.graphs import case
 
 pytestmark = pytest.mark.gpu
@@ -22,21 +23,6 @@ TOL = 1e-5
 
 def gold(name):
     return np.load(os.path.join(ROOT, "tests", "golden", name))
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return 0.0 if b.size == 0 else float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    return torch.device("cuda:0")
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
 
 
 def graph_from(g, dev, weight=None, x=None):

@@ -30,9 +30,10 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+from tests.gpu_util import T, dev, misaligned, plan_structure
 from tests.graphs import CASES, boundary_csr, case
 from tests.test_gpu_dispatch import (SLOPE, TINY, U32, assert_within, check_softmax, es_logits, fp16_bound,
-                                     gat_logits32, misaligned, softmax_bwd64)
+                                     gat_logits32, softmax_bwd64)
 
 pytestmark = pytest.mark.gpu
 
@@ -61,28 +62,15 @@ def within(got, ref, bnd, what):
     WORST[test] = max(WORST.get(test, 0.0), ratio)
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
 def graph_np(name):
     """(rowptr, colind, n_cols) int32 CSR of a case; "bounds" is boundary_csr(64)."""
     return boundary_csr(64) if name == "bounds" else case(name)
 
 
 def structure(name, rp, ci, n_cols, dev):
-    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES, CSRStructure
+    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES
 
-    return CSRStructure(T(rp, dev), T(ci, dev), n_cols=n_cols, chunk_edges=64 if name == "bounds" else DEFAULT_CHUNK_EDGES)
+    return plan_structure(rp, ci, n_cols, dev, chunk=64 if name == "bounds" else DEFAULT_CHUNK_EDGES)
 
 
 def place(a, kind, dev):

@@ -11,32 +11,12 @@ import torch
 
 from tests import graphs
 from tests.compgcn_ref import compgcn_aggregate_fp64
+from tests.gpu_util import dev, misaligned, row_err
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HUBS = ["hub", "two_hubs"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    import cogdl_b200  # noqa: F401
-
-    torch.backends.cuda.matmul.allow_tf32 = False
-    return torch.device("cuda:0")
-
-
-def err(got, ref, bound=None):
-    """max |got - ref| / max(|ref|, row scale of ref, bound).  bound: the same sum over |terms| (abs_problem); a sum
-    of terms that cancels (sub with F = 1, or a dR' row of many signed gradients) is known in fp32 only to a few ulps
-    of the sum of the magnitudes, whatever the order of summation."""
-    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
-    if ref.numel() == 0:
-        return 0.0
-    scale = torch.maximum(ref.abs(), ref.abs().amax(dim=1, keepdim=True))
-    if bound is not None:
-        scale = torch.maximum(scale, bound.detach().double().cpu().abs())
-    return float(((got - ref).abs() / scale.clamp_min(1e-30)).max())
 
 
 def abs_problem(opn, x, rel):
@@ -59,14 +39,6 @@ def typed_coo(name, T, dev, seed=0):
     return to(row[perm]), to(ci[perm]), to(typ), max(n, n_cols)
 
 
-def misaligned(t):
-    """A contiguous copy of t whose data starts 4 bytes past a 16-byte boundary (forces the scalar lanes)."""
-    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
-    out = buf[1:].view(t.shape)
-    out.copy_(t)
-    return out
-
-
 @pytest.mark.parametrize("chunk", [None, 16])
 @pytest.mark.parametrize("opn", ["sub", "mult"])
 @pytest.mark.parametrize("T", [1, 3, 475])
@@ -83,7 +55,7 @@ def test_forward_matches_fp64(dev, name, F, T, opn, chunk):
     w_in, w_out = compgcn_aggregate_fp64(row, col, typ, x, rel, opn)
     b_in, b_out = compgcn_aggregate_fp64(row, col, typ, *abs_problem(opn, x, rel), opn)
     assert a_in.shape == a_out.shape == (N, F)
-    assert err(a_in, w_in, b_in) <= 1e-5 and err(a_out, w_out, b_out) <= 1e-5
+    assert row_err(a_in, w_in, b_in) <= 1e-5 and row_err(a_out, w_out, b_out) <= 1e-5
 
 
 @pytest.mark.parametrize("opn", ["sub", "mult"])
@@ -99,7 +71,7 @@ def test_misaligned_inputs(dev, name, F, opn):
     a_in, a_out = compgcn_aggregate((row, col), typ, x, rel, opn, chunk_edges=16)
     w_in, w_out = compgcn_aggregate_fp64(row, col, typ, x, rel, opn)
     b_in, b_out = compgcn_aggregate_fp64(row, col, typ, *abs_problem(opn, x, rel), opn)
-    assert err(a_in, w_in, b_in) <= 1e-5 and err(a_out, w_out, b_out) <= 1e-5
+    assert row_err(a_in, w_in, b_in) <= 1e-5 and row_err(a_out, w_out, b_out) <= 1e-5
 
 
 def _grads(aggregate, x0, rel0, G):
@@ -128,8 +100,8 @@ def test_gradients_match_fp64_autograd(dev, name, F, opn, chunk):
     fp64 = lambda a, b: compgcn_aggregate_fp64(row, col, typ, a, b, opn)  # noqa: E731
     ex, erel = _grads(fp64, x.double(), rel.double(), G.double())
     bx, brel = _grads(fp64, *abs_problem(opn, x, rel), G.double().abs())
-    assert err(dx, ex, bx) <= 1e-5
-    assert err(drel, erel, brel) <= 1e-5
+    assert row_err(dx, ex, bx) <= 1e-5
+    assert row_err(drel, erel, brel) <= 1e-5
     if name in HUBS:
         assert int(torch.bincount(typ).min()) > 10 * (chunk or DEFAULT_CHUNK_EDGES)
 
@@ -200,7 +172,7 @@ def test_empty_half_gives_zeros(dev, E):
     a_in, a_out = compgcn_aggregate((row, col), typ, x, rel, "mult")
     assert torch.equal(a_in, torch.zeros_like(a_in))
     w_in, w_out = compgcn_aggregate_fp64(row, col, typ, x, rel, "mult")
-    assert err(a_out, w_out) <= 1e-6
+    assert row_err(a_out, w_out) <= 1e-6
     (a_in.sum() + a_out.sum()).backward()
     assert x.grad.shape == x.shape and rel.grad.shape == rel.shape
 

@@ -10,6 +10,7 @@ import torch
 
 from tests import graphs
 from tests.disengcn_ref import disen_routing_fp64, normalize_channels_fp64, route_step_fp64
+from tests.gpu_util import dev, misaligned, plan_structure, row_err
 
 pytestmark = pytest.mark.gpu
 
@@ -17,27 +18,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SQUARE = [name for name in graphs.CASES if name != "rect"]
 
 
-@pytest.fixture(scope="module")
-def dev():
-    import cogdl_b200  # noqa: F401
-
-    torch.backends.cuda.matmul.allow_tf32 = False
-    return torch.device("cuda:0")
-
-
-def err(got, ref):
-    """max |got - ref| / max(|ref|, row scale of ref)."""
-    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
-    if ref.numel() == 0:
-        return 0.0
-    if ref.dim() == 1:                       # a vector (a bias gradient) is one row
-        ref, got = ref[None, :], got[None, :]
-    scale = torch.maximum(ref.abs(), ref.abs().amax(dim=1, keepdim=True)).clamp_min(1e-30)
-    return float(((got - ref).abs() / scale).max())
-
-
 def route_err(got, want, norm):
-    """err() of u = out |u| rather than of out, with the fp64 |u| [n, K] of the step that made `want`.  The last
+    """row_err() of u = out |u| rather than of out, with the fp64 |u| [n, K] of the step that made `want`.  The last
     normalisation multiplies any rounding of u by 1 / |u|: where a + c nearly cancels (|u| -> 0: routinely for
     d = 1, where c = +-1) out is ill-conditioned in the layer itself, not in the kernel.  Channels whose fp64 |u|
     is below 1e-6 decide their direction by rounding and are left out."""
@@ -47,27 +29,18 @@ def route_err(got, want, norm):
     scale = norm.double().cpu()[..., None] * keep
     u_got = torch.where(keep, got.detach().double().cpu().reshape(n, K, -1) * scale, 0.0)
     u_want = torch.where(keep, want.detach().double().cpu().reshape(n, K, -1) * scale, 0.0)
-    return err(u_got.reshape(n, F), u_want.reshape(n, F))
+    return row_err(u_got.reshape(n, F), u_want.reshape(n, F))
 
 
 def structure(name, dev, chunk=None):
-    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES, CSRStructure
+    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES
 
     rp, ci, n_cols = graphs.case(name)
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols,
-                        chunk_edges=DEFAULT_CHUNK_EDGES if chunk is None else chunk)
+    return plan_structure(rp, ci, n_cols, dev, chunk=DEFAULT_CHUNK_EDGES if chunk is None else chunk)
 
 
 def unit_channels(n, K, d, dev, gen):
     return normalize_channels_fp64(torch.randn(n, K * d, device=dev, generator=gen), K).float()
-
-
-def misaligned(t):
-    """A contiguous copy of t whose data starts 4 bytes past a 16-byte boundary (forces the scalar lanes)."""
-    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
-    out = buf[1:].view(t.shape)
-    out.copy_(t)
-    return out
 
 
 @pytest.mark.parametrize("chunk", [None, 16])
@@ -109,7 +82,7 @@ def test_disen_routing_seven_iterations(dev, name, K, d):
     for tau, bar in ((0.1, 1e-4), (1.0, 1e-5), (5.0, 1e-5)):
         got = disen_routing(st, h, K, 7, tau)
         assert route_err(got, *disen_routing_fp64(st.rowptr, st.colind, h, K, 7, tau, with_norm=True)) <= bar, tau
-    assert err(disen_routing(st, h, K, 0, 1.0), normalize_channels_fp64(h, K)) <= 1e-6   # no iterations: c
+    assert row_err(disen_routing(st, h, K, 0, 1.0), normalize_channels_fp64(h, K)) <= 1e-6   # no iterations: c
 
 
 @pytest.mark.parametrize("K,d", [(16, 4), (8, 8), (8, 2), (2, 32)])
@@ -130,8 +103,8 @@ def test_step_gradients_match_fp64_autograd(dev, name, K, d):
     for tau in (0.5, 1.0):
         got = grads(lambda q, c: DisenRouteFunction.apply(st, q, c, K, tau), torch.float32)
         want = grads(lambda q, c: route_step_fp64(st.rowptr, st.colind, q, c, K, tau), torch.float64)
-        assert err(got[0], want[0]) <= 1e-4, ("dq", tau)
-        assert err(got[1], want[1]) <= 1e-4, ("dc", tau)
+        assert row_err(got[0], want[0]) <= 1e-4, ("dq", tau)
+        assert row_err(got[1], want[1]) <= 1e-4, ("dc", tau)
 
 
 @pytest.mark.parametrize("K,d", [(16, 4), (8, 8), (4, 16)])
@@ -158,7 +131,7 @@ def test_layer_chain_gradients_match_fp64_autograd(dev, name, K, d):
     got = grads(lambda h: disen_routing(st, h, K, 7, 1.0), torch.float32)
     want = grads(lambda h: disen_routing_fp64(st.rowptr, st.colind, h, K, 7, 1.0), torch.float64)
     for name_, g, w in zip(("x", "W", "b"), got, want):
-        assert err(g, w) <= 1e-4, name_
+        assert row_err(g, w) <= 1e-4, name_
 
 
 @pytest.mark.parametrize("name", ["hub", "two_hubs"])

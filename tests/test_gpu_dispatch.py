@@ -40,40 +40,13 @@ import torch
 
 import oracle
 from tests.dispatch_table import TABLE
+from tests.gpu_util import T, check_counters, dev, misaligned, plan_structure
 from tests.graphs import boundary_csr, case
 
 pytestmark = pytest.mark.gpu
 
 U32 = 2.0 ** -24                      # unit roundoff of fp32
 TINY = float(np.finfo(np.float32).tiny)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
-def misaligned(t):
-    """A contiguous copy of t whose data starts one element past the allocation (not 16-byte aligned)."""
-    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
-    out = buf[1:].view(t.shape)
-    out.copy_(t)
-    return out
-
-
-def structure(rp, ci, n_cols, dev, c):
-    from cogdl_b200.structure import CSRStructure
-
-    chunk, seg_cost = {"none": (0, None), "chunks": (c.chunk, 0), "default": (c.chunk, None)}[c.plan]
-    return CSRStructure(T(rp, dev), T(ci, dev), n_cols=n_cols, chunk_edges=chunk, seg_cost=seg_cost)
 
 
 def csr64(rp, ci, vals, n_cols):
@@ -118,7 +91,7 @@ def _peer_call(dev, c, rp, ci, n_cols, val_d, X):
     for o in (1, 2):
         m = (ci >= bounds[o]) & (ci < bounds[o + 1])
         enc[m] = bounds[1] + (o << shift) + (ci[m] - bounds[o])
-    st = structure(rp, enc, n_cols, dev, c)
+    st = plan_structure(rp, enc, n_cols, dev, c.plan, c.chunk)
     shards = [T(X[bounds[o]:bounds[o + 1]], dev) for o in range(3)]
     ptrs = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in shards])
     y = torch.empty((rp.shape[0] - 1, c.F), device=dev)
@@ -143,10 +116,10 @@ def run_spmm(dev, c):
     val_d = None if val is None else T(val, dev)
     Xd = T(X, dev) if c.aligned else misaligned(T(X, dev))
     if c.src == "one":
-        st = structure(rp, ci, n_cols, dev, c)
+        st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
         y = spmm_raw(st, val_d, Xd, panels=c.panels)
     elif c.src == "two":
-        st = structure(rp, ci, n_cols, dev, c)
+        st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
         n0 = 400
         y = spmm_2src_raw(st, val_d, Xd[:n0], Xd[n0:])
     else:
@@ -197,7 +170,7 @@ def run_spmm_f16(dev, c):
     X = X.astype(np.float16)
     val = rng.random(ci.shape[0]).astype(np.float16) if c.weighted else None
     zero_row = plant_cancelling_row(rp, ci, val, X, c.chunk if c.plan != "none" else 1 << 30) if c.weighted else None
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     Xd = T(X, dev) if c.aligned else misaligned(T(X, dev))
     y = spmm_raw(st, None if val is None else T(val, dev), Xd)
     check_kernel(c)
@@ -222,7 +195,7 @@ def run_sddmm(dev, c):
     rng = np.random.default_rng(300 + c.H * 1000 + c.F)
     D1 = rng.standard_normal((n, c.H, c.F)).astype(np.float32)
     D2 = rng.standard_normal((n_cols, c.H, c.F)).astype(np.float32)
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     d1 = T(D1, dev)
     d2 = T(D2, dev) if c.aligned else misaligned(T(D2, dev))
     if c.H == 1:
@@ -253,7 +226,7 @@ def run_mhspmm(dev, c):
         mask = rng.random((nnz, c.H)) < 0.3
         eff = np.where(mask, np.float32(0), att * scale).astype(np.float32)
         att = np.where(mask, -att, att).astype(np.float32)
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     if c.perm:
         # the transposed pass (grad_feat of the GAT aggregation): rows of A^T, attention read through the permutation
         st, p = st.csc()
@@ -299,7 +272,7 @@ def run_scatter_max(dev, c):
         np.add.at(cnt, (ref_id[ok], cols), 1)
         assert_within(gx, want, cnt * U32 * mag + TINY, c.id)
         return
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     Xd = T(X, dev) if c.aligned else misaligned(T(X, dev))
     out, arg = scatter_max_fwd_raw(st, Xd)
     check_kernel(c)
@@ -388,18 +361,13 @@ def softmax_bwd64(rp, y, g, dact):
     return out, bound, grow, gbound + deg[:, None] * U32 * gmag + TINY
 
 
-def check_counters(c, st):
-    if c.plan != "none" and st.plan.n_chunks > 0:
-        assert int(st.plan.counters.abs().sum()) == 0, f"{c.id}: arrival counters not back at zero"
-
-
 def run_edge_softmax(dev, c):
     from cogdl_b200.operators._raw import edge_softmax_bwd_raw, edge_softmax_fwd_raw
 
     rp, ci, n_cols = es_graph(c)
     rng = np.random.default_rng(600 + c.H * 10 + c.chunk)
     x = es_logits(rp, c.H, rng, c.masked, c.chunk)
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     if c.op == "edge_softmax":
         got = edge_softmax_fwd_raw(st, T(x, dev) if c.aligned else misaligned(T(x, dev)))
         check_kernel(c)
@@ -411,7 +379,7 @@ def run_edge_softmax(dev, c):
         check_kernel(c)
         ref, bound, _, _ = softmax_bwd64(rp, y, g, 1.0)
         assert_within(got.cpu().numpy(), ref, bound, c.id)
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 def gat_logits32(rp, ci, hl, hr):
@@ -430,7 +398,7 @@ def run_gat_fwd(dev, c):
     hl = rng.standard_normal((n, c.H)).astype(np.float32)
     hr = rng.uniform(-20, 90, (n, c.H)).astype(np.float32)          # logits spread over ~90 in a row
     feat = rng.standard_normal((n, c.H, c.F)).astype(np.float32)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     scale = np.float32(1.0 / (1.0 - P_DROP))
     seed = 0x5EED + c.H
     drop = (seed, drop_below(P_DROP), float(scale)) if c.drop else None
@@ -451,7 +419,7 @@ def run_gat_fwd(dev, c):
         A = csr64(rp, ci, eff[:, h], n)
         f64 = feat[:, h, :].astype(np.float64)
         assert_within(got[:, h, :], A @ f64, deg * U32 * (abs(A) @ np.abs(f64)) + TINY, f"{c.id} head {h}")
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 def run_gat_attn_bwd(dev, c):
@@ -470,7 +438,7 @@ def run_gat_attn_bwd(dev, c):
     z = gat_logits32(rp, ci, hl, hr)[0]
     assert np.all(z[first] == 0)
     dact = np.where(z > 0, 1.0, np.float64(SLOPE))
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     y, g, ds = att, d_att, None
     if c.drop:
         scale = np.float32(1.0 / (1.0 - P_DROP))
@@ -485,7 +453,7 @@ def run_gat_attn_bwd(dev, c):
     ref, bound, grow, gbound = softmax_bwd64(rp, y, g, dact)
     assert_within(d_edge.cpu().numpy(), ref, bound, f"{c.id} d_edge")
     assert_within(g_row.cpu().numpy(), grow, gbound, f"{c.id} g_row")
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 RUN = {"spmm": run_spmm, "spmm_f16": run_spmm_f16, "sddmm": run_sddmm, "mhspmm": run_mhspmm,

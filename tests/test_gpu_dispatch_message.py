@@ -57,6 +57,7 @@ import pytest
 import torch
 
 from tests.dispatch_table import MESSAGE_TABLE
+from tests.gpu_util import T, check_counters, dev, misaligned, plan_structure
 from tests.graphs import boundary_csc, boundary_csr, case
 
 pytestmark = pytest.mark.gpu
@@ -68,27 +69,6 @@ LN2 = float(np.log(2.0))
 EPS = 1e-7
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
-def misaligned(t):
-    """A contiguous copy of t whose data starts one element past the allocation (not 16-byte aligned)."""
-    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
-    out = buf[1:].view(t.shape)
-    out.copy_(t)
-    return out
-
-
 def graph_of(c):
     if c.graph == "bounds":
         return boundary_csr(c.chunk)
@@ -97,23 +77,10 @@ def graph_of(c):
     return case(c.graph)
 
 
-def structure(rp, ci, n_cols, dev, c):
-    from cogdl_b200.structure import CSRStructure
-
-    chunk, seg_cost = {"none": (0, None), "chunks": (c.chunk, 0), "default": (c.chunk, None)}[c.plan]
-    return CSRStructure(T(rp, dev), T(ci, dev), n_cols=n_cols, chunk_edges=chunk, seg_cost=seg_cost)
-
-
 def check_kernel(c):
     from cogdl_b200 import _cabi
 
     assert _cabi.last_kernel() == c.kernel, f"{c.id}: launched {_cabi.last_kernel()!r}"
-
-
-def check_counters(c, *structures):
-    for st in structures:
-        if st.chunk_edges > 0 and st.plan.n_chunks > 0:
-            assert int(st.plan.counters.abs().sum()) == 0, f"{c.id}: arrival counters not back at zero"
 
 
 def has_chunks(c, st):
@@ -234,7 +201,7 @@ def run_sa_fwd(dev, c):
     rp, ci, n = graph_of(c)
     rng = np.random.default_rng(1000 + c.F)
     x, A = sa_inputs(c, rp, ci, n, rng)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     beta_d = torch.tensor([c.beta], dtype=torch.float32, device=dev)
     out, lse2, q = sa_fwd_call(dev, c, st, x, A, beta_d, c.want_q)
     check_kernel(c)
@@ -249,7 +216,7 @@ def run_sa_fwd(dev, c):
     assert np.all(out.cpu().numpy()[empty] == 0) and np.all(lse2.cpu().numpy()[empty] == 0)
     if c.plan != "none":
         has_chunks(c, st)
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 def run_sa_bwd(dev, c):
@@ -258,7 +225,7 @@ def run_sa_bwd(dev, c):
     rp, ci, n = graph_of(c)
     rng = np.random.default_rng(2000 + c.F)
     x, A = sa_inputs(c, rp, ci, n, rng)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     beta_d = torch.tensor([c.beta], dtype=torch.float32, device=dev)
     Ad = None if A is None else T(A, dev)
     out, lse2, _ = softmax_aggr_fwd_raw(st, T(x, dev), beta_d, EPS, Ad, want_lse=True)
@@ -289,7 +256,8 @@ def run_sa_bwd(dev, c):
         assert_within(got, dpre, eb + TINY, f"{c.id} dA")
     else:
         assert da is None
-    check_counters(c, st, st_t)
+    check_counters(st, c.id)
+    check_counters(st_t, c.id)
 
 
 # ------------------------------------------------------------------------------------------ DisenGCN
@@ -344,7 +312,7 @@ def run_disen_fwd(dev, c):
     rp, ci, n = graph_of(c)
     rng = np.random.default_rng(3000 + c.F * 10 + c.K)
     q, cc = disen_inputs(c, rp, ci, n, rng)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     qd, cd = T(q, dev), T(cc, dev)
     if not c.aligned:
         qd, cd = misaligned(qd), misaligned(cd)
@@ -373,7 +341,7 @@ def run_disen_fwd(dev, c):
         assert_within(np.where(okk, lse2.cpu().numpy(), 0), np.where(okk, lse64, 0), lb, f"{c.id} lse2")
     else:
         assert lse2 is None and r is None
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 def run_disen_bwd(dev, c):
@@ -382,7 +350,7 @@ def run_disen_bwd(dev, c):
     rp, ci, n = graph_of(c)
     rng = np.random.default_rng(4000 + c.F * 10 + c.K)
     q, cc = disen_inputs(c, rp, ci, n, rng)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     qd, cd = T(q, dev), T(cc, dev)
     gd = T(rng.standard_normal((n, c.F)).astype(np.float32), dev)
     if not c.aligned:
@@ -433,7 +401,8 @@ def run_disen_bwd(dev, c):
     dc64 = gu.reshape(n, -1) + col_sum(flat(term), ci, n)
     dcb = col_sum(flat(rho_e[..., None] * tmag), ci, n) + (d + 4) * U32 * GU.reshape(n, -1) + U32 * np.abs(dc64) + TINY
     assert_nan_within(f(dc), dc64, dcb, f"{c.id} dc")
-    check_counters(c, st, st_t)
+    check_counters(st, c.id)
+    check_counters(st_t, c.id)
 
 
 # ------------------------------------------------------------------------------------------ CompGCN
@@ -447,7 +416,7 @@ def run_comp(dev, c):
     w = rng.standard_normal(nnz).astype(np.float32)
     a = rng.standard_normal((n, c.F)).astype(np.float32)
     b = rng.standard_normal((c.T, c.F)).astype(np.float32)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     y = comp_aggr_raw(st, T(idx2, dev), T(w, dev), T(a, dev), T(b, dev), c.comp).cpu().numpy()
     check_kernel(c)
     has_chunks(c, st)
@@ -466,7 +435,7 @@ def run_comp(dev, c):
     terms = w[:, None].astype(np.float64) * {"mult": a64 * b64, "sub": a64 - b64, "copy": a64}[c.comp]
     ref = seg_reduce(np.add, terms, rp)
     assert_within(y, ref, (deg[:, None] + 2) * U32 * seg_reduce(np.add, np.abs(terms), rp) + TINY, c.id)
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 # ------------------------------------------------------------------------------------------ fused layers
@@ -522,7 +491,7 @@ def run_fused(dev, c):
 
     rp, ci, n = graph_of(c)
     rng = np.random.default_rng(6000 + c.F)
-    st = structure(rp, ci, n, dev, c)
+    st = plan_structure(rp, ci, n, dev, c.plan, c.chunk)
     x = T(rng.standard_normal((n, 128)).astype(np.float32), dev)
     val = T(rng.random(ci.size).astype(np.float32), dev) if c.weighted and c.op != "fused_sage_max" else None
     rs = T((rng.random(n) + 0.5).astype(np.float32), dev) if c.row_scale else None
@@ -535,7 +504,7 @@ def run_fused(dev, c):
         has_chunks(c, st)
     else:
         assert st.plan.n_chunks == 0, f"{c.id}: the structure should have no hub rows"
-    check_counters(c, st)
+    check_counters(st, c.id)
     # the aggregated tile, as the kernel forms it
     if c.op == "fused_sage_max":
         A32 = scatter_max_fwd_raw(st, x)[0].cpu().numpy()
@@ -571,7 +540,7 @@ def run_fused(dev, c):
     E, Mg, steps = emulate(A32, Woh)
     assert np.all(steps <= 3)
     assert_within(got, E, 2.0 ** -22 * steps * Mg + TINY, f"{c.id} split emulation")
-    check_counters(c, st)
+    check_counters(st, c.id)
 
 
 RUN = {"sa_fwd": run_sa_fwd, "sa_bwd": run_sa_bwd, "disen_fwd": run_disen_fwd, "disen_bwd": run_disen_bwd,

@@ -37,24 +37,12 @@ import torch
 from tests import graphs
 from tests import spgemm_oracle as so
 from tests.dispatch_table import SPG_COUNT, SPG_DA, SPG_DA_DB, SPG_DB, SPG_FILL, SPGEMM_TABLE
+from tests.gpu_util import T, dev
 from tests.test_gpu_spspmm import run_and_check, to_dev
 
 pytestmark = pytest.mark.gpu
 
 U32 = 2.0 ** -24
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
 
 
 def raw_product(dev, a, b, m, k, n, dirty):

@@ -19,18 +19,11 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import dev
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-5
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    return torch.device("cuda:0")
 
 
 def rowwise_err(got, ref):

@@ -6,24 +6,11 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gpu_util import dev, plan_structure, row_err
 from tests.graphs import case
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    return torch.device("cuda:0")
-
-
-def err(got, ref):
-    got, ref = got.double().cpu(), ref.double().cpu()
-    scale = torch.maximum(ref.abs(), ref.abs().amax(dim=1, keepdim=True)).clamp_min(1e-30)
-    return float(((got - ref).abs() / scale).max())
 
 
 def ref_layer(rp, ci, val, x, W, b, relu):
@@ -38,12 +25,6 @@ def ref_layer(rp, ci, val, x, W, b, relu):
     return torch.relu(out) if relu else out
 
 
-def st_of(rp, ci, n_cols, dev, chunk=64):
-    from cogdl_b200.structure import CSRStructure
-
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk)
-
-
 def test_identity_graph_is_a_plain_gemm(dev):
     """A = I: OUT = X.W^T + b -- exercises the operand layouts, descriptors and the accumulator fragment layout only."""
     from cogdl_b200.operators.fused_gcn import fused_gcn_raw
@@ -53,20 +34,20 @@ def test_identity_graph_is_a_plain_gemm(dev):
     ci = np.arange(n, dtype=np.int32)
     g = torch.Generator(device=dev).manual_seed(0)
     x = torch.randn(n, 128, device=dev, generator=g)
-    st = st_of(rp, ci, n, dev)
+    st = plan_structure(rp, ci, n, dev, chunk=64)
     eye = torch.eye(128, device=dev)
     out = fused_gcn_raw(st, None, x, eye, None, False)     # W = I: OUT must be X itself (three-term split is exact)
     # (bit-exact if the tensor core adds the three terms without dropping bits; only 1e-6 is REQUIRED)
-    assert err(out, x) <= 1e-6, f"A-operand layout / accumulator read-back broken: max diff {float((out - x).abs().max())}"
+    assert row_err(out, x) <= 1e-6, f"A-operand layout / accumulator read-back broken: max diff {float((out - x).abs().max())}"
     W = torch.randn(128, 128, device=dev, generator=g) / 11.3
     b = torch.randn(128, device=dev, generator=g)
     out = fused_gcn_raw(st, None, x, W, b, False)
-    assert err(out, ref_layer(rp, ci, None, x, W, b, False)) <= TOL
+    assert row_err(out, ref_layer(rp, ci, None, x, W, b, False)) <= TOL
     for fout in (16, 40, 7, 100):                          # N padding and the masked / unvectorised stores
         Wn, bn = W[:fout].contiguous(), b[:fout].contiguous()
         out = fused_gcn_raw(st, None, x, Wn, bn, True)
         assert out.shape == (n, fout)
-        assert err(out, ref_layer(rp, ci, None, x, Wn, bn, True)) <= TOL, fout
+        assert row_err(out, ref_layer(rp, ci, None, x, Wn, bn, True)) <= TOL, fout
 
 
 @pytest.mark.parametrize("name", ["tiny", "ragged", "hub", "two_hubs", "empty_graph"])
@@ -86,16 +67,16 @@ def test_fused_layer_matches_reference_order_fp64(dev, name, fout, weighted):
     W = torch.randn(fout, 128, device=dev, generator=g) / 11.3
     b = torch.randn(fout, device=dev, generator=g)
     for chunk in (64, 16):
-        st = st_of(rp, ci, n_cols, dev, chunk)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk)
         for relu in (False, True):
             out = fused_gcn_raw(st, val, x, W, b, relu)
-            assert err(out, ref_layer(rp, ci, val, x, W, b, relu)) <= TOL, (chunk, relu)
+            assert row_err(out, ref_layer(rp, ci, val, x, W, b, relu)) <= TOL, (chunk, relu)
             out = fused_gcn_raw(st, val, x, W, b, relu, cache_rowsum=False)      # hub weight sums inside the kernel
-            assert err(out, ref_layer(rp, ci, val, x, W, b, relu)) <= TOL, (chunk, relu, "no cached row sums")
+            assert row_err(out, ref_layer(rp, ci, val, x, W, b, relu)) <= TOL, (chunk, relu, "no cached row sums")
         # W = I, no bias: the fused kernel's aggregated tile is the SpMM output (re-assembled from its three bf16 terms)
         if fout == 128:
             out = fused_gcn_raw(st, val, x, torch.eye(128, device=dev), None, False)
-            assert err(out, spmm_raw(st, val, x)) <= 1e-6, chunk
+            assert row_err(out, spmm_raw(st, val, x)) <= 1e-6, chunk
         assert int(st.plan.counters.abs().sum()) == 0
 
 
@@ -127,13 +108,13 @@ def test_fused_layer_module_and_autograd_names_pre_pass_and_layer(dev):
     launches = cogdl_b200._cabi.last_kernel().split(" + ")
     assert len(launches) == 2 and launches[0].startswith("cogdl_b200::stream_kernel<"), launches
     assert launches[1].startswith("cogdl_b200::fg::fused_layer_kernel<gcn,"), launches
-    assert err(yb, ya) <= 2e-5
+    assert row_err(yb, ya) <= 2e-5
     g = torch.randn_like(ya)
     ya.backward(g)
     yb.backward(g)
     for pa, pb in zip(a.parameters(), b.parameters()):
-        assert err(pb.grad.reshape(1, -1), pa.grad.reshape(1, -1)) <= 1e-4
-    assert err(x2.grad, x.grad) <= 1e-4
+        assert row_err(pb.grad.reshape(1, -1), pa.grad.reshape(1, -1)) <= 1e-4
+    assert row_err(x2.grad, x.grad) <= 1e-4
 
 
 def test_fused_layer_full_arxiv_shape(dev):
@@ -153,4 +134,4 @@ def test_fused_layer_full_arxiv_shape(dev):
     b = torch.randn(128, device=dev, generator=gen) * 0.1
     out = fused_gcn_raw(st, g.raw_edge_weight, x, W, b, True)
     ref = ref_layer(rp.numpy().astype(np.int32), col.numpy().astype(np.int32), w, x, W, b, True)
-    assert err(out, ref) <= TOL
+    assert row_err(out, ref) <= TOL

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import dev, plan_structure, row_err
 from tests.graphs import case
 
 pytestmark = pytest.mark.gpu
@@ -14,26 +15,9 @@ TOL = 1e-5
 AGGS = ["sum_weighted", "sum_unweighted", "mean_baked", "mean_in_norm", "max"]
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    torch.backends.cuda.matmul.allow_tf32 = False
+@pytest.fixture(scope="module", autouse=True)
+def _no_cudnn_tf32():
     torch.backends.cudnn.allow_tf32 = False
-    return torch.device("cuda:0")
-
-
-def err(got, ref):
-    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
-    scale = torch.maximum(ref.abs(), ref.abs().amax(dim=1, keepdim=True)).clamp_min(1e-30)
-    return float(((got - ref).abs() / scale).max())
-
-
-def st_of(rp, ci, n_cols, dev, chunk=64):
-    from cogdl_b200.structure import CSRStructure
-
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk)
 
 
 def inputs(kind, rp, ci, dev, g):
@@ -87,16 +71,16 @@ def test_identity_graph_layout(dev, aggr):
     ci = np.arange(n, dtype=np.int32)
     g = torch.Generator(device=dev).manual_seed(0)
     x = torch.randn(n, 128, device=dev, generator=g)
-    st = st_of(rp, ci, n, dev)
+    st = plan_structure(rp, ci, n, dev, chunk=64)
     eye = torch.cat([torch.zeros(128, 128, device=dev), torch.eye(128, device=dev)], dim=1)
     for fout in (128, 16, 40, 7, 100):                     # N padding and the masked / unvectorised stores
         out = fused_sage_raw(st, None, None, x, eye[:fout].contiguous(), None, aggr, False)
         assert out.shape == (n, fout)
-        assert err(out, x[:, :fout]) <= 1e-6, f"operand layout / read-back broken at Fout={fout}"
+        assert row_err(out, x[:, :fout]) <= 1e-6, f"operand layout / read-back broken at Fout={fout}"
     W = torch.randn(100, 256, device=dev, generator=g) / 16
     b = torch.randn(100, device=dev, generator=g)
     out = fused_sage_raw(st, None, None, x, W, b, aggr, True)
-    assert err(out, ref_layer(x, x.cpu(), W, b, True)) <= TOL
+    assert row_err(out, ref_layer(x, x.cpu(), W, b, True)) <= TOL
 
 
 @pytest.mark.parametrize("name", ["tiny", "ragged", "hub", "two_hubs", "empty_graph"])
@@ -113,10 +97,10 @@ def test_fused_sage_matches_reference_order_fp64(dev, name, kind, fout):
     b = torch.randn(fout, device=dev, generator=g)
     agg = oracle_agg(rp, ci, val, row_scale, aggr, x)
     for chunk in (64, 16):
-        st = st_of(rp, ci, n_cols, dev, chunk)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk)
         for relu in (False, True):
             out = fused_sage_raw(st, val, row_scale, x, W, b, aggr, relu)
-            assert err(out, ref_layer(x, agg, W, b, relu)) <= TOL, (chunk, relu)
+            assert row_err(out, ref_layer(x, agg, W, b, relu)) <= TOL, (chunk, relu)
         assert int(st.plan.counters.abs().sum()) == 0
 
 
@@ -132,9 +116,9 @@ def test_aggregated_tile_is_the_unfused_aggregation(dev, name, kind):
     val, row_scale, aggr = inputs(kind, rp, ci, dev, g)
     eye = torch.cat([torch.zeros(128, 128, device=dev), torch.eye(128, device=dev)], dim=1)
     for chunk in (64, 16):
-        st = st_of(rp, ci, n_cols, dev, chunk)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk)
         out = fused_sage_raw(st, val, row_scale, x, eye, None, aggr, False)
-        assert err(out, unfused_agg(st, val, row_scale, aggr, x)) <= 1e-6, chunk
+        assert row_err(out, unfused_agg(st, val, row_scale, aggr, x)) <= 1e-6, chunk
         assert int(st.plan.counters.abs().sum()) == 0
 
 
@@ -183,13 +167,13 @@ def check_layers(a, b, gr_a, gr_b, x, fused_expected=True):
     # with hub rows the fused layer records its pre-pass first: the fused kernel is the last launch named
     last = cogdl_b200._cabi.last_kernel().split(" + ")[-1]
     assert last.startswith("cogdl_b200::fg::fused_layer_kernel<sage-") == fused_expected, cogdl_b200._cabi.last_kernel()
-    assert err(yb, ya) <= 2e-5
+    assert row_err(yb, ya) <= 2e-5
     gout = torch.randn_like(ya)
     ya.backward(gout)
     yb.backward(gout)
     for pa, pb in zip(a.parameters(), b.parameters()):
-        assert err(pb.grad.reshape(1, -1), pa.grad.reshape(1, -1)) <= 1e-4
-    assert err(xb.grad, xa.grad) <= 1e-4
+        assert row_err(pb.grad.reshape(1, -1), pa.grad.reshape(1, -1)) <= 1e-4
+    assert row_err(xb.grad, xa.grad) <= 1e-4
 
 
 @pytest.mark.parametrize("aggr", ["mean", "sum", "max"])
@@ -246,7 +230,7 @@ def test_fused_sage_full_arxiv_shape(dev, aggr):
     n, e = synth.SHAPES["arxiv"]
     rp, col = synth.powerlaw_csr(n, e, seed=0)
     rp32, ci32 = rp.numpy().astype(np.int32), col.numpy().astype(np.int32)
-    st = st_of(rp32, ci32, n, dev)
+    st = plan_structure(rp32, ci32, n, dev, chunk=64)
     gen = torch.Generator(device=dev).manual_seed(2)
     x = torch.randn(n, 128, device=dev, generator=gen)
     W = torch.randn(128, 256, device=dev, generator=gen) / 16
@@ -254,4 +238,4 @@ def test_fused_sage_full_arxiv_shape(dev, aggr):
     val, row_scale, raw = inputs("mean_in_norm" if aggr == "mean" else "max", rp32, ci32, dev, gen)
     out = fused_sage_raw(st, val, row_scale, x, W, b, raw, True)
     ref = ref_layer(x, oracle_agg(rp32, ci32, val, row_scale, raw, x), W, b, True)
-    assert err(out, ref) <= TOL
+    assert row_err(out, ref) <= TOL

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from tests.gat_dropout_ref import drop_below, gat_attention_fp64, gat_dropout_fp64, keep_mask
+from tests.gpu_util import dev, plan_structure, rel
 from tests.graphs import case
 
 pytestmark = pytest.mark.gpu
@@ -22,28 +23,6 @@ TOL = 1e-5
 GRAPHS = [("hub", 16), ("hub", 256), ("two_hubs", 64), ("ragged", 256), ("ragged", 0), ("tiny", 0)]
 # (H, F): the widths of the existing GAT tests; F = 8 at H = 1 takes the narrow-group gather, H = 3 the generic softmax
 SHAPES = [(8, 16), (8, 128), (1, 64), (1, 8), (3, 5)]
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    if b.size == 0:
-        return 0.0
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def structure(rp, ci, n_cols, dev, chunk):
-    from cogdl_b200.structure import CSRStructure
-
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk)
 
 
 def inputs(name, H, F, dev, seed=12):
@@ -69,7 +48,7 @@ def test_p0_through_dropout_entry_points_is_bit_identical(dev, name, chunk, H, F
     from cogdl_b200.operators._raw import gat_attn_bwd_raw, gat_fwd_raw, mhsddmm_raw, mhspmm_raw
 
     rp, ci, n, h_l, h_r, feat = inputs(name, H, F, dev)
-    st = structure(rp, ci, n, dev, chunk)
+    st = plan_structure(rp, ci, n, dev, chunk=chunk)
     out0, att0 = gat_fwd_raw(st, h_l, h_r, feat, 0.2, True)
     out1, att1 = gat_fwd_raw(st, h_l, h_r, feat, 0.2, True, drop=drop_args(987654321, 0.0))
     assert torch.equal(out0, out1) and torch.equal(att0, att1)
@@ -89,7 +68,7 @@ def test_forward_and_mask_vs_fp64(dev, name, chunk, H, F, p):
     from cogdl_b200.operators._raw import gat_fwd_raw
 
     rp, ci, n, h_l, h_r, feat = inputs(name, H, F, dev)
-    st = structure(rp, ci, n, dev, chunk)
+    st = plan_structure(rp, ci, n, dev, chunk=chunk)
     seed = 0xABCDEF0123 + 7 * H + F
     out, att = gat_fwd_raw(st, h_l, h_r, feat, 0.2, True, drop=drop_args(seed, p))
     keep = keep_mask(seed, ci.size, H, p)
@@ -113,7 +92,7 @@ def test_gradients_vs_fp64_autograd(dev, name, chunk, H, F):
 
     p, seed = 0.5, 4242 + H
     rp, ci, n, h_l, h_r, feat = inputs(name, H, F, dev)
-    st = structure(rp, ci, n, dev, chunk)
+    st = plan_structure(rp, ci, n, dev, chunk=chunk)
     xs = [t.clone().requires_grad_(True) for t in (h_l, h_r, feat)]
     out = FusedGATFunction.apply(xs[0], xs[1], st, None, None, None, 0.2, xs[2], p, seed)
     G = torch.randn_like(out)
@@ -221,7 +200,7 @@ def test_kernel_names_list_every_launch_with_the_dropout_flag(dev):
     from cogdl_b200.operators._raw import gat_attn_bwd_raw, gat_fwd_raw, mhsddmm_raw
 
     rp, ci, n, h_l, h_r, feat = inputs("hub", 8, 128, dev)
-    st = structure(rp, ci, n, dev, 256)
+    st = plan_structure(rp, ci, n, dev, chunk=256)
     _, att = gat_fwd_raw(st, h_l, h_r, feat, 0.2, True, drop=drop_args(1, 0.5))
     assert _cabi.last_kernel() == ("cogdl_b200::es_stats_kernel<MODE=2> + cogdl_b200::es_main_kernel<MODE=2,CAP=2048,WARPS=8,DROP>"
                                    " + cogdl_b200::stream_kernel<float4,NV=1,multihead+drop,SRC_ONE,U=8,MINB=3,prefetch>"
@@ -231,7 +210,7 @@ def test_kernel_names_list_every_launch_with_the_dropout_flag(dev):
     assert _cabi.last_kernel() == ("cogdl_b200::es_stats_kernel<MODE=3,DROP> + "
                                    "cogdl_b200::es_main_kernel<MODE=3,CAP=2048,WARPS=8,DROP> cp.async.bulk tiles")
     rp1, ci1, n1, hl1, hr1, f1 = inputs("hub", 1, 8, dev)
-    gat_fwd_raw(structure(rp1, ci1, n1, dev, 256), hl1, hr1, f1, 0.2, True, drop=drop_args(1, 0.5))
+    gat_fwd_raw(plan_structure(rp1, ci1, n1, dev, chunk=256), hl1, hr1, f1, 0.2, True, drop=drop_args(1, 0.5))
     assert _cabi.last_kernel() == ("cogdl_b200::es_stats_kernel<MODE=2> + cogdl_b200::es_main_kernel<MODE=2,CAP=512,WARPS=8,DROP>"
                                    " + cogdl_b200::mhspmm_kernel<float4,GROUP=2,no_perm,drop>")
 
@@ -243,7 +222,7 @@ def test_bad_arguments_raise_the_library_error(dev):
     from cogdl_b200.structure import _ptr, _stream
 
     rp, ci, n, h_l, h_r, feat = inputs("tiny", 8, 16, dev)
-    st = structure(rp, ci, n, dev, 256)
+    st = plan_structure(rp, ci, n, dev, chunk=256)
     out = torch.empty(n, 8, 16, device=dev)
     att = torch.empty(ci.size, 8, device=dev)
     plan, keep = st.plan_struct(_scratch("gat_fwd", st, 8, 16))

@@ -11,38 +11,18 @@ import torch
 
 from tests import graphs
 from tests.genconv_ref import genconv_aggregate_fp64
+from tests.gpu_util import dev, plan_structure, row_err
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.fixture(scope="module")
-def dev():
-    import cogdl_b200  # noqa: F401
-
-    torch.backends.cuda.matmul.allow_tf32 = False
-    return torch.device("cuda:0")
-
-
-def err(got, ref):
-    """max |got - ref| / max(|ref|, row scale of ref)."""
-    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
-    if ref.numel() == 0:
-        return 0.0
-    if ref.dim() == 1:
-        ref, got = ref[:, None], got[:, None]
-    scale = torch.maximum(ref.abs(), ref.abs().amax(dim=1, keepdim=True)).clamp_min(1e-30)
-    return float(((got - ref).abs() / scale).max())
-
-
 def structure(name, dev, chunk=None):
-    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES, CSRStructure
+    from cogdl_b200.structure import DEFAULT_CHUNK_EDGES
 
     rp, ci, n_cols = graphs.case(name)
-    st = CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols,
-                      chunk_edges=DEFAULT_CHUNK_EDGES if chunk is None else chunk)
-    return st, rp, ci, n_cols
+    return plan_structure(rp, ci, n_cols, dev, chunk=DEFAULT_CHUNK_EDGES if chunk is None else chunk), rp, ci, n_cols
 
 
 @pytest.mark.parametrize("chunk", [None, 16])
@@ -60,11 +40,11 @@ def test_forward_matches_fp64(dev, name, F, edge, chunk):
         got = genconv_aggregate(st, x, "softmax_sg", beta=beta, edge_term=a)
         want = genconv_aggregate_fp64(st.rowptr, st.colind, x, "softmax_sg", beta=beta, edge_term=a)
         assert got.shape == (st.n_rows, F)
-        assert err(got, want) <= 1e-5, f"beta={beta}"
+        assert row_err(got, want) <= 1e-5, f"beta={beta}"
     for aggr in ("softmax", "mean", "sum") + (() if edge else ("max", "powermean")):
         got = genconv_aggregate(st, x, aggr, edge_term=a, p=2.0)
         want = genconv_aggregate_fp64(st.rowptr, st.colind, x, aggr, edge_term=a, p=2.0)
-        assert err(got, want) <= 1e-5, aggr
+        assert row_err(got, want) <= 1e-5, aggr
 
 
 def test_large_logits(dev):
@@ -76,7 +56,7 @@ def test_large_logits(dev):
     beta = torch.full((1,), 20.0, device=dev)                     # beta * m up to 80
     got = genconv_aggregate(st, x, "softmax_sg", beta=beta)
     assert torch.isfinite(got).all()
-    assert err(got, genconv_aggregate_fp64(st.rowptr, st.colind, x, "softmax_sg", beta=20.0)) <= 1e-5
+    assert row_err(got, genconv_aggregate_fp64(st.rowptr, st.colind, x, "softmax_sg", beta=20.0)) <= 1e-5
 
 
 @pytest.mark.parametrize("aggr", ["softmax_sg", "softmax", "mean", "sum"])
@@ -104,11 +84,11 @@ def test_gradients_match_fp64_autograd(dev, name, edge, aggr):
     got = grads(lambda x_, a_, b_: genconv_aggregate(st, x_, aggr, beta=b_, edge_term=a_), torch.float32)
     want = grads(lambda x_, a_, b_: genconv_aggregate_fp64(st.rowptr, st.colind, x_, aggr, beta=b_, edge_term=a_),
                  torch.float64)
-    assert err(got[0], want[0]) <= 1e-4
+    assert row_err(got[0], want[0]) <= 1e-4
     if edge:
-        assert err(got[1], want[1]) <= 1e-4
+        assert row_err(got[1], want[1]) <= 1e-4
     if aggr == "softmax_sg":
-        assert err(got[2], want[2]) <= 1e-4
+        assert row_err(got[2], want[2]) <= 1e-4
     else:
         assert got[2] is None
 
@@ -180,7 +160,7 @@ def test_full_arxiv_shape_forward(dev):
     x = torch.randn(st.n_cols, 128, device=dev, generator=torch.Generator(device=dev).manual_seed(0))
     got = genconv_aggregate(st, x, "softmax_sg", beta=1.0)
     want = genconv_aggregate_fp64(st.rowptr, st.colind, x, "softmax_sg", beta=1.0)
-    assert err(got, want) <= 1e-5
+    assert row_err(got, want) <= 1e-5
 
 
 def test_reference_deepergcn_through_install():

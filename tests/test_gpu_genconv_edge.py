@@ -36,22 +36,15 @@ import torch
 from tests import graphs
 from tests.genconv_edge_table import GE_BWD_BLOCKS, GE_WARPS, TABLE, wide_csr
 from tests.genconv_ref import genconv_aggregate_fp64
-from tests.test_gpu_dispatch_message import (EPS, LN2, LOG2E, RATIOS, TINY, U32, assert_within, check_counters,
-                                             col_sum, edge_rows, misaligned, sa_fwd64, sa_inputs, sa_m, seg_reduce)
-from tests.test_gpu_genconv import err, structure
+from tests.gpu_util import check_counters, dev, misaligned, row_err
+from tests.test_gpu_dispatch_message import (EPS, LN2, LOG2E, RATIOS, TINY, U32, assert_within, col_sum, edge_rows,
+                                             sa_fwd64, sa_inputs, sa_m, seg_reduce)
+from tests.test_gpu_genconv import structure
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SOFTMAX_AGGRS = ("softmax_sg", "softmax", "mean", "sum")
-
-
-@pytest.fixture(scope="module")
-def dev():
-    import cogdl_b200  # noqa: F401
-
-    torch.backends.cuda.matmul.allow_tf32 = False
-    return torch.device("cuda:0")
 
 
 def operands(st, F, D, dev, seed=0):
@@ -78,10 +71,10 @@ def test_forward_matches_fp64(dev, name, F, D, chunk):
     for beta in (0.0, 0.5, 1.0, 4.0):
         got = genconv_aggregate(st, x, "softmax_sg", beta=beta, edge_attr=attr, edge_weight=w)
         assert got.shape == (st.n_rows, F)
-        assert err(got, fp64(st, x, attr, w, "softmax_sg", beta)) <= 1e-5, f"beta={beta}"
+        assert row_err(got, fp64(st, x, attr, w, "softmax_sg", beta)) <= 1e-5, f"beta={beta}"
     for aggr in ("softmax", "mean", "sum"):
         got = genconv_aggregate(st, x, aggr, edge_attr=attr, edge_weight=w)
-        assert err(got, fp64(st, x, attr, w, aggr)) <= 1e-5, aggr
+        assert row_err(got, fp64(st, x, attr, w, aggr)) <= 1e-5, aggr
 
 
 def q_fp64(st, x, attr, w, beta, eps=1e-7):
@@ -127,15 +120,15 @@ def test_gradients_match_fp64_autograd(dev, name, aggr):
 
     want = _grads(exact, x, w, beta, r, torch.float64, need_b=need_b)
     got = _grads(mine, x, w, beta, r, torch.float32, need_b=need_b)
-    assert err(got[1], want[1]) <= 1e-4
-    assert err(got[2], want[2]) <= 1e-4
+    assert row_err(got[1], want[1]) <= 1e-4
+    assert row_err(got[2], want[2]) <= 1e-4
     if need_b:
-        assert err(got[3], want[3]) <= 1e-4
+        assert row_err(got[3], want[3]) <= 1e-4
     else:
         assert got[3] is None
     # only W needs grad: no dx; only x: no dW (and the frozen W costs no dW pass)
     only_w = _grads(mine, x, w, beta, r, torch.float32, need_x=False, need_b=False)
-    assert only_w[1] is None and err(only_w[2], want[2]) <= 1e-4
+    assert only_w[1] is None and row_err(only_w[2], want[2]) <= 1e-4
     assert torch.equal(only_w[2], got[2])
     only_x = _grads(mine, x, w, beta, r, torch.float32, need_w=False, need_b=False)
     assert only_x[2] is None and torch.equal(only_x[1], got[1])
@@ -168,7 +161,7 @@ def test_bit_identical_to_edge_term_kernels(dev, name, F, aggr):
     (out_b * r).sum().backward()
     assert torch.equal(out_a, out_b)
     assert torch.equal(xa.grad, xb.grad)
-    assert err(wa.grad, term.grad.T.double() @ attr.double()) <= 1e-5
+    assert row_err(wa.grad, term.grad.T.double() @ attr.double()) <= 1e-5
 
 
 @pytest.mark.parametrize("name", ["hub", "two_hubs"])
@@ -359,7 +352,7 @@ def test_table_row(dev, c):
         if c.graph.startswith("bounds") or c.partials_offset:
             assert st.plan.n_chunks > 0
         _check_fwd(c, rp, out, lse2, q, m, dm)
-        check_counters(c, st)
+        check_counters(st, c.id)
     else:
         out, lse2, _ = genconv_edge_fwd_raw(st, xd, attr_d, w_d, beta_d, EPS, want_lse=True)
         g = np.random.default_rng(3 + c.F).standard_normal((st.n_rows, c.F)).astype(np.float32)
@@ -376,7 +369,8 @@ def test_table_row(dev, c):
             for a, b in zip((dx, dw), again):
                 assert (a is None and b is None) or torch.equal(a, b), f"{c.id}: not reproducible"
         _check_bwd(c, st, rp, ci, n, attr, g, out, lse2, dx, dw, pre, m, dm, flip)
-        check_counters(c, st, st_t)
+        check_counters(st, c.id)
+        check_counters(st_t, c.id)
     print(" ".join(f"[{k}: worst err/bound {v:.3g}]" for k, v in RATIOS.items()))
 
 
@@ -412,7 +406,7 @@ def test_no_edge_sized_tensor(dev):
     assert xg.grad is not None and wg.grad is not None
     with torch.no_grad():
         got = genconv_aggregate(st, x, "softmax_sg", beta=1.0, edge_attr=attr, edge_weight=w)
-    assert err(got, fp64(st, x, attr, w, "softmax_sg", 1.0)) <= 1e-5
+    assert row_err(got, fp64(st, x, attr, w, "softmax_sg", 1.0)) <= 1e-5
 
 
 def test_errors(dev):

@@ -24,24 +24,15 @@ import scipy.sparse as sp
 import torch
 
 from tests.gin_grand_table import TABLE
+from tests.gpu_util import bits, dev, misaligned, plan_structure
 from tests.graphs import boundary_csr, case
 from tests.test_gpu_autograd import (GraphCase, MODES, SQUARE, bound, incoming, place, same_bits, sum_ref, within)
-from tests.test_gpu_label_prop import bits, misaligned, structure
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 A_COEF, B_COEF, ORDER = 0.8, 1.3, 8
 ORDERS = (0, 1, 2, 8)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
 
 
 def row_inputs(c, dev):
@@ -78,7 +69,7 @@ def test_row_is_the_unfused_sequence_bit_for_bit_and_near_fp64(dev, c):
     from cogdl_b200.operators.grand import div_scale
 
     rp, ci, n_cols, n, X, Z, r, val = row_inputs(c, dev)
-    st = structure(rp, ci, n_cols, dev, c.plan, c.chunk)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     t = spmm_raw(st, val, X, panels=c.panels)
     if r is not None:
         t = r.view(-1, 1) * t
@@ -127,7 +118,7 @@ def test_accum_entry_rejects_overlapping_outputs(dev):
     from cogdl_b200.operators._raw import spmm_accum_raw
 
     rp, ci, n_cols = case("two_hubs")
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev, chunk=64)
     n = rp.shape[0] - 1
     X = torch.randn(n, 16, device=dev)
     acc = torch.zeros(n, 16, device=dev)

@@ -13,6 +13,7 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+from tests.gpu_util import bits, dev, misaligned, plan_structure
 from tests.graphs import boundary_csr, case
 from tests.label_prop_table import TABLE
 
@@ -20,34 +21,6 @@ pytestmark = pytest.mark.gpu
 
 A_COEF, B_COEF = 0.8, 1 - 0.8   # alpha = 0.8 of the smooth phase, (1 - alpha) rounded in fp64 first, as Python does
 CLAMP_LO, CLAMP_HI = -0.75, 0.5
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def structure(rp, ci, n_cols, dev, plan="default", chunk=64):
-    from cogdl_b200.structure import CSRStructure
-
-    chunk, seg_cost = {"none": (0, None), "chunks": (chunk, 0), "default": (chunk, None)}[plan]
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk,
-                        seg_cost=seg_cost)
-
-
-def misaligned(t):
-    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
-    out = buf[1:].view(t.shape)
-    out.copy_(t)
-    return out
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 def inputs(c, dev):
@@ -87,7 +60,7 @@ def test_step_is_the_unfused_sequence_bit_for_bit_and_near_fp64(dev, c):
     from cogdl_b200.operators.label_prop import label_prop_raw, pin_mask
 
     rp, ci, n_cols, X, Z, r, val, nid = inputs(c, dev)
-    st = structure(rp, ci, n_cols, dev, c.plan, c.chunk)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     n = rp.shape[0] - 1
     clamp = (CLAMP_LO, CLAMP_HI) if c.clamp else None
     pin = pin_mask(n, nid, dev) if nid is not None else None
@@ -123,7 +96,7 @@ def test_step_is_the_unfused_sequence_bit_for_bit_and_near_fp64(dev, c):
 def special_inputs(dev, F=40, plan="default"):
     """A hub graph with empty rows, X and Z holding NaN, +-inf and -0.0."""
     rp, ci, n = case("two_hubs")
-    st = structure(rp, ci, n, dev, plan)
+    st = plan_structure(rp, ci, n, dev, plan, 64)
     g = torch.Generator().manual_seed(11)
     X = torch.randn(n, F, generator=g)
     Z = torch.randn(n, F, generator=g)

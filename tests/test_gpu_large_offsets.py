@@ -34,6 +34,7 @@ import scipy.sparse as sp
 import torch
 
 from tests import large_offset_table as LT
+from tests.gpu_util import plan_structure
 from tests.test_gpu_dispatch import SLOPE, TINY, U32, check_softmax, gat_logits32, softmax_bwd64
 
 pytestmark = pytest.mark.gpu
@@ -72,12 +73,8 @@ def D(a):
 
 
 def structure(rp, ci, n_cols, plan):
-    from cogdl_b200.structure import CSRStructure
-
-    chunk, seg = {"none": (0, None), "chunks": (LT.CHUNK, 0), "default": (LT.CHUNK, None)}[plan]
-    rp = rp if isinstance(rp, torch.Tensor) else D(rp.astype(np.int32))
-    ci = ci if isinstance(ci, torch.Tensor) else D(ci.astype(np.int32))
-    return CSRStructure(rp, ci, n_cols=n_cols, chunk_edges=chunk, seg_cost=seg)
+    int32 = lambda a: a if isinstance(a, torch.Tensor) else a.astype(np.int32)  # noqa: E731
+    return plan_structure(int32(rp), int32(ci), n_cols, DEV, plan, LT.CHUNK)
 
 
 def last_kernel():

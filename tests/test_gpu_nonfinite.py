@@ -22,6 +22,7 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import T, check_counters, dev, plan_structure
 from tests.graphs import boundary_csr, case
 from tests.nonfinite_table import PANEL_F, PLAN_FORMS, SPMM_PANELS, TABLE
 from tests.test_gpu_dispatch import softmax64
@@ -34,34 +35,20 @@ TINY = float(np.finfo(np.float32).tiny)
 BF16_OVERFLOW = float.fromhex("0x1.fefp127")     # the smallest fp32 that rounds to a bf16 infinity
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
 def graph_of(c, chunk):
     return boundary_csr(chunk or 16) if c.graph == "bounds" else case(c.graph)
 
 
 def structure(rp, ci, n_cols, dev, form):
-    from cogdl_b200.structure import CSRStructure
-
     _, chunk, seg_cost = form
-    return CSRStructure(T(rp, dev), T(ci, dev), n_cols=n_cols, chunk_edges=chunk, seg_cost=seg_cost)
+    return plan_structure(rp, ci, n_cols, dev, chunk=chunk, seg_cost=seg_cost)
 
 
-def check_counters(st, what):
+def check_hub_plan(st, what):
+    """A planned structure has hub chunks, and the call left their arrival counters at zero."""
     if st.chunk_edges > 0:
         assert st.plan.n_chunks > 0, f"{what}: the graph should have hub rows at chunk {st.chunk_edges}"
-        assert int(st.plan.counters.abs().sum()) == 0, f"{what}: arrival counters not back at zero"
+    check_counters(st, what)
 
 
 def rows_of(rp):
@@ -154,7 +141,7 @@ def run_spmm(dev, c, form):
         got = spmm_raw(st, T(w, dev), T(X, dev), panels=panels).cpu().numpy()
         ref, bound = spmm64(rp, ci, w, X)
         check(got, ref, bound, f"{c.id} {form[0]} F={F} panels={panels}")
-        check_counters(st, c.id)
+        check_hub_plan(st, c.id)
         # rows the plan does not split: equal to the oracle's CSR-order fp32 sum (NaN where it is NaN)
         want = oracle.spmm_csr(rp, ci, w, X)
         assert np.array_equal(got[~split], want[~split], equal_nan=True), \
@@ -188,7 +175,7 @@ def run_spmm_f16(dev, c, form):
     deg = np.diff(rp)[:, None]
     check(got, ref16, 2.0 ** -11 * np.abs(ref) + deg * U32 * mag + 2.0 ** -24, f"{c.id} {form[0]}")
     assert np.isinf(got[:, 2]).any() and np.isinf(got[:, 3]).any()
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def run_residual(dev, c, form):
@@ -209,7 +196,7 @@ def run_residual(dev, c, form):
             ref = a * agg + b * Z.astype(np.float64)
         check(got, ref, a * bound + 2 * U32 * (np.abs(a * agg) + np.abs(b * np.nan_to_num(Z, posinf=0, neginf=0))),
               f"{c.id} {form[0]} a={a} b={b}")
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def run_sddmm(dev, c, form):
@@ -246,7 +233,7 @@ def run_mhspmm(dev, c, form):
     for h in range(c.H):
         ref, bound = spmm64(rp, ci, att[:, h], feat[:, h, :])
         check(got[:, h], ref, bound, f"{c.id} {form[0]} head {h}")
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def run_scatter_max(dev, c, form):
@@ -265,7 +252,7 @@ def run_scatter_max(dev, c, form):
     assert not np.isnan(ref).any() and np.isinf(ref).any()
     assert np.array_equal(out.cpu().numpy(), ref), f"{c.id} {form[0]}: max differs"
     assert np.array_equal(arg.cpu().numpy(), ref_id), f"{c.id} {form[0]}: argmax differs"
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def run_edge_softmax(dev, c, form):
@@ -291,7 +278,7 @@ def run_edge_softmax(dev, c, form):
         y, t, Tm, d = softmax64(rp, x)
     check(got, y, y * ((d + 3) * 2.0 ** -22 + d * U32 + (2 * t + 2 * Tm) * 2.0 ** -23) + 2.0 ** -126,
           f"{c.id} {form[0]}")
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def sa64(rp, ci, x, A, beta):
@@ -337,7 +324,7 @@ def run_softmax_aggr(dev, c, form):
         out, _, _ = softmax_aggr_fwd_raw(st, T(x, dev), beta_d, EPS, None if A is None else T(A, dev))
         ref, bound = sa64(rp, ci, x, A, beta)
         check(out.cpu().numpy(), ref, bound, f"{c.id} {form[0]} beta={beta}")
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def run_genconv_edge(dev, c, form):
@@ -354,7 +341,7 @@ def run_genconv_edge(dev, c, form):
     A = (attr.astype(np.float64) @ W.astype(np.float64).T).astype(np.float32)
     ref, bound = sa64(rp, ci, x, A, 1.0)
     check(out.cpu().numpy(), ref, bound + 2.0 ** -12 * np.abs(np.nan_to_num(ref)), f"{c.id} {form[0]}")
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 def run_fused(dev, c, form):
@@ -443,7 +430,7 @@ def fused_case(dev, c, form, relu):
     else:
         check(got, ref, 2.0 ** -15 * np.where(np.isfinite(mag), mag, 0) + TINY, f"{c.id} {form[0]} relu={relu}",
               nan_superset=not relu)
-    check_counters(st, c.id)
+    check_hub_plan(st, c.id)
 
 
 RUN = {

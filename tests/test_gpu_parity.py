@@ -10,38 +10,12 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import T, dev, plan_structure, rel
 from tests.graphs import CASES, case
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-5
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    if b.size == 0:
-        return 0.0
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def structure(rp, ci, n_cols, dev, chunk=256, seg_cost=None):
-    from cogdl_b200.structure import CSRStructure
-
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk,
-                        seg_cost=seg_cost)
-
-
-def T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
 
 
 # ------------------------------------------------------------------------------------ SpMM
@@ -59,7 +33,7 @@ def test_spmm_matches_oracle(dev, name, F, weighted):
     # chunk 0: no hub plan -> strictly sequential -> bit exact everywhere; seg_cost 0: a plan without segments, so
     # every width runs the row kernel with hub chunks
     for chunk, seg_cost in ((0, None), (256, None), (256, 0)):
-        st = structure(rp, ci, n_cols, dev, chunk, seg_cost)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk, seg_cost=seg_cost)
         y = spmm_raw(st, None if val is None else T(val, dev), T(X, dev)).cpu().numpy()
         assert y.shape == ref.shape
         deg = np.diff(rp)
@@ -74,7 +48,7 @@ def test_spmm_deterministic_with_hubs(dev):
     rp, ci, n_cols = case("hub")
     rng = np.random.default_rng(2)
     X, val = T(rng.standard_normal((n_cols, 128)).astype(np.float32), dev), T(rng.random(ci.shape[0]).astype(np.float32), dev)
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev)
     assert st.plan.n_hub_rows == 1 and st.plan.n_chunks == 6
     y0 = spmm_raw(st, val, X)
     for _ in range(5):
@@ -90,7 +64,7 @@ def test_spmm_half(dev):
     X = rng.standard_normal((n_cols, 128)).astype(np.float16)
     val = rng.random(ci.shape[0]).astype(np.float16)
     ref = oracle.spmm_csr(rp, ci, val.astype(np.float32), X.astype(np.float32))
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev)
     y = spmm_raw(st, T(val, dev), T(X, dev))
     assert y.dtype == torch.float16
     # fp16 storage, fp32 accumulate: error budget = one fp16 rounding of the result
@@ -105,7 +79,7 @@ def test_spmm_two_source(dev):
     X = rng.standard_normal((n_cols, 128)).astype(np.float32)
     val = rng.random(ci.shape[0]).astype(np.float32)
     ref = oracle.spmm_csr(rp, ci, val, X)
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev)
     n0 = 123
     y = spmm_2src_raw(st, T(val, dev), T(X[:n0], dev), T(X[n0:], dev)).cpu().numpy()
     assert np.array_equal(y, ref)
@@ -136,7 +110,7 @@ def test_spmm_peer_form_single_gpu(dev, F):
         m = (ci >= bounds[o]) & (ci < bounds[o + 1])
         enc[m] = bounds[1] + (o << shift) + (ci[m] - bounds[o])
     shards = [T(X[bounds[o]:bounds[o + 1]], dev) for o in range(3)]
-    st = structure(rp, enc, n_cols, dev)
+    st = plan_structure(rp, enc, n_cols, dev)
     ptrs = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in shards])
     y = torch.empty((n, F), device=dev)
     plan, keep = st.plan_struct(_scratch("spmm", st, F))
@@ -160,7 +134,7 @@ def test_sddmm_matches_oracle(dev, name, F):
     D1 = rng.standard_normal((n, F)).astype(np.float32)
     D2 = rng.standard_normal((n_cols, F)).astype(np.float32)
     ref = oracle.sddmm_csr(rp, ci, D1, D2)
-    out = sddmm_raw(structure(rp, ci, n_cols, dev), T(D1, dev), T(D2, dev)).cpu().numpy()
+    out = sddmm_raw(plan_structure(rp, ci, n_cols, dev), T(D1, dev), T(D2, dev)).cpu().numpy()
     assert rel(out, ref) <= TOL
 
 
@@ -169,7 +143,7 @@ def test_sddmm_matches_oracle(dev, name, F):
 def test_csr2csc_bit_exact(dev, name):
     rp, ci, n_cols = case(name)
     colptr, rowind, perm = oracle.csr2csc(rp, ci, n_cols)
-    st_t, p = structure(rp, ci, n_cols, dev).csc()
+    st_t, p = plan_structure(rp, ci, n_cols, dev).csc()
     assert np.array_equal(st_t.rowptr.cpu().numpy(), colptr)
     assert np.array_equal(st_t.colind.cpu().numpy(), rowind)
     assert np.array_equal(p.cpu().numpy(), perm)
@@ -200,7 +174,7 @@ def test_edge_softmax_fwd_bwd(dev, name, H):
     # chunk 256: tiles of 2048 floats or the warp kernel (H >= 16); 64 / 16: the 512- and 1024-float tiles,
     # many chunks per hub row (split-row statistics), cp.async.bulk staging when H % 4 == 0; 0: no plan
     for chunk in (256, 64, 16, 0):
-        st = structure(rp, ci, n_cols, dev, chunk)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk)
         y = edge_softmax_fwd_raw(st, T(e, dev))
         gin = edge_softmax_bwd_raw(st, T(yref, dev), T(g, dev))
         assert rel(y.cpu().numpy(), yref) <= TOL, chunk
@@ -235,7 +209,7 @@ def test_gat_attention_backward_and_colsum(dev, name, H):
     hl, hr = rng.standard_normal((n, H)).astype(np.float32), rng.standard_normal((n, H)).astype(np.float32)
     de_ref, gr_ref, gc_ref = oracle.gat_attn_bwd(rp, ci, att, d_att, hl, hr, 0.2)
     for chunk in (256, 16, 0):
-        st = structure(rp, ci, n_cols, dev, chunk)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk)
         de, gr = gat_attn_bwd_raw(st, T(att, dev), T(d_att, dev), T(hl, dev), T(hr, dev), 0.2)
         assert rel(de.cpu().numpy(), de_ref) <= TOL and rel(gr.cpu().numpy(), gr_ref) <= TOL, chunk
         st_t, perm = st.csc()
@@ -260,7 +234,7 @@ def test_mhspmm_and_mhsddmm(dev, name, H, F):
     ref = oracle.mhspmm(rp, ci, att, feat)
     ref_sd = oracle.mhsddmm(rp, ci, grad, feat)
     for chunk, seg_cost in ((0, None), (256, None), (256, 0)):   # seg_cost 0: row kernel with hub chunks
-        st = structure(rp, ci, n_cols, dev, chunk, seg_cost)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk, seg_cost=seg_cost)
         out = mhspmm_raw(st, T(att, dev), T(feat, dev)).cpu().numpy()
         unsplit = np.diff(rp) <= chunk if chunk else np.ones(n, bool)
         assert np.array_equal(out[unsplit], ref[unsplit])
@@ -280,7 +254,7 @@ def test_mhspmm_transpose_with_fused_perm(dev):
     grad = rng.standard_normal((rp.shape[0] - 1, H, F)).astype(np.float32)
     colptr, rowind, perm = oracle.csr2csc(rp, ci, n_cols)
     ref = oracle.mhspmm(colptr, rowind, att, grad, perm=perm)
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev)
     st_t, p = st.csc()
     out = mhspmm_raw(st_t, T(att, dev), T(grad, dev), perm=p).cpu().numpy()
     assert rel(out, ref) <= TOL
@@ -299,7 +273,7 @@ def test_scatter_max_fwd_bwd(dev, name, F):
     X = np.round(rng.standard_normal((n_cols, F)) * 4).astype(np.float32) / 4
     ref, ref_id = oracle.scatter_max_fwd(rp, ci, X)
     for chunk, seg_cost in ((0, None), (256, None), (256, 0)):   # seg_cost 0: row kernel with hub chunks
-        out, arg = scatter_max_fwd_raw(structure(rp, ci, n_cols, dev, chunk, seg_cost), T(X, dev))
+        out, arg = scatter_max_fwd_raw(plan_structure(rp, ci, n_cols, dev, chunk=chunk, seg_cost=seg_cost), T(X, dev))
         assert np.array_equal(out.cpu().numpy(), ref)         # max is exact
         assert np.array_equal(arg.cpu().numpy(), ref_id)      # integer output: bit exact, ties included
     g = rng.standard_normal((n, F)).astype(np.float32)
@@ -314,7 +288,7 @@ def test_scatter_max_reference_semantics_agree_on_positive_features(dev):
     rp, ci, n_cols = case("ragged")
     X = (np.random.default_rng(11).random((n_cols, 64)) + 0.01).astype(np.float32)
     ref, ref_id = oracle.scatter_max_fwd(rp, ci, X, reference_semantics=True)
-    out, arg = scatter_max_fwd_raw(structure(rp, ci, n_cols, dev), T(X, dev))
+    out, arg = scatter_max_fwd_raw(plan_structure(rp, ci, n_cols, dev), T(X, dev))
     has = np.diff(rp) > 0
     assert np.array_equal(out.cpu().numpy()[has], ref[has]) and np.array_equal(arg.cpu().numpy()[has], ref_id[has])
 
@@ -326,7 +300,7 @@ def test_scatter_max_and_mhspmm_name_their_kernel(dev):
     from cogdl_b200.operators._raw import mhspmm_raw, scatter_max_fwd_raw, spmm_raw
 
     rp, ci, n_cols = case("hub")
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev)
     rng = np.random.default_rng(15)
     spmm_raw(st, None, T(rng.standard_normal((n_cols, 128)).astype(np.float32), dev))
     assert "stream_kernel<" in _cabi.last_kernel()
@@ -355,7 +329,7 @@ def test_fused_gat_forward(dev, name, H, F):
     h_r = rng.standard_normal((n, H)).astype(np.float32)
     feat = rng.standard_normal((n, H, F)).astype(np.float32)
     ref, ref_att = oracle.gat_fwd(rp, ci, h_l, h_r, feat, 0.2, return_att=True)
-    out, att = gat_fwd_raw(structure(rp, ci, n_cols, dev), T(h_l, dev), T(h_r, dev), T(feat, dev), 0.2, True)
+    out, att = gat_fwd_raw(plan_structure(rp, ci, n_cols, dev), T(h_l, dev), T(h_r, dev), T(feat, dev), 0.2, True)
     assert rel(out.cpu().numpy(), ref) <= TOL
     assert rel(att.cpu().numpy(), ref_att) <= TOL
 
@@ -420,7 +394,7 @@ def test_errors_are_raised_not_swallowed(dev):
     from cogdl_b200.operators._raw import spmm_raw
 
     rp, ci, n_cols = case("tiny")
-    st = structure(rp, ci, n_cols, dev)
+    st = plan_structure(rp, ci, n_cols, dev)
     with pytest.raises(ValueError):
         spmm_raw(st, torch.ones(3, device=dev), torch.ones(n_cols, 4, device=dev))  # wrong nnz
     with pytest.raises(RuntimeError):
@@ -441,7 +415,7 @@ def test_stream_spmm_on_hub_chunks_matches_the_oracle(dev, F):
     rng = np.random.default_rng(21)
     X = rng.standard_normal((n_cols, F)).astype(np.float32)
     val = rng.random(ci.shape[0]).astype(np.float32)
-    st = structure(rp, ci, n_cols, dev, chunk=64)
+    st = plan_structure(rp, ci, n_cols, dev, chunk=64)
     y = spmm_raw(st, T(val, dev), T(X, dev)).cpu().numpy()
     ref = oracle.spmm_csr(rp, ci, val, X)
     unsplit = np.diff(rp) <= 64
@@ -469,7 +443,7 @@ def test_sddmm_stream_and_row_forms_match_the_oracle(dev, name, H, F):
         run = lambda st: mhsddmm_raw(st, T(grad, dev), T(feat, dev))
     # stream form (default plan), row form with hub chunks (plan without segments), row form without a plan
     for chunk, seg_cost in ((64, None), (64, 0), (0, None)):
-        st = structure(rp, ci, n_cols, dev, chunk, seg_cost)
+        st = plan_structure(rp, ci, n_cols, dev, chunk=chunk, seg_cost=seg_cost)
         out = run(st).cpu().numpy()
         assert rel(out, ref) <= TOL, f"chunk={chunk} seg_cost={seg_cost}"
         if chunk:

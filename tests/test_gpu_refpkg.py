@@ -25,16 +25,12 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gpu_util import rel
 from tests.refpkg import import_reference, reference_dir
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-4
-
-
-def rel(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
 
 
 def gat_exact_grads(state, graph, target, nhead=8, slope=0.2):

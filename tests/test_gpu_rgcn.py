@@ -19,25 +19,15 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gpu_util import bits, dev, misaligned, rel
 from tests.graphs import boundary_csr, case
 from tests.rgcn_table import TABLE
 from tests.test_gpu_autograd import bound, rows_of
-from tests.test_gpu_label_prop import bits, misaligned
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TOL = 1e-5
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    torch.backends.cuda.matmul.allow_tf32 = False
-    return torch.device("cuda:0")
 
 
 def row_inputs(c, dev):
@@ -142,11 +132,6 @@ def params(dev, seed=4):
     V = torch.randn(B, F_IN, F_OUT, generator=g) / 5
     dout = torch.randn(N, F_OUT, generator=g)
     return x, alpha, V, dout
-
-
-def rel(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
 
 
 def test_rgcn_conv_and_aggregate_against_fp64_autograd(dev):

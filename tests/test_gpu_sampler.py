@@ -9,16 +9,9 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import dev
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    return torch.device("cuda:0")
 
 
 def graph(n, e, seed, hub=None, empty=0.2):

@@ -9,20 +9,13 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+from tests.gpu_util import dev
+
 pytestmark = pytest.mark.gpu
 
 # H a power of two with H * chunk_edges <= 2048: the edge-softmax kernels take their split-row path, which uses the
 # partials; F = K * d with d a power of two for the routing
 N, H, F, K, B, T, D = 1500, 4, 32, 4, 2, 3, 4
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")

@@ -37,6 +37,7 @@ import torch
 
 from tests import test_gpu_dispatch
 from tests.gat_dropout_ref import keep_mask
+from tests.gpu_util import dev
 from tests.graphs import boundary_csc, boundary_csr, case
 from tests.hgn_table import ALPHA, CHUNK, MAX_TABLE, TABLE
 from tests.simple_hgn_ref import HgnConvStandIn, aggregate_fp64, hgn_attention_fp64
@@ -50,15 +51,6 @@ GOLDEN = os.path.join(ROOT, "tests", "golden", "simple_hgn.npz")
 SLOPE, F = 0.2, 4
 U32 = 2.0 ** -24
 TINY = float(np.finfo(np.float32).tiny)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
 
 
 def close(a, b, what):
@@ -125,7 +117,7 @@ def run(rs, ins, c, seed):
     return out, att, leaves
 
 
-def bits(a):
+def np_bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
@@ -177,7 +169,7 @@ def test_row_against_fp64(dev, c):
         alpha32 = np.float32(c.alpha)
         keep32 = np.float32(np.float32(1) - alpha32)
         want_mix = ((want_mix * keep32).astype(np.float32) + (np_["res"] * alpha32).astype(np.float32))
-    assert np.array_equal(bits(mix_n), bits(want_mix)), f"{c.id}: mix differs from its fp32 emulation"
+    assert np.array_equal(np_bits(mix_n), np_bits(want_mix)), f"{c.id}: mix differs from its fp32 emulation"
     assert torch.equal(mix_inf.view(torch.int32), mix.view(torch.int32)), f"{c.id}: the inference call's mix differs"
 
     # the layer: forward and backward through the autograd function
@@ -199,7 +191,7 @@ def test_row_against_fp64(dev, c):
     sd = gn[rows].astype(np.float64) * h64[ci]
     assert_within(dm, sd.sum(-1), F * U32 * np.abs(sd).sum(-1) + TINY, f"{c.id} d m")
     if c.res:
-        assert np.array_equal(bits(leaves["res"].grad.cpu().numpy()), bits(dm * np.float32(c.alpha))), "d res"
+        assert np.array_equal(np_bits(leaves["res"].grad.cpu().numpy()), np_bits(dm * np.float32(c.alpha))), "d res"
     gs = np.float32((1.0 - (c.alpha if c.res else 0.0)) * scale)    # the layer's grad_scale, rounded once
     d_edge, g_row = hgn_attn_bwd_raw(st, rs.type, att, torch.from_numpy(dm).to(dev), ins["h_l"], ins["h_r"],
                                      ins["h_e"], SLOPE, float(gs))

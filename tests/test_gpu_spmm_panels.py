@@ -9,28 +9,10 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import bits, dev, plan_structure
 from tests.graphs import case
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def structure(rp, ci, n_cols, dev, chunk):
-    from cogdl_b200.structure import CSRStructure
-
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk)
-
-
-def bits(y):
-    return y.contiguous().view(torch.int32)
 
 
 @pytest.mark.parametrize("name", ["hub", "two_hubs", "ragged", "rect"])
@@ -46,7 +28,7 @@ def test_panels_bitwise_equal_single_pass(dev, name, F, weighted, chunk):
     X = rng.standard_normal((n_cols, F)).astype(np.float32)
     val = rng.random(ci.shape[0]).astype(np.float32) if weighted else None
     ref = oracle.spmm_csr(rp, ci, val, X)
-    st = structure(rp, ci, n_cols, dev, chunk)
+    st = plan_structure(rp, ci, n_cols, dev, chunk=chunk)
     assert st.plan.n_segs > 0
     x_d = torch.from_numpy(X).to(dev)
     v_d = None if val is None else torch.from_numpy(val).to(dev)
@@ -67,7 +49,7 @@ def test_forced_panels_out_of_range_is_an_error(dev):
     from cogdl_b200.operators._raw import spmm_raw
 
     rp, ci, n_cols = case("hub")
-    st = structure(rp, ci, n_cols, dev, 256)
+    st = plan_structure(rp, ci, n_cols, dev, chunk=256)
     for F, P in ((128, 3), (128, 8), (40, 2), (512, 2), (192, 2), (384, 4)):
         with pytest.raises(CogdlB200Error):
             spmm_raw(st, None, torch.randn(n_cols, F, device=dev), panels=P)
@@ -94,7 +76,7 @@ def test_automatic_panel_count_follows_x_size(dev, x_rows, F):
     rng = np.random.default_rng(4)
     rp = np.arange(0, 4001 * 6, 6, dtype=np.int32)[:4001]
     ci = rng.integers(0, x_rows, int(rp[-1])).astype(np.int32)
-    st = structure(rp, ci, x_rows, dev, 256)
+    st = plan_structure(rp, ci, x_rows, dev, chunk=256)
     x = torch.randn(x_rows, F, device=dev)
     y = spmm_raw(st, None, x)
     P = expected_auto_panels(x_rows * F * 4, F)

@@ -13,6 +13,7 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+from tests.gpu_util import bits, dev, misaligned, plan_structure
 from tests.graphs import boundary_csr, case
 from tests.spmm_residual_table import TABLE
 
@@ -21,32 +22,8 @@ pytestmark = pytest.mark.gpu
 A_COEF, B_COEF = 0.9, 0.1       # (1 - alpha, alpha) of alpha = 0.1: 0.9 is not an fp32 value, so the rounding shows
 
 
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
 def graph_of(c):
     return boundary_csr(c.chunk) if c.graph == "bounds" else case(c.graph)
-
-
-def structure(rp, ci, n_cols, dev, c):
-    from cogdl_b200.structure import CSRStructure
-
-    chunk, seg_cost = {"none": (0, None), "chunks": (c.chunk, 0), "default": (c.chunk, None)}[c.plan]
-    return CSRStructure(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), n_cols=n_cols, chunk_edges=chunk,
-                        seg_cost=seg_cost)
-
-
-def misaligned(t):
-    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
-    out = buf[1:].view(t.shape)
-    out.copy_(t)
-    return out
 
 
 def inputs(c, dev):
@@ -62,17 +39,13 @@ def inputs(c, dev):
     return rp, ci, n_cols, X, Z, r, val
 
 
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
 @pytest.mark.parametrize("c", TABLE, ids=lambda c: c.id)
 def test_forward_is_the_unfused_sequence_bit_for_bit(dev, c):
     from cogdl_b200 import _cabi
     from cogdl_b200.operators._raw import spmm_raw, spmm_residual_raw
 
     rp, ci, n_cols, X, Z, r, val = inputs(c, dev)
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     y = spmm_residual_raw(st, val, X, Z, A_COEF, B_COEF, r, panels=c.panels)
     assert _cabi.last_kernel() == c.kernel, f"{c.id}: launched {_cabi.last_kernel()!r}"
     t = spmm_raw(st, val, X, panels=c.panels)
@@ -104,7 +77,7 @@ def test_gradients_match_fp64(dev, c):
     from cogdl_b200.operators.spmm_residual import SpmmResidualFunction
 
     rp, ci, n_cols, X, Z, r, val = inputs(c, dev)
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     n = rp.shape[0] - 1
     x = X.detach().clone().requires_grad_(True)
     z = Z.detach().clone().requires_grad_(True) if Z is not None else None
@@ -138,7 +111,7 @@ def test_symmetric_backward_runs_over_the_matrix_itself(dev):
 
     c = RCase("two_hubs", 40, "", row_scale=True)
     rp, ci, n_cols, X, Z, r, val = inputs(c, dev)
-    st = structure(rp, ci, n_cols, dev, c)
+    st = plan_structure(rp, ci, n_cols, dev, c.plan, c.chunk)
     x = X.detach().clone().requires_grad_(True)
     g = torch.randn(rp.shape[0] - 1, 40, device=dev)
     SpmmResidualFunction.apply(st, x, Z, val, A_COEF, B_COEF, r, True).backward(g)
@@ -153,7 +126,7 @@ def test_aliased_output_is_rejected(dev):
     from cogdl_b200.structure import _ptr, _stream
 
     rp, ci, n = boundary_csr(64)
-    st = structure(rp, ci, n, dev, type("C", (), {"plan": "default", "chunk": 64})())
+    st = plan_structure(rp, ci, n, dev, chunk=64)
     X = torch.randn(n, 32, device=dev)
     Z = torch.randn(n, 32, device=dev)
     plan, keep = st.plan_struct(_scratch("spmm", st, 32))

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 import oracle
+from tests.gpu_util import bits, dev
 
 pytestmark = pytest.mark.gpu
 
@@ -49,19 +50,6 @@ def graph(name):
 GRAPHS = ["empty_runs", "slab_aligned", "unit_rows", "hubs", "mixed"]
 # panel counts the SpMM accepts at each width (a panel is 32, 64 or 128 floats); F = 9 takes the scalar lean loop
 WIDTHS = {9: [1], 40: [1], 64: [1, 2], 128: [1, 2, 4], 256: [1, 2, 4]}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available()
-    import cogdl_b200  # noqa: F401
-
-    assert cogdl_b200._cabi.load().cogdl_b200_check_device() == 0, cogdl_b200._cabi.last_error()
-    return torch.device("cuda:0")
-
-
-def bits(y):
-    return y.contiguous().view(torch.int32)
 
 
 @pytest.mark.parametrize("name", GRAPHS)

@@ -9,20 +9,13 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gpu_util import dev
 from tests import graphs
 from tests import spgemm_oracle as so
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    import cogdl_b200  # noqa: F401
-
-    torch.backends.cuda.matmul.allow_tf32 = False
-    return torch.device("cuda:0")
 
 
 def coo_of(rp, ci, seed, shuffle=True):
