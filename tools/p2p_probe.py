@@ -6,6 +6,7 @@ import sys
 
 import torch
 import torch.distributed as dist
+from gpu_timing import event_times
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
@@ -30,18 +31,14 @@ def main():
         peer = (rank + 1) % world
         idx = torch.randint(0, n, (1 << 18,), device=dev, dtype=torch.int32)
         out = torch.empty((idx.numel(), F), device=dev)
-        for _ in range(3):
-            _cabi.call("cogdl_b200_gather_rows_f32", _ptr(idx), ctypes.c_void_p(hdl.buffer_ptrs[peer]), _ptr(out),
-                       idx.numel(), F, _stream(dev))
+
+        def gather(times):
+            for _ in range(times):
+                _cabi.call("cogdl_b200_gather_rows_f32", _ptr(idx), ctypes.c_void_p(hdl.buffer_ptrs[peer]), _ptr(out),
+                           idx.numel(), F, _stream(dev))
+        gather(3)
         torch.cuda.synchronize()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(5):
-            _cabi.call("cogdl_b200_gather_rows_f32", _ptr(idx), ctypes.c_void_p(hdl.buffer_ptrs[peer]), _ptr(out),
-                       idx.numel(), F, _stream(dev))
-        b.record()
-        torch.cuda.synchronize()
-        ms = a.elapsed_time(b) / 5
+        ms = event_times(lambda: gather(5), 1, 0, flush=False)[0] / 1e3 / 5
         ok = bool((out == float(peer + 1)).all())
         print(f"[rank {rank}] peer gather of {idx.numel()} x 512 B rows from rank {peer}: correct={ok} {ms:.3f} ms "
               f"= {idx.numel() * 512 / ms / 1e6:.1f} GB/s", flush=True)

@@ -3,6 +3,7 @@ import os
 import sys
 
 import torch
+from gpu_timing import flush_l2
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
@@ -19,9 +20,8 @@ fout = int(sys.argv[1]) if len(sys.argv) > 1 else 128
 x = torch.randn(n, 128, device=dev)
 lin = torch.nn.Linear(128, fout).to(dev)
 W, b = lin.weight.detach().contiguous(), lin.bias.detach().contiguous()
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
 for _ in range(4):
-    flush.zero_()
+    flush_l2()
     fused_gcn_raw(st, w, x, W, b, True)
 torch.cuda.synchronize()
 print("done")

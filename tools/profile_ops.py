@@ -4,6 +4,7 @@ import os
 import sys
 
 import torch
+from gpu_timing import flush_l2
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
@@ -21,19 +22,18 @@ logits = (torch.randn(st.nnz, H, device=dev) * 3).clamp_(-10, 10)
 x = torch.randn(n, F, device=dev)
 h = torch.randn(n, H, F, device=dev)
 hl, hr = torch.randn(n, H, device=dev), torch.randn(n, H, device=dev)
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
 for it in range(3):
-    flush.zero_()
+    flush_l2()
     att = edge_softmax_fwd_raw(st, logits)
-    flush.zero_()
+    flush_l2()
     edge_softmax_bwd_raw(st, att, logits)
-    flush.zero_()
+    flush_l2()
     gat_fwd_raw(st, hl, hr, h, 0.2, True)
-    flush.zero_()
+    flush_l2()
     mhsddmm_raw(st, h, h)
-    flush.zero_()
+    flush_l2()
     sddmm_raw(st, x, x)
-    flush.zero_()
+    flush_l2()
     spmm_raw(st, w, x)
 torch.cuda.synchronize()
 print("done")

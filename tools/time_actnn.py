@@ -13,21 +13,15 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from gpu_timing import card, event_times
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
 
 
 class GCNII(nn.Module):
@@ -67,16 +61,8 @@ def step_time(model, g, x, y, warmup, reps):
         step()
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
-    times = []
-    for _ in range(reps):
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        step()
-        e.record()
-        torch.cuda.synchronize()
-        times.append(s.elapsed_time(e))
-    times.sort()
-    return times[len(times) // 2], torch.cuda.max_memory_allocated() / 2 ** 30
+    times = sorted(event_times(step, reps, 0, flush=False))
+    return times[len(times) // 2] / 1e3, torch.cuda.max_memory_allocated() / 2 ** 30
 
 
 def graph(n, e, f, seed):
@@ -115,16 +101,14 @@ def main():
     C = torch.rand(169343, device="cuda") * 100
     target = 2 * C.numel()
     dev_bits = kernels.allocate_bits(C, target)
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for _ in range(3):
         kernels.allocate_bits(C, target)
     torch.cuda.synchronize()
-    s.record()
-    for _ in range(20):
-        kernels.allocate_bits(C, target)
-    e.record()
-    torch.cuda.synchronize()
-    res["alloc_device_ms"] = round(s.elapsed_time(e) / 20, 3)
+
+    def twenty():     # each result is dropped before the next call, so its block is reused
+        for _ in range(20):
+            kernels.allocate_bits(C, target)
+    res["alloc_device_ms"] = round(event_times(twenty, 1, 0, flush=False)[0] / 1e3 / 20, 3)
     import time
 
     t0 = time.perf_counter()

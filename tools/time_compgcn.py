@@ -16,15 +16,14 @@ Writes time_compgcn.json to OUT_DIR with the card name and power limit read in t
 
     python tools/time_compgcn.py OUT_DIR
 """
-import hashlib
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import numpy as np
 import torch
+from gpu_timing import digest, event_times, peak_above, write_result
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -36,42 +35,8 @@ from tests.refpkg import import_reference  # noqa: E402
 if len(sys.argv) != 2:
     sys.exit(__doc__)
 out_dir = sys.argv[1]
-os.makedirs(out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
-
-
-def timed(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return statistics.median(ts)
-
-
-def peak_above(fn):
-    torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.max_memory_allocated() - base
-
-
-def sha(t):
-    return hashlib.sha256(t.detach().contiguous().cpu().numpy().tobytes()).hexdigest()[:16]
-
-
 def make_kg(n_ent, n_rel, n_tri, seed):
     """Seeded KG: relation frequencies Zipf(1) over a random relation order, entity ranks from a power law (hubs),
     each triple plus its reverse (type t + n_rel), the COO shuffled.  int64 tensors on the device."""
@@ -104,7 +69,7 @@ def with_forward(fwd, fn):
         CompGCNLayer.forward = FUSED
 
 
-res = {"card": card, "fb15k237": {}, "wikikg2": {}, "sha256": {}}
+res = {"fb15k237": {}, "wikikg2": {}, "sha256": {}}
 
 # ---------------------------------------------------------------------------------------------- (a)
 N, R = 14541, 237
@@ -124,18 +89,20 @@ def build():
     torch.cuda.synchronize()
 
 
-fb["structure_build_us"] = timed(build, reps=10)
+fb["structure_build_us"] = statistics.median(event_times(build, 10, 3, flush=True))
 fb["hub_rows_2N"] = cs.csr.plan.n_hub_rows
 for F in (100, 200):
     gen = torch.Generator(device=dev).manual_seed(F)
     x = torch.randn(N, F, device=dev, generator=gen)
     relt = torch.randn(2 * R + 1, F, device=dev, generator=gen)
-    t_sp = timed(lambda: spmm_raw(cs.csr, cs.w, x))
-    t_mult = timed(lambda: comp_aggr_raw(cs.csr, cs.type, cs.w, x, relt, "mult"))
-    t_sub = timed(lambda: comp_aggr_raw(cs.csr, cs.type, cs.w, x, relt, "sub"))
+    t_sp = statistics.median(event_times(lambda: spmm_raw(cs.csr, cs.w, x), 20, 3, flush=True))
+    t_mult = statistics.median(
+        event_times(lambda: comp_aggr_raw(cs.csr, cs.type, cs.w, x, relt, "mult"), 20, 3, flush=True))
+    t_sub = statistics.median(
+        event_times(lambda: comp_aggr_raw(cs.csr, cs.type, cs.w, x, relt, "sub"), 20, 3, flush=True))
     fb[f"aggr_F{F}"] = {"spmm_us": t_sp, "fused_mult_us": t_mult, "fused_sub_us": t_sub,
                         "ratio_mult": t_mult / t_sp, "ratio_sub": t_sub / t_sp}
-    res["sha256"][f"fb_aggr_mult_F{F}"] = sha(comp_aggr_raw(cs.csr, cs.type, cs.w, x, relt, "mult"))
+    res["sha256"][f"fb_aggr_mult_F{F}"] = digest(comp_aggr_raw(cs.csr, cs.type, cs.w, x, relt, "mult"))
 
 # CompGCNLayer, F_in 100 -> F_out 200
 F_IN, F_OUT = 100, 200
@@ -158,15 +125,15 @@ def layer_fwd_bwd():
 
 for name, fwd in (("original", ORIGINAL), ("fused", FUSED)):
     with torch.no_grad():
-        t_f = with_forward(fwd, lambda: timed(layer_fwd, reps=10))
-    t_fb = with_forward(fwd, lambda: timed(layer_fwd_bwd, reps=10))
+        t_f = with_forward(fwd, lambda: statistics.median(event_times(layer_fwd, 10, 3, flush=True)))
+    t_fb = with_forward(fwd, lambda: statistics.median(event_times(layer_fwd_bwd, 10, 3, flush=True)))
     m_fb = with_forward(fwd, lambda: peak_above(layer_fwd_bwd))
     fb[f"layer_{name}"] = {"fwd_us": t_f, "fwd_bwd_us": t_fb, "fwd_bwd_peak_bytes": m_fb}
 with torch.no_grad():
     y_o = with_forward(ORIGINAL, layer_fwd)[0]
     y_f = layer_fwd()[0]
 fb["layer_fused_vs_original_max_rel"] = float((y_f - y_o).abs().max() / y_o.abs().max())
-res["sha256"]["fb_layer_fused"] = sha(y_f)
+res["sha256"]["fb_layer_fused"] = digest(y_f)
 fb["layer_fwd_bwd_speedup"] = fb["layer_original"]["fwd_bwd_us"] / fb["layer_fused"]["fwd_bwd_us"]
 fb["layer_fwd_speedup"] = fb["layer_original"]["fwd_us"] / fb["layer_fused"]["fwd_us"]
 
@@ -175,7 +142,7 @@ torch.manual_seed(1)
 model = LinkPredictCompGCN(N, R, 200, layers=2, dropout=0.3, opn="sub").to(dev).eval()
 with torch.no_grad():
     for name, fwd in (("original", ORIGINAL), ("fused", FUSED)):
-        t = with_forward(fwd, lambda: timed(lambda: model.predict(graph), reps=10))
+        t = with_forward(fwd, lambda: statistics.median(event_times(lambda: model.predict(graph), 10, 3, flush=True)))
         m = with_forward(fwd, lambda: peak_above(lambda: model.predict(graph)))
         fb[f"predict_{name}"] = {"us": t, "peak_bytes": m}
 fb["predict_speedup"] = fb["predict_original"]["us"] / fb["predict_fused"]["us"]
@@ -200,12 +167,11 @@ G = torch.randn(N, F_OUT, device=dev)
 torch.cuda.synchronize()
 structure.clear_structure_cache()
 wk["first_fwd_bwd_peak_bytes"] = peak_above(layer_fwd_bwd)       # includes the structure build
-wk["fwd_bwd_us"] = timed(layer_fwd_bwd, reps=5, warm=1)
+wk["fwd_bwd_us"] = statistics.median(event_times(layer_fwd_bwd, 5, 1, flush=True))
 with torch.no_grad():
-    wk["fwd_us"] = timed(layer_fwd, reps=5, warm=1)
+    wk["fwd_us"] = statistics.median(event_times(layer_fwd, 5, 1, flush=True))
 wk["fwd_bwd_peak_bytes"] = peak_above(layer_fwd_bwd)
-res["sha256"]["wikikg2_layer"] = sha(layer_fwd()[0])
+res["sha256"]["wikikg2_layer"] = digest(layer_fwd()[0])
 print(json.dumps(wk, indent=1), flush=True)
-print(json.dumps({"card": card, "sha256": res["sha256"]}))
-with open(os.path.join(out_dir, "time_compgcn.json"), "w") as f:
-    json.dump(res, f, indent=1)
+write_result(out_dir, "time_compgcn", res)
+print(json.dumps({"card": res["card"], "sha256": res["sha256"]}))

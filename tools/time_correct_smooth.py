@@ -16,31 +16,16 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+from gpu_timing import card, event_times
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 SHAPES = {"arxiv": (169343, 1166243, 40), "products": (2449029, 61859140, 47)}
 NPROP, CORRECT_ALPHA, SMOOTH_ALPHA, TRAIN_SHARE = 50, 1.0, 0.8, 0.54
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
-
-
-def timed(fn):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    out = fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e), out
 
 
 def loops(g1, g2, labels, nid, fused):
@@ -110,7 +95,7 @@ def main():
             t = {False: [], True: []}
             for _ in range(a.rounds):
                 for fused in (False, True):
-                    t[fused].append(timed(lambda: loops(g1, g2, labels, nid, fused))[0])
+                    t[fused].append(event_times(lambda: loops(g1, g2, labels, nid, fused), 1, 0, flush=False)[0] / 1e3)
         u, f = statistics.median(t[False]), statistics.median(t[True])
         r = {"nodes": n, "edges": int(rp[-1]), "C": C, "unfused_ms": round(u, 2), "fused_ms": round(f, 2),
              "ratio": round(f / u, 3), "bit_identical": same,
@@ -128,12 +113,15 @@ def main():
             logits = torch.randn(n, C, device=dev)
             pt = {False: [], True: []}
             outs = {}
+
+            def postprocess(fused):
+                outs[fused] = model.postprocess(graph, logits)
             with torch.no_grad():
                 for k in range(a.rounds + 1):
                     for fused in (False, True):
                         if fused:
                             cogdl_b200.install(correct_smooth=True)
-                        ms, outs[fused] = timed(lambda: model.postprocess(graph, logits))
+                        ms = event_times(lambda: postprocess(fused), 1, 0, flush=False)[0] / 1e3
                         cogdl_b200.uninstall_correct_smooth()
                         if k > 0:
                             pt[fused].append(ms)

@@ -13,14 +13,13 @@ and power limit read in the same run.
 
     python tools/time_disengcn.py OUT_DIR
 """
-import hashlib
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+from gpu_timing import digest, event_times, peak_above, write_result
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -32,46 +31,12 @@ from cogdl_b200.operators.edge_softmax import EdgeSoftmaxFunction  # noqa: E402
 if len(sys.argv) != 2:
     sys.exit(__doc__)
 out_dir = sys.argv[1]
-os.makedirs(out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 torch.backends.cudnn.allow_tf32 = False
 PEAK = 3.35e12
 T, TAU, F, IN = 7, 1.0, 64, 128
 
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
-
-
-def timed(fn, reps=20):
-    for _ in range(3):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return statistics.median(ts)
-
-
-def sha(t):
-    return hashlib.sha256(t.detach().contiguous().cpu().numpy().tobytes()).hexdigest()[:16]
-
-
-def peak_above(fn):
-    torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.max_memory_allocated() - base
-
-
 def step_bytes(E, N, F, K):
     # per edge: column index + gathered c row; per row: rowptr, q and c rows, out row (+ lse2, r in training)
     return E * (4 + 4 * F) + N * (4 + 12 * F)
@@ -134,10 +99,10 @@ def fwd_bwd(fn):
     return call
 
 
-res = {"card": card, "arxiv": {"n": n, "nnz": E, "F": F, "T": T}, "sha256": {}, "peak_bytes": {}, "parity": {},
+res = {"arxiv": {"n": n, "nnz": E, "F": F, "T": T}, "sha256": {}, "peak_bytes": {}, "parity": {},
        "bytes": {}, "rounds": []}
 variants = {"spmm_raw_us": lambda: spmm_raw(st, None, xf)}
-res["sha256"]["spmm_raw"] = sha(spmm_raw(st, None, xf))
+res["sha256"]["spmm_raw"] = digest(spmm_raw(st, None, xf))
 for K in (16, 8):
     c = act(x).detach().reshape(n, K, F // K)
     c = (c / c.pow(2).sum(-1, keepdim=True).sqrt()).reshape(n, F).contiguous()
@@ -151,9 +116,9 @@ for K in (16, 8):
         got, want = fused_layer(K)(x), reference_layer(K)(x)
     res["parity"][f"K{K}_fused_vs_reference_max_row_rel_err"] = float(
         ((got - want).abs() / want.abs().amax(1, keepdim=True).clamp_min(1e-30)).max())
-    res["sha256"][f"K{K}_fused_step"] = sha(disen_route_fwd_raw(st, c, c, K, TAU)[0])
-    res["sha256"][f"K{K}_fused_layer"] = sha(got)
-    res["sha256"][f"K{K}_reference_layer"] = sha(want)
+    res["sha256"][f"K{K}_fused_step"] = digest(disen_route_fwd_raw(st, c, c, K, TAU)[0])
+    res["sha256"][f"K{K}_fused_layer"] = digest(got)
+    res["sha256"][f"K{K}_reference_layer"] = digest(want)
     for name, fn in (("fused", fused_layer(K)), ("reference", reference_layer(K))):
         res["peak_bytes"][f"K{K}_{name}_layer_fwd_bwd"] = peak_above(fwd_bwd(fn))
         W.grad = b.grad = None
@@ -196,8 +161,8 @@ except ImportError as ex:
     print(f"(b) skipped: {ex}")
 
 for rnd in range(2):
-    rr = {k: timed(fn) for k, fn in variants.items()}
-    rr.update({k: timed(fn, reps=10) / 1e3 for k, fn in steps.items()})
+    rr = {k: statistics.median(event_times(fn, 20, 3, flush=True)) for k, fn in variants.items()}
+    rr.update({k: statistics.median(event_times(fn, 10, 3, flush=True)) / 1e3 for k, fn in steps.items()})
     res["rounds"].append(rr)
     for k, v in rr.items():
         print(f"round {rnd} {k:40s} {v:10.1f}" if k.endswith("_us") else f"round {rnd} {k:40s} {v:10.3f}")
@@ -225,12 +190,11 @@ st2.plan
 h2 = torch.randn(np_, F, device=dev, generator=torch.Generator(device=dev).manual_seed(2))
 with torch.no_grad():
     out2 = cogdl_b200.disen_routing(st2, h2, 16, T, TAU)
-    res["products"] = {"n": np_, "nnz": st2.nnz, "F": F, "K": 16, "T": T, "sha256": sha(out2)}
+    res["products"] = {"n": np_, "nnz": st2.nnz, "F": F, "K": 16, "T": T, "sha256": digest(out2)}
     del out2
     res["products"]["peak_bytes_above_inputs"] = peak_above(lambda: cogdl_b200.disen_routing(st2, h2, 16, T, TAU))
-    res["products"]["fused_layer_fwd_ms"] = timed(lambda: cogdl_b200.disen_routing(st2, h2, 16, T, TAU), reps=5) / 1e3
+    res["products"]["fused_layer_fwd_ms"] = statistics.median(
+        event_times(lambda: cogdl_b200.disen_routing(st2, h2, 16, T, TAU), 5, 3, flush=True)) / 1e3
 res["products"]["reference_one_EKd_tensor_bytes"] = st2.nnz * F * 4
 print(json.dumps({k: res[k] for k in ("summary", "peak_bytes", "products", "parity", "sha256", "kernel")}, indent=1))
-print(card)
-with open(os.path.join(out_dir, "time_disengcn.json"), "w") as f:
-    json.dump(res, f, indent=1)
+write_result(out_dir, "time_disengcn", res)

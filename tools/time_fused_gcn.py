@@ -4,6 +4,7 @@ import statistics
 import sys
 
 import torch
+from gpu_timing import card, event_times
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
@@ -17,22 +18,12 @@ rp, col = synth.powerlaw_csr(n, e, seed=0)
 w = synth.sym_norm_weights(rp, col).to(dev)
 st = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n)
 st.plan
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
 x = torch.randn(n, 128, device=dev)
+print("card:", card(), flush=True)
 
 
-def timed(fn, reps=20):
-    for _ in range(3):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
+def median_min(fn):
+    ts = event_times(fn, 20, 3, flush=True)
     return statistics.median(ts), min(ts)
 
 
@@ -43,8 +34,8 @@ for fout in (128, 40):
         torch.backends.cuda.matmul.allow_tf32 = tf32
         torch.backends.cudnn.allow_tf32 = tf32
         tag = "tf32" if tf32 else "fp32"
-        print(f"Fout={fout} unfused gemm({tag})+bias -> spmm -> relu", timed(lambda: torch.relu_(spmm_raw(st, w, torch.addmm(b, x, W.t())))))
-        print(f"Fout={fout} unfused spmm -> gemm({tag}) -> relu      ", timed(lambda: torch.relu_(spmm_raw(st, w, x) @ W.t())))
+        print(f"Fout={fout} unfused gemm({tag})+bias -> spmm -> relu", median_min(lambda: torch.relu_(spmm_raw(st, w, torch.addmm(b, x, W.t())))))
+        print(f"Fout={fout} unfused spmm -> gemm({tag}) -> relu      ", median_min(lambda: torch.relu_(spmm_raw(st, w, x) @ W.t())))
     torch.backends.cuda.matmul.allow_tf32 = False
-    print(f"Fout={fout} spmm alone (F=128)                       ", timed(lambda: spmm_raw(st, w, x)))
-    print(f"Fout={fout} FUSED wgmma                               ", timed(lambda: fused_gcn_raw(st, w, x, W, b, True)))
+    print(f"Fout={fout} spmm alone (F=128)                       ", median_min(lambda: spmm_raw(st, w, x)))
+    print(f"Fout={fout} FUSED wgmma                               ", median_min(lambda: fused_gcn_raw(st, w, x, W, b, True)))

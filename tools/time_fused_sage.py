@@ -11,14 +11,13 @@ on the command line, with the card name and power limit read in the same run.
 
     python tools/time_fused_sage.py OUT_DIR
 """
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 import torch.nn.functional as F
+from gpu_timing import event_times, write_result
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
@@ -30,36 +29,17 @@ from cogdl_b200.operators.fused_sage import fused_sage_raw  # noqa: E402
 if len(sys.argv) != 2:
     sys.exit(__doc__)
 out_dir = sys.argv[1]
-os.makedirs(out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 torch.backends.cudnn.allow_tf32 = False
 
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
 n, e = synth.SHAPES["arxiv"]
 rp, col = synth.powerlaw_csr(n, e, seed=0)
 st = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n)
 st.plan
 deg = (rp[1:] - rp[:-1]).float()
 inv = torch.where(deg > 0, 1.0 / deg.clamp_min(1), torch.zeros_like(deg)).to(dev).view(n, 1)
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
 x = torch.randn(n, 128, device=dev)
-
-
-def timed(fn, reps=20):
-    for _ in range(3):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return statistics.median(ts)
 
 
 def agg_of(aggr):
@@ -95,7 +75,7 @@ def step_fn(aggr, fused):
     return step
 
 
-res = {"card": card, "shape": {"n": n, "nnz": st.nnz, "in_feats": 128}, "unit": "us (layer), ms (train step)",
+res = {"shape": {"n": n, "nnz": st.nnz, "in_feats": 128}, "unit": "us (layer), ms (train step)",
        "rounds": []}
 layers = {(a, f): layer_variants(a, f) for a in ("mean", "max") for f in (128, 40)}
 steps = {(a, fu): step_fn(a, fu) for a in ("mean", "max") for fu in (False, True)}
@@ -103,14 +83,12 @@ for rnd in range(2):
     r = {}
     for (aggr, fout), variants in layers.items():
         for name, fn in variants.items():
-            r[f"{aggr}_F{fout}_{name}_us"] = timed(fn)
+            r[f"{aggr}_F{fout}_{name}_us"] = statistics.median(event_times(fn, 20, 3, flush=True))
     for (aggr, fused), fn in steps.items():
-        r[f"train_step_{aggr}_{'fused' if fused else 'unfused'}_ms"] = timed(fn) / 1e3
+        r[f"train_step_{aggr}_{'fused' if fused else 'unfused'}_ms"] = statistics.median(event_times(fn, 20, 3, flush=True)) / 1e3
     res["rounds"].append(r)
     for k, v in r.items():
         print(f"round {rnd} {k:45s} {v:10.1f}" if k.endswith("_us") else f"round {rnd} {k:45s} {v:10.3f}")
 layers[("mean", 128)]["fused"]()
 res["kernel_mean"] = cogdl_b200._cabi.last_kernel()
-print(card)
-with open(os.path.join(out_dir, "time_fused_sage.json"), "w") as f:
-    json.dump(res, f, indent=1)
+write_result(out_dir, "time_fused_sage", res)

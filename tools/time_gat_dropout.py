@@ -18,11 +18,11 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 import torch.nn.functional as F
+from gpu_timing import event_times, peak_above, write_result
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -34,12 +34,8 @@ ap = argparse.ArgumentParser()
 ap.add_argument("out_dir")
 ap.add_argument("--steps", type=int, default=20)
 args = ap.parse_args()
-os.makedirs(args.out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
-print("card:", card, flush=True)
 
 import_reference()
 import cogdl.layers.gat_layer as gl  # noqa: E402
@@ -70,16 +66,7 @@ def measure(step, modules, variants, steps):
     for _ in range(steps):
         for v in variants:
             set_variant(v, modules)
-            torch.cuda.synchronize()
-            base = torch.cuda.memory_allocated()
-            torch.cuda.reset_peak_memory_stats()
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            step()
-            b.record()
-            torch.cuda.synchronize()
-            times[v].append(a.elapsed_time(b) * 1e3)
-            peaks[v] = max(peaks[v], torch.cuda.max_memory_allocated() - base)
+            peaks[v] = max(peaks[v], peak_above(lambda: times[v].extend(event_times(step, 1, 0, flush=False))))
     return {v: {"us": statistics.median(times[v]), "peak_mb": peaks[v] / 2 ** 20} for v in variants}
 
 
@@ -91,7 +78,7 @@ def power_law_graph(n, e, f, seed):
     return Graph(x=x, edge_index=(row, col)), rp.numel() - 1, col.numel()
 
 
-result = {"card": card}
+result = {}
 
 # ---- (a) arxiv: 2-layer GAT training step
 graph, n, nnz = power_law_graph(169343, 1166243, 128, seed=0)
@@ -137,5 +124,4 @@ except torch.cuda.OutOfMemoryError as e:       # the unfused path does not fit: 
     res_b["unfused"] = {"error": f"out of memory: {str(e).splitlines()[0]}"}
 result["products_gat_layer_fwd_bwd"] = res_b
 print("products GATLayer fwd+bwd:", json.dumps(res_b), flush=True)
-with open(os.path.join(args.out_dir, "time_gat_dropout.json"), "w") as f:
-    json.dump(result, f, indent=1)
+write_result(args.out_dir, "time_gat_dropout", result)

@@ -20,23 +20,17 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from gpu_timing import alternate, card
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 HBM_BYTES_PER_S = 3.35e12      # H100 SXM data sheet
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
 
 
 class GCNII(nn.Module):
@@ -94,19 +88,6 @@ class APPNP(nn.Module):
         return preds
 
 
-def timed(fn, reps):
-    times = []
-    for _ in range(reps):
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        fn()
-        e.record()
-        torch.cuda.synchronize()
-        times.append(s.elapsed_time(e))
-    times.sort()
-    return times[len(times) // 2]
-
-
 def burst(fn, n=50):
     """fn run n times back to back: one event window times all n launches."""
     def run():
@@ -122,17 +103,13 @@ def train_step(model, g, x, y):
     return step
 
 
-def alternate(fns, warmup, reps, rounds):
-    """{name: median over rounds of the per-round median ms}, the names run in turn within each round."""
-    for fn in fns.values():
-        for _ in range(warmup):
-            fn()
-    torch.cuda.synchronize()
-    per = {k: [] for k in fns}
-    for _ in range(rounds):
-        for k, fn in fns.items():
-            per[k].append(timed(fn, reps))
-    return {k: round(sorted(v)[len(v) // 2], 3) for k, v in per.items()}, {k: [round(t, 3) for t in v] for k, v in per.items()}
+def round_medians(fns, warmup, reps, rounds):
+    """{name: median over rounds of the per-round median ms}, {name: per-round medians}; the names take turns within
+    each round.  The median of an even count is its upper middle value."""
+    upper_median = lambda v: sorted(v)[len(v) // 2]  # noqa: E731
+    per = {k: [upper_median(ts[i:i + reps]) / 1e3 for i in range(0, len(ts), reps)]
+           for k, (ts, _) in alternate(fns, rounds, reps, warmup, flush=False).items()}
+    return {k: round(upper_median(v), 3) for k, v in per.items()}, {k: [round(t, 3) for t in v] for k, v in per.items()}
 
 
 def main():
@@ -161,7 +138,7 @@ def main():
         torch.manual_seed(0)
         models[fused] = GCNII(128, 256, 40, 16, 0.5, fused).cuda().train()
     models[True].load_state_dict(models[False].state_dict())
-    med, raw = alternate({"unfused": train_step(models[False], g, x, y), "fused": train_step(models[True], g, x, y)},
+    med, raw = round_medians({"unfused": train_step(models[False], g, x, y), "fused": train_step(models[True], g, x, y)},
                          a.warmup, a.reps, a.rounds)
     res["gcnii_16x256_step_ms"] = med
     res["gcnii_ratio"] = round(med["fused"] / med["unfused"], 3)
@@ -179,7 +156,7 @@ def main():
         torch.manual_seed(0)
         models[fused] = APPNP(128, 64, 40, 0.5, 0.1, 10, fused).cuda().train()
     models[True].load_state_dict(models[False].state_dict())
-    med, raw = alternate({"unfused": train_step(models[False], g, x, y), "fused": train_step(models[True], g, x, y)},
+    med, raw = round_medians({"unfused": train_step(models[False], g, x, y), "fused": train_step(models[True], g, x, y)},
                          a.warmup, a.reps, a.rounds)
     res["appnp_k10_c40_step_ms"] = med
     res["appnp_ratio"] = round(med["fused"] / med["unfused"], 3)
@@ -208,7 +185,7 @@ def main():
                "residual_row_scale_only": lambda: spmm_residual_raw(st, val, h, None, 1.0, 0.0, r),
                "residual_z_row_scale": lambda: spmm_residual_raw(st, val, h, z, 0.9, 0.1, r),
                "unfused_z": lambda: 0.9 * spmm_raw(st, val, h) + 0.1 * z}
-        med, _ = alternate({k: burst(f, B) for k, f in fns.items()}, 1, a.reps, a.rounds)
+        med, _ = round_medians({k: burst(f, B) for k, f in fns.items()}, 1, a.reps, a.rounds)
         med = {k + "_us": round(v / B * 1e3, 1) for k, v in med.items()}
         med["read_z_once_us_arithmetic"] = round(n * Fw * 4 / HBM_BYTES_PER_S * 1e6, 1)
         for k in ("residual_z", "residual_no_z", "residual_row_scale_only", "residual_z_row_scale"):

@@ -16,10 +16,10 @@ the card name and power limit read in the same run.
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+from gpu_timing import event_times, peak_above, write_result
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -31,32 +31,11 @@ from cogdl_b200.operators.edge_softmax import EdgeSoftmaxFunction  # noqa: E402
 if len(sys.argv) != 2:
     sys.exit(__doc__)
 out_dir = sys.argv[1]
-os.makedirs(out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 torch.backends.cudnn.allow_tf32 = False
 PEAK = 3.35e12
 
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
-
-
-def timed(fn, reps=20):
-    for _ in range(3):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return statistics.median(ts)
-
-
 def fwd_bytes(E, N, F, edge=False, lse=False):
     return E * (4 * F + 4) + N * (4 * F + 4) + (E * 4 * F if edge else 0) + (N * 4 * F if lse else 0)
 
@@ -150,12 +129,12 @@ try:
 except ImportError as ex:
     print(f"(b) skipped: {ex}")
 
-res = {"card": card, "arxiv": {"n": n, "nnz": E, "F": F}, "fused_vs_reference_fwd_max_row_rel_err": parity,
+res = {"arxiv": {"n": n, "nnz": E, "F": F}, "fused_vs_reference_fwd_max_row_rel_err": parity,
        "bytes": {"fwd": fwd_bytes(E, n, F), "fwd_train": fwd_bytes(E, n, F, lse=True), "bwd": bwd_bytes(E, n, F)},
        "rounds": []}
 for rnd in range(2):
-    rr = {k: timed(fn) for k, fn in variants_a.items()}
-    rr.update({k: timed(fn, reps=20) / 1e3 for k, fn in variants_b.items()})
+    rr = {k: statistics.median(event_times(fn, 20, 3, flush=True)) for k, fn in variants_a.items()}
+    rr.update({k: statistics.median(event_times(fn, 20, 3, flush=True)) / 1e3 for k, fn in variants_b.items()})
     res["rounds"].append(rr)
     for k, v in rr.items():
         print(f"round {rnd} {k:34s} {v:10.1f}" if k.endswith("_us") else f"round {rnd} {k:34s} {v:10.3f}")
@@ -180,17 +159,14 @@ st2 = cogdl_b200.CSRStructure.from_int64(rp2, col2)
 del rp2, col2
 st2.plan
 x2 = torch.randn(np_, 256, device=dev)
-torch.cuda.synchronize()
-base = torch.cuda.memory_allocated()
-torch.cuda.reset_peak_memory_stats()
+ts = []
 with torch.no_grad():
-    t2 = timed(lambda: cogdl_b200.genconv_aggregate(st2, x2, "softmax_sg", beta=beta), reps=20)
-res["products"] = {"n": np_, "nnz": st2.nnz, "F": 256, "fused_fwd_us": t2,
-                   "peak_bytes_above_inputs": torch.cuda.max_memory_allocated() - base,
+    peak = peak_above(lambda: ts.extend(
+        event_times(lambda: cogdl_b200.genconv_aggregate(st2, x2, "softmax_sg", beta=beta), 20, 3, flush=True)))
+t2 = statistics.median(ts)
+res["products"] = {"n": np_, "nnz": st2.nnz, "F": 256, "fused_fwd_us": t2, "peak_bytes_above_inputs": peak,
                    "unfused_one_EF_tensor_bytes": st2.nnz * 256 * 4,
                    "fwd_bytes": fwd_bytes(st2.nnz, np_, 256),
                    "fused_fwd_hbm_fraction": fwd_bytes(st2.nnz, np_, 256) / (t2 * 1e-6) / PEAK}
 print(json.dumps({k: res[k] for k in ("summary", "products", "kernel", "fused_vs_reference_fwd_max_row_rel_err")}, indent=1))
-print(card)
-with open(os.path.join(out_dir, "time_genconv.json"), "w") as f:
-    json.dump(res, f, indent=1)
+write_result(out_dir, "time_genconv", res)

@@ -18,10 +18,10 @@ Writes time_genconv_edge.json to OUT_DIR with the card name and power limit read
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+from gpu_timing import event_times, peak_above, write_result
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -32,7 +32,6 @@ from cogdl_b200.operators._raw import spmm_raw  # noqa: E402
 if len(sys.argv) != 2:
     sys.exit(__doc__)
 out_dir = sys.argv[1]
-os.makedirs(out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 torch.backends.cudnn.allow_tf32 = False
 PEAK_BW, PEAK_FP32 = 3.35e12, 67e12
@@ -40,35 +39,7 @@ PROTEINS = (132_534, 79_122_504)
 D = 8
 
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
 HBM = torch.cuda.get_device_properties(dev).total_memory
-
-
-def timed(fn, reps=20):
-    for _ in range(3):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return statistics.median(ts)
-
-
-def peak_of(fn):
-    """Bytes allocated above what is live before one call of fn."""
-    torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.max_memory_allocated() - base
 
 
 def byte_model(E, N, F, fused, bwd=False):
@@ -133,7 +104,7 @@ def aggregation_variants(st, F, run_existing_bwd):
 def run_rounds(variants):
     rounds = []
     for rnd in range(2):
-        rr = {k: timed(fn) for k, fn in variants.items()}
+        rr = {k: statistics.median(event_times(fn, 20, 3, flush=True)) for k, fn in variants.items()}
         rounds.append(rr)
         for k, t in rr.items():
             print(f"round {rnd} {k:28s} {t:12.1f}")
@@ -142,7 +113,7 @@ def run_rounds(variants):
 
 def report(st, F, variants, rounds, med, parity, skipped):
     E, N = st.nnz, st.n_rows
-    peaks = {k.replace("_us", "_peak_bytes"): peak_of(fn) for k, fn in variants.items()}
+    peaks = {k.replace("_us", "_peak_bytes"): peak_above(fn) for k, fn in variants.items()}
     bm = {"fused_fwd": byte_model(E, N, F, True), "existing_fwd": byte_model(E, N, F, False),
           "fused_bwd": byte_model(E, N, F, True, bwd=True), "existing_bwd": byte_model(E, N, F, False, bwd=True)}
     flops = 2 * E * F * D
@@ -158,7 +129,7 @@ def report(st, F, variants, rounds, med, parity, skipped):
             "not_run": skipped}
 
 
-res = {"card": card, "hbm_bytes": HBM}
+res = {"hbm_bytes": HBM}
 
 # ---------------------------------------------------------------------------------------------- (a)
 st = structures(*PROTEINS, self_loops=False)
@@ -204,15 +175,11 @@ try:
         torch.nn.functional.binary_cross_entropy_with_logits(model(graph), y).backward()
         opt.step()
 
-    torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    step()
-    torch.cuda.synchronize()
-    peak, peak_above = torch.cuda.max_memory_allocated(), torch.cuda.max_memory_allocated() - base
-    times = [timed(step, reps=10) / 1e3 for _ in range(2)]
+    step_peak_above = peak_above(step)
+    peak = torch.cuda.max_memory_allocated()
+    times = [statistics.median(event_times(step, 10, 3, flush=True)) / 1e3 for _ in range(2)]
     res["deepergcn_step"] = {"layers": 14, "hidden": 128, "step_ms_rounds": times, "step_ms": statistics.median(times),
-                             "max_memory_allocated": peak, "peak_above_inputs": peak_above, "kernel_after_step":
+                             "max_memory_allocated": peak, "peak_above_inputs": step_peak_above, "kernel_after_step":
                              cogdl_b200._cabi.last_kernel(),
                              "original_saved_edge_terms_bytes": 13 * st.nnz * 128 * 4}
     print(json.dumps(res["deepergcn_step"]))
@@ -228,6 +195,4 @@ variants, parity = aggregation_variants(st, 128, True)
 rounds, med = run_rounds(variants)
 res["arxiv"] = report(st, 128, variants, rounds, med, parity, {})
 print(json.dumps({"arxiv": res["arxiv"]["summary"]}))
-print(card)
-with open(os.path.join(out_dir, "time_genconv_edge.json"), "w") as f:
-    json.dump(res, f, indent=1)
+write_result(out_dir, "time_genconv_edge", res)

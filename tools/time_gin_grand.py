@@ -18,11 +18,11 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 import torch.nn.functional as F
+from gpu_timing import card, event_times
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -32,21 +32,16 @@ GRAND_RUNS = [("cora", 1433), ("cora", 128), ("pubmed", 500), ("pubmed", 128), (
 ORDER, SAMPLE, DROPNODE, HIDDEN, CLASSES = 8, 4, 0.5, 32, 7
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
-
-
-def timed(fn, iters):
+def per_call_ms(fn, iters):
+    """ms per call over one CUDA-event window of `iters` back-to-back calls of fn, after one warm-up call, and the last
+    call's result."""
     fn()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        out = fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters, out
+    last = [None]
+
+    def loop():
+        for _ in range(iters):
+            last[0] = fn()
+    return event_times(loop, 1, 0, flush=False)[0] / 1e3 / iters, last[0]
 
 
 def graph(name, dev, norm):
@@ -119,7 +114,7 @@ def main():
         outs = {}
         for _ in range(a.rounds):
             for fused in (False, True):
-                ms, outs[fused] = timed(lambda: gin_step(g, x, eps, G, fused), a.iters)
+                ms, outs[fused] = per_call_ms(lambda: gin_step(g, x, eps, G, fused), a.iters)
                 t[fused].append(ms)
         same = all(torch.equal(p.view(torch.int32), q.view(torch.int32)) for p, q in zip(outs[True], outs[False]))
         res[f"gin_arxiv_F{Fd}"] = {"fused_ms": statistics.median(t[True]), "unfused_ms": statistics.median(t[False]),
@@ -136,10 +131,10 @@ def main():
         outs = {}
         for _ in range(a.rounds):
             for fused in (False, True):
-                ms, outs[fused] = timed(lambda: rand_prop(g, x.clone(), fused), a.iters)
+                ms, outs[fused] = per_call_ms(lambda: rand_prop(g, x.clone(), fused), a.iters)
                 t[("rand_prop", fused)].append(ms)
                 with torch.no_grad():
-                    ms, _ = timed(lambda: grand_forward(g, x, l1, l2, fused), max(1, a.iters // 4))
+                    ms, _ = per_call_ms(lambda: grand_forward(g, x, l1, l2, fused), max(1, a.iters // 4))
                 t[("forward", fused)].append(ms)
         same = torch.equal(outs[True].view(torch.int32), outs[False].view(torch.int32))
         for k in ("rand_prop", "forward"):

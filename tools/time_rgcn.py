@@ -19,16 +19,14 @@ Writes time_rgcn.json to OUT_DIR with the card name and power limit read in the 
 
     python tools/time_rgcn.py OUT_DIR
 """
-import hashlib
 import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
+from gpu_timing import digest, event_times, host_times, peak_above, write_result
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -40,42 +38,8 @@ from tests.refpkg import import_reference  # noqa: E402
 if len(sys.argv) != 2:
     sys.exit(__doc__)
 out_dir = sys.argv[1]
-os.makedirs(out_dir, exist_ok=True)
 torch.backends.cuda.matmul.allow_tf32 = False
 dev = torch.device("cuda")
-card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                      capture_output=True, text=True).stdout.strip()
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
-
-
-def timed(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    ts = []
-    for _ in range(reps):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return statistics.median(ts)
-
-
-def peak_above(fn):
-    torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.max_memory_allocated() - base
-
-
-def sha(t):
-    return hashlib.sha256(t.detach().contiguous().cpu().numpy().tobytes()).hexdigest()[:16]
-
-
 def make_kg(n_ent, n_rel, n_tri, seed):
     """Seeded KG: relation frequencies Zipf(1) over a random relation order, entity ranks from a power law (hubs), the
     COO shuffled.  int64 tensors on the device."""
@@ -143,7 +107,7 @@ def on_gpu_graph(row, col, typ):
     return g
 
 
-res = {"card": card, "fb15k237": {}, "wikikg2": {}, "sha256": {}}
+res = {"fb15k237": {}, "wikikg2": {}, "sha256": {}}
 
 # ---------------------------------------------------------------------------------------------- (a)
 N, R, F, BASES = 14541, 237, 200, 5
@@ -158,8 +122,8 @@ gen = torch.Generator(device=dev).manual_seed(1)
 x = torch.randn(N, F, device=dev, generator=gen)
 coef = torch.randn(R, BASES, device=dev, generator=gen)
 vals = [(val * coef[rs.type.long(), b]).contiguous() for b in range(BASES)]
-t_sp = timed(lambda: spmm_raw(st, val, x))
-t_agg = timed(lambda: rgcn_aggr_raw(st, rs.type, val, coef, x))
+t_sp = statistics.median(event_times(lambda: spmm_raw(st, val, x), 20, 3, flush=True))
+t_agg = statistics.median(event_times(lambda: rgcn_aggr_raw(st, rs.type, val, coef, x), 20, 3, flush=True))
 
 
 def five():
@@ -167,10 +131,10 @@ def five():
         spmm_raw(st, v, x)
 
 
-t_five = timed(five)
+t_five = statistics.median(event_times(five, 20, 3, flush=True))
 fb["aggr_F200_B5"] = {"spmm_us": t_sp, "fanout_us": t_agg, "five_spmm_us": t_five, "vs_spmm": t_agg / t_sp,
                       "vs_five_spmm": t_agg / t_five}
-res["sha256"]["fb_aggr"] = sha(rgcn_aggr_raw(st, rs.type, val, coef, x))
+res["sha256"]["fb_aggr"] = digest(rgcn_aggr_raw(st, rs.type, val, coef, x))
 print(json.dumps(fb, indent=1), flush=True)
 
 torch.manual_seed(0)
@@ -189,8 +153,8 @@ def layer_fwd_bwd():
 
 for name, fwd in (("original", ORIGINAL), ("corrected_loop", corrected_forward), ("installed", INSTALLED)):
     with torch.no_grad():
-        t_f = with_forward(fwd, lambda: timed(layer_fwd, reps=10))
-    t_fb = with_forward(fwd, lambda: timed(layer_fwd_bwd, reps=10))
+        t_f = with_forward(fwd, lambda: statistics.median(event_times(layer_fwd, 10, 3, flush=True)))
+    t_fb = with_forward(fwd, lambda: statistics.median(event_times(layer_fwd_bwd, 10, 3, flush=True)))
     m_fb = with_forward(fwd, lambda: peak_above(layer_fwd_bwd))
     fb[f"layer_{name}"] = {"fwd_us": t_f, "fwd_bwd_us": t_fb, "fwd_bwd_peak_bytes": m_fb}
     print(name, fb[f"layer_{name}"], flush=True)
@@ -198,7 +162,7 @@ with torch.no_grad():
     y_c = with_forward(corrected_forward, layer_fwd)
     y_i = layer_fwd()
 fb["installed_vs_corrected_loop_max_rel"] = float((y_i - y_c).abs().max() / y_c.abs().max())
-res["sha256"]["fb_layer_installed"] = sha(y_i)
+res["sha256"]["fb_layer_installed"] = digest(y_i)
 for k in ("fwd_us", "fwd_bwd_us", "fwd_bwd_peak_bytes"):
     fb[f"layer_{k}_original_over_installed"] = fb["layer_original"][k] / fb["layer_installed"][k]
     fb[f"layer_{k}_corrected_over_installed"] = fb["layer_corrected_loop"][k] / fb["layer_installed"][k]
@@ -208,7 +172,7 @@ model = LinkPredictRGCN(N, R, 200, 2, "basis", BASES).to(dev).eval()
 pgraph = on_gpu_graph(row, col, typ)
 with torch.no_grad():
     for name, fwd in (("original", ORIGINAL), ("installed", INSTALLED)):
-        t = with_forward(fwd, lambda: timed(lambda: model.predict(pgraph), reps=10))
+        t = with_forward(fwd, lambda: statistics.median(event_times(lambda: model.predict(pgraph), 10, 3, flush=True)))
         m = with_forward(fwd, lambda: peak_above(lambda: model.predict(pgraph)))
         fb[f"predict_{name}"] = {"us": t, "peak_bytes": m}
 fb["predict_speedup"] = fb["predict_original"]["us"] / fb["predict_installed"]["us"]
@@ -224,16 +188,8 @@ def loss_step():
 
 for name, fwd in (("original", ORIGINAL), ("installed", INSTALLED)):
     np.random.seed(3)
-    ts = []
     try:
-        for i in range(6):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            with_forward(fwd, loss_step)
-            torch.cuda.synchronize()
-            if i > 0:
-                ts.append((time.perf_counter() - t0) * 1e6)
-        fb[f"loss_step_{name}_us"] = statistics.median(ts)
+        fb[f"loss_step_{name}_us"] = statistics.median(host_times(lambda: with_forward(fwd, loss_step), 5, 1))
     except RuntimeError as e:    # the original raises on the GPU: loss() samples the edge types on the host
         fb[f"loss_step_{name}_us"] = f"raises: {str(e).splitlines()[0][:120]}"
 
@@ -253,16 +209,11 @@ torch.manual_seed(0)
 layer = RGCNLayer(F, F, R, "basis", BASES).to(dev).train()
 xl = torch.randn(N, F, device=dev, requires_grad=True)
 G = torch.randn(N, F, device=dev)
-torch.cuda.synchronize()
-t0 = time.perf_counter()
-layer_fwd_bwd()
-torch.cuda.synchronize()
-wk["first_fwd_bwd_with_build_us"] = (time.perf_counter() - t0) * 1e6
-wk["fwd_bwd_us"] = timed(layer_fwd_bwd, reps=5, warm=1)
+wk["first_fwd_bwd_with_build_us"] = host_times(layer_fwd_bwd, 1, 0)[0]
+wk["fwd_bwd_us"] = statistics.median(event_times(layer_fwd_bwd, 5, 1, flush=True))
 wk["fwd_bwd_peak_bytes"] = peak_above(layer_fwd_bwd)
 wk["inputs_bytes"] = torch.cuda.memory_allocated()
 print(json.dumps(wk, indent=1), flush=True)
 
-with open(os.path.join(out_dir, "time_rgcn.json"), "w") as f:
-    json.dump(res, f, indent=1)
+write_result(out_dir, "time_rgcn", res)
 print(json.dumps(res["sha256"]))

@@ -19,11 +19,10 @@ shape.  Usage: python tools/time_simple_hgn.py [--shapes mag,small] [--reps 5]
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
+from gpu_timing import card, host_times, peak_above
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
@@ -32,15 +31,6 @@ from cogdl_b200.operators._raw import gat_fwd_raw, hgn_attn_raw, mhspmm_raw  # n
 
 SHAPES = {"mag": (1939743, 21111007, 4), "small": (20000, 125000, 2)}
 SLOPE, P, ALPHA, F_IN, HID = 0.2, 0.5, 0.05, 128, 64
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        q = f"nvidia-smi unavailable ({e})"
-    return q
 
 
 def make_graph(N, E_half, R, dev, seed=0):
@@ -91,27 +81,9 @@ class Conv(torch.nn.Module):
         return out, att.detach()
 
 
-def timed(fn, reps):
+def median_s(fn, reps):
     """Median seconds of fn() over reps runs, each ended by a device synchronise, after one warm-up run."""
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        ts.append(time.perf_counter() - t0)
-    return sorted(ts)[len(ts) // 2]
-
-
-def peak_above_start(fn):
-    """Bytes: the peak allocated during fn() above what was allocated when it started."""
-    torch.cuda.synchronize()
-    start = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.memory_stats()["allocated_bytes.all.peak"] - start
+    return sorted(host_times(fn, reps, 1))[reps // 2] / 1e6
 
 
 def run_shape(name, reps, dev):
@@ -137,7 +109,7 @@ def run_shape(name, reps, dev):
     fwd_bwd(True)                              # build the cached structures (transpose, plan, type grouping) first
     fwd_bwd(False)
     for fused in (True, False):
-        res_row[f"peak_gb_{'fused' if fused else 'unfused'}"] = round(peak_above_start(lambda: fwd_bwd(fused)) / 1e9, 3)
+        res_row[f"peak_gb_{'fused' if fused else 'unfused'}"] = round(peak_above(lambda: fwd_bwd(fused)) / 1e9, 3)
     res_row["peak_saved_gb"] = round(res_row["peak_gb_unfused"] - res_row["peak_gb_fused"], 3)
     for r, tag in ((res, ""), (None, "_nores")):   # what the forward keeps alive for the backward (output included)
         for fused in (True, False):
@@ -156,7 +128,7 @@ def run_shape(name, reps, dev):
         t = {}
         for _ in range(2):                    # alternate fused and unfused
             for fused in (True, False):
-                t.setdefault(fused, []).append(timed(lambda: fn(fused), reps))
+                t.setdefault(fused, []).append(median_s(lambda: fn(fused), reps))
         res_row[f"{what}_ms_fused"] = round(1e3 * min(t[True]), 3)
         res_row[f"{what}_ms_unfused"] = round(1e3 * min(t[False]), 3)
         res_row[f"{what}_speedup"] = round(min(t[False]) / min(t[True]), 3)
@@ -169,9 +141,9 @@ def run_shape(name, reps, dev):
         he = (conv.a_e * (conv.edge_emb @ conv.W_e).view(-1, 8, conv.edge_feats)).sum(-1)
         rs = cogdl_b200.structure.rgcn_structure_for(st, etype)
         att = torch.rand(E, 8, device=dev)
-        t_typed = timed(lambda: hgn_attn_raw(st, rs.type, hl, hr, he, SLOPE, False), reps)
-        t_gat = timed(lambda: gat_fwd_raw(st, hl, hr, h, SLOPE, False), reps)
-        t_agg = timed(lambda: mhspmm_raw(st, att, h), reps)
+        t_typed = median_s(lambda: hgn_attn_raw(st, rs.type, hl, hr, he, SLOPE, False), reps)
+        t_gat = median_s(lambda: gat_fwd_raw(st, hl, hr, h, SLOPE, False), reps)
+        t_agg = median_s(lambda: mhspmm_raw(st, att, h), reps)
     res_row["typed_attention_ms"] = round(1e3 * t_typed, 3)
     res_row["gat_attention_ms"] = round(1e3 * (t_gat - t_agg), 3)
     res_row["typed_over_gat"] = round(t_typed / max(t_gat - t_agg, 1e-9), 3)
@@ -191,7 +163,7 @@ def run_shape(name, reps, dev):
     t = {}
     for _ in range(2):
         for fused in (True, False):
-            t.setdefault(fused, []).append(timed(lambda: step(fused), reps))
+            t.setdefault(fused, []).append(median_s(lambda: step(fused), reps))
     res_row["step_ms_fused"] = round(1e3 * min(t[True]), 3)
     res_row["step_ms_unfused"] = round(1e3 * min(t[False]), 3)
     res_row["step_speedup"] = round(min(t[False]) / min(t[True]), 3)

@@ -5,12 +5,12 @@ Inputs are seeded, so the hashes of two builds match exactly when the builds com
   python tools/time_spmm.py              # every workload below
   python tools/time_spmm.py 128 40       # only the SpMM (default plan) at these widths
 """
-import hashlib
 import os
 import statistics
 import sys
 
 import torch
+from gpu_timing import card, digest, event_times
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
@@ -24,42 +24,27 @@ w = synth.sym_norm_weights(rp, col).to(dev)
 st = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n)
 st.plan
 st_noplan = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n, chunk_edges=0)
-flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
+print("card:", card(), flush=True)
 
 
 def randn(*shape, seed):
     return torch.randn(*shape, device=dev, generator=torch.Generator(device=dev).manual_seed(seed))
 
 
-def digest(out):
-    h = hashlib.sha256()
-    for t in out if isinstance(out, tuple) else (out,):
-        h.update(t.contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()[:16]
-
-
-def run(label, fn, algo=None):
-    for _ in range(3):
-        out = fn()
-    ts = []
-    for _ in range(30):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
+def report(label, fn, algo=None):
+    out = fn()
+    ts = event_times(fn, 30, 2, flush=True)
     med = statistics.median(ts)
     rate = f"{algo / med / 1e3:7.0f} GB/s" if algo else " " * 12
-    print(f"{label:32s} median {med:8.1f} us min {min(ts):8.1f} us {rate}  sha256 {digest(out)}  [{_cabi.last_kernel()}]")
+    out = out if isinstance(out, tuple) else (out,)
+    print(f"{label:32s} median {med:8.1f} us min {min(ts):8.1f} us {rate}  sha256 {digest(*out)}  [{_cabi.last_kernel()}]")
 
 
 def spmm(F, structure=st, tag="", weights=(w, None)):
     x = randn(n, F, seed=F)
     for wt in weights:
         algo = st.nnz * (4 * F + (8 if wt is not None else 4)) + n * (4 * F + 4)
-        run(f"spmm F={F} {'weighted' if wt is not None else 'unweighted'}{tag}", lambda: spmm_raw(structure, wt, x), algo)
+        report(f"spmm F={F} {'weighted' if wt is not None else 'unweighted'}{tag}", lambda: spmm_raw(structure, wt, x), algo)
 
 
 if sys.argv[1:]:
@@ -71,7 +56,7 @@ for F in (7, 16, 32):
 spmm(128, st_noplan, " chunk_edges=0")
 for H, F in ((8, 8), (4, 8), (1, 16)):
     att, feat = torch.rand(st.nnz, H, device=dev, generator=torch.Generator(device=dev).manual_seed(H)), randn(n, H, F, seed=F)
-    run(f"mhspmm H={H} F={F}", lambda: mhspmm_raw(st, att, feat))
+    report(f"mhspmm H={H} F={F}", lambda: mhspmm_raw(st, att, feat))
 for F in (4, 7, 8, 16, 40, 128, 256):
     x = randn(n, F, seed=F)
-    run(f"scatter_max F={F}", lambda: scatter_max_fwd_raw(st, x))
+    report(f"scatter_max F={F}", lambda: scatter_max_fwd_raw(st, x))

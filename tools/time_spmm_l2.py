@@ -19,24 +19,17 @@ to this tree's, the launched kernel, the card's name, power limit and max SM clo
 active after the run.  No DRAM traffic is measured: the byte figures printed are computed from the shapes.
 """
 import argparse
-import hashlib
 import json
 import os
 import statistics
 import subprocess
 import sys
 
+from gpu_timing import card, digest, event_times
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = 128
 FOLDS = (1, 2, 4)
-
-
-def card(query):
-    try:
-        return subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as ex:  # noqa: BLE001
-        return f"nvidia-smi unavailable ({ex})"
 
 
 def worker(tree, steps):
@@ -54,7 +47,6 @@ def worker(tree, steps):
     rp, col = synth.powerlaw_csr(n, e, seed=0, self_loops=True)
     w = synth.sym_norm_weights(rp, col).to(dev)
     gen = torch.Generator(device=dev).manual_seed(0)
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
     variants = {}
     st = cogdl_b200.CSRStructure.from_int64(rp.to(dev), col.to(dev), n_cols=n)
     st.plan
@@ -72,23 +64,13 @@ def worker(tree, steps):
     for name, fn in variants.items():
         y = fn()
         torch.cuda.synchronize()
-        info[name] = {"kernel": _cabi.last_kernel(), "sha256": hashlib.sha256(y.cpu().numpy().tobytes()).hexdigest()}
+        info[name] = {"kernel": _cabi.last_kernel(), "sha256": digest(y)}
         for _ in range(3):
             fn()
     torch.cuda.synchronize()
     print(json.dumps({"ready": info, "nnz": int(col.numel()), "n": n}), flush=True)
     for line in sys.stdin:
-        fn = variants[line.strip()]
-        evs = []
-        for _ in range(steps):
-            flush.zero_()
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            fn()
-            b.record()
-            evs.append((a, b))
-        torch.cuda.synchronize()
-        print(json.dumps([a.elapsed_time(b) * 1e3 for a, b in evs]), flush=True)
+        print(json.dumps(event_times(variants[line.strip()], steps, 0, flush=True, sync_each=False)), flush=True)
 
 
 def single_use_bytes(n, nnz, panels, edge_row):
@@ -109,7 +91,7 @@ def main():
         worker(args.worker, args.steps)
         return
 
-    print("card:", card("name,power.limit,clocks.max.sm"), flush=True)
+    print("card:", card(), flush=True)
     trees = {"this": ROOT}
     for d in args.base:
         trees[os.path.basename(os.path.normpath(d))] = os.path.abspath(d)

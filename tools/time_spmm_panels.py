@@ -14,47 +14,15 @@ medians, and the card's name, power limit and max SM clock.
 import argparse
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+from gpu_timing import alternate, card
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import cogdl_b200  # noqa: E402
 from cogdl_b200 import _cabi, synth  # noqa: E402
 from cogdl_b200.operators._raw import spmm_raw  # noqa: E402
-
-
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as ex:  # noqa: BLE001
-        return f"nvidia-smi unavailable ({ex})"
-
-
-def run(variants, rounds, steps, flush):
-    """variants: {name: fn}; returns {name: (all times us, per-round medians)}."""
-    out = {k: ([], []) for k in variants}
-    for fn in variants.values():
-        for _ in range(3):
-            fn()
-    torch.cuda.synchronize()
-    for _ in range(rounds):
-        for name, fn in variants.items():
-            evs = []
-            for _ in range(steps):
-                flush.zero_()
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record()
-                fn()
-                b.record()
-                evs.append((a, b))
-            torch.cuda.synchronize()
-            ts = [a.elapsed_time(b) * 1e3 for a, b in evs]
-            out[name][0].extend(ts)
-            out[name][1].append(statistics.median(ts))
-    return out
 
 
 def report(res, base, notes):
@@ -77,7 +45,6 @@ def main():
     n, e = synth.SHAPES["arxiv"]
     rp, col = synth.powerlaw_csr(n, e, seed=0, self_loops=True)
     w = synth.sym_norm_weights(rp, col).to(dev)
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
     gen = torch.Generator(device=dev).manual_seed(0)
 
     if args.mode == "fold":
@@ -90,7 +57,7 @@ def main():
             x = torch.randn(m, F, device=dev, generator=gen)
             variants[f"k={k}"] = (lambda st=st, x=x: spmm_raw(st, w, x, panels=1))   # the single-pass kernel
             notes[f"k={k}"] = f"X {m * F * 4 / 1e6:.1f} MB"
-        res = run(variants, args.rounds, args.steps, flush)
+        res = alternate(variants, args.rounds, args.steps, 3, flush=True, sync_each=False)
         variants["k=1"]()
         notes["k=1"] += ", " + _cabi.last_kernel()
         print(f"fold curve: arxiv shape, weighted, F={F}, nnz={int(col.numel())}", flush=True)
@@ -110,7 +77,7 @@ def main():
             y = fn()
             notes[name] = ("bitwise == P=1" if torch.equal(y.view(torch.int32), y1.view(torch.int32)) else "DIFFERS from P=1") + \
                 ", " + _cabi.last_kernel()
-        res = run(variants, args.rounds, args.steps, flush)
+        res = alternate(variants, args.rounds, args.steps, 3, flush=True, sync_each=False)
         print(f"panel sweep: arxiv shape, weighted, F={F}, X {n * F * 4 / 1e6:.1f} MB", flush=True)
         report(res, "P=1", notes)
 

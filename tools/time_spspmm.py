@@ -9,37 +9,23 @@ the card's name and power limit read in the same run.  Prints one JSON line and 
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
+from gpu_timing import card, event_times, peak_above
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
-
-
-def timed(fn, warmup, reps):
+def median_ms_peak(fn, warmup, reps):
+    """Median ms (upper middle value of an even count) and peak GiB above the start over `reps` calls."""
     for _ in range(warmup):
         fn()
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
     times = []
-    for _ in range(reps):
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        fn()
-        e.record()
-        torch.cuda.synchronize()
-        times.append(s.elapsed_time(e))
+    peak = peak_above(lambda: times.extend(event_times(fn, reps, 0, flush=False)))
     times.sort()
-    return times[len(times) // 2], (torch.cuda.max_memory_allocated() - base) / 2**30
+    return times[len(times) // 2] / 1e3, peak / 2**30
 
 
 def products(index, n_rows, index_b):
@@ -76,9 +62,9 @@ def compare(name, ia, va, ib, vb, m, k, n, warmup, reps, backward=False):
     idx, _ = cogdl_b200.spspmm(ia, va, ib, vb, m, k, n)
     nnz = idx.shape[1]
     prods = products(A.indices(), k, B.indices())
-    t_ours, mem_ours = timed(ours, warmup, reps)
+    t_ours, mem_ours = median_ms_peak(ours, warmup, reps)
     try:
-        t_ref, mem_ref = timed(torch_mm, warmup, reps)
+        t_ref, mem_ref = median_ms_peak(torch_mm, warmup, reps)
     except RuntimeError as e:            # torch's sparse backward may not cover a case: report it, do not hide it
         t_ref, mem_ref = None, str(e).splitlines()[0]
     return {"workload": name, "m": m, "k": k, "n": n, "nnz_a": int(A._nnz()), "nnz_b": int(B._nnz()), "nnz_c": nnz,
@@ -149,7 +135,7 @@ def gtn_step(warmup, reps):
         torch.nn.functional.cross_entropy(model(graph), y).backward()
         opt.step()
 
-    t, mem = timed(step, warmup, reps)
+    t, mem = median_ms_peak(step, warmup, reps)
     return {"workload": "reference GTN training step through install(spspmm=True)", "ms": round(t, 3),
             "peak_gb": round(mem, 4)}
 
