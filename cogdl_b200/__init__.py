@@ -19,9 +19,13 @@ from .operators import csrspmm, csr_edge_softmax, csrmhspmm, scatter_max, fused_
 from .operators import genconv_aggregate, disen_routing, compgcn_aggregate, spspmm, coo_spmm  # noqa: E402,F401
 from .operators import spmm_residual, label_propagate, gin_aggregate, random_propagate  # noqa: E402,F401
 from .operators import rgcn_aggregate, rgcn_conv, hgn_attention  # noqa: E402,F401
+from .operators import (  # noqa: E402,F401
+    batch_sum_pooling, batch_mean_pooling, batch_max_pooling, graph_readout, set2set_attention, sort_pool,
+)
+from .structure import membership_for  # noqa: E402,F401
 from .install import (  # noqa: E402,F401
     install, uninstall_actnn, uninstall_appnp, uninstall_correct_smooth, uninstall_gat, uninstall_gcnii, uninstall_gin,
-    uninstall_grand, uninstall_rgcn, uninstall_spspmm, install_simple_hgn, uninstall_simple_hgn,
+    uninstall_grand, uninstall_readout, uninstall_rgcn, uninstall_spspmm, install_simple_hgn, uninstall_simple_hgn,
 )
 from . import sampling  # noqa: E402,F401
 

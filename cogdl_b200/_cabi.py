@@ -86,6 +86,8 @@ SIGNATURES = {
     "cogdl_b200_scatter_max_scratch_bytes": (_i64, [_i64, _i64]),
     "cogdl_b200_scatter_max_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_scatter_max_bwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "cogdl_b200_sort_pool_max_k": (_i64, []),
+    "cogdl_b200_sort_pool_select": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "cogdl_b200_gat_fwd_scratch_bytes": (_i64, [_i64, _i64, _i64]),
     "cogdl_b200_gat_fwd_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _i64, _i64, _i64, _plan_p, _vp]),
     "cogdl_b200_gat_fwd_dropout_f32": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, ctypes.c_uint64, ctypes.c_uint64, _f32,

@@ -43,6 +43,12 @@ rgcn=True rebinds `cogdl.layers.rgcn_layer.RGCNLayer.forward` (RGCN, LinkPredict
 relational sum with cogdl_b200.rgcn_conv (uninstall_rgcn()).  This deliberately differs from the original for more than
 one relation: the original aggregates every edge with the weight of the first relation that has edges (see
 rgcn_forward).
+readout=True rebinds cogdl.utils.batch_{sum,mean,max}_pooling (and every cogdl module attribute bound to them) to the
+deterministic, sync-free cogdl_b200 readouts, and `cogdl.models.nn.gin.GIN.forward`, `cogdl.models.nn.sortpool.SortPool.forward`
+and `cogdl.layers.set2set.Set2Set.forward` to gin_model_forward / sortpool_forward / set2set_forward (graph_readout,
+sort_pool, set2set_attention); InfoGraph and GCC take the pooling function at construction, so install before building
+models.  set2set_forward deliberately differs from an original that cannot run (see set2set_forward;
+uninstall_readout()).
 The Simple-HGN example's layer (examples/simple_hgn/conv.py, myGATConv) is not part of the cogdl package, so it has no
 install() flag: install_simple_hgn(conv_cls) rebinds the class the caller passes to simple_hgn_forward, which sends the
 attention to cogdl_b200.hgn_attention (uninstall_simple_hgn(conv_cls)).
@@ -568,6 +574,154 @@ def uninstall_simple_hgn(conv_cls):
     _restore_forward(conv_cls)
 
 
+_READOUT_NAMES = ("batch_sum_pooling", "batch_mean_pooling", "batch_max_pooling")
+_readout_state = {"originals": None, "rebound": []}
+
+
+def _readout_supported(x, batch):
+    """A readout the kernels take: x [N, F] fp32 and batch [N] integers, both on the GPU."""
+    return (torch.is_tensor(x) and torch.is_tensor(batch) and x.is_cuda and batch.is_cuda and x.dtype == torch.float32
+            and x.dim() == 2 and batch.dim() == 1 and x.shape[0] == batch.numel() and not batch.dtype.is_floating_point)
+
+
+def _pooling(mode):
+    from .operators.readout import graph_readout
+
+    name = f"batch_{mode}_pooling"
+
+    def pool(x, batch):
+        if not _readout_supported(x, batch):
+            return _readout_state["originals"][name](x, batch)
+        return graph_readout([x], batch, mode)
+
+    pool.__name__ = pool.__qualname__ = name
+    pool.__doc__ = (f"cogdl.utils.{name} (cogdl/utils/utils.py) on cogdl_b200.{name}: deterministic, and no host read "
+                    "once the batch's membership is cached; B is max(batch) + 1 and a graph id without nodes pools to 0 "
+                    "(the original's mean counts only the ids present).  CPU or non-fp32 input runs the original.")
+    pool._cogdl_b200 = True
+    return pool
+
+
+def gin_model_forward(self, batch):
+    """GIN.forward (cogdl/models/nn/gin.py:95-115) with its per-layer sum pooling (a scatter_add_ per layer after a host
+    read of max(batch)) as one cogdl_b200.graph_readout over the layer outputs; the layers, BatchNorm, ReLU, linears and
+    dropout are the model's own, called in its order.  CPU or non-fp32 features run the original."""
+    import torch.nn.functional as F
+
+    from .operators.readout import graph_readout
+
+    from .structure import membership_for
+
+    h = batch.x
+    if not _readout_supported(h, batch.batch):
+        return type(self)._cogdl_b200_original_forward(self, batch)
+    membership_for(batch.batch)     # a new batch's host reads happen here, before the layers are queued
+    layer_rep = [h]
+    for i in range(self.num_layers - 1):
+        h = F.relu(self.batch_norm[i](self.gin_layers[i](batch, h)))
+        layer_rep.append(h)
+    pooled = graph_readout(layer_rep, batch.batch, "sum")
+    final_score, off = 0, 0
+    for i, rep in enumerate(layer_rep):
+        final_score += self.dropout(self.linear_prediction[i](pooled[:, off:off + rep.shape[1]]))
+        off += rep.shape[1]
+    return final_score
+
+
+def sortpool_forward(self, batch):
+    """SortPool.forward (cogdl/models/nn/sortpool.py:105-136) with the padding to [B, max_n, F], the fill value, the
+    sort of the padded rows, the cut to k and the zeroing of the fill (two host reads) replaced by cogdl_b200.sort_pool.
+    The SAGE layers, the per-row h.sort(dim=-1), conv1d, the linears and dropout are the model's own.  Ties of the last
+    channel go to the lower node index (the original's CUDA sort is not stable).  CPU or non-fp32 features and k above
+    the kernel's maximum run the original."""
+    import torch.nn.functional as F
+
+    from .operators._raw import sort_pool_max_k
+    from .operators.readout import sort_pool
+
+    from .structure import membership_for
+
+    h = batch.x
+    if not _readout_supported(h, batch.batch) or self.k > sort_pool_max_k():
+        return type(self)._cogdl_b200_original_forward(self, batch)
+    membership_for(batch.batch)     # a new batch's host reads happen here, before the layers are queued
+    for i in range(self.num_layers):
+        h = F.relu(self.gnn_convs[i](batch, h))
+    h, _ = h.sort(dim=-1)
+    h = sort_pool(h, batch.batch, self.k)
+    batch_size = h.shape[0]
+    h = F.relu(self.conv1d(h.permute(0, 2, 1))).view(batch_size, -1)
+    h = F.relu(self.fc1(h))
+    h = F.dropout(h, p=self.dropout, training=self.training)
+    return self.fc2(h)
+
+
+def set2set_forward(self, x, batch):
+    """Set2Set.forward (cogdl/layers/set2set.py:46-62) with the attention read of every step in
+    cogdl_b200.set2set_attention; the LSTM and the concatenation are the layer's own.
+
+    A deliberate divergence from the original, which cannot run: it calls `edge_softmax(e, batch)`, which is
+    cogdl.utils.edge_softmax(graph, edge_val) with a tensor for the graph.  This computes what the layer's docstring
+    states, a = softmax over graph g's nodes of <x_i, q_g> and r_g = sum_i a_i x_i, with B = max(batch) + 1 and 0 for a
+    graph id without nodes.  CPU or non-fp32 input or LSTM weights run the original."""
+    from .operators.readout import set2set_attention
+    from .structure import membership_for
+
+    if not _readout_supported(x, batch) or any(p.dtype != torch.float32 for p in self.lstm.parameters()):
+        return type(self)._cogdl_b200_original_forward(self, x, batch)
+    batch_size = membership_for(batch).num_graphs
+    h = (x.new_zeros((self.num_layers, batch_size, self.in_channels)),
+         x.new_zeros((self.num_layers, batch_size, self.in_channels)))
+    q_star = x.new_zeros(batch_size, self.out_channels)
+    for _ in range(self.processing_steps):
+        q, h = self.lstm(q_star.unsqueeze(0), h)
+        q = q.view(batch_size, self.in_channels)
+        q_star = torch.cat([q, set2set_attention(x, q, batch)], dim=-1)
+    return q_star
+
+
+def install_readout():
+    """Rebind cogdl.utils.batch_{sum,mean,max}_pooling, and every attribute of an imported cogdl.* module bound to them,
+    to the cogdl_b200 readouts; GIN.forward to gin_model_forward, SortPool.forward to sortpool_forward and
+    Set2Set.forward to set2set_forward.  InfoGraph and GCC take the pooling function when a model is constructed, so
+    install before building models.  Idempotent; uninstall_readout() restores everything."""
+    import cogdl.layers.set2set as s2s
+    import cogdl.models.nn.gin as gm
+    import cogdl.models.nn.sortpool as sp
+    import cogdl.utils.utils as uu
+
+    st = _readout_state
+    if st["originals"] is None:
+        st["originals"] = {n: getattr(uu, n) for n in _READOUT_NAMES}
+        st["new"] = {n: _pooling(n.split("_")[1]) for n in _READOUT_NAMES}
+    by_id = {id(st["originals"][n]): st["new"][n] for n in _READOUT_NAMES}
+    patched = []
+    for mname, mod in list(sys.modules.items()):
+        if mod is None or not (mname == "cogdl" or mname.startswith("cogdl.")):
+            continue
+        for attr, val in list(vars(mod).items()):
+            new = by_id.get(id(val))
+            if new is not None:
+                st["rebound"].append((mod, attr, val))
+                setattr(mod, attr, new)
+                patched.append(f"{mname}.{attr}")
+    return (patched + _rebind_forward(gm.GIN, gin_model_forward, "cogdl.models.nn.gin.GIN.forward")
+            + _rebind_forward(sp.SortPool, sortpool_forward, "cogdl.models.nn.sortpool.SortPool.forward")
+            + _rebind_forward(s2s.Set2Set, set2set_forward, "cogdl.layers.set2set.Set2Set.forward"))
+
+
+def uninstall_readout():
+    import cogdl.layers.set2set as s2s
+    import cogdl.models.nn.gin as gm
+    import cogdl.models.nn.sortpool as sp
+
+    for mod, attr, old in reversed(_readout_state["rebound"]):
+        setattr(mod, attr, old)
+    _readout_state["rebound"] = []
+    for cls in (gm.GIN, sp.SortPool, s2s.Set2Set):
+        _restore_forward(cls)
+
+
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
 _spspmm_state = {"stub": None, "rebound": []}
 
@@ -672,7 +826,7 @@ def uninstall_actnn():
 
 
 def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
-            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False, rgcn=False):
+            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False, rgcn=False, readout=False):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
@@ -776,4 +930,6 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
         patched += install_grand()
     if rgcn:
         patched += install_rgcn()
+    if readout:
+        patched += install_readout()
     return patched

@@ -25,3 +25,7 @@ from .gin import gin_aggregate, GinAggregateFunction  # noqa: F401
 from .grand import random_propagate  # noqa: F401
 from .rgcn import rgcn_aggregate, rgcn_conv, RgcnAggregateFunction, RgcnConvFunction  # noqa: F401
 from .simple_hgn import hgn_attention, HgnAttentionFunction  # noqa: F401
+from .readout import (  # noqa: F401
+    batch_sum_pooling, batch_mean_pooling, batch_max_pooling, graph_readout, set2set_attention, sort_pool,
+    ReadoutFunction, Set2SetAttentionFunction, SortPoolFunction,
+)

@@ -214,6 +214,34 @@ def scatter_max_bwd_raw(grad, argmax, n_src):
     return gx
 
 
+def sort_pool_max_k():
+    """The largest k of the SortPool readout (COGDL_B200_SORT_POOL_MAX_K)."""
+    return int(_cabi.load().cogdl_b200_sort_pool_max_k())
+
+
+def sort_pool_select_raw(st: CSRStructure, keys, k):
+    """SortPool's per-graph top-k over the membership CSR st (row g: graph g's nodes) by keys [st.n_cols] fp32 (read as
+    their bit patterns): (idx [st.n_rows, k] int32, the selection CSR of st.n_rows * k rows and st.n_cols columns, run
+    without a hub plan); see cogdl_b200_sort_pool_select."""
+    dev = require_cuda(keys)
+    k = int(k)
+    if not 1 <= k <= sort_pool_max_k():
+        raise ValueError(f"k = {k}; the SortPool readout takes 1 to {sort_pool_max_k()}")
+    if keys.dtype != torch.float32 or keys.numel() != st.n_cols:
+        raise ValueError(f"keys must be float32 [{st.n_cols}], got {keys.dtype} {tuple(keys.shape)}")
+    bits = keys.contiguous().view(torch.int32)
+    B = st.n_rows
+    m = (st.rowptr[1:] - st.rowptr[:-1]).clamp(max=k)
+    off = (torch.cumsum(m, 0) - m).to(torch.int32)
+    idx = torch.empty((B, k), dtype=torch.int32, device=dev)
+    sel_rowptr = torch.empty(B * k + 1, dtype=torch.int32, device=dev)
+    sel_colind = torch.empty(min(B * k, st.n_cols), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _cabi.call("cogdl_b200_sort_pool_select", _ptr(st.rowptr), _ptr(st.colind), _ptr(bits), st.n_cols, B, k,
+                   _ptr(off), _ptr(idx), _ptr(sel_rowptr), _ptr(sel_colind), _stream(dev))
+    return idx, CSRStructure(sel_rowptr, sel_colind, n_cols=st.n_cols, chunk_edges=0)
+
+
 def attn_dropout_args(p):
     """(drop_below, scale) of attention dropout with probability p, 0 <= p < 1: an (edge, head) is kept iff
     draw(seed, edge, head) >= drop_below = floor(p * 2^64), a kept attention is multiplied by scale = 1 / (1 - p)."""

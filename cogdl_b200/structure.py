@@ -350,6 +350,76 @@ def clear_structure_cache():
     _COMP_CACHE.clear()
     _COO_CACHE.clear()
     _RGCN_CACHE.clear()
+    _MEMBER_CACHE.clear()
+
+
+class Membership(NamedTuple):
+    """What the readouts of one `batch` vector read: `st`, the membership CSR (B rows, one per graph, whose columns are
+    that graph's nodes in ascending order); `st_t`, its transpose (N rows, one edge per node: the node's graph), with
+    `perm` its permutation; `inv_count` [B], 1 / n_g in fp32 (0 for an empty graph: the mean's row scale) and
+    `inv_count_node` [N], inv_count of each node's graph (the mean's backward over st_t)."""
+    st: CSRStructure
+    st_t: CSRStructure
+    perm: torch.Tensor
+    inv_count: torch.Tensor
+    inv_count_node: torch.Tensor
+
+    @property
+    def num_graphs(self):
+        return self.st.n_rows
+
+
+# Membership cache, keyed on the storage identity, size and stride of the batch vector and the graph count asked for:
+# every readout of a forward and its backward share one entry, and the entry made when the graph count is read from
+# the device serves every later call on that batch without a host read.
+member_cache_stats = {"hit": 0, "miss": 0}
+_MEMBER_CACHE = IdentityCache(8, member_cache_stats)
+
+
+def membership_for(batch, num_graphs=None):
+    """The cached Membership of a graph-id vector `batch` ([N] integers on the device, node i in graph batch[i], sorted
+    or not).  B = num_graphs, or max(batch) + 1 when None; graph ids without nodes are empty rows.
+
+    Built on the device with the stable COO -> CSR sort (a sorted batch gives colind = arange(N)); the CSR's hub plan
+    is built here too, and the transpose needs none, so the readouts and their backward never read the host.  Building
+    reads the batch's smallest and largest id once (one host sync per batch vector, which also checks them) and the
+    plan's sizes; `batch` itself is never copied to the host."""
+    from .data import coo2csr_index
+
+    require_cuda(batch)
+    if batch.dim() != 1 or batch.dtype.is_floating_point or batch.dtype.is_complex or batch.dtype == torch.bool:
+        raise TypeError(f"batch must be a 1-D integer tensor, got {batch.dtype} {tuple(batch.shape)}")
+    key = (batch.data_ptr(), batch.numel(), tuple(batch.stride()), str(batch.device), batch.dtype,
+           None if num_graphs is None else int(num_graphs))
+    mb = _MEMBER_CACHE.get(key)
+    if mb is not None:
+        return mb
+    member_cache_stats["miss"] += 1
+    dev, N = batch.device, batch.numel()
+    if N >= 2**31:
+        raise ValueError("batch too large for int32 indices on one device")
+    lo, hi = (int(v) for v in torch.stack([batch.min(), batch.max()]).tolist()) if N > 0 else (0, -1)
+    B = hi + 1 if num_graphs is None else int(num_graphs)
+    if lo < 0 or hi >= B:
+        raise ValueError(f"graph id {lo if lo < 0 else hi} is out of range for {B} graphs")
+    if B >= 2**31:
+        raise ValueError(f"{B} graphs do not fit int32 indices")
+    rowptr, reindex = coo2csr_index(batch, B)
+    st = CSRStructure.from_int64(rowptr, reindex, n_cols=N)
+    st.plan                                             # built now: its sizes are read on the host
+    # The transpose needs no sort: row q is node q with its one edge, column batch[q], and perm[q] is node q's CSR
+    # slot.  With one edge per row it has no hub rows, so it runs without a plan (no host read).
+    perm = torch.empty(N, dtype=torch.int32, device=dev)
+    perm[st.colind.long()] = torch.arange(N, dtype=torch.int32, device=dev)
+    st_t = CSRStructure(torch.arange(N + 1, dtype=torch.int32, device=dev), batch.to(torch.int32).contiguous(),
+                        n_cols=B, chunk_edges=0)
+    st._csc = (st_t, perm)
+    count = (rowptr[1:] - rowptr[:-1]).float()
+    inv_count = torch.where(count > 0, 1.0 / count.clamp_min(1.0), torch.zeros_like(count))
+    inv_count_node = inv_count[st_t.colind.long()].contiguous()
+    mb = Membership(st, st_t, perm, inv_count, inv_count_node)
+    _MEMBER_CACHE.put(key, (batch,), mb, 4 * (3 * N + 3 * B))
+    return mb
 
 
 class CompStructure:

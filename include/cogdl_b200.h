@@ -321,6 +321,27 @@ COGDL_B200_API int cogdl_b200_scatter_max_bwd_f32(const float *g, const int32_t 
                                    cogdl_b200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * SortPool readout: the per-graph top-k selection.
+ * Replaces  the padding, sorting and cutting of SortPool.forward   cogdl/models/nn/sortpool.py:105-126
+ * (rowptr, colind) is the membership CSR: row g lists graph g's nodes (in ascending node order), n_graphs rows.
+ * key_bits [n_x_rows] holds each node's key as the bit pattern of an IEEE binary32 value (SortPool's last channel),
+ * ordered with integer operations only: every NaN above +inf, -0 equal to +0.
+ * For each graph, the r-th of its min(k, n_g) nodes with the largest key, in descending key order with ties to the
+ * lower node index (a stable descending torch.sort), is written to idx[g, r]; idx is -1 for r >= n_g.  The same
+ * selection is written as a CSR of n_graphs * k rows: row g * k + r holds that node, or nothing for r >= n_g
+ * (sel_rowptr [n_graphs * k + 1], sel_colind [sum of min(k, n_g)]), so cogdl_b200_spmm_csr_f32_ex over it with unit
+ * values gathers the pooled rows and cogdl_b200_scatter_max_bwd_f32 with idx as the argmax scatters their gradient.
+ * sel_off [n_graphs] must hold the exclusive prefix sum of min(k, n_g).  idx [n_graphs, k] int32.
+ * 1 <= k <= cogdl_b200_sort_pool_max_k() (= COGDL_B200_SORT_POOL_MAX_K), else COGDL_B200_EINVAL before any launch.
+ * ------------------------------------------------------------------------------------- */
+#define COGDL_B200_SORT_POOL_MAX_K 1024
+COGDL_B200_API int64_t cogdl_b200_sort_pool_max_k(void);
+COGDL_B200_API int cogdl_b200_sort_pool_select(const int32_t *rowptr, const int32_t *colind, const uint32_t *key_bits,
+                                int64_t n_x_rows, int64_t n_graphs, int64_t k, const int32_t *sel_off,
+                                int32_t *idx, int32_t *sel_rowptr, int32_t *sel_colind,
+                                cogdl_b200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * "Next" rows (SURVEY 8f).
  *
  * GAT forward: e = leakyrelu(h_l[i,h] + h_r[col,h]); a = softmax_row(e); out = sum a*feat.
