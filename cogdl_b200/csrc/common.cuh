@@ -188,9 +188,9 @@ __device__ __forceinline__ float4 sub_rn(float4 a, float4 b) {
 }
 // Attention that carries a dropout mask in its sign bit (GAT attention dropout, edge_softmax.cu MODE 2): a dropped
 // entry reads as 0, a kept one as a * scale.  The BIT is tested, not a < 0: a dropped softmax that underflowed to 0
-// is stored as -0.0.
+// is stored as -0.0.  A dropped entry is |a| * 0, not a selected 0, so a dropped NaN stays NaN (torch's a * mask * scale).
 __device__ __forceinline__ float drop_att(float a, float scale) {
-  return (__float_as_uint(a) >> 31) ? 0.f : __fmul_rn(a, scale);
+  return __fmul_rn(fabsf(a), __int_as_float(~(__float_as_int(a) >> 31) & __float_as_int(scale)));
 }
 template <typename VecT> __device__ __forceinline__ VecT vzero();
 template <> __device__ __forceinline__ float4 vzero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }

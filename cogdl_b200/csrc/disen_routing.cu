@@ -111,6 +111,9 @@ __device__ __forceinline__ void dr_fwd_finish(const DrFwdParams &p, int row, int
   using VecT = typename DrVec<W>::T;
   float u[W];
   dr_load<W>(p.c, (int64_t)row * p.FV + cv, ok, u);
+  // a +Inf logit is its channel's max, and exp(z - max) = exp(Inf - Inf) is NaN in the softmax this restates: the
+  // online state counted it as 1, so S is replaced by NaN here.  All logits -inf: S = 0, and acc / S is NaN.
+  S = M < CUDART_INF_F ? S : CUDART_NAN_F;
 #pragma unroll
   for (int k = 0; k < W; ++k) u[k] = any ? u[k] + acc[k] / S : u[k];
   const float nrm = sqrtf(chan_sum(dr_dot<W>(u, u), p.L, mask));
@@ -149,7 +152,9 @@ __global__ void __launch_bounds__(256) disen_route_fwd_kernel(const DrFwdParams 
     dr_load<W>(p.q, (int64_t)w.row * FV + cv, ok, qi);
 #pragma unroll
     for (int k = 0; k < W; ++k) acc[k] = 0.f;
-    float M = -CUDART_INF_F, S = 0.f;
+    // M starts at -FLT_MAX, not -inf: a -inf logit (a large q against its c) then gives e = 0 wherever it falls, where
+    // -inf - (-inf) would make the channel NaN
+    float M = -FLT_MAX, S = 0.f;
     for (int off = 0; off < maxdeg; off += GROUP) {
       const int cnt = min(GROUP, w.hb - w.lb - off);   // <= 0 once this item's edges are done
       const int cidx = gl < cnt ? ld_stream(p.colind + w.lb + off + gl) : 0;
@@ -172,7 +177,7 @@ __global__ void __launch_bounds__(256) disen_route_fwd_kernel(const DrFwdParams 
           dr_unpack(xv[u], x);
           const float z = __fmul_rn(chan_sum(dr_dot<W>(qi, x), p.L, FULL), p.zs);
           if (ok && j + u < cnt) {
-            const float dd = z - M;                 // M = -inf on the first edge: e = 0, S = 1, acc = x
+            const float dd = z - M;                 // first edge (z > -FLT_MAX): dd > 0, e = 0, S = 1, acc = x
             const float e = exp2f(-fabsf(dd));
             if (dd > 0.f) {
               S = fmaf(S, e, 1.f);

@@ -3,8 +3,8 @@
 //   TYPED (MODES 2, 3): the logit gains a per-edge-type term, leakyrelu(h_l[row,h] + h_r[col,h] + h_e[type[p],h]),
 //          h_e [T, H] staged in shared memory by the kernel (`tab`), type [nnz] int32 in CSR slot order;
 //   MIX   (MODE 2, TYPED only): besides the signed softmax (out, nullable), the kernel writes the attention the layer
-//          returns, mix = (1 - alpha) * (dropped ? 0 : a * keep_scale) + alpha * res[p,h]; without MIX it is
-//          (dropped ? 0 : a * keep_scale).
+//          returns, mix = (1 - alpha) * a * (dropped ? 0 : keep_scale) + alpha * res[p,h]; without MIX it is
+//          a * (dropped ? 0 : keep_scale), a product, so a dropped NaN stays NaN.
 // edge_softmax.cu launches them with TYPED = MIX = false.
 #pragma once
 #include "common.cuh"
@@ -59,7 +59,8 @@ __device__ __forceinline__ float es_mark(const EsParams &p, int64_t edge, int he
 template <bool DROP>
 __device__ __forceinline__ void es_unmark(const EsParams &p, float &y, float &g) {
   if (DROP) {
-    g = (__float_as_uint(y) >> 31) ? 0.f : __fmul_rn(g, p.scale);
+    // a product with 0, not a select: a NaN or Inf gradient of a dropped entry gives NaN, as torch's g * mask * scale
+    g = __fmul_rn(g, __int_as_float(~(__float_as_int(y) >> 31) & __float_as_int(p.scale)));
     y = fabsf(y);
   }
 }
@@ -72,7 +73,8 @@ __device__ __forceinline__ void es_put(const EsParams &p, int64_t k, float a) {
     return;
   }
   if (p.out) st_stream(p.out + k, a);
-  float m = (__float_as_uint(a) >> 31) ? 0.f : __fmul_rn(a, p.keep_scale);
+  // |a| * (kept ? keep_scale : 0), a product and not a select: a dropped NaN stays NaN
+  float m = __fmul_rn(fabsf(a), __int_as_float(~(__float_as_int(a) >> 31) & __float_as_int(p.keep_scale)));
   if (MIX) m = __fadd_rn(__fmul_rn(m, p.keep), __fmul_rn(__ldg(p.res + k), p.alpha));
   st_stream(p.mix + k, m);
 }

@@ -6,7 +6,7 @@
 //   a[p,h]   = softmax over row i of leakyrelu(h_l[i,h] + h_r[j,h] + h_e[t,h])
 //   att[p,h] = a, with the sign bit set when dropped (the GAT-dropout carrier: the same mask, seed and keep rule as
 //              cogdl_b200_gat_fwd_dropout_f32), written only when a gradient is needed
-//   mix[p,h] = (1 - alpha) * (dropped ? 0 : a * scale) + alpha * res[p,h]    (without res: dropped ? 0 : a * scale)
+//   mix[p,h] = (1 - alpha) * a * (dropped ? 0 : scale) + alpha * res[p,h]    (without res: a * (dropped ? 0 : scale))
 // mix is what the layer aggregates (cogdl_b200_mhspmm_f32) and returns; no other [nnz, H] tensor is written.
 //
 // Backward (MODE 3 with the type term): given att and d mix (= mhsddmm(d out, h)),

@@ -42,7 +42,7 @@ __global__ void __launch_bounds__(256) softmax_aggr_fwd_kernel(const SaFwdParams
     const bool ok = cv < FV;
     float M[W], S[W], T[W], Q[W];
 #pragma unroll
-    for (int k = 0; k < W; ++k) { M[k] = -CUDART_INF_F; S[k] = 0.f; T[k] = 0.f; Q[k] = 0.f; }
+    for (int k = 0; k < W; ++k) { M[k] = SA_M0; S[k] = 0.f; T[k] = 0.f; Q[k] = 0.f; }
     for (int e0 = w.lb; e0 < w.hb; e0 += 32) {
       const int cnt = min(32, w.hb - e0);
       const int c = lane < cnt ? ld_stream(p.colind + e0 + lane) : 0;
@@ -79,14 +79,14 @@ __global__ void __launch_bounds__(256) softmax_aggr_fwd_kernel(const SaFwdParams
       st_cg(pp + 2 * FV, pack(T));
       if (WANT_Q) st_cg(pp + 3 * FV, pack(Q));
     } else if (ok) {
-      sa_finish<W, WANT_Q>(p, (int64_t)w.row * FV + cv, M, S, T, Q);
+      sa_finish<W, WANT_Q>(p, (int64_t)w.row * FV + cv, M, S, T, Q, w.hb > w.lb);
     }
   }
   if (w.is_chunk && hub_arrive_last<32>(w, p.hub, lane)) {
     for (int cv = lane; cv < FV; cv += 32) {
       float M[W], S[W], T[W], Q[W];
 #pragma unroll
-      for (int k = 0; k < W; ++k) { M[k] = -CUDART_INF_F; S[k] = 0.f; T[k] = 0.f; Q[k] = 0.f; }
+      for (int k = 0; k < W; ++k) { M[k] = SA_M0; S[k] = 0.f; T[k] = 0.f; Q[k] = 0.f; }
       for (int q = 0; q < w.n_row_chunks; ++q) {   // chunk order: deterministic
         const VecT *pp = P + (int64_t)(w.first + q) * K * FV + cv;
         float Mc[W], Sc[W], Tc[W], Qc[W];
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(256) softmax_aggr_fwd_kernel(const SaFwdParams
 #pragma unroll
         for (int k = 0; k < W; ++k) sa_merge(Mc[k], Sc[k], Tc[k], WANT_Q ? Qc[k] : 0.f, M[k], S[k], T[k], Q[k]);
       }
-      sa_finish<W, WANT_Q>(p, (int64_t)w.row * FV + cv, M, S, T, Q);
+      sa_finish<W, WANT_Q>(p, (int64_t)w.row * FV + cv, M, S, T, Q, true);
     }
   }
 }

@@ -9,9 +9,14 @@
 
 #include <math_constants.h>
 
+#include <cfloat>
+
 namespace cogdl_b200 {
 
 constexpr float SA_LOG2E = 1.4426950408889634f;
+// The running max M starts at -FLT_MAX, not -inf: a -inf logit (a negative beta times a message past ~2^127) then
+// gives d = -inf and weight 0 wherever it falls, where -inf - (-inf) would make the row NaN.
+constexpr float SA_M0 = -FLT_MAX;
 constexpr int SA_UNROLL = 4;   // gathers in flight per lane (8 measured slower: 573-625 vs 472-515 us, arxiv F = 128)
 
 template <int W> struct SaVec;
@@ -40,7 +45,8 @@ struct SaFwdParams {
   HubView hub;         // partials: [n_chunks][3 or 4][FV] vectors
 };
 
-// One edge into the online state.  M = -inf on entry gives d = +inf, e = 0: S = 1, T = m, M = z.
+// One edge into the online state.  M = SA_M0 on entry gives d > 0 and S = 1, T = m, M = z for any z above -FLT_MAX;
+// z = -inf gives e = 0 and adds nothing (T += 0 * m: NaN for an infinite m, as exp(-inf) * m is in the softmax).
 template <bool WANT_Q>
 __device__ __forceinline__ void sa_step(float m, float b2, float &M, float &S, float &T, float &Q) {
   const float z = m * b2;
@@ -58,7 +64,8 @@ __device__ __forceinline__ void sa_step(float m, float b2, float &M, float &S, f
   }
 }
 
-// Fold a chunk's partial state into (M, S, T, Q); M = -inf on entry takes the partial as it is.
+// Fold a chunk's partial state into (M, S, T, Q); M = SA_M0 on entry takes the partial as it is (a chunk's M is at
+// least SA_M0, so no -inf - (-inf) forms here either).
 __device__ __forceinline__ void sa_merge(float Mc, float Sc, float Tc, float Qc, float &M, float &S, float &T, float &Q) {
   const float Mn = fmaxf(M, Mc);
   const float a = exp2f(M - Mn), b = exp2f(Mc - Mn);
@@ -70,14 +77,15 @@ __device__ __forceinline__ void sa_merge(float Mc, float Sc, float Tc, float Qc,
 
 template <int W, bool WANT_Q>
 __device__ __forceinline__ void sa_finish(const SaFwdParams &p, int64_t off, const float (&M)[W], const float (&S)[W],
-                                          const float (&T)[W], const float (&Q)[W]) {
+                                          const float (&T)[W], const float (&Q)[W], bool any) {
   using VecT = typename SaVec<W>::T;
   float o[W], l[W], q[W];
 #pragma unroll
   for (int k = 0; k < W; ++k) {
-    const bool any = S[k] != 0.f;          // degree-0 rows: out = 0 (a scatter_add of nothing); a NaN S is not one
-    // a +Inf logit is its row's max, and exp(z - max) = exp(Inf - Inf) is NaN in the softmax this restates: the
-    // online state counted it as 1, so the row's sums are replaced by NaN here
+    // `any` comes from the CSR: degree-0 rows give out = 0 (a scatter_add of nothing), while a row whose logits are
+    // all -inf has S = 0 and gives T / S = NaN, as the softmax does.  A +Inf logit is its row's max, and
+    // exp(z - max) = exp(Inf - Inf) is NaN in the softmax this restates: the online state counted it as 1, so the
+    // row's sums are replaced by NaN here
     const float s = M[k] < CUDART_INF_F ? S[k] : CUDART_NAN_F;
     o[k] = any ? T[k] / s : 0.f;
     l[k] = any ? M[k] + log2f(s) : 0.f;

@@ -73,7 +73,7 @@ struct StreamParams {
   const int *idx2;
   const float *B;
   // multi-head form with DROP: the attention carries an attention-dropout mask in its sign bit (edge_softmax.cu,
-  // MODE 2); a kept entry is read as att * drop_scale, a dropped one as 0 (drop_att, common.cuh).  Read only by
+  // MODE 2); a kept entry is read as att * drop_scale, a dropped one as |att| * 0 (drop_att, common.cuh).  Read only by
   // the multi-head form, which takes the DROP instantiation iff drop_scale > 0.
   float drop_scale;
   SpmmEpilogue epi;   // the plain SpMM's store epilogue

@@ -38,20 +38,36 @@ def test_every_named_entry_is_in_the_header():
 
 # Every row id.  A row that goes missing from the table fails here, even when its entry point keeps other rows.
 ROW_IDS = {
+    "disen_route_fwd-overflow-K3F6",
     "edge_softmax-logits-H1",
     "edge_softmax-logits-H4",
+    "edge_softmax_bwd-grad_out-H4",
+    "edge_softmax_bwd-saved-H4",
+    "gat_attn_bwd-grad_out-H4",
+    "gat_attn_bwd-saved-H4",
+    "gat_attn_bwd_dropout-grad_out-H4",
+    "gat_attn_bwd_dropout-saved-H4",
     "gcn_fused-features-K128",
     "gcn_fused-overflow-K128",
     "genconv_edge_fwd-features-F67",
+    "hgn_attn-logits-H4",
+    "hgn_attn_bwd-grad_out-H4",
+    "hgn_attn_bwd-saved-H4",
     "mhspmm-attention-H4F11",
+    "mhspmm_dropout-attention-H4F11",
     "residual-Z-F67",
+    "residual_dcoef-b_dev-F67",
     "sage_fused-max-features-K128",
     "sage_fused-mean-features-K128",
     "sage_fused-sum-features-K128",
     "scatter_max-features-F67",
+    "scatter_max_bwd-grad_out-F67",
     "sddmm-features-F67",
+    "softmax_aggr_bwd-grad_out-F67",
+    "softmax_aggr_bwd-overflow-F67",
     "softmax_aggr_fwd-edge_term-F67",
     "softmax_aggr_fwd-features-F67",
+    "softmax_aggr_fwd-overflow-F67",
     "spmm-features-F67",
     "spmm-weights-F67",
     "spmm_f16-overflow-F66",
