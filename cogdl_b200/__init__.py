@@ -24,8 +24,9 @@ from .operators import (  # noqa: E402,F401
 )
 from .structure import membership_for  # noqa: E402,F401
 from .install import (  # noqa: E402,F401
-    install, uninstall_actnn, uninstall_appnp, uninstall_correct_smooth, uninstall_gat, uninstall_gcnii, uninstall_gin,
-    uninstall_grand, uninstall_readout, uninstall_rgcn, uninstall_spspmm, install_simple_hgn, uninstall_simple_hgn,
+    install, uninstall, uninstall_actnn, uninstall_appnp, uninstall_compgcn, uninstall_correct_smooth, uninstall_disengcn,
+    uninstall_gat, uninstall_gcnii, uninstall_genconv, uninstall_gin, uninstall_grand, uninstall_readout, uninstall_rgcn,
+    uninstall_spspmm, install_simple_hgn, uninstall_simple_hgn,
 )
 from . import sampling  # noqa: E402,F401
 

@@ -4,60 +4,98 @@ Plug-in point (SURVEY 8b): the module-global dict `cogdl.utils.spmm_utils.CONFIG
 `cogdl.operators.*` module attributes; layer modules capture the callables at construction
 (SpMM.__init__ cogdl/utils/spmm_utils.py:131, EdgeSoftmax.__init__ :195, MultiHeadSpMM.__init__
 :234-235, MaxAggregator.__init__ cogdl/layers/sage_layer.py:22-25), so call install() BEFORE
-building models.  Two levels are patched:
+building models.
 
-  1. operator level -- CONFIGS["fast_spmm" | "csr_edge_softmax" | "csrmhspmm" | "fused_gat_func"]
-     and cogdl.operators.{spmm.csrspmm, edge_softmax.csr_edge_softmax, mhspmm.csrmhspmm,
-     scatter_max.scatter_max, fused_gat.fused_gat_func}, with the *_flag latches set so the lazy
-     initialisers do not overwrite them;
-  2. dispatch level -- every already-imported cogdl module attribute that IS the reference's
-     spmm / edge_softmax / mh_spmm / fused_gat_op function (or SpMM / EdgeSoftmax / MultiHeadSpMM
-     / FusedGATOp class) is rebound to this package's version, which keeps the int32 CSR, hub
-     plan and transpose cached on the graph instead of re-casting per call.
+Every change install() makes goes through one primitive, _rebind(feature, owner, name, new): owner is an object
+(a class or module, set with setattr) or a dict (sys.modules, CONFIGS).  It records (feature, owner, name, old) in
+one undo log, old being _MISSING when owner had no such name of its own, and does nothing when owner.name already
+is new: that is what makes a repeated install() a no-op.  A function of this module that it puts in place is
+marked with the attribute _cogdl_b200 (True), so a caller can tell it from the reference's; install() never reads
+the mark.  A replacement that falls back to the original finds it at owner._cogdl_b200_original_<name>, set (and
+logged) by the same call, and read at call time, so assigning it routes the fallback elsewhere.  uninstall_<flag>() replays that flag's records newest first, uninstall() the whole log.
 
-With genconv=True, `cogdl.layers.deepergcn_layer.GENConv.forward` (DeeperGCN, RevGCN) is also rebound, to
-genconv_forward below, which sends the aggregation to cogdl_b200.genconv_aggregate.  The original forward stays
-reachable as GENConv._cogdl_b200_original_forward (uninstall_genconv() restores it).  disengcn=True does the same for
-`cogdl.layers.disengcn_layer.DisenGCNLayer.forward` (DisenGCN), with disengcn_forward and cogdl_b200.disen_routing
-(uninstall_disengcn()).  compgcn=True rebinds `cogdl.models.nn.compgcn.CompGCNLayer.forward` (CompGCN) to
-compgcn_forward, which sends the message passing to cogdl_b200.compgcn_aggregate (uninstall_compgcn()).
-gat=True rebinds `cogdl.layers.gat_layer.GATLayer.forward` (GAT and every model built on GATLayer) to gat_forward, which
-sends the attention, its dropout and the aggregation to the fused GAT kernels (uninstall_gat()).
-spspmm=True provides torch_sparse's spspmm / spmm (cogdl_b200.spspmm / coo_spmm) to GTN, SRGCN and Graph U-Net, through a
-`torch_sparse` stand-in module when the real package is missing (install_spspmm, uninstall_spspmm()).
-actnn=True provides the `actnn` API (cogdl_b200.actnn) to ActGCN, GCNII(actnn=True), GraphSAGE(actnn=True) and the trainer's
---actnn, through an `actnn` stand-in package when the real one does not import (install_actnn, uninstall_actnn()).
-gcnii=True rebinds `cogdl.layers.gcnii_layer.GCNIILayer.forward` (GCNII) to gcnii_forward and appnp=True
-`cogdl.models.nn.ppnp.PPNP.forward` (APPNP) to appnp_forward; both send the initial-residual propagation to
-cogdl_b200.spmm_residual (uninstall_gcnii(), uninstall_appnp()).
-correct_smooth=True rebinds the module globals `outcome_correlation` and `diffusion` of `cogdl.models.nn.correct_smooth`
-(Correct & Smooth, CorrectSmoothMLP) to outcome_correlation / diffusion below: the propagation loops with the clamp or
-the row reset go to cogdl_b200.label_propagate, the p = 1 diffusion steps to cogdl_b200.spmm_residual.  The originals
-stay reachable as `_cogdl_b200_original_outcome_correlation` / `_cogdl_b200_original_diffusion` on that module
-(uninstall_correct_smooth() restores them).
-gin=True rebinds `cogdl.layers.gin_layer.GINLayer.forward` (GIN, InfoGraph, GCC) and `cogdl.layers.gine_layer.GINELayer.forward`
-to gin_forward / gine_forward, which send `(1 + eps) * x + spmm(graph, x)` to cogdl_b200.gin_aggregate (uninstall_gin()).
-grand=True rebinds `cogdl.models.nn.grand.Grand.rand_prop` (GRAND) to grand_rand_prop, which keeps the reference's DropNode
-draw and sends the propagation to cogdl_b200.random_propagate (uninstall_grand()).
-rgcn=True rebinds `cogdl.layers.rgcn_layer.RGCNLayer.forward` (RGCN, LinkPredictRGCN) to rgcn_forward, which computes the
-relational sum with cogdl_b200.rgcn_conv (uninstall_rgcn()).  This deliberately differs from the original for more than
-one relation: the original aggregates every edge with the weight of the first relation that has edges (see
-rgcn_forward).
-readout=True rebinds cogdl.utils.batch_{sum,mean,max}_pooling (and every cogdl module attribute bound to them) to the
-deterministic, sync-free cogdl_b200 readouts, and `cogdl.models.nn.gin.GIN.forward`, `cogdl.models.nn.sortpool.SortPool.forward`
-and `cogdl.layers.set2set.Set2Set.forward` to gin_model_forward / sortpool_forward / set2set_forward (graph_readout,
-sort_pool, set2set_attention); InfoGraph and GCC take the pooling function at construction, so install before building
-models.  set2set_forward deliberately differs from an original that cannot run (see set2set_forward;
-uninstall_readout()).
-The Simple-HGN example's layer (examples/simple_hgn/conv.py, myGATConv) is not part of the cogdl package, so it has no
-install() flag: install_simple_hgn(conv_cls) rebinds the class the caller passes to simple_hgn_forward, which sends the
-attention to cogdl_b200.hgn_attention (uninstall_simple_hgn(conv_cls)).
+The base step (always) fills CONFIGS and the cogdl.operators.* modules, seeding a module that is not imported yet,
+routes the sampler to the device, and, with rebind_dispatch, rebinds every imported cogdl.* module attribute that IS
+the reference's spmm / edge_softmax / mh_spmm / fused_gat_op (or SpMM / EdgeSoftmax / MultiHeadSpMM / FusedGATOp
+class) to this package's version, which keeps the int32 CSR, hub plan and transpose cached on the graph.  Each flag
+is one entry of _FEATURES: the class methods it rebinds, or for correct_smooth, spspmm, actnn and readout a small
+installer; what each replacement computes and when it falls back is documented on the replacement.  The Simple-HGN
+example's layer is not part of the cogdl package, so install_simple_hgn(conv_cls) takes the class.
 """
+import importlib
 import sys
+import types
+from functools import partial
 
 import torch
 
 from .structure import graph_operands, unsupported_operands
+
+_MISSING = object()
+_log = []   # (feature, owner, name, old), oldest first
+
+
+def _put(owner, name, value):
+    if isinstance(owner, dict):
+        if value is _MISSING:
+            owner.pop(name, None)
+        else:
+            owner[name] = value
+    elif value is _MISSING:
+        if name in vars(owner):
+            delattr(owner, name)
+    else:
+        setattr(owner, name, value)
+
+
+def _rebind(feature, owner, name, new, label=None, keep_original=False):
+    """owner.name (owner[name] for a dict) = new, logged under feature; nothing when it already is new.  With
+    keep_original, the value it replaces also goes to owner._cogdl_b200_original_<name>.  Returns [label] when it
+    rebinds and a label is given, else []."""
+    own = owner if isinstance(owner, dict) else vars(owner)
+    current = own.get(name, _MISSING) if own is owner else getattr(owner, name, _MISSING)
+    if current is new:
+        return []
+    if keep_original:
+        _rebind(feature, owner, "_cogdl_b200_original_" + name, current)
+    if isinstance(new, types.FunctionType) and new.__module__ == __name__:
+        new._cogdl_b200 = True     # tells a caller the name holds one of this module's replacements
+    _log.append((feature, owner, name, own.get(name, _MISSING)))
+    _put(owner, name, new)
+    return [label] if label else []
+
+
+def _undo(feature=None):
+    """Put back what `feature` rebound (everything when None), newest first."""
+    for i in reversed(range(len(_log))):
+        f, owner, name, old = _log[i]
+        if feature is None or f == feature:
+            _put(owner, name, old)
+            del _log[i]
+
+
+def _rebind_everywhere(feature, pairs):
+    """Rebind every attribute of an imported cogdl.* module that is the first of one of the (original, replacement)
+    pairs to the second."""
+    by_id = {id(old): new for old, new in pairs}
+    patched = []
+    for mname, mod in list(sys.modules.items()):
+        if mod is None or not (mname == "cogdl" or mname.startswith("cogdl.")):
+            continue
+        for attr, val in list(vars(mod).items()):
+            if id(val) in by_id:
+                patched += _rebind(feature, mod, attr, by_id[id(val)], f"{mname}.{attr}")
+    return patched
+
+
+def _rebind_methods(feature, targets):
+    """Rebind each (module, class, attribute, replacement) of targets, keeping the original for the fallback."""
+    patched = []
+    for mname, cname, attr, new in targets:
+        cls = getattr(importlib.import_module(mname), cname)
+        patched += _rebind(feature, cls, attr, new, f"{mname}.{cname}.{attr}", keep_original=True)
+    return patched
+
 
 _GENCONV_KERNEL_AGGRS = ("softmax_sg", "softmax", "mean", "sum", "max", "powermean")
 
@@ -111,33 +149,6 @@ def _fused_edge_encoder_weight(encoder, attr, F):
     return w
 
 
-def _rebind_forward(cls, forward, name, attr="forward"):
-    """cls.<attr> (forward by default) = forward, keeping the original at cls._cogdl_b200_original_<attr>; idempotent."""
-    if getattr(getattr(cls, attr), "_cogdl_b200", False):
-        return []
-    setattr(cls, "_cogdl_b200_original_" + attr, getattr(cls, attr))
-    forward._cogdl_b200 = True
-    setattr(cls, attr, forward)
-    return [name]
-
-
-def _restore_forward(cls, attr="forward"):
-    if getattr(getattr(cls, attr), "_cogdl_b200", False):
-        setattr(cls, attr, getattr(cls, "_cogdl_b200_original_" + attr))
-
-
-def install_genconv():
-    import cogdl.layers.deepergcn_layer as dl
-
-    return _rebind_forward(dl.GENConv, genconv_forward, "cogdl.layers.deepergcn_layer.GENConv.forward")
-
-
-def uninstall_genconv():
-    import cogdl.layers.deepergcn_layer as dl
-
-    _restore_forward(dl.GENConv)
-
-
 def disengcn_forward(self, graph, x):
     """DisenGCNLayer.forward (cogdl/layers/disengcn_layer.py:40-91) with the routing in the sm_90a kernels: the
     layer's own weight, bias and activation give h, and cogdl_b200.disen_routing does the per-channel
@@ -152,18 +163,6 @@ def disengcn_forward(self, graph, x):
         return original(self, graph, x)
     h = self.activation(torch.matmul(x, self.weight) + self.bias)
     return disen_routing(graph_operands(graph).st, h, K, self.iterations, self.tau)
-
-
-def install_disengcn():
-    import cogdl.layers.disengcn_layer as dl
-
-    return _rebind_forward(dl.DisenGCNLayer, disengcn_forward, "cogdl.layers.disengcn_layer.DisenGCNLayer.forward")
-
-
-def uninstall_disengcn():
-    import cogdl.layers.disengcn_layer as dl
-
-    _restore_forward(dl.DisenGCNLayer)
 
 
 def compgcn_forward(self, graph, x, rel_embed):
@@ -196,18 +195,6 @@ def compgcn_forward(self, graph, x, rel_embed):
     return self.activation(out), torch.matmul(rel_embed, self.weight_rel)[:-1]
 
 
-def install_compgcn():
-    import cogdl.models.nn.compgcn as cm
-
-    return _rebind_forward(cm.CompGCNLayer, compgcn_forward, "cogdl.models.nn.compgcn.CompGCNLayer.forward")
-
-
-def uninstall_compgcn():
-    import cogdl.models.nn.compgcn as cm
-
-    _restore_forward(cm.CompGCNLayer)
-
-
 def gat_forward(self, graph, x):
     """GATLayer.forward (cogdl/layers/gat_layer.py:59-86) with the attention, its dropout and the aggregation in the
     fused sm_90a GAT kernels, for any graph (the backward uses the cached transpose, not is_symmetric()).  The layer's
@@ -236,18 +223,6 @@ def gat_forward(self, graph, x):
     return out
 
 
-def install_gat():
-    import cogdl.layers.gat_layer as gl
-
-    return _rebind_forward(gl.GATLayer, gat_forward, "cogdl.layers.gat_layer.GATLayer.forward")
-
-
-def uninstall_gat():
-    import cogdl.layers.gat_layer as gl
-
-    _restore_forward(gl.GATLayer)
-
-
 def gcnii_forward(self, graph, x, init_x):
     """GCNIILayer.forward (cogdl/layers/gcnii_layer.py:24-30) with the propagation `(1 - alpha) * spmm(graph, x) +
     alpha * init_x` in one cogdl_b200.spmm_residual launch, and the identity mapping `beta * linear(s) + (1 - beta) * s`
@@ -270,18 +245,6 @@ def gcnii_forward(self, graph, x, init_x):
     if self.residual:
         h = h + x
     return h
-
-
-def install_gcnii():
-    import cogdl.layers.gcnii_layer as gl
-
-    return _rebind_forward(gl.GCNIILayer, gcnii_forward, "cogdl.layers.gcnii_layer.GCNIILayer.forward")
-
-
-def uninstall_gcnii():
-    import cogdl.layers.gcnii_layer as gl
-
-    _restore_forward(gl.GCNIILayer)
 
 
 def appnp_forward(self, graph):
@@ -309,18 +272,6 @@ def appnp_forward(self, graph):
         for _ in range(self.niter):
             preds = spmm_residual(graph, preds, local_preds, 1 - self.alpha, self.alpha)
     return preds
-
-
-def install_appnp():
-    import cogdl.models.nn.ppnp as pm
-
-    return _rebind_forward(pm.PPNP, appnp_forward, "cogdl.models.nn.ppnp.PPNP.forward")
-
-
-def uninstall_appnp():
-    import cogdl.models.nn.ppnp as pm
-
-    _restore_forward(pm.PPNP)
 
 
 def _correct_smooth_module():
@@ -375,22 +326,12 @@ def diffusion(g, x, nhtop, p=1, alpha=0.5):
 
 def install_correct_smooth():
     """Rebind cogdl.models.nn.correct_smooth.outcome_correlation and diffusion (resolved as module globals at call
-    time by CorrectSmooth.__call__ and CorrectSmoothMLP.forward), keeping the originals on the module; idempotent."""
+    time by CorrectSmooth.__call__ and CorrectSmoothMLP.forward), keeping the originals on the module."""
     cs = _correct_smooth_module()
     patched = []
     for name, new in (("outcome_correlation", outcome_correlation), ("diffusion", diffusion)):
-        if getattr(cs, name) is not new:
-            setattr(cs, "_cogdl_b200_original_" + name, getattr(cs, name))
-            setattr(cs, name, new)
-            patched.append(f"cogdl.models.nn.correct_smooth.{name}")
+        patched += _rebind("correct_smooth", cs, name, new, f"cogdl.models.nn.correct_smooth.{name}", keep_original=True)
     return patched
-
-
-def uninstall_correct_smooth():
-    cs = _correct_smooth_module()
-    for name, new in (("outcome_correlation", outcome_correlation), ("diffusion", diffusion)):
-        if getattr(cs, name) is new:
-            setattr(cs, name, getattr(cs, "_cogdl_b200_original_" + name))
 
 
 def _gin_unsupported(self, graph, x):
@@ -418,22 +359,6 @@ def gine_forward(self, graph, x):
     return gin_forward(self, graph, x)
 
 
-def install_gin():
-    import cogdl.layers.gin_layer as gl
-    import cogdl.layers.gine_layer as gel
-
-    return (_rebind_forward(gl.GINLayer, gin_forward, "cogdl.layers.gin_layer.GINLayer.forward")
-            + _rebind_forward(gel.GINELayer, gine_forward, "cogdl.layers.gine_layer.GINELayer.forward"))
-
-
-def uninstall_gin():
-    import cogdl.layers.gin_layer as gl
-    import cogdl.layers.gine_layer as gel
-
-    _restore_forward(gl.GINLayer)
-    _restore_forward(gel.GINELayer)
-
-
 def grand_rand_prop(self, graph, x):
     """Grand.rand_prop (cogdl/models/nn/grand.py:98-104): the reference's own drop_node (the same torch.bernoulli on the
     CPU generator and `masks.to(device) * x`, so a seeded run draws the same mask; `x * (1 - p)` in eval mode), then the
@@ -445,18 +370,6 @@ def grand_rand_prop(self, graph, x):
         return type(self)._cogdl_b200_original_rand_prop(self, graph, x)
     x = self.drop_node(x)
     return random_propagate(graph, x, self.order)
-
-
-def install_grand():
-    import cogdl.models.nn.grand as gm
-
-    return _rebind_forward(gm.Grand, grand_rand_prop, "cogdl.models.nn.grand.Grand.rand_prop", attr="rand_prop")
-
-
-def uninstall_grand():
-    import cogdl.models.nn.grand as gm
-
-    _restore_forward(gm.Grand, attr="rand_prop")
 
 
 _RGCN_EYE = {}
@@ -508,18 +421,6 @@ def rgcn_forward(self, graph, x):
     return h_result
 
 
-def install_rgcn():
-    import cogdl.layers.rgcn_layer as rl
-
-    return _rebind_forward(rl.RGCNLayer, rgcn_forward, "cogdl.layers.rgcn_layer.RGCNLayer.forward")
-
-
-def uninstall_rgcn():
-    import cogdl.layers.rgcn_layer as rl
-
-    _restore_forward(rl.RGCNLayer)
-
-
 def simple_hgn_forward(self, graph, x, res_attn=None):
     """myGATConv.forward of CogDL's Simple-HGN example (examples/simple_hgn/conv.py) with the attention, its dropout,
     the residual-attention blend and the aggregation in cogdl_b200.hgn_attention.  The layer's own feat_drop, x @ W,
@@ -567,15 +468,16 @@ def simple_hgn_forward(self, graph, x, res_attn=None):
 def install_simple_hgn(conv_cls):
     """Rebind conv_cls.forward (the Simple-HGN example's myGATConv, which is not part of the cogdl package, so the
     caller passes the class) to simple_hgn_forward; the original stays at conv_cls._cogdl_b200_original_forward."""
-    return _rebind_forward(conv_cls, simple_hgn_forward, f"{conv_cls.__module__}.{conv_cls.__qualname__}.forward")
+    return _rebind(("simple_hgn", conv_cls), conv_cls, "forward", simple_hgn_forward,
+                   f"{conv_cls.__module__}.{conv_cls.__qualname__}.forward", keep_original=True)
 
 
 def uninstall_simple_hgn(conv_cls):
-    _restore_forward(conv_cls)
+    _undo(("simple_hgn", conv_cls))
 
 
 _READOUT_NAMES = ("batch_sum_pooling", "batch_mean_pooling", "batch_max_pooling")
-_readout_state = {"originals": None, "rebound": []}
+_POOLING = []   # (original, replacement): built once per process, so every install rebinds the same objects
 
 
 def _readout_supported(x, batch):
@@ -584,21 +486,20 @@ def _readout_supported(x, batch):
             and x.dim() == 2 and batch.dim() == 1 and x.shape[0] == batch.numel() and not batch.dtype.is_floating_point)
 
 
-def _pooling(mode):
-    from .operators.readout import graph_readout
-
-    name = f"batch_{mode}_pooling"
+def _pooling(name, original):
+    mode = name.split("_")[1]
 
     def pool(x, batch):
+        from .operators.readout import graph_readout
+
         if not _readout_supported(x, batch):
-            return _readout_state["originals"][name](x, batch)
+            return original(x, batch)
         return graph_readout([x], batch, mode)
 
     pool.__name__ = pool.__qualname__ = name
     pool.__doc__ = (f"cogdl.utils.{name} (cogdl/utils/utils.py) on cogdl_b200.{name}: deterministic, and no host read "
                     "once the batch's membership is cached; B is max(batch) + 1 and a graph id without nodes pools to 0 "
                     "(the original's mean counts only the ids present).  CPU or non-fp32 input runs the original.")
-    pool._cogdl_b200 = True
     return pool
 
 
@@ -684,66 +585,39 @@ def install_readout():
     """Rebind cogdl.utils.batch_{sum,mean,max}_pooling, and every attribute of an imported cogdl.* module bound to them,
     to the cogdl_b200 readouts; GIN.forward to gin_model_forward, SortPool.forward to sortpool_forward and
     Set2Set.forward to set2set_forward.  InfoGraph and GCC take the pooling function when a model is constructed, so
-    install before building models.  Idempotent; uninstall_readout() restores everything."""
-    import cogdl.layers.set2set as s2s
-    import cogdl.models.nn.gin as gm
-    import cogdl.models.nn.sortpool as sp
+    install before building models."""
+    import cogdl.layers.set2set  # noqa: F401  (imported before the scan, so their bindings are rebound too)
+    import cogdl.models.nn.gin  # noqa: F401
+    import cogdl.models.nn.sortpool  # noqa: F401
     import cogdl.utils.utils as uu
 
-    st = _readout_state
-    if st["originals"] is None:
-        st["originals"] = {n: getattr(uu, n) for n in _READOUT_NAMES}
-        st["new"] = {n: _pooling(n.split("_")[1]) for n in _READOUT_NAMES}
-    by_id = {id(st["originals"][n]): st["new"][n] for n in _READOUT_NAMES}
-    patched = []
-    for mname, mod in list(sys.modules.items()):
-        if mod is None or not (mname == "cogdl" or mname.startswith("cogdl.")):
-            continue
-        for attr, val in list(vars(mod).items()):
-            new = by_id.get(id(val))
-            if new is not None:
-                st["rebound"].append((mod, attr, val))
-                setattr(mod, attr, new)
-                patched.append(f"{mname}.{attr}")
-    return (patched + _rebind_forward(gm.GIN, gin_model_forward, "cogdl.models.nn.gin.GIN.forward")
-            + _rebind_forward(sp.SortPool, sortpool_forward, "cogdl.models.nn.sortpool.SortPool.forward")
-            + _rebind_forward(s2s.Set2Set, set2set_forward, "cogdl.layers.set2set.Set2Set.forward"))
-
-
-def uninstall_readout():
-    import cogdl.layers.set2set as s2s
-    import cogdl.models.nn.gin as gm
-    import cogdl.models.nn.sortpool as sp
-
-    for mod, attr, old in reversed(_readout_state["rebound"]):
-        setattr(mod, attr, old)
-    _readout_state["rebound"] = []
-    for cls in (gm.GIN, sp.SortPool, s2s.Set2Set):
-        _restore_forward(cls)
+    if not _POOLING:
+        _POOLING.extend((getattr(uu, n), _pooling(n, getattr(uu, n))) for n in _READOUT_NAMES)
+    return _rebind_everywhere("readout", _POOLING) + _rebind_methods("readout", (
+        ("cogdl.models.nn.gin", "GIN", "forward", gin_model_forward),
+        ("cogdl.models.nn.sortpool", "SortPool", "forward", sortpool_forward),
+        ("cogdl.layers.set2set", "Set2Set", "forward", set2set_forward)))
 
 
 _SPSPMM_MODULES = ("cogdl.models.nn.gtn", "cogdl.models.nn.srgcn", "cogdl.utils.srgcn_utils", "cogdl.models.nn.graph_unet")
-_spspmm_state = {"stub": None, "rebound": []}
 
 
 def install_spspmm():
     """torch_sparse's spspmm / spmm for GTN, SRGCN and Graph U-Net.  Without a loadable torch_sparse, a module of that
     name providing exactly those two functions goes into sys.modules, so the models import; an importable torch_sparse
-    is left alone.  Either way the two names are rebound in those of the four model modules already imported."""
-    import types
-
+    is left alone.  Either way the two names are rebound in those of the four model modules already imported (models
+    imported while the stand-in was there keep their binding after uninstall_spspmm())."""
     from .operators.spspmm import coo_spmm, spspmm
 
     patched = []
-    if _spspmm_state["stub"] is None and "torch_sparse" not in sys.modules:
+    if "torch_sparse" not in sys.modules:
         try:
             import torch_sparse  # noqa: F401
         except (ImportError, OSError):   # missing, or a binary build that does not load (undefined symbol)
             stub = types.ModuleType("torch_sparse")
             stub.__doc__ = "spspmm and spmm of cogdl_b200, seeded by cogdl_b200.install(spspmm=True)"
             stub.spspmm, stub.spmm = spspmm, coo_spmm
-            sys.modules["torch_sparse"] = _spspmm_state["stub"] = stub
-            patched.append("torch_sparse")
+            patched += _rebind("spspmm", sys.modules, "torch_sparse", stub, "torch_sparse")
     for mname in _SPSPMM_MODULES:
         mod = sys.modules.get(mname)
         if mod is None:
@@ -751,49 +625,32 @@ def install_spspmm():
         for attr, new in (("spspmm", spspmm), ("spmm", coo_spmm)):
             if attr == "spmm" and mname != "cogdl.utils.srgcn_utils":
                 continue   # srgcn.py's `spmm` is cogdl.utils.spmm (the graph SpMM), not torch_sparse's
-            old = getattr(mod, attr, None)
-            if old is not None and old is not new:
-                _spspmm_state["rebound"].append((mod, attr, old))
-                setattr(mod, attr, new)
-                patched.append(f"{mname}.{attr}")
+            if getattr(mod, attr, None) is not None:
+                patched += _rebind("spspmm", mod, attr, new, f"{mname}.{attr}")
     return patched
-
-
-def uninstall_spspmm():
-    """Undo install_spspmm: restore the rebound names and take the torch_sparse stand-in out of sys.modules (models
-    imported while it was there keep their binding)."""
-    for mod, attr, old in reversed(_spspmm_state["rebound"]):
-        setattr(mod, attr, old)
-    _spspmm_state["rebound"] = []
-    stub = _spspmm_state["stub"]
-    if stub is not None and sys.modules.get("torch_sparse") is stub:
-        del sys.modules["torch_sparse"]
-    _spspmm_state["stub"] = None
 
 
 _ACTNN_SUBMODULES = ("conf", "ops", "qscheme", "qbnscheme", "layers", "utils")
 _ACTNN_NAMES = {"cogdl.operators.linear": ("quantize_activation", "dequantize_activation", "config", "empty_cache"),
                 "cogdl.operators.spmm": ("quantize_activation", "dequantize_activation")}
-_actnn_state = {"stub": None, "rebound": []}
 
 
 def install_actnn():
     """The `actnn` API for CogDL's activation-compressed models.  Without an importable actnn, cogdl_b200.actnn and its
     submodules go into sys.modules as `actnn` and `actnn.<name>`, so the models' imports resolve to them; an importable
     actnn is left alone.  cogdl.operators.linear imports actnn inside a try at import time: if it was imported before,
-    its names are bound here."""
+    its names are bound here.  Modules imported while the stand-in was there keep their binding after
+    uninstall_actnn()."""
     from . import actnn as stub
 
     patched = []
-    if _actnn_state["stub"] is None and "actnn" not in sys.modules:
+    if "actnn" not in sys.modules:
         try:
             import actnn  # noqa: F401
         except (ImportError, OSError):   # missing, or a binary build that does not load
-            sys.modules["actnn"] = stub
+            patched += _rebind("actnn", sys.modules, "actnn", stub, "actnn")
             for name in _ACTNN_SUBMODULES:
-                sys.modules["actnn." + name] = getattr(stub, name)
-            _actnn_state["stub"] = stub
-            patched.append("actnn")
+                _rebind("actnn", sys.modules, "actnn." + name, getattr(stub, name))
     actnn_mod = sys.modules["actnn"]
     for mname, attrs in _ACTNN_NAMES.items():
         mod = sys.modules.get(mname)
@@ -801,44 +658,58 @@ def install_actnn():
             continue
         for attr in attrs:
             src = actnn_mod.conf if attr == "config" else (actnn_mod.utils if attr == "empty_cache" else actnn_mod.ops)
-            new, old = getattr(src, attr), getattr(mod, attr, None)
-            if old is not new:
-                _actnn_state["rebound"].append((mod, attr, old))
-                setattr(mod, attr, new)
-                patched.append(f"{mname}.{attr}")
+            patched += _rebind("actnn", mod, attr, getattr(src, attr), f"{mname}.{attr}")
     return patched
 
 
-def uninstall_actnn():
-    """Undo install_actnn: restore the bound names and take the actnn stand-in out of sys.modules (modules imported
-    while it was there keep their binding)."""
-    for mod, attr, old in reversed(_actnn_state["rebound"]):
-        if old is None:
-            delattr(mod, attr)
-        else:
-            setattr(mod, attr, old)
-    _actnn_state["rebound"] = []
-    if _actnn_state["stub"] is not None:
-        for name in ("actnn",) + tuple("actnn." + n for n in _ACTNN_SUBMODULES):
-            if sys.modules.get(name) is not None and getattr(sys.modules[name], "__name__", "").startswith("cogdl_b200."):
-                del sys.modules[name]
-    _actnn_state["stub"] = None
+def _host_sampler(name):
+    """The reference's own host function install() found at cogdl.data.data.<name>, for CPU graphs (no CPU path in
+    this package)."""
+    import cogdl.data.data as ref_data
+
+    original = getattr(ref_data, "_cogdl_b200_original_" + name)
+    if original is None:
+        raise RuntimeError("cogdl.operators.sample failed to load and the graph is on the CPU")
+    return original
 
 
-def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
-            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False, rgcn=False, readout=False):
+def sample_adj_c(indptr, indices, node_idx, num_neighbors=-1, replace=True):
+    """cogdl.data.data.sample_adj_c (what Graph.sample_adj calls, cogdl/data/data.py:792-832; SURVEY 8f-4): CUDA graphs
+    go to the device sampler, CPU graphs to the reference's own host function."""
+    from . import sampling
+
+    if not indptr.is_cuda:
+        return _host_sampler("sample_adj_c")(indptr, indices, node_idx, num_neighbors, replace)
+    node_idx = torch.as_tensor(node_idx, dtype=torch.int64).to(indptr.device)
+    rp, ci, nodes, edges = sampling.sample_adj(indptr, indices, node_idx, num_neighbors, replace)
+    # data.py:818-820 pads row_ptr for the new (edge-less) nodes with a CPU tensor; hand it over padded
+    pad = nodes.numel() + 1 - rp.numel()
+    if pad > 0:
+        rp = torch.cat([rp, rp[-1:].expand(pad)])
+    return rp, ci, nodes, edges
+
+
+def subgraph_c(indptr, indices, node_idx):
+    """cogdl.data.data.subgraph_c (what Graph.csr_subgraph calls, cogdl/data/data.py:856-874), routed as sample_adj_c."""
+    from . import sampling
+
+    if not indptr.is_cuda:
+        return _host_sampler("subgraph_c")(indptr, indices, node_idx)
+    return sampling.subgraph(indptr, indices, node_idx.to(indptr.device))
+
+
+def _install_base(rebind_dispatch):
     import cogdl.utils.spmm_utils as ref_su  # raises ImportError if cogdl is not importable
 
     from . import operators as ops
     from .utils import spmm_utils as su
 
-    ref_su.CONFIGS.update({
+    for key, value in {
         "fast_spmm": ops.csrspmm, "csr_edge_softmax": ops.csr_edge_softmax, "csrmhspmm": ops.csrmhspmm,
         "fused_gat_func": ops.fused_gat_func,
         "spmm_flag": True, "mh_spmm_flag": True, "fused_gat_flag": True,
-    })
-    import types
-
+    }.items():
+        _rebind("base", ref_su.CONFIGS, key, value)
     import cogdl.operators as ref_ops_pkg
 
     for mod_name, attrs in (
@@ -855,81 +726,71 @@ def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, 
             # and the reference's import-time JIT build of its own CUDA sources never runs.
             mod = types.ModuleType(mod_name)
             mod.__doc__ = "seeded by cogdl_b200.install()"
-            sys.modules[mod_name] = mod
-            setattr(ref_ops_pkg, mod_name.rsplit(".", 1)[1], mod)
+            _rebind("base", sys.modules, mod_name, mod)
+            _rebind("base", ref_ops_pkg, mod_name.rsplit(".", 1)[1], mod)
         for k, v in attrs.items():
-            setattr(mod, k, v)
+            _rebind("base", mod, k, v)
+    import cogdl.data.data as ref_data
 
     patched = []
-    # Device sampler (SURVEY 8f-4): Graph.sample_adj / csr_subgraph (cogdl/data/data.py:792-874) resolve the
-    # module globals `sample_adj_c` / `subgraph_c`.  CUDA graphs go to the device sampler; CPU graphs keep
-    # the reference's own host functions (they are not ours to replace: no CPU path in this package).
-    import cogdl.data.data as ref_data
-    from . import sampling
-
-    ref_sample, ref_subgraph = getattr(ref_data, "sample_adj_c", None), getattr(ref_data, "subgraph_c", None)
-    if not getattr(ref_sample, "_cogdl_b200", False):
-        def sample_adj_c(indptr, indices, node_idx, num_neighbors=-1, replace=True):
-            if not indptr.is_cuda:
-                if ref_sample is None:
-                    raise RuntimeError("cogdl.operators.sample failed to load and the graph is on the CPU")
-                return ref_sample(indptr, indices, node_idx, num_neighbors, replace)
-            import torch
-
-            node_idx = torch.as_tensor(node_idx, dtype=torch.int64).to(indptr.device)
-            rp, ci, nodes, edges = sampling.sample_adj(indptr, indices, node_idx, num_neighbors, replace)
-            # data.py:818-820 pads row_ptr for the new (edge-less) nodes with a CPU tensor; hand it over padded
-            pad = nodes.numel() + 1 - rp.numel()
-            if pad > 0:
-                rp = torch.cat([rp, rp[-1:].expand(pad)])
-            return rp, ci, nodes, edges
-
-        def subgraph_c(indptr, indices, node_idx):
-            if not indptr.is_cuda:
-                if ref_subgraph is None:
-                    raise RuntimeError("cogdl.operators.sample failed to load and the graph is on the CPU")
-                return ref_subgraph(indptr, indices, node_idx)
-            return sampling.subgraph(indptr, indices, node_idx.to(indptr.device))
-
-        sample_adj_c._cogdl_b200 = subgraph_c._cogdl_b200 = True
-        ref_data.sample_adj_c, ref_data.subgraph_c = sample_adj_c, subgraph_c
-        patched += ["cogdl.data.data.sample_adj_c", "cogdl.data.data.subgraph_c"]
+    for name, new in (("sample_adj_c", sample_adj_c), ("subgraph_c", subgraph_c)):
+        patched += _rebind("base", ref_data, name, new, f"cogdl.data.data.{name}", keep_original=True)
     if rebind_dispatch:
         names = ["spmm", "edge_softmax", "mh_spmm", "fused_gat_op", "check_fused_gat", "SpMM", "EdgeSoftmax",
                  "MultiHeadSpMM", "FusedGATOp"]
-        originals = {id(getattr(ref_su, n)): getattr(su, n) for n in names if hasattr(ref_su, n)}
-        for mname, mod in list(sys.modules.items()):
-            if mod is None or not (mname == "cogdl" or mname.startswith("cogdl.")):
-                continue
-            for attr, val in list(vars(mod).items()):
-                new = originals.get(id(val))
-                if new is not None and val is not new:
-                    setattr(mod, attr, new)
-                    patched.append(f"{mname}.{attr}")
-    if genconv:
-        patched += install_genconv()
-    if disengcn:
-        patched += install_disengcn()
-    if compgcn:
-        patched += install_compgcn()
-    if spspmm:
-        patched += install_spspmm()
-    if gat:
-        patched += install_gat()
-    if actnn:
-        patched += install_actnn()
-    if gcnii:
-        patched += install_gcnii()
-    if appnp:
-        patched += install_appnp()
-    if correct_smooth:
-        patched += install_correct_smooth()
-    if gin:
-        patched += install_gin()
-    if grand:
-        patched += install_grand()
-    if rgcn:
-        patched += install_rgcn()
-    if readout:
-        patched += install_readout()
+        patched += _rebind_everywhere("base", [(getattr(ref_su, n), getattr(su, n)) for n in names if hasattr(ref_su, n)])
     return patched
+
+
+_FEATURES = {   # install() flag -> the class methods it rebinds (module, class, attribute, replacement) or its
+                # installer, in the order install() applies them
+    "genconv": (("cogdl.layers.deepergcn_layer", "GENConv", "forward", genconv_forward),),
+    "disengcn": (("cogdl.layers.disengcn_layer", "DisenGCNLayer", "forward", disengcn_forward),),
+    "compgcn": (("cogdl.models.nn.compgcn", "CompGCNLayer", "forward", compgcn_forward),),
+    "spspmm": install_spspmm,
+    "gat": (("cogdl.layers.gat_layer", "GATLayer", "forward", gat_forward),),
+    "actnn": install_actnn,
+    "gcnii": (("cogdl.layers.gcnii_layer", "GCNIILayer", "forward", gcnii_forward),),
+    "appnp": (("cogdl.models.nn.ppnp", "PPNP", "forward", appnp_forward),),
+    "correct_smooth": install_correct_smooth,
+    "gin": (("cogdl.layers.gin_layer", "GINLayer", "forward", gin_forward),
+            ("cogdl.layers.gine_layer", "GINELayer", "forward", gine_forward)),
+    "grand": (("cogdl.models.nn.grand", "Grand", "rand_prop", grand_rand_prop),),
+    "rgcn": (("cogdl.layers.rgcn_layer", "RGCNLayer", "forward", rgcn_forward),),
+    "readout": install_readout,
+}
+
+
+def _install(feature):
+    how = _FEATURES[feature]
+    return how() if callable(how) else _rebind_methods(feature, how)
+
+
+def install(rebind_dispatch=True, genconv=False, disengcn=False, compgcn=False, spspmm=False, gat=False, actnn=False,
+            gcnii=False, appnp=False, correct_smooth=False, gin=False, grand=False, rgcn=False, readout=False):
+    """Register the backend in the imported cogdl package, plus each feature whose flag is set; returns the names
+    rebound, in the order rebound (a repeated call rebinds nothing and returns [])."""
+    flags = locals()    # the keyword arguments, by name
+    patched = _install_base(rebind_dispatch)
+    for feature in _FEATURES:
+        if flags[feature]:
+            patched += _install(feature)
+    return patched
+
+
+def uninstall():
+    """Put back everything install() and install_simple_hgn() rebound."""
+    _undo()
+
+
+install_genconv, uninstall_genconv = partial(_install, "genconv"), partial(_undo, "genconv")
+install_disengcn, uninstall_disengcn = partial(_install, "disengcn"), partial(_undo, "disengcn")
+install_compgcn, uninstall_compgcn = partial(_install, "compgcn"), partial(_undo, "compgcn")
+install_gat, uninstall_gat = partial(_install, "gat"), partial(_undo, "gat")
+install_gcnii, uninstall_gcnii = partial(_install, "gcnii"), partial(_undo, "gcnii")
+install_appnp, uninstall_appnp = partial(_install, "appnp"), partial(_undo, "appnp")
+install_gin, uninstall_gin = partial(_install, "gin"), partial(_undo, "gin")
+install_grand, uninstall_grand = partial(_install, "grand"), partial(_undo, "grand")
+install_rgcn, uninstall_rgcn = partial(_install, "rgcn"), partial(_undo, "rgcn")
+uninstall_spspmm, uninstall_actnn = partial(_undo, "spspmm"), partial(_undo, "actnn")
+uninstall_correct_smooth, uninstall_readout = partial(_undo, "correct_smooth"), partial(_undo, "readout")
